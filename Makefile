@@ -1,9 +1,9 @@
-# Builds everything in-tree: the product library (hand-written sm_100a CUDA behind the C ABI),
+# Builds everything in-tree: the product library (hand-written sm_90a (H100) CUDA behind the C ABI),
 # the synthetic tipset builder and the CPU oracle (test infrastructure).
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CSRC      := ipc_filecoin_proofs_b200/csrc
-NVFLAGS   := -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr
+NVFLAGS   := -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr
 CU_SRCS   := $(CSRC)/store.cu $(CSRC)/events.cu $(CSRC)/storage.cu $(CSRC)/witness.cu $(CSRC)/prims.cu $(CSRC)/parallel.cu $(CSRC)/verify.cu $(CSRC)/capi.cu
 CU_OBJS   := $(CU_SRCS:.cu=.o)
 CU_HDRS   := $(wildcard $(CSRC)/*.cuh) include/ipcfp.h
@@ -11,7 +11,8 @@ LIB       := ipc_filecoin_proofs_b200/libipcfp.so
 
 all: $(LIB) synth/libipcfp_synth.so oracle/liboracle.so
 
-$(CSRC)/%.o: $(CSRC)/%.cu $(CU_HDRS)
+# objects depend on this file too: a change of NVFLAGS (the target architecture) rebuilds them
+$(CSRC)/%.o: $(CSRC)/%.cu $(CU_HDRS) Makefile
 	$(NVCC) $(NVFLAGS) $(EXTRA_NVFLAGS) -c $< -o $@
 
 $(CSRC)/bundle_json.o: $(CSRC)/bundle_json.cpp include/ipcfp.h
@@ -29,7 +30,7 @@ endif
 LIB_OUT ?= $(LIB)
 
 $(LIB_OUT): $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o $(CSRC)/exports.map
-	$(NVCC) -shared -gencode arch=compute_100a,code=sm_100a $(LIB_LDFLAGS) -o $@ $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o -lcudart -ldl
+	$(NVCC) -shared -gencode arch=compute_90a,code=sm_90a $(LIB_LDFLAGS) -o $@ $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o -lcudart -ldl
 
 synth/libipcfp_synth.so: synth/synth.cpp synth/synth.h synth/cpu_crypto.h
 	$(CXX) -O2 -std=c++17 -fPIC -shared -pthread -o $@ synth/synth.cpp

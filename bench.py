@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — receipts/sec scanned (+ witness bytes/sec) of the event-proof hot path on B200.
+"""bench.py — receipts/sec scanned (+ witness bytes/sec) of the event-proof hot path on H100.
 
   python bench.py --gpus N --steps K --warmup W            # this engine (CUDA, through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU algorithm (oracle), host cores
+  python bench.py ... --dump-outputs DIR                    # also write the last timed step's results as DIR/<name>.npy
 
 One "step" = one generate_event_proof over the synthetic tipset of BASELINE.json configs[3]
 (1 M receipts x 8 events, 0.1 % match rate, events-AMT bit widths 3/5): message-AMT walk + execution
@@ -55,7 +56,7 @@ def build_tipset(world, rank):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -114,20 +115,46 @@ def dist_env():
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (700 W card; not a measured figure)"
 
 
-def pass1_traffic():
-    """dram bytes per k_pass1 launch from the committed ncu --set full capture, if any."""
+def gpu_info(gpu_index):
+    """Name and power limit of the card the numbers were measured on."""
     try:
-        with open(os.path.join(ROOT, "profiles", "pass1_traffic.json")) as f:
-            return json.load(f).get("dram_bytes_per_launch")
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clk = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clk)}
     except Exception:
         return None
+
+
+def dump_outputs(dirpath, res):
+    """Writes what generate_event_proof returned (an EventResultPy) as DIR/<name>.npy, float64 for indices and counts, float32 for bytes.
+    The witness is large (≈ 147 k blocks, 51 MB at 1 M receipts): a fixed, seeded sample of its rows is written, the same rows for CIDs,
+    lengths and block bytes, so that two builds given the same arguments can be compared array for array (≈ 30 MB in all)."""
+    from ipc_filecoin_proofs_b200 import _abi as A
+    os.makedirs(dirpath, exist_ok=True)
+    w = res.witness
+    m = w.n_blocks
+    rows = np.arange(m) if m <= 16384 else np.sort(np.random.default_rng(0).choice(m, 16384, replace=False))
+    blocks = np.frombuffer(b"".join(w.block(int(i)) for i in rows), dtype=np.uint8)[: 8 << 20]
+    raw = np.frombuffer(res.raw_proofs.tobytes(), dtype=A.EventProofC).reshape(-1) if len(res.proofs) else None
+    fields = ("exec_index", "event_index", "emitter", "n_topics", "data_len", "data_off", "topics_off")
+    out = {
+        "counts": np.array([len(res.matching), len(res.proofs), m, w.total_bytes, res.n_exec], dtype=np.float64),
+        "matching": res.matching.astype(np.float64),
+        "proof_fields": np.stack([raw[f].astype(np.float64) for f in fields], axis=1) if raw is not None else np.zeros((0, len(fields))),
+        "proof_message_cids": np.array([list(p.message_cid) for p in res.proofs], dtype=np.float32).reshape(-1, A.CID_LEN),
+        "proof_data_blob": res.data_blob.astype(np.float32),
+        "witness_sample_rows": rows.astype(np.float64),
+        "witness_cids": w.cids[rows].astype(np.float32),
+        "witness_lengths": w.lengths[rows].astype(np.float64),
+        "witness_block_bytes": blocks.astype(np.float32),
+    }
+    for k, v in out.items():
+        np.save(os.path.join(dirpath, k + ".npy"), v)
+    return sorted(out)
 
 
 WORKLOAD = ("BASELINE.json configs[3] per GPU: 1M receipts x 8 events, 0.1% match, events-AMT bit-widths 3/5; generate_event_proof "
@@ -141,7 +168,7 @@ def config_dict(world, n_local, **extra):
     d.update({"workload": WORKLOAD + ("" if world == 1 else f"; N={world}: ONE {world}M-receipt tipset sharded by receipt index range (configs[4] shape at N=8), "
                                  "in-library NCCL protocol: all-to-all + all-reduce for the first-seen dedup of the execution order, all-gather of the witness CID sets"),
          "receipts_per_gpu": int(n_local), "receipts_total": int(n_local) * world,
-         "l2": "inputs (1.15 GB/GPU) exceed the 126 MB L2; no flush needed"})
+         "l2": "inputs (1.15 GB/GPU) exceed the 50 MB L2; no flush needed"})
     d.update(extra)
     return d
 
@@ -325,7 +352,8 @@ def run_engine(args, world, rank, local):
 
     stats = {}
 
-    def step_resident(full=True):
+    def step_resident(full=True, keep=False):
+        """keep: return the result instead of freeing it (the caller frees it outside the timed region)."""
         out = run_shard(store, tip)
         r = out.contents
         m = int(r.witness.n_blocks)
@@ -340,6 +368,8 @@ def run_engine(args, world, rank, local):
                      pass1_bytes=int(r.pass1_bytes), pass1_nodes=int(r.pass1_nodes),
                      d2h_bytes=int(r.n_matching) * 4 + int(r.n_proofs) * C.sizeof(A.EventProofC) + int(r.data_blob_size) +
                      int(r.witness.n_blocks) * (38 + 8 + 4) + int(r.witness.blob_size))
+        if keep:
+            return out
         L.ipcfp_event_result_free(out)
 
     def barrier():
@@ -366,9 +396,10 @@ def run_engine(args, world, rank, local):
     t_wall0 = time.time()
     ev0.record(ext_stream)
     step_wall = []
-    for _ in range(args.steps):
+    last_out = None
+    for i in range(args.steps):
         _t = time.perf_counter()
-        step_resident(False)
+        last_out = step_resident(False, keep=bool(args.dump_outputs) and i == args.steps - 1)
         step_wall.append(1e3 * (time.perf_counter() - _t))
         for k in phase:
             phase[k].append(stats["ms"][k])
@@ -376,6 +407,11 @@ def run_engine(args, world, rank, local):
     torch.cuda.synchronize()
     t_wall1 = time.time()
     barrier()
+    if last_out is not None:
+        if rank == 0:
+            names = dump_outputs(args.dump_outputs, A.event_result_from_c(last_out.contents))
+            log(f"last timed step's results written to {args.dump_outputs}: {', '.join(names)}")
+        L.ipcfp_event_result_free(last_out)
     launches = api.kernel_launch_count() - launches0
     # CUDA events on the engine stream bracket the K steps on every rank (each step ends with the results on the host); max over ranks
     dev_ms = ev0.elapsed_time(ev1)
@@ -542,9 +578,9 @@ def run_engine(args, world, rank, local):
             "step_hbm": {"algorithmic_bytes_per_step_per_gpu": int(step_bytes), "achieved_gbs": step_bytes / (dev_ms_max / args.steps / 1e3) / 1e9,
                          "frac_of_peak": step_bytes / (dev_ms_max / args.steps / 1e3) / 1e9 / peak,
                          "note": "whole step incl. the PCIe copy of the results: pass-1 bytes + witness blocks read and written once + message-AMT nodes"},
-            "roofline": {"kernel": os.environ.get("IPCFP_PASS1_STAGE", "k_pass1_occ8") + " (pass 1, csrc/events.cu)", "bound": "hbm", "achieved": achieved, "peak": peak,
+            "roofline": {"kernel": os.environ.get("IPCFP_PASS1_STAGE", "k_pass1_stage 128x4x1") + " (pass 1, csrc/events.cu)", "bound": "hbm", "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": pass1_traffic(), "algorithmic_bytes_per_launch": stats["pass1_bytes"], "ms_per_launch": p1,
+                         "traffic": None, "algorithmic_bytes_per_launch": stats["pass1_bytes"], "ms_per_launch": p1,
                          "peak_source": peak_src},
             "cpu_baseline": cpu_baseline,
             "e2e": {"value": n_total / (e2e_ms / 1e3), "unit": "receipts/s", "ms_per_step": e2e_ms, "steps": e2e_steps,
@@ -555,6 +591,7 @@ def run_engine(args, world, rank, local):
             "storage": storage,
             "gpu_launches": int(launches),
             "clocks": clocks,
+            "gpu": gpu_info(local),
         }
         print(json.dumps(line), flush=True)
     if comm is not None:
@@ -575,7 +612,11 @@ def main():
     ap.add_argument("--impl", default="engine", choices=["engine", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-storage", action="store_true", help="skip the HAMT storage-lookup section (configs[2])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned (rank 0) as DIR/<name>.npy (float32/float64, < 64 MB)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     world, rank, local = dist_env()
     if args.impl == "reference":
         run_reference(args, world, rank)

@@ -1,11 +1,11 @@
-/* ipcfp.h — C ABI of the B200-native witness-generation engine.
+/* ipcfp.h — C ABI of the H100-native witness-generation engine.
  *
  * Drop-in boundary for ONE path of consensus-shipyard/ipc-filecoin-proofs: the two-pass
  * receipt/event AMT scan and the HAMT storage-slot lookup. Every entry point cites the
  * reference interface it replaces (paths relative to the reference repo root). The header
  * is bindgen-ready: plain pointers and sizes, POD structs, no C++ or torch types.
  *
- * All compute behind these calls runs in hand-written sm_100a CUDA kernels. There is no
+ * All compute behind these calls runs in hand-written sm_90a CUDA kernels. There is no
  * CPU implementation in this library: without a CUDA device every call fails with
  * IPCFP_ERR_NO_DEVICE.
  *

@@ -22,7 +22,7 @@ LIB_PATH = os.path.join(_HERE, "libipcfp.so")
 
 
 def build_lib(force=False, jobs=8):
-    """Compile the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA library in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     if force or not os.path.exists(LIB_PATH):
         subprocess.check_call(["make", "-C", _ROOT, "-j%d" % jobs, os.path.relpath(LIB_PATH, _ROOT)])
     else:

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host utilities of the B200 witness-generation engine.
+// common.cuh — shared device/host utilities of the H100 witness-generation engine.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

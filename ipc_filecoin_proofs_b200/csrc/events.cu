@@ -84,7 +84,7 @@ __device__ __forceinline__ void pass1_body(const Pass1Args& a) {
     if ((threadIdx.x & 31) == 0 && nodes) { atomicAdd(a.stats, (unsigned long long)nodes); atomicAdd(a.stats + 1, (unsigned long long)bytes); }
 }
 // the same kernel at three register budgets (resident CTAs per SM: 6 → 80 regs, 8 → 64, 10 → 48);
-// IPCFP_PASS1_MINB selects one at run time for tuning, 8 is the measured default
+// IPCFP_PASS1_MINB selects one at run time. The default pass 1 is the staged kernel (pass1_stage.cuh): faster on H100 (DESIGN.md §4)
 __global__ void __launch_bounds__(128, 6) k_pass1(Pass1Args a) { pass1_body(a); }
 __global__ void __launch_bounds__(128, 8) k_pass1_occ8(Pass1Args a) { pass1_body(a); }
 __global__ void __launch_bounds__(128, 10) k_pass1_occ10(Pass1Args a) { pass1_body(a); }
@@ -160,9 +160,9 @@ __global__ void k_check_exec(const uint32_t* __restrict__ match_rel, uint64_t n_
 }
 // a.per_warp: one matching receipt per WARP (lane 0 walks). A matching receipt is a chain of dependent accesses (hash probe → record →
 // strict decode of a 349–413 B node, 7 levels at 1 M receipts, then its events AMT), and 32 lanes on 32 different paths execute that
-// chain serialised by divergence: 1 020 matches in 8 CTAs kept 8 of 148 SMs busy for 0.14 ms (profiles/r1_ncu_full_final.txt). One warp
-// per match is the shape that took k_read_slots from 0.85 to 0.125 ms (storage.cu); above 16 384 matches the grid fills the machine
-// either way and one match per thread is kept. Same per-item code, so results are identical by construction.
+// chain serialised by divergence: ≈ 1 000 matches in 8 CTAs keep 8 of the GPU's 132 SMs busy. One warp per match is the shape
+// k_read_slots uses for the same reason (storage.cu); above 16 384 matches the grid fills the machine either way and one match per
+// thread is kept. Same per-item code, so results are identical by construction.
 __global__ void __launch_bounds__(128) k_pass2(Pass2Args a) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a.per_warp) { if (threadIdx.x & 31) return; t >>= 5; }
@@ -777,12 +777,13 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     p1.match_bits = match_bits.p; p1.cnt = cnt.p; p1.nbytes = nby.p; p1.err = dw; p1.stats = dw + 4;
     if (N) {
         // kernel variant: read per call so that one process can sweep them (tools/profile_step.py)
-        //   IPCFP_PASS1_STAGE=<chunk>x<slots>x<chunks per pass>   warp-cooperative shared-memory staging (pass1_stage.cuh)
+        //   IPCFP_PASS1_STAGE=<chunk>x<slots>x<chunks per pass>   warp-cooperative shared-memory staging (pass1_stage.cuh); default 128x4x1
         //   IPCFP_PASS1_RING=<chunk>x<slots>                      per-lane cp.async rings (pass1_ring.cuh, round-1 experiment)
         //   IPCFP_PASS1_MINB=6|8|10, IPCFP_PASS1_TUNE=<bits>      thread-per-node kernel straight from the arena (round 1)
         const char* stage_env = getenv("IPCFP_PASS1_STAGE");
         const char* ring_env = getenv("IPCFP_PASS1_RING");
-        const int minb = getenv("IPCFP_PASS1_MINB") ? atoi(getenv("IPCFP_PASS1_MINB")) : 8;
+        const char* minb_env = getenv("IPCFP_PASS1_MINB");
+        const int minb = minb_env ? atoi(minb_env) : 8;
         p1.tune = (uint32_t)(getenv("IPCFP_PASS1_TUNE") ? atoi(getenv("IPCFP_PASS1_TUNE")) : 0);
         auto launch_stage = [&](auto kern, int warps, size_t warp_bytes) {
             const size_t smem = warps * warp_bytes;
@@ -810,6 +811,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         else if (is(ring_env, "256x2")) launch_ring(k_pass1_ring<256, 2>, 128 * (256 * 2 + 16));
         else if (getenv("IPCFP_PASS1_W16") && atoi(getenv("IPCFP_PASS1_W16")) == 6) k_pass1_w16_occ6<<<div_up(N, 128), 128, 0, st>>>(p1);
         else if (getenv("IPCFP_PASS1_W16")) k_pass1_w16<<<div_up(N, 128), 128, 0, st>>>(p1);
+        else if (!minb_env) launch_stage(k_pass1_stage<128, 4, 1, 4, 3>, 4, StageGeom<128, 4, 1>::WARP_BYTES);
         else if (minb >= 10) k_pass1_occ10<<<div_up(N, 128), 128, 0, st>>>(p1);
         else if (minb >= 8) k_pass1_occ8<<<div_up(N, 128), 128, 0, st>>>(p1);
         else k_pass1<<<div_up(N, 128), 128, 0, st>>>(p1);

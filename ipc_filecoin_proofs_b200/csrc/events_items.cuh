@@ -50,8 +50,7 @@ template <int MODE, int WINMODE = 0>
 __device__ __forceinline__ void node_events(Rd& r, const uint8_t* p, const AmtNodeHdr& h, uint32_t nv, uint64_t base, const Matcher& m,
                                             WalkOut& wo, EmitCtx* ec, uint32_t tune = 0) {
     for (uint32_t v = 0; v < nv && !r.err; v++) {
-        // rolling prefetch: 2 lines ahead of the dependent walk — measured best of 0/2/3/4/6 (profiles/r1_pass1_prefetch_sweep.txt);
-        // IPCFP_PASS1_TUNE: bits 4..7 = other distance in lines, bit 1 = off
+        // rolling prefetch: 2 lines ahead of the dependent walk; IPCFP_PASS1_TUNE: bits 4..7 = other distance in lines, bit 1 = off
         const uint32_t ahead = (tune >> 4) & 15u ? 128u * ((tune >> 4) & 15u) : 256u;
         if (!(tune & 2) && r.pos + ahead < r.n) prefetch_l2(r.p + r.pos + ahead);
         if ((tune & 1) && r.pos + 128 < r.n) prefetch_l1(r.p + r.pos + 128);  // experiment: next line into L1

@@ -1,4 +1,4 @@
-// hashes.cuh — device hash functions of the engine (sm_100a).
+// hashes.cuh — device hash functions of the engine (sm_90a).
 //   K1  Blake2b-256  (RFC 7693)    : CID verification of ingested IPLD blocks
 //                                     (multihash-codetable Code::Blake2b256, reference events/utils.rs:65)
 //   K2  Keccak-256   (pad 0x01)    : topic0 / storage-slot keys (reference common/evm.rs:62-88, storage/utils.rs:5-12)

@@ -1,7 +1,7 @@
 // pass1_ring.cuh — EXPERIMENT (round 2): pass 1 with a per-lane shared-memory ring fed by cp.async.
 //
-// Why: k_pass1 is bound by the dependent chain "load 16-byte window → parse head → next address" — 58 % of warp time
-// is long_scoreboard at the first use of a window, DRAM active 60 %, issue active 43 % (profiles/r1_ncu_full_v4_pass1.txt).
+// Why: k_pass1 is bound by the dependent chain "load 16-byte window → parse head → next address": most warp time is spent
+// waiting on the first use of a window (long_scoreboard), with neither DRAM nor issue saturated.
 // Here every lane streams its node through a private ring of NSLOT chunks of CH bytes (chunk-aligned in the arena, so
 // cp.async's 16-byte alignment holds for any block offset): chunks are requested NSLOT-1 ahead of the parser, windows
 // come from shared memory (≈ 30 cycles) and L1 is bypassed (cp.async.cg). Only the fast path reads the ring; the strict

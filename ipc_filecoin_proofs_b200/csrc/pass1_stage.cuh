@@ -1,9 +1,9 @@
 // pass1_stage.cuh — pass 1 (find_matching_events pass 1, reference events/generator.rs:206-239) with the node bytes STAGED
 // THROUGH SHARED MEMORY by warp-cooperative, coalesced 16-byte copies.
 //
-// Why (profiles/r1_ncu_full_v4_pass1.txt, DESIGN.md §4): the thread-per-node kernel reads each lane's node straight from the
-// arena, so every 8-byte window load of a warp touches 32 different 128-byte lines = 32 L1 wavefronts; ≈ 80 such loads per node
-// put ≈ 550 k wavefronts per SM into a kernel of ≈ 650 k cycles — the L1 wavefront queue, not HBM, is what it runs at.
+// Why (DESIGN.md §4): the thread-per-node kernel reads each lane's node straight from the arena, so every 8-byte window load of a
+// warp touches 32 different 128-byte lines = 32 L1 wavefronts; with ≈ 80 such loads per node the L1 wavefront queue, not HBM, can
+// be what the kernel runs at.
 //
 // Here a warp owns 32 receipts (lane = receipt, as before: DAG-CBOR is sequential, one lane parses one node) but the BYTES travel
 // differently: every lane has a ring of NSLOT chunks of CH bytes in shared memory; a fill pass moves, for every node of the warp,

@@ -20,8 +20,8 @@
 namespace ipcfp {
 
 // One WARP per proof / lookup, lane 0 walks. The walk is a chain of data-dependent branches over a different node in every lane:
-// 32 lookups in one warp execute one lane at a time (measured: 1.5 active lanes per instruction, 0.85 ms for ANY batch up to 64 k
-// lookups), so a lookup per warp costs the same issue slots, finishes 32 lookups' worth earlier and spreads a small batch over all SMs.
+// 32 lookups in one warp execute close to one lane at a time (the kernel time hardly depends on the batch size), so a lookup per warp
+// costs the same issue slots, finishes 32 lookups' worth earlier and spreads a small batch over all SMs.
 __global__ void __launch_bounds__(128) k_storage_proofs(StorageArgs a) {
     uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= a.n || (threadIdx.x & 31)) return;
@@ -48,7 +48,7 @@ struct SlotArgs {
     uint32_t per_warp;
 };
 // a.per_warp: one lookup per warp (small and medium batches: latency); else one per thread with the strict decoder, whose uniform
-// head-by-head loop keeps the lanes of a warp closer together (large batches: 60 M lookups/s at 64 k, measured)
+// head-by-head loop keeps the lanes of a warp closer together (large batches, where the grid fills the GPU either way)
 __global__ void __launch_bounds__(128) k_read_slots(SlotArgs a) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a.per_warp) { if (threadIdx.x & 31) return; t >>= 5; }

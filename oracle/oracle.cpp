@@ -12,7 +12,7 @@
 //   src/proofs/common/decode.rs:17-124      get_actor_state, parse_evm_state, HeaderLite
 //   src/proofs/generator.rs:25-95           generate_proof_bundle
 //   src/proofs/events/verifier.rs:51-290, src/proofs/storage/verifier.rs:24-170   verifiers
-// The crates' arithmetic ([UPSTREAM], not under /root/reference) is restated from their
+// The crates' arithmetic ([UPSTREAM], not in the reference tree) is restated from their
 // published formats: SURVEY.md Appendix A; the decode contract is written down in DESIGN.md §3.
 //
 // Deliberately mirrors the reference's allocation behaviour (get() clones the block, every

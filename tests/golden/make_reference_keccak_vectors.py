@@ -12,15 +12,17 @@ topdown-messenger/lib/forge-std/, and that library's sources and test-suite carr
   * every mixed-case address literal: solc only accepts it when its EIP-55 checksum — keccak256 of the lower-case hex — is right.
 
 Keccak-256 is on the hot path (topic0 = keccak256(event signature), events/generator.rs:30-35 via common/evm.rs:62-69; mapping slots,
-storage/utils.rs:5-12). These are the only vectors under /root/reference that pin anything the path computes; AMT / HAMT / DAG-CBOR stay
-unpinned by the reference. Run HERE (needs /root/reference); the JSON is what travels. No hashing happens in this script: it only copies
+storage/utils.rs:5-12). These are the only vectors in the reference tree that pin anything the path computes; AMT / HAMT / DAG-CBOR stay
+unpinned by the reference. Usage: make_reference_keccak_vectors.py <reference checkout>; the JSON is what the tests read. No hashing happens in this script: it only copies
 constants and states how each expected value is derived, the tests do the hashing with the implementation under test."""
 import json
 import os
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+if len(sys.argv) != 2:
+    raise SystemExit(__doc__.splitlines()[0] + "\nusage: make_reference_keccak_vectors.py <reference checkout>")
+REF = sys.argv[1]
 FORGE = os.path.join(REF, "topdown-messenger", "lib", "forge-std")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_keccak_vectors.json")
 
