@@ -140,29 +140,46 @@ __device__ __forceinline__ uint32_t bits_below(const uint32_t* __restrict__ bits
     return (uint32_t)prefix[r >> 5] + (uint32_t)__popc(bits[r >> 5] & ((1u << (r & 31)) - 1u));
 }
 // idx = [A: mA ranks ascending][B: m - mA ranks ascending], A and B disjoint. Entry i goes to its merged position f.
-__global__ void k_witness_emit(const uint32_t* __restrict__ idx, const uint64_t* __restrict__ offs, uint64_t m, uint64_t mA, uint64_t baseB,
-                               const uint32_t* __restrict__ bitsA, const uint64_t* __restrict__ prefixA, const uint32_t* __restrict__ bitsB,
-                               const uint64_t* __restrict__ prefixB, StoreView v, uint8_t* cids, uint64_t* out_offs, uint32_t* out_lens, uint32_t* out_idx,
-                               int by_ref) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const uint32_t r = idx[i];
-    uint64_t f;
-    if (i < mA) f = i + (m > mA ? bits_below(bitsB, prefixB, r) : 0u);
-    else f = (i - mA) + bits_below(bitsA, prefixA, r);
-    const uint32_t b = v.block_at_rank[r];
-    out_offs[f] = by_ref ? v.offsets[b] : offs[i] + (i >= mA ? baseB : 0);   // by reference: where the block sits in the blob the store was created from
-    out_lens[f] = v.lengths[b];
-    out_idx[f] = b;
-    uint8_t* o = cids + 38 * f;
-    uint32_t c = v.cls[b];
+// The 38-byte CID records are built in shared memory and stored by the warp as 2-byte units (38·f is always even): the lanes of a
+// warp nearly always hold consecutive positions, so each store instruction covers 64 contiguous bytes. One byte store per lane at a
+// 38-byte stride touched a sector per lane, 38 times over.
+#define EMIT_THREADS 256
+__global__ void __launch_bounds__(EMIT_THREADS) k_witness_emit(const uint32_t* __restrict__ idx, const uint64_t* __restrict__ offs, uint64_t m,
+                                                               uint64_t mA, uint64_t baseB, const uint32_t* __restrict__ bitsA,
+                                                               const uint64_t* __restrict__ prefixA, const uint32_t* __restrict__ bitsB,
+                                                               const uint64_t* __restrict__ prefixB, StoreView v, uint8_t* cids, uint64_t* out_offs,
+                                                               uint32_t* out_lens, uint32_t* out_idx, int by_ref) {
+    __shared__ uint16_t rec[EMIT_THREADS][19];
+    __shared__ uint64_t pos[EMIT_THREADS];
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < m) {
+        const uint32_t r = idx[i];
+        uint64_t f;
+        if (i < mA) f = i + (m > mA ? bits_below(bitsB, prefixB, r) : 0u);
+        else f = (i - mA) + bits_below(bitsA, prefixA, r);
+        const uint32_t b = v.block_at_rank[r];
+        out_offs[f] = by_ref ? v.offsets[b] : offs[i] + (i >= mA ? baseB : 0);   // by reference: where the block sits in the blob the store was created from
+        out_lens[f] = v.lengths[b];
+        out_idx[f] = b;
+        pos[threadIdx.x] = f;
+        uint8_t* o = (uint8_t*)rec[threadIdx.x];
+        uint32_t c = v.cls[b];
 #pragma unroll
-    for (int k = 0; k < 6; k++) o[k] = v.class_prefix[c][k];
-    Digest d = v.digests[b];
+        for (int k = 0; k < 6; k++) o[k] = v.class_prefix[c][k];
+        Digest d = v.digests[b];
 #pragma unroll
-    for (int w = 0; w < 4; w++)
+        for (int w = 0; w < 4; w++)
 #pragma unroll
-        for (int k = 0; k < 8; k++) o[6 + 8 * w + k] = (uint8_t)(d.w[w] >> (8 * k));
+            for (int k = 0; k < 8; k++) o[6 + 8 * w + k] = (uint8_t)(d.w[w] >> (8 * k));
+    }
+    __syncwarp();
+    const uint32_t lane = threadIdx.x & 31, w0 = threadIdx.x - lane;
+    const uint64_t first = i - lane;
+    const uint32_t nrec = first < m ? (uint32_t)std::min<uint64_t>(32, m - first) : 0;
+    for (uint32_t u = lane; u < nrec * 19; u += 32) {
+        const uint32_t q = u / 19, k = u - 19 * q;
+        ((uint16_t*)(cids + 38 * pos[w0 + q]))[k] = rec[w0 + q][k];
+    }
 }
 
 WitnessBuilder::WitnessBuilder(Store* store) : s(store) {
@@ -273,7 +290,7 @@ void WitnessBuilder::finish_start(uint64_t mB_, uint64_t bytesB_, WitnessOut& ou
     AsyncBuf<uint64_t> d_offs(m + 8, st);
     AsyncBuf<uint8_t> d_cids(m * 38 + 64, st);
     if (m) {
-        k_witness_emit<<<div_up(m, 256), 256, 0, st>>>(idx.p, offs.p, m, mA, bytesA, bitsA.p, word_prefix.p, bitsB.p, word_prefixB.p, s->view, d_cids.p, d_offs.p,
+        k_witness_emit<<<div_up(m, EMIT_THREADS), EMIT_THREADS, 0, st>>>(idx.p, offs.p, m, mA, bytesA, bitsA.p, word_prefix.p, bitsB.p, word_prefixB.p, s->view, d_cids.p, d_offs.p,
                                                        d_lens.p, d_idx.p, by_ref ? 1 : 0);
         IPCFP_LAUNCH_CHECK();
     }
