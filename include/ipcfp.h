@@ -196,6 +196,13 @@ typedef struct ipcfp_event_result {
     float _pad0;
     uint64_t union_part_first;
     uint64_t n_union_part;
+    /* IPCFP_RESULT_JSON only (NULL / 0 otherwise): the EventProofBundle as JSON, byte for byte what ipcfp_event_result_to_json renders
+     * for the same call made without the flag. NUL-terminated, json_len bytes without the NUL, owned by the result. ms_json: device time
+     * of the rendering and its copy to the host. */
+    const char* json;
+    uint64_t json_len;
+    float ms_json;
+    float _pad1;
 } ipcfp_event_result;
 
 typedef struct ipcfp_storage_proof {
@@ -249,6 +256,13 @@ typedef struct ipcfp_bundle {
  * host already has; WitnessCollector::materialize (src/proofs/common/witness.rs:43-56) becomes a gather over the caller's blocks. */
 #define IPCFP_WITNESS_BY_REFERENCE 0x8u
 #define IPCFP_SHARDED_UNION_FULL 0x4u    /* … every rank receives the WHOLE merged list (all-gather + merge of `world` lists on every rank) instead of its partition */
+/* JSON result (ipcfp_generate_event_proof, ipcfp_generate_event_proof_resident): the result also carries `json`, the serde_json text of
+ * EventProofBundle (src/proofs/events/bundle.rs:5-30), rendered on the device — the text ipcfp_event_result_to_json gives for the same call
+ * without the flag. Block bytes are read from the store itself, so IPCFP_RESULT_JSON | IPCFP_WITNESS_BY_REFERENCE is the combination for a
+ * caller who wants the wire format: the text, without the ≈ 51 MB (per 1 M receipts) copy of the witness blob it already contains. With
+ * IPCFP_SCAN_SKIP_TX_AMTS the text renders what that result holds. Costs one extra host synchronisation per call. Sharded calls
+ * (ipcfp_generate_event_proof_shard*, _sharded) refuse the flag with IPCFP_ERR_UNSUPPORTED: a shard's result is not an EventProofBundle. */
+#define IPCFP_RESULT_JSON 0x10u
 
 /* generate_event_proof (src/proofs/events/generator.rs:60-107): base witness, message-AMT
  * recording, execution order, two-pass scan (find_matching_events :180-307), materialise. */

@@ -23,6 +23,7 @@ pub const IPCFP_SCAN_SKIP_TX_AMTS: u32 = 0x1;
 pub const IPCFP_SHARDED_UNION_TO_HOST: u32 = 0x2;
 pub const IPCFP_SHARDED_UNION_FULL: u32 = 0x4;
 pub const IPCFP_WITNESS_BY_REFERENCE: u32 = 0x8;
+pub const IPCFP_RESULT_JSON: u32 = 0x10;
 pub const IPCFP_COMM_ID_BYTES: usize = 128;
 
 #[repr(C)] pub struct ipcfp_store { _p: [u8; 0] }
@@ -64,6 +65,7 @@ pub struct ipcfp_event_result {
     pub union_cids_dev: *const c_void, pub n_union_cids: u64, pub union_cids: *const u8, pub total_matching: u64, pub total_proofs: u64,
     pub ms_exchange: f32, pub ms_fetch: f32, pub ms_union: f32, pub _pad0: f32,
     pub union_part_first: u64, pub n_union_part: u64,
+    pub json: *const c_char, pub json_len: u64, pub ms_json: f32, pub _pad1: f32,
 }
 #[repr(C)]
 pub struct ipcfp_storage_proof {

@@ -28,6 +28,7 @@ SCAN_SKIP_TX_AMTS = 0x1
 SHARDED_UNION_TO_HOST = 0x2
 SHARDED_UNION_FULL = 0x4
 WITNESS_BY_REFERENCE = 0x8
+RESULT_JSON = 0x10
 COMM_ID_BYTES = 128
 
 
@@ -116,6 +117,10 @@ class EventResultC(C.Structure):
         ("_pad0", C.c_float),
         ("union_part_first", C.c_uint64),
         ("n_union_part", C.c_uint64),
+        ("json", C.c_void_p),
+        ("json_len", C.c_uint64),
+        ("ms_json", C.c_float),
+        ("_pad1", C.c_float),
     ]
 
 
@@ -254,6 +259,7 @@ class EventResultPy:
     pass1_nodes: int = 0
     raw_proofs: np.ndarray = None   # packed ipcfp_event_proof records (for the verifier)
     data_blob: np.ndarray = None
+    json: str = None        # IPCFP_RESULT_JSON: the EventProofBundle text rendered on the device
 
 
 def event_result_from_c(r):
@@ -268,9 +274,12 @@ def event_result_from_c(r):
         topics = [db[p.topics_off + 32 * k: p.topics_off + 32 * (k + 1)] for k in range(p.n_topics)]
         proofs.append(EventProofPy(int(p.exec_index), int(p.event_index), int(p.emitter), topics,
                                    db[p.data_off:p.data_off + p.data_len], bytes(p.message_cid)))
-    return EventResultPy(matching, proofs, witness_from_c(r.witness), int(r.n_exec),
-                         dict(total=r.ms_total, pass1=r.ms_pass1, pass2=r.ms_pass2, txamt=r.ms_txamt, witness=r.ms_witness),
-                         int(r.pass1_bytes), int(r.pass1_nodes), raw, data)
+    timings = dict(total=r.ms_total, pass1=r.ms_pass1, pass2=r.ms_pass2, txamt=r.ms_txamt, witness=r.ms_witness)
+    text = None
+    if r.json:
+        text = C.string_at(r.json, int(r.json_len)).decode()
+        timings["json"] = r.ms_json
+    return EventResultPy(matching, proofs, witness_from_c(r.witness), int(r.n_exec), timings, int(r.pass1_bytes), int(r.pass1_nodes), raw, data, text)
 
 
 def pack_event_proofs(proofs):

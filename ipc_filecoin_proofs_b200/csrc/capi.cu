@@ -125,7 +125,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_json_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }

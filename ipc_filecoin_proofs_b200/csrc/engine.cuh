@@ -71,7 +71,7 @@ struct Store {
     DevBuf<unsigned long long> dev_words;  // [0] error word, [1..] counters
     PinnedBuf<uint64_t> host_words;
     PinnedArray stage;                     // pinned staging (from the process-wide pool) for small per-call uploads: spec, tipset CIDs, walk tables
-    cudaEvent_t ev[10] = {};
+    cudaEvent_t ev[12] = {};
     ~Store();
     void use() const { IPCFP_CUDA(cudaSetDevice(device)); }
 };
@@ -192,6 +192,7 @@ struct WitnessOut {
     PinnedArray cids, offsets, lengths, blob;
     PinnedArray sorted_idx;       // host copy of the block indices in Cid order (u32[n])
     AsyncBuf<uint8_t> cids_dev;   // the same sorted CIDs in device memory (n*38), for the multi-GPU union
+    AsyncBuf<uint32_t> idx_dev;   // block index of every entry in device memory (n), for the JSON renderer
     uint64_t n = 0, blob_size = 0;
     void fill(ipcfp_witness& w) const {
         w.n_blocks = n; w.cids = cids.as<uint8_t>(); w.offsets = offsets.as<uint64_t>(); w.lengths = lengths.as<uint32_t>();
@@ -221,6 +222,23 @@ struct WitnessBuilder {
     void finish_join(WitnessOut& out);                                              // … wait for both streams
 };
 void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out);
+
+// json.cu — IPCFP_RESULT_JSON: the EventProofBundle text of one call from what is on the device after k_witness_emit (all pointers device)
+struct JsonInputs {
+    const ipcfp_event_proof* proofs;   // n_proofs slots as pass 2 wrote them (skipped slots included)
+    uint64_t n_proofs;
+    const uint8_t* blob;               // topics / data bytes the proofs index
+    const uint8_t* cids;               // m*38, sorted witness CIDs
+    const uint32_t* idx;               // m, block index of every witness entry
+    uint64_t m;
+    int64_t parent_epoch, child_epoch;
+    uint32_t n_parents;
+    const uint8_t* parent_cids;        // n_parents*38
+    const uint8_t* child_cid;          // 38
+};
+// enqueues on the store's stream, synchronises it once (the exact length), enqueues the rendering and the copy into `out` (pinned,
+// NUL-terminated; the text is there once the stream has drained); returns the length of the text
+uint64_t render_event_json(Store* s, const JsonInputs& in, PinnedArray& out);
 // ord[0..m) = the permutation that sorts the blocks idx[0..m) in `Cid` Ord (stable); runs on the store's stream (ingest: the ranks)
 size_t sort_by_cid_ws_bytes(uint64_t m);
 void sort_by_cid(Store* s, const uint32_t* idx_dev, uint32_t* ord, uint64_t m, void* workspace);

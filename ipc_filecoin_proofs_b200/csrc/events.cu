@@ -401,6 +401,7 @@ struct EventResultBox {
     PinnedArray matching, proofs, blob;
     WitnessOut wit;
     PinnedArray union_host;       // sharded calls with IPCFP_SHARDED_UNION_TO_HOST
+    PinnedArray json;             // IPCFP_RESULT_JSON: the EventProofBundle text
     AsyncBuf<RawCid> shard_exec;  // shard mode: this shard's slice of the raw execution list, kept on the device
 };
 
@@ -483,6 +484,8 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     const auto t_enter = std::chrono::steady_clock::now();
     static thread_local std::chrono::steady_clock::time_point t_last_exit = t_enter;
     if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+    // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
+    if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
     if (!sharded) { lo = 0; hi = td.n_receipts; }
     if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
     const uint64_t N = hi - lo;
@@ -923,6 +926,15 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
             publish_words_on(s, sw, dw + 18, 18, 1);
         } else xch->witness_union_partitioned(sw, box->wit.cids_dev.p, box->wit.n, xch->union_piece_cap(false), &union_dev, 320);   // [size, overflow] per rank → hw[320 ..)
     }
+    // IPCFP_RESULT_JSON: render the bundle from the device copies (json.cu) while the witness blob copy, if any, is still on the wire
+    uint64_t json_len = 0;
+    if (flags & IPCFP_RESULT_JSON) {
+        IPCFP_CUDA(cudaEventRecord(s->ev[10], st));
+        JsonInputs ji{d_proofs.p, n_proofs, d_blob.p, box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n,
+                      td.parent_epoch, td.child_epoch, td.n_parents, sa.parent_cids, sa.child_cid};
+        json_len = render_event_json(s, ji, box->json);
+        IPCFP_CUDA(cudaEventRecord(s->ev[11], st));
+    }
     wbuild.finish_join(box->wit);
     if (xch) {
         IPCFP_CUDA(cudaStreamSynchronize(xch->stream()));
@@ -962,6 +974,10 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[3], s->ev[4])); r.ms_pass2 = ms;
     IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[4], s->ev[5])); r.ms_witness = ms;
     r.pass1_bytes = pass1_bytes; r.pass1_nodes = pass1_nodes;
+    if (flags & IPCFP_RESULT_JSON) {
+        r.json = box->json.as<char>(); r.json_len = json_len;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[10], s->ev[11])); r.ms_json = ms;
+    }
     r.shard_raw_total = nraw_total;
     if (sharded) { r.n_exec = 0; r.shard_exec_count = nraw; box->shard_exec = std::move(exec_raw); r.shard_exec_dev = box->shard_exec.p; }
     if (xch) {

@@ -308,6 +308,7 @@ void WitnessBuilder::finish_start(uint64_t mB_, uint64_t bytesB_, WitnessOut& ou
         if (want_sorted_idx) IPCFP_CUDA(cudaMemcpyAsync(out.sorted_idx.p, d_idx.p, m * 4, cudaMemcpyDeviceToHost, st));
     }
     out.cids_dev = std::move(d_cids);
+    out.idx_dev = std::move(d_idx);
     dblobB_keep = std::move(dblobB);
 }
 void WitnessBuilder::finish_join(WitnessOut& out) {
