@@ -397,7 +397,10 @@ ipcfp_status ipcfp_exec_fetch(int device, const void* seg_dev, uint64_t nseg, ui
 /* Device-resident copy of a result's sorted witness CIDs (n*38 bytes) for the collective. */
 ipcfp_status ipcfp_witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap_cids, uint64_t* n);
 /* Merge all-gathered CID lists on the device: gathered = world*cap*38 bytes, counts[world];
- * out_dev receives the sorted unique union (cap_out*38), *n_out its length. */
+ * out_dev receives the sorted unique union (cap_out*38), *n_out its length.
+ * Every CID must carry the first CID's 6-byte prefix (version, codec, multihash code, size): the order is the raw byte order,
+ * which is `Cid` order only within one prefix. Otherwise IPCFP_ERR_UNSUPPORTED, with ipcfp_last_error_index() the first
+ * position (counted over the segments' valid entries, in order) whose prefix differs, and *n_out = 0. */
 ipcfp_status ipcfp_merge_witness_cids(int device, const void* gathered_dev, const uint64_t* counts, uint32_t world,
                                       uint64_t cap, void* out_dev, uint64_t cap_out, uint64_t* n_out);
 

@@ -27,15 +27,20 @@ template <class F> static ipcfp_status guard(F f) {
 
 // ------------------------------------------------------------------------------------------ multi-GPU merge
 // gathered: world segments of `cap` 38-byte CIDs, counts[r] valid in segment r. Sort + unique on the device.
+// first = the first valid entry; *mixed receives the smallest position whose 6 prefix bytes differ from first's.
 struct SortCid { uint8_t b[38]; };
 __global__ void k_merge_keys(const uint8_t* __restrict__ g, const uint64_t* __restrict__ seg_off, uint32_t world, uint64_t cap, uint64_t total,
-                             uint32_t* keys, uint32_t* vals) {
+                             const uint8_t* __restrict__ first, uint32_t* keys, uint32_t* vals, unsigned long long* mixed) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     uint32_t r = 0;
     while (r + 1 < world && i >= seg_off[r + 1]) r++;
     uint64_t src = (uint64_t)r * cap + (i - seg_off[r]);
     const uint8_t* c = g + 38 * src;
+    bool same = true;
+#pragma unroll
+    for (int k = 0; k < 6; k++) same &= c[k] == first[k];
+    if (!same) atomicMin(mixed, (unsigned long long)i);
     keys[i] = ((uint32_t)c[6] << 24) | ((uint32_t)c[7] << 16) | ((uint32_t)c[8] << 8) | c[9];
     vals[i] = (uint32_t)src;
 }
@@ -74,14 +79,17 @@ __global__ void k_merge_emit(const uint8_t* __restrict__ g, const uint32_t* __re
 
 void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
                         uint64_t* n_out) {
-    // NOTE: raw byte order == `Cid` Ord for CIDs sharing one prefix (the homogeneous Filecoin chain
-    // case); stores with several CID prefixes must merge on the host (see DESIGN.md §6).
+    // The order is the raw byte order of the 38 bytes, which is `Cid` Ord only among CIDs that share one prefix (the varint
+    // multihash code does not sort bytewise): lists with several prefixes are refused, like the sharded call refuses such stores.
     check_device(device);
     std::vector<uint64_t> seg(world + 1, 0);
     for (uint32_t r = 0; r < world; r++) { if (counts[r] > cap) throw Error(IPCFP_ERR_INVALID_ARG, "count exceeds segment capacity"); seg[r + 1] = seg[r] + counts[r]; }
     uint64_t total = seg[world];
     *n_out = 0;
     if (!total) return;
+    uint32_t r0 = 0;
+    while (!counts[r0]) r0++;
+    const uint8_t* first = (const uint8_t*)gathered + 38ull * r0 * cap;
     cudaStream_t st = nullptr;
     AsyncBuf<uint64_t> d_seg(world + 1, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_seg.p, seg.data(), (world + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -89,15 +97,19 @@ void merge_witness_cids(int device, const void* gathered, const uint64_t* counts
     unsigned nb = radix_blocks(total);
     AsyncBuf<uint32_t> hist((size_t)256 * nb + 256, st);
     AsyncBuf<uint64_t> scan_tmp((size_t)256 * nb + 256, st), scratch(scan_scratch_elems(std::max<uint64_t>((uint64_t)256 * nb, total)) + 8, st),
-        wp((total + 31) / 32 + 8, st), cnt(1, st);
-    k_merge_keys<<<div_up(total, 256), 256, 0, st>>>((const uint8_t*)gathered, d_seg.p, world, cap, total, keys.p, vals.p); IPCFP_LAUNCH_CHECK();
+        wp((total + 31) / 32 + 8, st), cnt(2, st);   // cnt[0] = unique count, cnt[1] = first mixed-prefix position
+    IPCFP_CUDA(cudaMemsetAsync(cnt.p + 1, 0xff, 8, st));
+    k_merge_keys<<<div_up(total, 256), 256, 0, st>>>((const uint8_t*)gathered, d_seg.p, world, cap, total, first, keys.p, vals.p,
+                                                     (unsigned long long*)cnt.p + 1); IPCFP_LAUNCH_CHECK();
     radix_sort_pairs(keys.p, vals.p, ka.p, va.p, total, 32, hist.p, scan_tmp.p, scratch.p, st);
     k_merge_tie_fix<<<div_up(total, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, keys.p, total); IPCFP_LAUNCH_CHECK();
     k_merge_unique_flags<<<div_up((total + 31) / 32 * 32, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, total, bits.p); IPCFP_LAUNCH_CHECK();
     bitmap_to_indices(bits.p, total, pos.p, cnt.p, wp.p, scratch.p, st);
-    uint64_t n = 0;
-    IPCFP_CUDA(cudaMemcpyAsync(&n, cnt.p, 8, cudaMemcpyDeviceToHost, st));
+    uint64_t h[2] = {0, 0};
+    IPCFP_CUDA(cudaMemcpyAsync(h, cnt.p, 16, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
+    if (h[1] != UINT64_MAX) throw Error(IPCFP_ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", h[1]);
+    const uint64_t n = h[0];
     if (n > cap_out) throw Error(IPCFP_ERR_INVALID_ARG, "output buffer too small for the merged witness CID list");
     k_merge_emit<<<div_up(n, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, pos.p, n, (uint8_t*)out); IPCFP_LAUNCH_CHECK();
     IPCFP_CUDA(cudaStreamSynchronize(st));

@@ -54,8 +54,12 @@ class NumpyShardOps:
 
     def merge_witness(self, gathered, counts, world, cap):
         import oracle
+        from ipc_filecoin_proofs_b200 import _abi as A
         g = gathered.numpy().reshape(world, cap, 38)
         allc = np.concatenate([g[w, :int(counts[w])] for w in range(world)])
+        mixed = np.flatnonzero((allc[:, :6] != allc[:1, :6]).any(axis=1)) if len(allc) else []
+        if len(mixed):   # the rule of ipcfp_merge_witness_cids
+            raise A.IpcfpError(A.ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", int(mixed[0]))
         return oracle.sort_unique_cids(allc).reshape(-1)
 
 
