@@ -348,6 +348,49 @@ ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* witness_store, const ipcfp
                                          uint8_t* results);
 
 /* ------------------------------------------------------------------------------------------
+ * verify_proof_bundle (src/proofs/verifier.rs:12-60) from the JSON text: parse, witness store and verification on the GPU.
+ * Accepts EventProofBundle and UnifiedProofBundle text. The result is, in every case, what this composition of the calls above gives:
+ *   1. ipcfp_bundle_from_json on the text: its failure status is returned (index UINT64_MAX);
+ *   2. trust (verify_trust_anchors / verify_trust_anchor): trusted_child is called once (if the bundle has a proof) with the child epoch
+ *      and child block CID, then trusted_parent once (if it has event proofs and the child is trusted) with the parent epoch and parent
+ *      tipset CIDs. Both run on the calling thread; non-zero = trusted; NULL = AcceptAll. Untrusted child: every result is false.
+ *      Untrusted parent: every event result is false;
+ *   3. if a trusted proof is left: a witness store of the blocks in bundle order with IPCFP_STORE_VERIFY_CIDS — a digest mismatch
+ *      returns IPCFP_ERR_CID_MISMATCH with the block's position in the bundle as the index (duplicates and up to 8 CID prefixes as in
+ *      ipcfp_store_create). With no trusted proof no store is built and the call succeeds whatever the blocks hold;
+ *   4. ipcfp_verify_storage_proofs on the trusted storage proofs, then ipcfp_verify_event_proofs on the trusted event proofs with
+ *      `filter` (check_event, may be NULL). A verifier failure fails the call; its index counts storage proofs first, then event proofs.
+ * Canonical text (what serde_json::to_string, ipcfp_bundle_to_json, ipcfp_event_result_to_json and IPCFP_RESULT_JSON write) is parsed
+ * on the device straight into the witness store (parsed_on_device = 1); any other spelling — whitespace, escapes, other key orders or
+ * fields, other CID spellings, upper-case hex, out-of-range values — is read by ipcfp_bundle_from_json instead (parsed_on_device = 0),
+ * with identical results. *out is released with ipcfp_bundle_verdict_free.
+ * ------------------------------------------------------------------------------------------ */
+typedef int (*ipcfp_trusted_parent_ts_fn)(void* ctx, int64_t parent_epoch, const uint8_t* parent_cids /* n_parents*38 */, uint32_t n_parents);
+typedef int (*ipcfp_trusted_child_header_fn)(void* ctx, int64_t child_epoch, const uint8_t* child_cid /* 38 */);
+typedef struct ipcfp_bundle_verdict {
+    ipcfp_tipset_desc tipset;                  /* the fields every proof shares, as ipcfp_parsed_bundle.tipset                   */
+    uint64_t n_storage_proofs;
+    const ipcfp_storage_proof* storage_proofs; /* as ipcfp_bundle_from_json returns them                                         */
+    const uint8_t* storage_results;            /* UnifiedVerificationResult.storage_results (0 / 1)                              */
+    uint64_t n_event_proofs;
+    const ipcfp_event_proof* event_proofs;
+    const uint8_t* event_results;              /* UnifiedVerificationResult.event_results (0 / 1)                                */
+    const uint8_t* data_blob;                  /* topics / data of event_proofs                                                  */
+    uint64_t data_blob_size;
+    uint64_t n_blocks;                         /* witness blocks in the bundle                                                   */
+    uint64_t witness_bytes;                    /* their decoded bytes (sum of the block lengths)                                 */
+    uint32_t parsed_on_device;                 /* 1: device parser; 0: text not in canonical form, read by ipcfp_bundle_from_json */
+    /* wall time of the call and of its phases, milliseconds (each phase ends in a host synchronisation): parse (text to PODs and
+     * block arrays, including the text's copy to the device), store (witness store with its CID check), verify (both verifiers) */
+    float ms_total, ms_parse, ms_store, ms_verify;
+    uint32_t _pad;
+} ipcfp_bundle_verdict;
+ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
+                                      ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
+                                      ipcfp_bundle_verdict** out);
+void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v);
+
+/* ------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU; the caller owns the communicator — torch.distributed / NCCL).
  * Receipts shard by index range; each rank scans its shard, then the per-shard witness CID sets
  * are all-gathered and merged (the BTreeSet union of src/proofs/common/witness.rs:24-40).

@@ -735,6 +735,30 @@ inline UnifiedVerificationResult verify_proof_bundle(const UnifiedProofBundle& b
     return r;
 }
 
+// verify_proof_bundle from the bundle's JSON text (EventProofBundle or UnifiedProofBundle), through ipcfp_verify_bundle_json: parse, witness
+// store and verification on the GPU (text not in serde_json's canonical form is read by the host parser, with the same results). Each
+// closure is called at most once, on this thread.
+inline UnifiedVerificationResult verify_proof_bundle_json(const std::string& text, const TrustedParentTs& is_trusted_parent_ts,
+                                                          const TrustedChildHeader& is_trusted_child_header, const EventProofSpec* check_event = nullptr,
+                                                          int device = 0) {
+    struct Ctx { const TrustedParentTs* parent; const TrustedChildHeader* child; } ctx{&is_trusted_parent_ts, &is_trusted_child_header};
+    auto tp = [](void* c, int64_t epoch, const uint8_t* cids, uint32_t n) -> int {
+        std::vector<Cid> parents;
+        for (uint32_t q = 0; q < n; q++) parents.push_back(Cid::from_bytes(cids + 38ull * q));
+        return (*static_cast<Ctx*>(c)->parent)(epoch, parents) ? 1 : 0;
+    };
+    auto tc = [](void* c, int64_t epoch, const uint8_t* cid) -> int { return (*static_cast<Ctx*>(c)->child)(epoch, Cid::from_bytes(cid)) ? 1 : 0; };
+    ipcfp_event_spec filter;
+    if (check_event) filter = spec_c(check_event->event_signature, check_event->topic_1, check_event->actor_id_filter);
+    ipcfp_bundle_verdict* v = nullptr;
+    check(ipcfp_verify_bundle_json(text.data(), text.size(), device, tp, tc, &ctx, check_event ? &filter : nullptr, &v), "verify_proof_bundle_json");
+    UnifiedVerificationResult r;
+    for (uint64_t i = 0; i < v->n_storage_proofs; i++) r.storage_results.push_back(v->storage_results[i] != 0);
+    for (uint64_t i = 0; i < v->n_event_proofs; i++) r.event_results.push_back(v->event_results[i] != 0);
+    ipcfp_bundle_verdict_free(v);
+    return r;
+}
+
 // ------------------------------------------------------------------------------------------ wire format (serde_json of the bundle structs)
 // to_json: what `serde_json::to_string(&bundle)` gives in the reference (common/bundle.rs:10-45, events/bundle.rs:5-30,
 // storage/bundle.rs:5-14) — struct field order, compact, ProofBlock.cid as the byte array cid 0.11's Serialize emits, block data as

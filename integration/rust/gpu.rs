@@ -23,7 +23,7 @@ use fvm_ipld_blockstore::Blockstore;
 use ipcfp_sys as sys;
 
 use crate::client::types::{ApiReceipt, ApiTipset};
-use crate::proofs::common::bundle::{ProofBlock, UnifiedProofBundle};
+use crate::proofs::common::bundle::{ProofBlock, UnifiedProofBundle, UnifiedVerificationResult};
 use crate::proofs::events::bundle::{EventData, EventProof, EventProofBundle};
 use crate::proofs::generator::{EventProofSpec, StorageProofSpec};
 use crate::proofs::storage::bundle::StorageProof;
@@ -673,6 +673,59 @@ pub fn verify_storage_proof_gpu(
         }
     }
     Ok(results)
+}
+
+struct TrustCtx<'a> {
+    parent: &'a dyn Fn(i64, &[Cid]) -> bool,
+    child: &'a dyn Fn(i64, &Cid) -> bool,
+}
+unsafe extern "C" fn trust_parent_tramp(ctx: *mut c_void, epoch: i64, cids: *const u8, n: u32) -> std::os::raw::c_int {
+    let t = &*(ctx as *const TrustCtx);
+    let raw = if n == 0 { &[][..] } else { std::slice::from_raw_parts(cids, n as usize * CID_LEN) };
+    let parsed: std::result::Result<Vec<Cid>, _> = raw.chunks(CID_LEN).map(Cid::try_from).collect();
+    parsed.map_or(0, |v| (t.parent)(epoch, &v) as std::os::raw::c_int)
+}
+unsafe extern "C" fn trust_child_tramp(ctx: *mut c_void, epoch: i64, cid: *const u8) -> std::os::raw::c_int {
+    let t = &*(ctx as *const TrustCtx);
+    Cid::try_from(std::slice::from_raw_parts(cid, CID_LEN)).map_or(0, |c| (t.child)(epoch, &c) as std::os::raw::c_int)
+}
+
+/// `verify_proof_bundle` (`src/proofs/verifier.rs:12-60`) straight from the bundle's JSON text (EventProofBundle or UnifiedProofBundle):
+/// the parse, the witness store and both verifiers run on the GPU; text not in serde_json's canonical form is read by the host parser
+/// with the same results. The trust closures are called at most once each, on this thread.
+pub fn verify_proof_bundle_json(
+    text: &str,
+    is_trusted_parent_ts: &dyn Fn(i64, &[Cid]) -> bool,
+    is_trusted_child_header: &dyn Fn(i64, &Cid) -> bool,
+    check_event: Option<&EventProofSpec>,
+    device: i32,
+) -> Result<UnifiedVerificationResult> {
+    let filter = match check_event {
+        Some(s) => Some(spec_c(&s.event_signature, &s.topic_1, s.actor_id_filter)?),
+        None => None,
+    };
+    let ctx = TrustCtx { parent: is_trusted_parent_ts, child: is_trusted_child_header };
+    let mut out = std::ptr::null_mut();
+    check(unsafe {
+        sys::ipcfp_verify_bundle_json(
+            text.as_ptr() as *const std::os::raw::c_char,
+            text.len() as u64,
+            device,
+            Some(trust_parent_tramp),
+            Some(trust_child_tramp),
+            &ctx as *const TrustCtx as *mut c_void,
+            filter.as_ref().map_or(std::ptr::null(), |f| &f.raw as *const _),
+            &mut out,
+        )
+    })?;
+    let v = unsafe { &*out };
+    let bools = |p: *const u8, n: u64| if n == 0 { vec![] } else { unsafe { std::slice::from_raw_parts(p, n as usize) }.iter().map(|&x| x != 0).collect() };
+    let res = UnifiedVerificationResult {
+        storage_results: bools(v.storage_results, v.n_storage_proofs),
+        event_results: bools(v.event_results, v.n_event_proofs),
+    };
+    unsafe { sys::ipcfp_bundle_verdict_free(out) };
+    Ok(res)
 }
 
 /// `calculate_storage_slot` / `compute_mapping_slot` (`src/proofs/storage/utils.rs:5-19`) on the GPU, batched.

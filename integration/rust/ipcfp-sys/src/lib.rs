@@ -84,6 +84,14 @@ pub struct ipcfp_slot_result { pub n: u64, pub found: *const u8, pub raw_len: *c
 pub struct ipcfp_parsed_bundle { pub tipset: ipcfp_tipset_desc, pub n_storage_proofs: u64, pub storage_proofs: *const ipcfp_storage_proof,
                                  pub n_event_proofs: u64, pub event_proofs: *const ipcfp_event_proof, pub data_blob: *const u8, pub data_blob_size: u64,
                                  pub witness: ipcfp_witness }
+pub type ipcfp_trusted_parent_ts_fn = Option<unsafe extern "C" fn(ctx: *mut c_void, parent_epoch: i64, parent_cids: *const u8, n_parents: u32) -> c_int>;
+pub type ipcfp_trusted_child_header_fn = Option<unsafe extern "C" fn(ctx: *mut c_void, child_epoch: i64, child_cid: *const u8) -> c_int>;
+#[repr(C)]
+pub struct ipcfp_bundle_verdict { pub tipset: ipcfp_tipset_desc, pub n_storage_proofs: u64, pub storage_proofs: *const ipcfp_storage_proof,
+                                  pub storage_results: *const u8, pub n_event_proofs: u64, pub event_proofs: *const ipcfp_event_proof,
+                                  pub event_results: *const u8, pub data_blob: *const u8, pub data_blob_size: u64, pub n_blocks: u64,
+                                  pub witness_bytes: u64, pub parsed_on_device: u32, pub ms_total: f32, pub ms_parse: f32, pub ms_store: f32,
+                                  pub ms_verify: f32, pub _pad: u32 }
 #[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness }
 
@@ -139,6 +147,10 @@ extern "C" {
                                      data_blob: *const u8, data_blob_size: u64, filter: *const ipcfp_event_spec, results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_storage_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_storage_proof, n_proofs: u64,
                                        results: *mut u8) -> ipcfp_status;
+    pub fn ipcfp_verify_bundle_json(json: *const c_char, len: u64, device: c_int, trusted_parent: ipcfp_trusted_parent_ts_fn,
+                                    trusted_child: ipcfp_trusted_child_header_fn, trust_ctx: *mut c_void, filter: *const ipcfp_event_spec,
+                                    out: *mut *mut ipcfp_bundle_verdict) -> ipcfp_status;
+    pub fn ipcfp_bundle_verdict_free(v: *mut ipcfp_bundle_verdict);
     pub fn ipcfp_comm_unique_id(id: *mut u8) -> ipcfp_status;
     pub fn ipcfp_comm_init(id: *const u8, world_size: u32, rank: u32, device: c_int, out: *mut *mut ipcfp_comm) -> ipcfp_status;
     pub fn ipcfp_comm_destroy(c: *mut ipcfp_comm);

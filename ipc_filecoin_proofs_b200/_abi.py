@@ -151,6 +151,33 @@ class ParsedBundleC(C.Structure):
     ]
 
 
+TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
+TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
+
+
+class BundleVerdictC(C.Structure):
+    """ipcfp_bundle_verdict (ipcfp_verify_bundle_json)."""
+    _fields_ = [
+        ("tipset", TipsetDesc),
+        ("n_storage_proofs", C.c_uint64),
+        ("storage_proofs", C.c_void_p),
+        ("storage_results", C.c_void_p),
+        ("n_event_proofs", C.c_uint64),
+        ("event_proofs", C.c_void_p),
+        ("event_results", C.c_void_p),
+        ("data_blob", C.c_void_p),
+        ("data_blob_size", C.c_uint64),
+        ("n_blocks", C.c_uint64),
+        ("witness_bytes", C.c_uint64),
+        ("parsed_on_device", C.c_uint32),
+        ("ms_total", C.c_float),
+        ("ms_parse", C.c_float),
+        ("ms_store", C.c_float),
+        ("ms_verify", C.c_float),
+        ("_pad", C.c_uint32),
+    ]
+
+
 class StorageResultC(C.Structure):
     _fields_ = [
         ("n_proofs", C.c_uint64),

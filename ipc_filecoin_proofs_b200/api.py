@@ -43,7 +43,7 @@ EXPORTS = [
     "ipcfp_store_stream", "ipcfp_exec_bucketize", "ipcfp_exec_dedup", "ipcfp_exec_fetch",
     "ipcfp_comm_unique_id", "ipcfp_comm_init", "ipcfp_comm_destroy", "ipcfp_generate_event_proof_sharded",
     "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
-    "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free",
+    "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
 ]
 
 
@@ -139,6 +139,10 @@ def lib():
         L.ipcfp_bundle_from_json.restype = C.c_int32
         L.ipcfp_bundle_from_json.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.POINTER(A.ParsedBundleC))]
         L.ipcfp_parsed_bundle_free.argtypes = [C.POINTER(A.ParsedBundleC)]
+        L.ipcfp_verify_bundle_json.restype = C.c_int32
+        L.ipcfp_verify_bundle_json.argtypes = [C.c_char_p, C.c_uint64, C.c_int, A.TrustedParentFn, A.TrustedChildFn, C.c_void_p, C.c_void_p,
+                                               C.POINTER(C.POINTER(A.BundleVerdictC))]
+        L.ipcfp_bundle_verdict_free.argtypes = [C.POINTER(A.BundleVerdictC)]
         _lib = L
     return _lib
 
@@ -376,6 +380,47 @@ class ParsedBundle:
             self.close()
         except Exception:
             pass
+
+
+class BundleVerdict:
+    """verify_proof_bundle (src/proofs/verifier.rs:12-60) from the JSON text (ipcfp_verify_bundle_json): storage_results / event_results
+    (UnifiedVerificationResult), the parsed proofs (raw PODs, as ParsedBundle has them), the shared tipset fields, the path taken
+    (parsed_on_device) and the phase times."""
+
+    def __init__(self, c):
+        n_s, n_e = int(c.n_storage_proofs), int(c.n_event_proofs)
+        self.storage_results = [bool(x) for x in A._arr(c.storage_results, n_s, np.uint8)] if n_s else []
+        self.event_results = [bool(x) for x in A._arr(c.event_results, n_e, np.uint8)] if n_e else []
+        self.storage_proofs_raw = A._arr(c.storage_proofs, n_s * C.sizeof(A.StorageProofC), np.uint8).copy() if n_s else np.zeros(0, np.uint8)
+        self.event_proofs_raw = A._arr(c.event_proofs, n_e * C.sizeof(A.EventProofC), np.uint8).copy() if n_e else np.zeros(0, np.uint8)
+        nb = int(c.data_blob_size)
+        self.data_blob = A._arr(c.data_blob, nb, np.uint8).copy() if nb else np.zeros(0, np.uint8)
+        t = c.tipset
+        P = int(t.n_parents)
+        self.tipset = dict(parent_epoch=int(t.parent_epoch), child_epoch=int(t.child_epoch),
+                           parent_cids=A._arr(t.parent_cids, P * A.CID_LEN, np.uint8).tobytes() if P else b"",
+                           child_cid=A._arr(t.child_cid, A.CID_LEN, np.uint8).tobytes() if t.child_cid else None,
+                           parent_state_root=A._arr(t.child_parent_state_root, A.CID_LEN, np.uint8).tobytes() if t.child_parent_state_root else None)
+        self.n_blocks, self.witness_bytes = int(c.n_blocks), int(c.witness_bytes)
+        self.parsed_on_device = bool(c.parsed_on_device)
+        self.ms = dict(total=c.ms_total, parse=c.ms_parse, store=c.ms_store, verify=c.ms_verify)
+
+
+def verify_bundle_json(text, trusted_parent=None, trusted_child=None, filter_spec=None, device=0):
+    """ipcfp_verify_bundle_json. trusted_parent(epoch, parent_cids: bytes) / trusted_child(epoch, child_cid: bytes) → bool, None = accept
+    all. filter_spec: an A.EventSpec (check_event) or None. → BundleVerdict; failures raise IpcfpError (status, index)."""
+    raw = text.encode() if isinstance(text, str) else bytes(text)
+    cb_p = A.TrustedParentFn(lambda ctx, e, p, n: int(bool(trusted_parent(int(e), C.string_at(p, 38 * n) if n else b""))))\
+        if trusted_parent else A.TrustedParentFn()
+    cb_c = A.TrustedChildFn(lambda ctx, e, c: int(bool(trusted_child(int(e), C.string_at(c, 38))))) if trusted_child else A.TrustedChildFn()
+    out = C.POINTER(A.BundleVerdictC)()
+    L = lib()
+    _check(L.ipcfp_verify_bundle_json(raw, len(raw), device, cb_p, cb_c, None, C.addressof(filter_spec) if filter_spec is not None else None,
+                                      C.byref(out)))
+    try:
+        return BundleVerdict(out.contents)
+    finally:
+        L.ipcfp_bundle_verdict_free(out)
 
 
 def verify_event_proofs(witness, ts, result, filter_spec=None, device=0):

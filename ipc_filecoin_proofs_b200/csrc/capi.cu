@@ -344,6 +344,17 @@ ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* s, const ipcfp_tipset_desc
     });
 }
 
+ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
+                                      ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
+                                      ipcfp_bundle_verdict** out) {
+    return guard([&] {
+        if (!json || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, filter);
+    });
+}
+void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v) { if (v) bundle_verdict_free(v); }
+
 ipcfp_status ipcfp_comm_unique_id(uint8_t id[IPCFP_COMM_ID_BYTES]) {
     return guard([&] {
         if (!id) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");

@@ -102,6 +102,12 @@ void hash_batch(int which, const uint8_t* blob, uint64_t blob_size, const uint64
                 uint8_t* out);
 void mapping_slots(const uint8_t* keys32, const uint64_t* slot_indices, uint64_t n, int device, uint8_t* out);
 void check_device(int device);
+// the pieces of store_create, for a caller that writes the blocks on the device itself (json_parse.cu):
+//   store_shell → store_alloc_blocks → (fill cids_dev, offsets, lengths, arena + 16) → store_index → store_verify_all
+Store* store_shell(int device);   // stream, events, counters; no block yet
+void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev);
+void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws);
+void store_verify_all(Store* s);
 // counters dev_words[first, first+count) → host_words (same indices) through mapped host memory: a tiny kernel
 // instead of a D2H copy, so the read-back never queues behind a large copy on the copy engine
 void publish_words(Store* s, uint32_t first, uint32_t count);
@@ -123,6 +129,14 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* t, T
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
                          const ipcfp_event_spec* filter, uint8_t* results);
 void verify_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results);
+// … the same with the proofs (and the data blob, padded by 16 bytes) already in device memory
+void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
+                             const ipcfp_event_spec* filter, uint8_t* results);
+void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* d_proofs, uint64_t n, uint8_t* results);
+// json_parse.cu — ipcfp_verify_bundle_json
+ipcfp_bundle_verdict* verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
+                                         ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter);
+void bundle_verdict_free(ipcfp_bundle_verdict* v);
 void event_result_free(ipcfp_event_result* r);
 void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n);
 void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,

@@ -306,15 +306,10 @@ static void compute_class_ranks(Store* s) {
     for (size_t r = 0; r < nc; r++) s->class_rank[order[r]] = (uint32_t)r;
 }
 
-Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size, uint64_t n,
-                    int device, uint32_t flags) {
+Store* store_shell(int device) {
     check_device(device);
-    if (n >= 0x7fffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^31 blocks in one store");
-    if (n && (!cids || !offsets || !lengths || (!blob && blob_size))) throw Error(IPCFP_ERR_INVALID_ARG, "null input array");
     std::unique_ptr<Store> s(new Store());
     s->device = device;
-    s->n = n;
-    s->blob_size = blob_size;
     {   // one process-wide pinned pool: result buffers are recycled across stores and calls
         static std::mutex pool_mu;
         static std::shared_ptr<PinnedPool> g_pool;
@@ -332,7 +327,13 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
         if (cudaDeviceGetDefaultMemPool(&mp, device) == cudaSuccess) { uint64_t thr = UINT64_MAX; cudaMemPoolSetAttribute(mp, cudaMemPoolAttrReleaseThreshold, &thr); }
     }
     IPCFP_CUDA(cudaMemsetAsync(s->dev_words.p, 0, 64 * 8, st));
+    return s.release();
+}
 
+void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev) {
+    if (n >= 0x7fffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^31 blocks in one store");
+    s->n = n;
+    s->blob_size = blob_size;
     // device allocations
     // (from the process-wide device pool: a store created right after one of similar size was destroyed allocates nothing)
     s->arena.alloc_pooled(blob_size + 48 + 512);   // + room for whole aligned chunks around the last block (pass-1 staging copies CH-aligned chunks)
@@ -346,8 +347,95 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
     uint64_t slots = 64;
     while (slots < 2 * n) slots <<= 1;
     s->table.alloc_pooled(slots);
-    DevBuf<uint8_t> cids_dev, sort_ws;
     cids_dev.alloc_pooled(n * 38 + 16);
+}
+
+// Class prefixes, `Cid` ranks, block records and the hash index of the n blocks whose CIDs are at cids_dev (n*38, device) and whose
+// offsets / lengths are in the store: everything of the ingest that does not touch block bytes. cids_host: the same CIDs on the host, or
+// null (the rare several-prefix path then reads them back). first_prefix: the first CID's 6 prefix bytes (host). Leaves the view
+// uploaded; the last synchronisation is the class check's.
+void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws) {
+    const uint64_t n = s->n;
+    cudaStream_t st = s->stream;
+    // CID classes: the first CID's prefix is class 0; anything else is discovered by the kernel
+    if (n) { std::array<uint8_t, 6> p0; memcpy(p0.data(), first_prefix, 6); s->class_prefix.push_back(p0); }
+    for (int attempt = 0; attempt < 2 && n; attempt++) {
+        compute_class_ranks(s);
+        fill_view(s);
+        unsigned long long* unknown = s->dev_words.p + 1;
+        IPCFP_CUDA(cudaMemsetAsync(unknown, 0, 8, st));
+        k_extract_digests<<<div_up(n, 256), 256, 0, st>>>(cids_dev, (uint32_t)n, s->view, s->digests.p, s->cls.p, unknown);
+        IPCFP_LAUNCH_CHECK();
+        IPCFP_CUDA(cudaMemcpyAsync(s->host_words.p, unknown, 8, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        if (s->host_words.p[0] == 0) break;
+        if (attempt == 1) throw Error(IPCFP_ERR_UNSUPPORTED, "internal: CID classes unresolved");
+        // rare path: several CID prefixes in one store — enumerate them on the host
+        std::vector<uint8_t> back;
+        if (!cids_host) {
+            back.resize(n * 38);
+            IPCFP_CUDA(cudaMemcpyAsync(back.data(), cids_dev, n * 38, cudaMemcpyDeviceToHost, st));
+            IPCFP_CUDA(cudaStreamSynchronize(st));
+        }
+        const uint8_t* cids = cids_host ? cids_host : back.data();
+        for (uint64_t i = 0; i < n; i++) {
+            std::array<uint8_t, 6> p;
+            memcpy(p.data(), cids + 38 * i, 6);
+            if (std::find(s->class_prefix.begin(), s->class_prefix.end(), p) == s->class_prefix.end()) {
+                if (s->class_prefix.size() >= IPCFP_MAX_CID_CLASSES) throw Error(IPCFP_ERR_UNSUPPORTED, "too many distinct CID prefixes in one store", i);
+                s->class_prefix.push_back(p);
+            }
+        }
+    }
+    if (!n) { fill_view(s); }
+    if (n) {
+        // `Cid` Ord rank of every block (one sort per store, under the blob copy): witness bitmaps are indexed by rank, so that every
+        // later call reads its witness out of the bitmap already in BTreeSet<Cid> order
+        sort_ws.alloc_pooled(n * 4 + 256 + sort_by_cid_ws_bytes(n));   // released (to the device pool) by the caller: after its final sync
+        uint32_t* iota = (uint32_t*)sort_ws.p;
+        k_iota<<<div_up(n, 256), 256, 0, st>>>(iota, (uint32_t)n); IPCFP_LAUNCH_CHECK();
+        sort_by_cid(s, iota, s->block_at_rank.p, n, sort_ws.p + ((n * 4 + 255) & ~(uint64_t)255));
+        k_invert_perm<<<div_up(n, 256), 256, 0, st>>>(s->block_at_rank.p, (uint32_t)n, s->rank_of.p); IPCFP_LAUNCH_CHECK();
+        k_build_recs<<<div_up(n, 256), 256, 0, st>>>((uint32_t)n, s->digests.p, s->cls.p, s->offsets.p, s->lengths.p, s->recs.p);
+        IPCFP_LAUNCH_CHECK();
+        k_build_index<<<div_up(n, 256), 256, 0, st>>>((uint32_t)n, s->digests.p, s->cls.p, (unsigned long long*)s->table.p, s->table.n - 1);
+        IPCFP_LAUNCH_CHECK();
+    }
+    upload_view(s);
+}
+
+// the classes whose multihash is Blake2b-256 (0xb220): the blocks IPCFP_STORE_VERIFY_CIDS checks
+static uint32_t blake2b_class_mask(const Store* s) {
+    uint32_t mask = 0;
+    for (size_t c = 0; c < s->class_prefix.size(); c++) {
+        uint64_t key[4];
+        parse_prefix(s->class_prefix[c].data(), key);
+        if (key[2] == 0xb220) mask |= 1u << c;
+    }
+    return mask;
+}
+
+// IPCFP_STORE_VERIFY_CIDS over every block of a store whose blocks are all on the device already; synchronises, sets first_bad
+void store_verify_all(Store* s) {
+    cudaStream_t st = s->stream;
+    unsigned long long* bad = s->dev_words.p + 2;
+    IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
+    if (s->n) { k_verify_cids<<<div_up(s->n, 128), 128, 0, st>>>(s->view, 0, (uint32_t)s->n, blake2b_class_mask(s), bad); IPCFP_LAUNCH_CHECK(); }
+    publish_words(s, 2, 1);
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    s->first_bad = s->host_words.p[2];
+}
+
+Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size, uint64_t n,
+                    int device, uint32_t flags) {
+    check_device(device);
+    if (n >= 0x7fffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^31 blocks in one store");
+    if (n && (!cids || !offsets || !lengths || (!blob && blob_size))) throw Error(IPCFP_ERR_INVALID_ARG, "null input array");
+    std::unique_ptr<Store> s(store_shell(device));
+    cudaStream_t st = s->stream;
+    DevBuf<uint8_t> cids_dev, sort_ws;   // released (to the device pool) when this function returns: after its final sync
+    store_alloc_blocks(s.get(), n, blob_size, cids_dev);
+    const uint64_t slots = s->table.n;
 
     // H2D. The CID array goes first so the index build overlaps the (much larger) blob copy.
     cudaStream_t st2;
@@ -390,51 +478,9 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
         IPCFP_CUDA(cudaEventRecord(chunk_ev[k], st2));
     }
 
-    // CID classes: the first CID's prefix is class 0; anything else is discovered by the kernel
-    if (n) { std::array<uint8_t, 6> p0; memcpy(p0.data(), cids, 6); s->class_prefix.push_back(p0); }
-    for (int attempt = 0; attempt < 2 && n; attempt++) {
-        compute_class_ranks(s.get());
-        fill_view(s.get());
-        unsigned long long* unknown = s->dev_words.p + 1;
-        IPCFP_CUDA(cudaMemsetAsync(unknown, 0, 8, st));
-        k_extract_digests<<<div_up(n, 256), 256, 0, st>>>(cids_dev.p, (uint32_t)n, s->view, s->digests.p, s->cls.p, unknown);
-        IPCFP_LAUNCH_CHECK();
-        IPCFP_CUDA(cudaMemcpyAsync(s->host_words.p, unknown, 8, cudaMemcpyDeviceToHost, st));
-        IPCFP_CUDA(cudaStreamSynchronize(st));
-        if (s->host_words.p[0] == 0) break;
-        if (attempt == 1) throw Error(IPCFP_ERR_UNSUPPORTED, "internal: CID classes unresolved");
-        // rare path: several CID prefixes in one store — enumerate them on the host
-        for (uint64_t i = 0; i < n; i++) {
-            std::array<uint8_t, 6> p;
-            memcpy(p.data(), cids + 38 * i, 6);
-            if (std::find(s->class_prefix.begin(), s->class_prefix.end(), p) == s->class_prefix.end()) {
-                if (s->class_prefix.size() >= IPCFP_MAX_CID_CLASSES) throw Error(IPCFP_ERR_UNSUPPORTED, "too many distinct CID prefixes in one store", i);
-                s->class_prefix.push_back(p);
-            }
-        }
-    }
-    if (!n) { fill_view(s.get()); }
-    if (n) {
-        // `Cid` Ord rank of every block (one sort per store, under the blob copy): witness bitmaps are indexed by rank, so that every
-        // later call reads its witness out of the bitmap already in BTreeSet<Cid> order
-        sort_ws.alloc_pooled(n * 4 + 256 + sort_by_cid_ws_bytes(n));   // released (to the device pool) when this function returns: after its final sync
-        uint32_t* iota = (uint32_t*)sort_ws.p;
-        k_iota<<<div_up(n, 256), 256, 0, st>>>(iota, (uint32_t)n); IPCFP_LAUNCH_CHECK();
-        sort_by_cid(s.get(), iota, s->block_at_rank.p, n, sort_ws.p + ((n * 4 + 255) & ~(uint64_t)255));
-        k_invert_perm<<<div_up(n, 256), 256, 0, st>>>(s->block_at_rank.p, (uint32_t)n, s->rank_of.p); IPCFP_LAUNCH_CHECK();
-        k_build_recs<<<div_up(n, 256), 256, 0, st>>>((uint32_t)n, s->digests.p, s->cls.p, s->offsets.p, s->lengths.p, s->recs.p);
-        IPCFP_LAUNCH_CHECK();
-        k_build_index<<<div_up(n, 256), 256, 0, st>>>((uint32_t)n, s->digests.p, s->cls.p, (unsigned long long*)s->table.p, s->table.n - 1);
-        IPCFP_LAUNCH_CHECK();
-    }
-    upload_view(s.get());
+    store_index(s.get(), cids_dev.p, cids, cids, sort_ws);
     if (verify) {
-        uint32_t mask = 0;
-        for (size_t c = 0; c < s->class_prefix.size(); c++) {
-            uint64_t key[4];
-            parse_prefix(s->class_prefix[c].data(), key);
-            if (key[2] == 0xb220) mask |= 1u << c;
-        }
+        const uint32_t mask = blake2b_class_mask(s.get());
         unsigned long long* bad = s->dev_words.p + 2;
         IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
         for (size_t k = 0; k < chunks.size(); k++) {   // chunk k is checked while chunk k+1 is on the wire

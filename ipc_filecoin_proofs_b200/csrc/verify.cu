@@ -55,17 +55,28 @@ void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event
     if (n && (!proofs || !results)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
     if (n == 0) return;
     cudaStream_t st = s->stream;
+    AsyncBuf<uint8_t> d_blob(blob_size + 16, st);
+    AsyncBuf<ipcfp_event_proof> d_proofs(n, st);
+    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_event_proof), cudaMemcpyHostToDevice, st));
+    if (blob_size) IPCFP_CUDA(cudaMemcpyAsync(d_blob.p, data_blob, blob_size, cudaMemcpyHostToDevice, st));
+    verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results);
+}
+
+// the proofs and their data blob (blob_size bytes + 16 of padding) already on the device, on the store's device
+void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
+                             const ipcfp_event_spec* filter, uint8_t* results) {
+    if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
+    if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
+    if (n == 0) return;
+    cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
     uint64_t* hw = s->host_words.p;
     const uint32_t P = t->n_parents;
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
-    AsyncBuf<uint8_t> d_cids(38ull * (2 * P + 2) + 64, st), d_blob(blob_size + 16, st), d_res(n + 16, st);
+    AsyncBuf<uint8_t> d_cids(38ull * (2 * P + 2) + 64, st), d_res(n + 16, st);
     AsyncBuf<uint32_t> d_flags(8, st);
-    AsyncBuf<ipcfp_event_proof> d_proofs(n, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_cids.p, t->child_cid, 38, cudaMemcpyHostToDevice, st));
     if (P) IPCFP_CUDA(cudaMemcpyAsync(d_cids.p + 38, t->parent_cids, 38ull * P, cudaMemcpyHostToDevice, st));
-    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_event_proof), cudaMemcpyHostToDevice, st));
-    if (blob_size) IPCFP_CUDA(cudaMemcpyAsync(d_blob.p, data_blob, blob_size, cudaMemcpyHostToDevice, st));
     uint8_t* d_tx = d_cids.p + 38ull * (P + 1);
     VerifyTipsetArgs ta;
     ta.store = s->view; ta.parent_cids = d_cids.p + 38; ta.child_cid = d_cids.p; ta.n_parents = P;
@@ -130,7 +141,7 @@ void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event
         IPCFP_CUDA(cudaStreamSynchronize(st));   // m is a stack object
     }
     VerifyEventArgs va;
-    va.store = s->view; va.proofs = d_proofs.p; va.n = n; va.blob = d_blob.p; va.blob_size = blob_size;
+    va.store = s->view; va.proofs = d_proofs; va.n = n; va.blob = d_blob; va.blob_size = blob_size;
     va.consistent = d_flags.p; va.receipts_root_blk = d_flags.p + 1;
     va.exec_raw = exo.exec_raw.p; va.exec_idx = exo.exec_idx.p; va.n_exec = exo.n_exec;
     va.filter = filter ? d_filter.p : nullptr; va.results = d_res.p; va.err = dw;
@@ -154,16 +165,24 @@ void verify_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_sto
     if (n && (!proofs || !results)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
     if (n == 0) return;
     cudaStream_t st = s->stream;
+    AsyncBuf<ipcfp_storage_proof> d_proofs(n, st);
+    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_storage_proof), cudaMemcpyHostToDevice, st));
+    verify_storage_proofs_dev(s, t, d_proofs.p, n, results);
+}
+
+// the proofs already on the device, on the store's device
+void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* d_proofs, uint64_t n, uint8_t* results) {
+    if (!t || !t->child_cid || !t->child_parent_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+    if (n == 0) return;
+    cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
     uint64_t* hw = s->host_words.p;
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
     AsyncBuf<uint8_t> d_in(128, st), d_res(n + 16, st);
-    AsyncBuf<ipcfp_storage_proof> d_proofs(n, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_in.p, t->child_cid, 38, cudaMemcpyHostToDevice, st));
     IPCFP_CUDA(cudaMemcpyAsync(d_in.p + 64, t->child_parent_state_root, 38, cudaMemcpyHostToDevice, st));
-    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_storage_proof), cudaMemcpyHostToDevice, st));
     VerifyStorageArgs a;
-    a.store = s->view; a.child_cid = d_in.p; a.state_root_json = d_in.p + 64; a.proofs = d_proofs.p; a.n = n; a.results = d_res.p; a.err = dw;
+    a.store = s->view; a.child_cid = d_in.p; a.state_root_json = d_in.p + 64; a.proofs = d_proofs; a.n = n; a.results = d_res.p; a.err = dw;
     k_verify_storage<<<div_up(n * 32, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK();
     IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
