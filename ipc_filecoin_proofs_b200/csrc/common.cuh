@@ -190,19 +190,6 @@ __device__ __forceinline__ void win_load(const uint8_t* q, uint64_t& w0, uint64_
     w0 = (uint64_t)__funnelshift_r(c0, c1, s) | ((uint64_t)__funnelshift_r(c1, c2, s) << 32);
     w1 = (uint64_t)__funnelshift_r(c2, c3, s) | ((uint64_t)__funnelshift_r(c3, c4, s) << 32);
 }
-// the same 16 bytes with TWO aligned 16-byte loads (32 bytes at q & ~15): a warp whose lanes read 32 different lines pays one L1
-// wavefront per lane and LOAD, so this costs 2/3 of win_load's wavefronts for ~5 more ALU instructions (may touch up to 31 bytes
-// past q and up to 15 before it: buffers are padded by ≥ 16 / 32 bytes)
-__device__ __forceinline__ void win_load16(const uint8_t* q, uint64_t& w0, uint64_t& w1) {
-    uintptr_t a = (uintptr_t)q;
-    const ulonglong2* b = (const ulonglong2*)(a & ~(uintptr_t)15);
-    const ulonglong2 x0 = b[0], x1 = b[1];
-    const bool up = (a & 8) != 0;
-    const uint64_t A = up ? x0.y : x0.x, B = up ? x1.x : x0.y, C = up ? x1.y : x1.x;
-    const uint32_t s = (uint32_t)(a & 7) * 8;
-    w0 = (A >> s) | ((B << 1) << (63 - s));
-    w1 = (B >> s) | ((C << 1) << (63 - s));
-}
 __device__ __forceinline__ Digest load_digest(const uint8_t* p) {
     uintptr_t a = (uintptr_t)p;
     const uint64_t* b = (const uint64_t*)(a & ~(uintptr_t)7);
@@ -214,7 +201,6 @@ __device__ __forceinline__ Digest load_digest(const uint8_t* p) {
     return d;
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 #endif
 
 }  // namespace ipcfp

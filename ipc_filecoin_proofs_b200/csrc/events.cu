@@ -5,9 +5,10 @@
 //   k_amt_level/...    record_transaction_amts (:148-177) and build_execution_order
 //                      (events/utils.rs:33-94) as ONE level-synchronous, order-preserving BFS
 //   k_dedup_*          first-seen dedup of the execution order (utils.rs:56-91)
-//   k_pass1            find_matching_events pass 1 (:206-239): one thread decodes one events-AMT
-//                      root node, tests (actor_id, topic_0, topic_1) on every StampedEvent, the
-//                      warp ballots the matching-receipt bitmap
+//   k_pass1_stage      find_matching_events pass 1 (:206-239, pass1_stage.cuh): one lane decodes one
+//                      events-AMT root node, its bytes staged through shared memory by the whole warp,
+//                      tests (actor_id, topic_0, topic_1) on every StampedEvent, the warp ballots the
+//                      matching-receipt bitmap
 //   k_pass2<EMIT>      pass 2 (:241-301): per matching receipt, receipts-AMT path walk + full
 //                      events-AMT walk, witness bits, EventProof records
 //   materialize_witness (witness.cu)   WitnessCollector::materialize (:104)
@@ -22,133 +23,13 @@
 #include "prims.cuh"
 #include "walk.cuh"
 #include "events_items.cuh"
-#include "pass1_ring.cuh"
 #include "pass1_stage.cuh"
 #include "rawcid.cuh"
 
 namespace ipcfp {
 
 // ------------------------------------------------------------------------------------------ pass 1 / pass 2 kernels (per-receipt code: events_items.cuh)
-// One thread per receipt: resolve its events root CID, decode the root node of its events AMT,
-// test every StampedEvent. The common single-node AMT (≤ 2^bw events) never leaves this
-// function; taller AMTs fall through to the generic walker.
-template <int WINMODE = 0>
-__device__ __forceinline__ void pass1_body(const Pass1Args& a) {
-    uint64_t i = a.lo + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool matched = false;
-    uint32_t bytes = 0, nodes = 0, np_ = 0, nb_ = 0;
-    // phase 1: Blockstore::get of the events root (hash probe); every lane takes part so the warp
-    // can be re-converged before the long decode
-    const bool valid = i < a.hi && a.has_root[i];
-    int32_t blk = -1;
-    if (valid) {
-        blk = store_lookup(a.store, a.events_roots + 38 * i);
-        if (blk < 0) report_error(a.err, ST_PASS1, i, DC_MISSING, 0);
-    }
-    uint32_t len = 0;
-    const uint8_t* p = nullptr;
-    if (blk >= 0) {
-        p = store_block(a.store, (uint32_t)blk, len);
-        const uint32_t first = (a.tune & 4) ? 2048u : ((a.tune & 8) ? 256u : 512u);
-        for (uint32_t o = 0; o < len && o < first; o += 128) prefetch_l2(p + o);  // first lines in flight before the dependent walk
-    }
-    __syncwarp();
-    // phase 2: decode the root node, test every event
-    if (blk >= 0) {
-        bytes = len + 38; nodes = 1;
-        Rd r(p, len);
-        uint32_t bw, height;
-        uint64_t cnt;
-        amt_root_begin(r, 3, bw, height, cnt);
-        AmtNodeHdr h;
-        amt_node_begin(r, bw, h);
-        uint32_t nv = rd_array(r);
-        WalkOut wo{0, 0, false};
-        node_events<WALK_COUNT, WINMODE>(r, p, h, nv, 0, a.m, wo, nullptr, a.tune);
-        amt_node_finish(r, h, nv, height);
-        if (r.err) report_error(a.err, ST_PASS1, i, DC_DECODE, r.err);
-        else if (h.nl) {
-            uint32_t detail = 0;
-            wo = WalkOut{0, 0, false};
-            uint32_t rc = walk_events<WALK_COUNT>(a.store_dev, (uint32_t)blk, a.m_dev, nullptr, wo, nullptr, &detail);
-            if (rc) { report_error(a.err, ST_PASS1, i, rc, detail); wo = WalkOut{0, 0, false}; }
-        }
-        matched = wo.any;
-        np_ = wo.nproofs; nb_ = wo.nbytes;
-    }
-    if (i < a.hi) { a.cnt[i - a.lo] = np_; a.nbytes[i - a.lo] = nb_; }
-    unsigned b = __ballot_sync(0xffffffffu, matched);
-    if ((threadIdx.x & 31) == 0) a.match_bits[((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5] = b;
-    // per-warp statistics (algorithmic bytes of the scan)
-    for (int o = 16; o; o >>= 1) { bytes += __shfl_xor_sync(0xffffffffu, bytes, o); nodes += __shfl_xor_sync(0xffffffffu, nodes, o); }
-    if ((threadIdx.x & 31) == 0 && nodes) { atomicAdd(a.stats, (unsigned long long)nodes); atomicAdd(a.stats + 1, (unsigned long long)bytes); }
-}
-// the same kernel at three register budgets (resident CTAs per SM: 6 → 80 regs, 8 → 64, 10 → 48);
-// IPCFP_PASS1_MINB selects one at run time. The default pass 1 is the staged kernel (pass1_stage.cuh): faster on H100 (DESIGN.md §4)
-__global__ void __launch_bounds__(128, 6) k_pass1(Pass1Args a) { pass1_body(a); }
-__global__ void __launch_bounds__(128, 8) k_pass1_occ8(Pass1Args a) { pass1_body(a); }
-__global__ void __launch_bounds__(128, 10) k_pass1_occ10(Pass1Args a) { pass1_body(a); }
-// windows through two 16-byte loads (2/3 of the L1 wavefronts of three 8-byte loads)
-__global__ void __launch_bounds__(128, 8) k_pass1_w16(Pass1Args a) { pass1_body<1>(a); }
-__global__ void __launch_bounds__(128, 6) k_pass1_w16_occ6(Pass1Args a) { pass1_body<1>(a); }
-
-// ---- EXPERIMENT (round 2): pass 1 through per-lane shared-memory rings, see pass1_ring.cuh. Same outputs as k_pass1;
-// a node the ring path cannot take (malformed head, links = taller AMT) is re-decoded by the arena path below.
-template <int CH, int NSLOT>
-__global__ void __launch_bounds__(128, (CH * NSLOT <= 256 ? 6 : 3)) k_pass1_ring(Pass1Args a, const uint8_t* arena_end) {
-    extern __shared__ __align__(16) uint8_t ring_smem[];
-    constexpr uint32_t STRIDE = CH * NSLOT + 16;      // 16-byte aligned rows, 4 banks apart
-    uint64_t i = a.lo + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool matched = false;
-    uint32_t bytes = 0, nodes = 0, np_ = 0, nb_ = 0;
-    const bool valid = i < a.hi && a.has_root[i];
-    int32_t blk = -1;
-    if (valid) {
-        blk = store_lookup(a.store, a.events_roots + 38 * i);
-        if (blk < 0) report_error(a.err, ST_PASS1, i, DC_MISSING, 0);
-    }
-    uint32_t len = 0;
-    const uint8_t* p = nullptr;
-    RingWin<CH, NSLOT> ring;
-    if (blk >= 0) {
-        p = store_block(a.store, (uint32_t)blk, len);
-        ring.init(ring_smem + threadIdx.x * STRIDE, p, len, arena_end);
-        ring.top_up(0);                                 // first NSLOT chunks in flight before the dependent walk
-    }
-    __syncwarp();
-    if (blk >= 0) {
-        bytes = len + 38; nodes = 1;
-        WalkOut wo{0, 0, false};
-        const bool taken = pass1_ring_item(ring, p, len, a.m, wo);
-        if (!taken) {                                    // the arena path decides (and reports) everything about this node
-            wo = WalkOut{0, 0, false};
-            Rd r(p, len);
-            uint32_t bw, height;
-            uint64_t cnt;
-            amt_root_begin(r, 3, bw, height, cnt);
-            AmtNodeHdr h;
-            amt_node_begin(r, bw, h);
-            uint32_t nv = rd_array(r);
-            node_events<WALK_COUNT>(r, p, h, nv, 0, a.m, wo, nullptr, 2u);
-            amt_node_finish(r, h, nv, height);
-            if (r.err) report_error(a.err, ST_PASS1, i, DC_DECODE, r.err);
-            else if (h.nl) {
-                uint32_t detail = 0;
-                wo = WalkOut{0, 0, false};
-                uint32_t rc = walk_events<WALK_COUNT>(a.store_dev, (uint32_t)blk, a.m_dev, nullptr, wo, nullptr, &detail);
-                if (rc) { report_error(a.err, ST_PASS1, i, rc, detail); wo = WalkOut{0, 0, false}; }
-            }
-            if (r.err) wo = WalkOut{0, 0, false};
-        }
-        matched = wo.any;
-        np_ = wo.nproofs; nb_ = wo.nbytes;
-    }
-    if (i < a.hi) { a.cnt[i - a.lo] = np_; a.nbytes[i - a.lo] = nb_; }
-    unsigned b = __ballot_sync(0xffffffffu, matched);
-    if ((threadIdx.x & 31) == 0) a.match_bits[((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5] = b;
-    for (int o = 16; o; o >>= 1) { bytes += __shfl_xor_sync(0xffffffffu, bytes, o); nodes += __shfl_xor_sync(0xffffffffu, nodes, o); }
-    if ((threadIdx.x & 31) == 0 && nodes) { atomicAdd(a.stats, (unsigned long long)nodes); atomicAdd(a.stats + 1, (unsigned long long)bytes); }
-}
+// Pass 1 is k_pass1_stage (pass1_stage.cuh).
 
 // exec.get(i) for every matching receipt against the GLOBAL execution order length (sharded calls: the order spans shards)
 __global__ void k_check_exec(const uint32_t* __restrict__ match_rel, uint64_t n_match, uint64_t lo, const unsigned long long* __restrict__ n_exec,
@@ -779,46 +660,10 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     p1.store = s->view; p1.store_dev = s->view_dev.p; p1.m_dev = d_matcher; p1.m = mh; p1.events_roots = td.events_roots.p; p1.has_root = td.has_root.p; p1.lo = lo; p1.hi = hi;
     p1.match_bits = match_bits.p; p1.cnt = cnt.p; p1.nbytes = nby.p; p1.err = dw; p1.stats = dw + 4;
     if (N) {
-        // kernel variant: read per call so that one process can sweep them (tools/profile_step.py)
-        //   IPCFP_PASS1_STAGE=<chunk>x<slots>x<chunks per pass>   warp-cooperative shared-memory staging (pass1_stage.cuh); default 128x4x1
-        //   IPCFP_PASS1_RING=<chunk>x<slots>                      per-lane cp.async rings (pass1_ring.cuh, round-1 experiment)
-        //   IPCFP_PASS1_MINB=6|8|10, IPCFP_PASS1_TUNE=<bits>      thread-per-node kernel straight from the arena (round 1)
-        const char* stage_env = getenv("IPCFP_PASS1_STAGE");
-        const char* ring_env = getenv("IPCFP_PASS1_RING");
-        const char* minb_env = getenv("IPCFP_PASS1_MINB");
-        const int minb = minb_env ? atoi(minb_env) : 8;
-        p1.tune = (uint32_t)(getenv("IPCFP_PASS1_TUNE") ? atoi(getenv("IPCFP_PASS1_TUNE")) : 0);
-        auto launch_stage = [&](auto kern, int warps, size_t warp_bytes) {
-            const size_t smem = warps * warp_bytes;
-            IPCFP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            kern<<<div_up(N, 32 * warps), 32 * warps, smem, st>>>(p1);
-        };
-        auto launch_ring = [&](auto kern, size_t smem) {
-            IPCFP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            kern<<<div_up(N, 128), 128, smem, st>>>(p1, (const uint8_t*)s->arena.p + s->arena.n);
-        };
-        auto is = [](const char* e, const char* v) { return e && !strcmp(e, v); };
-        if (is(stage_env, "lean128x4x1")) launch_stage(k_pass1_stage<128, 4, 1, 4, 3, 1>, 4, StageGeom<128, 4, 1>::WARP_BYTES);
-        else if (is(stage_env, "lean128x4x1w2")) launch_stage(k_pass1_stage<128, 4, 1, 2, 6, 1>, 2, StageGeom<128, 4, 1>::WARP_BYTES);
-        else if (is(stage_env, "lean64x8x2")) launch_stage(k_pass1_stage<64, 8, 2, 4, 3, 1>, 4, StageGeom<64, 8, 2>::WARP_BYTES);
-        else if (is(stage_env, "lean128x4x2")) launch_stage(k_pass1_stage<128, 4, 2, 4, 3, 1>, 4, StageGeom<128, 4, 2>::WARP_BYTES);
-        else if (is(stage_env, "128x4x1")) launch_stage(k_pass1_stage<128, 4, 1, 4, 3>, 4, StageGeom<128, 4, 1>::WARP_BYTES);
-        else if (is(stage_env, "128x4x1w2")) launch_stage(k_pass1_stage<128, 4, 1, 2, 6>, 2, StageGeom<128, 4, 1>::WARP_BYTES);
-        else if (is(stage_env, "128x4x2")) launch_stage(k_pass1_stage<128, 4, 2, 4, 3>, 4, StageGeom<128, 4, 2>::WARP_BYTES);
-        else if (is(stage_env, "64x8x2")) launch_stage(k_pass1_stage<64, 8, 2, 4, 3>, 4, StageGeom<64, 8, 2>::WARP_BYTES);
-        else if (is(stage_env, "64x4x2")) launch_stage(k_pass1_stage<64, 4, 2, 8, 3>, 8, StageGeom<64, 4, 2>::WARP_BYTES);
-        else if (is(stage_env, "256x2x1")) launch_stage(k_pass1_stage<256, 2, 1, 4, 3>, 4, StageGeom<256, 2, 1>::WARP_BYTES);
-        else if (is(stage_env, "256x4x1")) launch_stage(k_pass1_stage<256, 4, 1, 2, 3>, 2, StageGeom<256, 4, 1>::WARP_BYTES);
-        else if (is(ring_env, "128x2")) launch_ring(k_pass1_ring<128, 2>, 128 * (128 * 2 + 16));
-        else if (is(ring_env, "128x4")) launch_ring(k_pass1_ring<128, 4>, 128 * (128 * 4 + 16));
-        else if (is(ring_env, "256x2")) launch_ring(k_pass1_ring<256, 2>, 128 * (256 * 2 + 16));
-        else if (getenv("IPCFP_PASS1_W16") && atoi(getenv("IPCFP_PASS1_W16")) == 6) k_pass1_w16_occ6<<<div_up(N, 128), 128, 0, st>>>(p1);
-        else if (getenv("IPCFP_PASS1_W16")) k_pass1_w16<<<div_up(N, 128), 128, 0, st>>>(p1);
-        else if (!minb_env) launch_stage(k_pass1_stage<128, 4, 1, 4, 3>, 4, StageGeom<128, 4, 1>::WARP_BYTES);
-        else if (minb >= 10) k_pass1_occ10<<<div_up(N, 128), 128, 0, st>>>(p1);
-        else if (minb >= 8) k_pass1_occ8<<<div_up(N, 128), 128, 0, st>>>(p1);
-        else k_pass1<<<div_up(N, 128), 128, 0, st>>>(p1);
-        IPCFP_LAUNCH_CHECK();
+        // 4 warps per CTA, 3 CTAs per SM; every lane has a ring of 4 chunks of 128 bytes, one chunk filled per pass (pass1_stage.cuh)
+        const int smem = 4 * StageGeom<128, 4, 1>::WARP_BYTES;
+        IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        k_pass1_stage<128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
     }
     IPCFP_CUDA(cudaEventRecord(s->ev[3], st));
     AsyncBuf<uint32_t> match_rel(N + 32, st);

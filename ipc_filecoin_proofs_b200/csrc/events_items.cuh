@@ -46,16 +46,14 @@ __device__ __forceinline__ void emit_proof(const uint8_t* p, const EvLog& ev, ui
 }
 
 // Decodes the values of one events-AMT node. Returns false on a decode error (r.err set).
-template <int MODE, int WINMODE = 0>
+// PREFETCH: an L2 prefetch 2 lines ahead of the dependent walk before every event (off in the staged pass 1's arena fallback).
+template <int MODE, bool PREFETCH = true>
 __device__ __forceinline__ void node_events(Rd& r, const uint8_t* p, const AmtNodeHdr& h, uint32_t nv, uint64_t base, const Matcher& m,
-                                            WalkOut& wo, EmitCtx* ec, uint32_t tune = 0) {
+                                            WalkOut& wo, EmitCtx* ec) {
     for (uint32_t v = 0; v < nv && !r.err; v++) {
-        // rolling prefetch: 2 lines ahead of the dependent walk; IPCFP_PASS1_TUNE: bits 4..7 = other distance in lines, bit 1 = off
-        const uint32_t ahead = (tune >> 4) & 15u ? 128u * ((tune >> 4) & 15u) : 256u;
-        if (!(tune & 2) && r.pos + ahead < r.n) prefetch_l2(r.p + r.pos + ahead);
-        if ((tune & 1) && r.pos + 128 < r.n) prefetch_l1(r.p + r.pos + 128);  // experiment: next line into L1
+        if (PREFETCH && r.pos + 256 < r.n) prefetch_l2(r.p + r.pos + 256);
         EvLog ev;
-        decode_stamped_event<WINMODE>(r, ev);
+        decode_stamped_event(r, ev);
         if (r.err) break;
         if (event_matches(p, ev, m)) {
             wo.any = true;
@@ -124,7 +122,6 @@ struct Pass1Args {
     uint32_t* nbytes;              // [i - lo] topics+data bytes of those events
     unsigned long long* err;
     unsigned long long* stats;     // [0] nodes scanned, [1] bytes scanned
-    uint32_t tune;                 // experiment bits (env IPCFP_PASS1_TUNE), 0 = default
 };
 
 // ------------------------------------------------------------------------------------------ receipts AMT

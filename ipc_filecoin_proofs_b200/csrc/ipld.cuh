@@ -219,11 +219,10 @@ __device__ __forceinline__ uint32_t win_byte(uint64_t w0, uint64_t w1, uint32_t 
     return (uint32_t)(w >> (8 * (k & 7))) & 0xffu;
 }
 // window source over global memory (the block arena)
-template <int WINMODE = 0> struct GlobalWinT {   // WINMODE 1: two 16-byte loads per window instead of three 8-byte loads
+struct GlobalWin {
     const uint8_t* p;
-    __device__ __forceinline__ void load(uint32_t pos, uint64_t& w0, uint64_t& w1) { if (WINMODE) win_load16(p + pos, w0, w1); else win_load(p + pos, w0, w1); }
+    __device__ __forceinline__ void load(uint32_t pos, uint64_t& w0, uint64_t& w1) { win_load(p + pos, w0, w1); }
 };
-typedef GlobalWinT<0> GlobalWin;
 template <class Win>
 __device__ __forceinline__ uint32_t fast_stamped_event_t(Win& win, uint32_t pos, uint32_t n, EvLog& ev) {
     if (n - pos < 3) return FAST_FAIL;
@@ -310,9 +309,8 @@ __device__ __forceinline__ uint32_t fast_stamped_event_t(Win& win, uint32_t pos,
     ev_finish(a, ev);
     return cur;
 }
-template <int WINMODE = 0>
 __device__ __forceinline__ uint32_t fast_stamped_event(const uint8_t* p, uint32_t pos, uint32_t n, EvLog& ev) {
-    GlobalWinT<WINMODE> g{p};
+    GlobalWin g{p};
     return fast_stamped_event_t(g, pos, n, ev);
 }
 // One StampedEvent at r.pos: fast path first, exact generic decoder on any deviation. The slow path
@@ -326,10 +324,9 @@ static __device__ __noinline__ uint32_t slow_stamped_event(const uint8_t* p, uin
     *err = r2.err;
     return r2.pos;
 }
-template <int WINMODE = 0>
 __device__ __forceinline__ void decode_stamped_event(Rd& r, EvLog& ev) {
     if (r.err) { ev.some = 0; ev.ntopics = 0; ev.emitter = 0; return; }
-    uint32_t np = fast_stamped_event<WINMODE>(r.p, r.pos, r.n, ev);
+    uint32_t np = fast_stamped_event(r.p, r.pos, r.n, ev);
     if (np == FAST_FAIL) {
         EvLog e2;
         uint32_t err = 0;

@@ -1,9 +1,9 @@
 // pass1_stage.cuh — pass 1 (find_matching_events pass 1, reference events/generator.rs:206-239) with the node bytes STAGED
 // THROUGH SHARED MEMORY by warp-cooperative, coalesced 16-byte copies.
 //
-// Why (DESIGN.md §4): the thread-per-node kernel reads each lane's node straight from the arena, so every 8-byte window load of a
-// warp touches 32 different 128-byte lines = 32 L1 wavefronts; with ≈ 80 such loads per node the L1 wavefront queue, not HBM, can
-// be what the kernel runs at.
+// Why (DESIGN.md §4): a kernel whose lanes read their nodes straight from the arena makes every 8-byte window load of a warp touch
+// 32 different 128-byte lines = 32 L1 wavefronts; with ≈ 80 such loads per node the L1 wavefront queue, not HBM, can be what the
+// kernel runs at.
 //
 // Here a warp owns 32 receipts (lane = receipt, as before: DAG-CBOR is sequential, one lane parses one node) but the BYTES travel
 // differently: every lane has a ring of NSLOT chunks of CH bytes in shared memory; a fill pass moves, for every node of the warp,
@@ -13,8 +13,8 @@
 // Chunks are CH-aligned in the ARENA (not in the block), so the 16-byte alignment cp.async needs holds for blocks at any offset.
 //
 // Only the canonical-shape fast path reads the ring. Anything else — an event the fast path declines, an event larger than the
-// ring can show at once, a node with links (taller AMT), any decode problem — goes through the same strict arena decoders as
-// k_pass1, so results are identical by construction; tests/host_fuzz/emu_stage.cu runs this very code on the CPU (with the
+// ring can show at once, a node with links (taller AMT), any decode problem — goes through the strict arena decoders of
+// events_items.cuh, so results are identical by construction; tests/host_fuzz/emu_stage.cu runs this very code on the CPU (with the
 // asynchronous copies modelled adversarially) against the arena path.
 #pragma once
 #include "events_items.cuh"
@@ -62,28 +62,6 @@ template <class GEO> struct StageWin {
         w0 = (uint64_t)__funnelshift_r(c0, c1, s) | ((uint64_t)__funnelshift_r(c1, c2, s) << 32);
         w1 = (uint64_t)__funnelshift_r(c2, c3, s) | ((uint64_t)__funnelshift_r(c3, c4, s) << 32);
     }
-    // the same without the residency test (the caller has checked that pos + 24 bytes have landed)
-    __device__ __forceinline__ void load_resident(uint32_t pos, uint64_t& w0, uint64_t& w1) const {
-        const uint32_t a = skew + pos, a0 = a & ~7u;
-        const uint32_t s = (a & 7) * 8;
-        const uint2 x0 = lds(a0), x1 = lds(a0 + 8), x2 = lds(a0 + 16);
-        const bool up = (s & 32) != 0;
-        const uint32_t c0 = up ? x0.y : x0.x, c1 = up ? x1.x : x0.y, c2 = up ? x1.y : x1.x, c3 = up ? x2.x : x1.y, c4 = up ? x2.y : x2.x;
-        w0 = (uint64_t)__funnelshift_r(c0, c1, s) | ((uint64_t)__funnelshift_r(c1, c2, s) << 32);
-        w1 = (uint64_t)__funnelshift_r(c2, c3, s) | ((uint64_t)__funnelshift_r(c3, c4, s) << 32);
-    }
-    // 32 resident bytes at node offset pos == w[0..3]? The first 8 bytes decide almost every time.
-    __device__ __forceinline__ bool eq32_resident(uint32_t pos, const uint64_t w[4]) const {
-        const uint32_t a = skew + pos, a0 = a & ~7u, s = (a & 7) * 8;
-        const uint2 x0 = lds(a0), x1 = lds(a0 + 8);
-        const uint64_t q0 = (uint64_t)x0.x | ((uint64_t)x0.y << 32), q1 = (uint64_t)x1.x | ((uint64_t)x1.y << 32);
-        if (((q0 >> s) | ((q1 << 1) << (63 - s))) != w[0]) return false;
-        uint64_t a_, b_;
-        load_resident(pos + 8, a_, b_);
-        if (a_ != w[1] || b_ != w[2]) return false;
-        load_resident(pos + 16, a_, b_);
-        return b_ == w[3];
-    }
     // 32 bytes at node offset pos == w[0..3]? (pos + 32 must be resident: checked by the caller)
     __device__ __forceinline__ bool eq32(uint32_t pos, const uint64_t w[4]) {
         uint64_t a, b;
@@ -93,128 +71,6 @@ template <class GEO> struct StageWin {
         return a == w[2] && b == w[3];
     }
 };
-
-// ---- lean event decode for pass 1 ------------------------------------------------------------------------------------------
-// Pass 1 only needs, per event: does it decode, does it match, and (for the proofs pass 2 will emit) how many topic / data bytes a
-// match carries. fast_stamped_event_t + ev_finish + event_matches keep every offset of every key for the emitter of pass 2; this
-// variant keeps bit masks and lengths only, compares t1 / t2 (or the head of `topics`) with the filter while the entry is in the
-// window, and never looks at the node again — ≈ 3× fewer instructions per event. Same acceptance as fast_stamped_event_t (the entry
-// shapes are decoded by the very same expressions), same meaning as ev_finish + event_matches; whatever it declines (LEAN_FAIL) goes
-// to the strict arena decoder; LEAN_SHORT = a byte it needs has not landed in the ring yet (res_end = node offset up to which
-// bytes are resident).
-#define LEAN_FAIL 0xffffffffu
-#define LEAN_SHORT 0xfffffffeu
-struct LeanOut { bool hit; uint32_t nbytes; };
-template <class Win>
-__device__ __forceinline__ uint32_t lean_stamped_event(Win& win, uint32_t pos, uint32_t n, uint32_t res_end, const Matcher& m, LeanOut& out) {
-    out.hit = false; out.nbytes = 0;
-    if (n - pos < 3) return LEAN_FAIL;
-    if (pos + 24 > res_end) return LEAN_SHORT;
-    uint64_t w0, w1;
-    win.load_resident(pos, w0, w1);
-    if ((w0 & 0xff) != 0x82) return LEAN_FAIL;
-    const uint32_t eb = (uint32_t)(w0 >> 8) & 0xff;
-    if (eb >= 0x1b) return LEAN_FAIL;
-    const uint32_t enb = eb < 24 ? 0 : (1u << (eb - 24));
-    const uint32_t be = __byte_perm((uint32_t)(w0 >> 16), 0, 0x0123);
-    const uint32_t earg = enb ? (be >> (32 - 8 * enb)) : eb;
-    const uint32_t emin = eb == 24 ? 24u : (eb == 25 ? 0x100u : (eb == 26 ? 0x10000u : 0u));
-    if (earg < emin) return LEAN_FAIL;
-    const uint32_t hb = (uint32_t)(w0 >> (16 + 8 * enb)) & 0xffu;
-    if ((hb & 0xe0) != 0x80 || (hb & 31) >= 24) return LEAN_FAIL;
-    const uint32_t ne = hb & 31;
-    uint32_t cur = pos + 3 + enb;
-    if (cur > n) return LEAN_FAIL;
-    const bool actor_ok = !m.has_actor || earg == m.actor;
-    uint32_t have = 0, lenok = 0, d_len = 0, tp_len = 0, da_len = 0;
-    bool m0 = false, m1 = false, mA = false;
-    for (uint32_t e = 0; e < ne; e++) {
-        if (n - cur < 5) return LEAN_FAIL;
-        if (cur + 24 > res_end) return LEAN_SHORT;
-        win.load_resident(cur, w0, w1);
-        const uint32_t lo = (uint32_t)w0, hi = (uint32_t)(w0 >> 32), ll = (uint32_t)w1 & 0xffu;
-        const uint32_t tidx = (hi & 0xffu) - (uint32_t)'1';
-        const uint32_t fl8 = (lo >> 8) & 0xffu;
-        bool canon = (lo & 0xffff00ffu) == 0x74620084u && fl8 < 24u && (hi & 0xff00ff00u) == 0x58001800u && tidx < 4u && ((hi >> 16) & 0xffu) >= 24u && ll >= 24u;
-        uint32_t kind = tidx, vlen = ll, voff = cur + 9;
-        if ((lo & 0xffff00ffu) == 0x64610084u && fl8 < 24u && (hi & 0xffu) == 0x18u && ((hi >> 8) & 0xffu) >= 24u) {
-            const uint32_t vb = (hi >> 16) & 0xffu, b7 = hi >> 24, l16 = (b7 << 8) | ll;
-            kind = 4;
-            if (vb - 0x40u < 0x18u) { vlen = vb - 0x40u; voff = cur + 7; canon = true; }
-            else if (vb == 0x58u && b7 >= 24u) { vlen = b7; voff = cur + 8; canon = true; }
-            else if (vb == 0x59u && l16 >= 256u) { vlen = l16; voff = cur + 9; canon = true; }
-        }
-        if (!canon) {
-            uint32_t b0 = (uint32_t)w0 & 0xff, fl = (uint32_t)(w0 >> 8) & 0xff, th = (uint32_t)(w0 >> 16) & 0xff;
-            if (b0 != 0x84 || fl >= 24) return LEAN_FAIL;
-            uint32_t klen = th - 0x60;
-            uint32_t k4 = (uint32_t)(w0 >> 24);
-            if (klen == 2) {
-                uint32_t idx = ((k4 >> 8) & 0xff) - (uint32_t)'1';
-                if ((k4 & 0xff) != 't' || idx >= 4) return LEAN_FAIL;
-                kind = idx;
-            } else if (klen == 1) {
-                if ((k4 & 0xff) != 'd') return LEAN_FAIL;
-                kind = 4;
-            } else if (klen == 6) {
-                uint64_t key = (w0 >> 24) | (w1 << 40);
-                if ((key & 0xffffffffffffull) != 0x736369706f74ull) return LEAN_FAIL;  // "topics"
-                kind = 5;
-            } else if (klen == 4) {
-                if (k4 != 0x61746164u) return LEAN_FAIL;          // "data"
-                kind = 6;
-            } else return LEAN_FAIL;
-            uint32_t k = 3 + klen;
-            uint32_t cb = win_byte(w0, w1, k);
-            uint32_t clen;
-            if (cb < 24) clen = 1;
-            else if (cb == 24 && win_byte(w0, w1, k + 1) >= 24) clen = 2;
-            else return LEAN_FAIL;
-            k += clen;
-            uint32_t vb = win_byte(w0, w1, k);
-            uint32_t vh;
-            if (vb >= 0x40 && vb < 0x58) { vlen = vb - 0x40; vh = 1; }
-            else if (vb == 0x58) { vlen = win_byte(w0, w1, k + 1); vh = 2; if (vlen < 24) return LEAN_FAIL; }
-            else if (vb == 0x59) { vlen = (win_byte(w0, w1, k + 1) << 8) | win_byte(w0, w1, k + 2); vh = 3; if (vlen < 256) return LEAN_FAIL; }
-            else return LEAN_FAIL;
-            voff = cur + k + vh;
-        }
-        if (voff > n || vlen > n - voff) return LEAN_FAIL;
-        // what extract_evm_log (common/evm.rs:13-59) will look at — last duplicate of a key wins (:14-17)
-        if (kind < 4) {
-            const uint32_t bit = 1u << kind;
-            have |= bit;
-            lenok = vlen == 32 ? (lenok | bit) : (lenok & ~bit);
-            if (kind < 2 && actor_ok) {                      // topic 0 / topic 1 against the filter, while the value is at hand
-                bool eq = false;
-                if (vlen == 32) {
-                    if (voff + 40 > res_end) return LEAN_SHORT;
-                    eq = win.eq32_resident(voff, kind == 0 ? m.t0 : m.t1);
-                }
-                if (kind == 0) m0 = eq; else m1 = eq;
-            }
-        } else if (kind == 4) { have |= 16; d_len = vlen; }
-        else if (kind == 5) {
-            have |= 32; tp_len = vlen;
-            mA = false;
-            if (actor_ok && vlen >= 64 && vlen % 32 == 0) {
-                if (voff + 72 > res_end) return LEAN_SHORT;
-                mA = win.eq32_resident(voff, m.t0) && win.eq32_resident(voff + 32, m.t1);
-            }
-        } else { have |= 64; da_len = vlen; }
-        cur = voff + vlen;
-    }
-    // ev_finish + event_matches: `topics` selects Case A (:20-30); Case B = leading t1.. run, every one of them 32 bytes (:45-56)
-    if (have & 32) {
-        if (tp_len % 32 == 0 && tp_len >= 64 && mA) { out.hit = true; out.nbytes = tp_len + ((have & 64) ? da_len : 0); }
-    } else {
-        const uint32_t present = have & 15;
-        const uint32_t lead = present == 15 ? 4 : (uint32_t)(__ffs((int)(~present & 15)) - 1);
-        const uint32_t lead_mask = (1u << lead) - 1;
-        if (lead >= 2 && (lenok & lead_mask) == lead_mask && m0 && m1) { out.hit = true; out.nbytes = 32 * lead + ((have & 16) ? d_len : 0); }
-    }
-    return cur;
-}
 
 // per-lane state of the staged scan (registers on the device)
 template <class GEO> struct StageLane {
@@ -272,40 +128,6 @@ template <class GEO> struct StageLane {
         // amt_node_finish for a node without links: values only at height 0, popcount == number of values, no trailing bytes
         state = 0;
         taken = !((nv && height != 0) || pc != nv || cur != len);
-    }
-    // one parse step with the lean decoder (pass 1's count mode): at most one event
-    __device__ __forceinline__ void step_lean(const Matcher& m) {
-        if (state == 1) {
-            const uint32_t need = skew + (len < 64 ? len : 64);
-            if (landed * GEO::CH < need && landed < nchunks) return;
-            begin();
-            if (state == 0) return;
-        }
-        if (state != 2) return;
-        if (vi >= nv) { finish(); return; }
-        StageWin<GEO> win{ring, skew, landed * GEO::CH, false};
-        const uint32_t res_end = landed * GEO::CH - skew;    // node offset up to which bytes have landed (landed ≥ 1 here: the header was read)
-        LeanOut lo;
-        uint32_t nx = lean_stamped_event(win, cur, len, res_end, m, lo);
-        if (nx == LEAN_SHORT && landed != front) return;      // the pass in flight brings more
-        if (nx >= LEAN_SHORT) {                               // declined, or larger than the ring can show: the exact decoder, from the arena
-            EvLog e2;
-            uint32_t err = 0;
-#if defined(IPCFP_STAGE_HOST_STATS) && !defined(__CUDA_ARCH__)
-            g_stage_slow_events++;
-#endif
-            nx = slow_stamped_event(p, cur, len, &e2, &err);
-            if (err) { state = 0; taken = false; return; }
-            lo.hit = event_matches(p, e2, m);
-            lo.nbytes = 32 * e2.ntopics + e2.data_len;
-        }
-#if defined(IPCFP_STAGE_HOST_STATS) && !defined(__CUDA_ARCH__)
-        g_stage_events++;
-#endif
-        if (lo.hit) { wo.any = true; wo.nproofs++; wo.nbytes += lo.nbytes; }
-        cur = nx;
-        vi++;
-        if (vi >= nv) finish();
     }
     // one parse step: at most one event
     __device__ __forceinline__ void step(const Matcher& m) {
@@ -379,7 +201,7 @@ __device__ __forceinline__ void cp_async16(uint8_t* dst_smem, const uint8_t* src
 #endif
 
 // W warps per CTA, each with its own rings; no CTA-wide synchronisation anywhere.
-template <int CH, int NSLOT, int CPP, int W, int MINB, int LEAN = 0>
+template <int CH, int NSLOT, int CPP, int W, int MINB>
 __global__ void __launch_bounds__(32 * W, MINB) k_pass1_stage(Pass1Args a) {
 #ifdef __CUDA_ARCH__
     using GEO = StageGeom<CH, NSLOT, CPP>;
@@ -417,9 +239,9 @@ __global__ void __launch_bounds__(32 * W, MINB) k_pass1_stage(Pass1Args a) {
         L.landed = L.front;
         if (!__any_sync(0xffffffffu, L.state != 0)) break;
         fill();
-        if (LEAN) L.step_lean(a.m); else L.step(a.m);
+        L.step(a.m);
     }
-    // phase 3: results; nodes the staged path did not take are decoded from the arena exactly as k_pass1 does
+    // phase 3: results; nodes the staged path did not take are decoded from the arena (node_events, walk_events)
     bool matched = false;
     uint32_t bytes = 0, nodes = 0, np_ = 0, nb_ = 0;
     if (blk >= 0) {
@@ -434,7 +256,7 @@ __global__ void __launch_bounds__(32 * W, MINB) k_pass1_stage(Pass1Args a) {
             AmtNodeHdr h;
             amt_node_begin(r, bw, h);
             uint32_t nv = rd_array(r);
-            node_events<WALK_COUNT>(r, p, h, nv, 0, a.m, wo, nullptr, 2u);
+            node_events<WALK_COUNT, false>(r, p, h, nv, 0, a.m, wo, nullptr);
             amt_node_finish(r, h, nv, height);
             if (r.err) { report_error(a.err, ST_PASS1, i, DC_DECODE, r.err); wo = WalkOut{0, 0, false}; }
             else if (h.nl) {

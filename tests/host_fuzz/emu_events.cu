@@ -4,7 +4,7 @@
 //   k_setup's sequence (TxMeta → AMT roots, receipts root validation, base witness)        mirrored here from header functions
 //   dense message-AMT walk                                                                 amt_item_dense + make_dense_plan (csrc/walk.cuh)
 //   first-seen dedup of the raw list                                                       restated here (a hash set)
-//   pass 1 per receipt                                                                     pass1_body's sequence, from node_events / walk_events
+//   pass 1 per receipt                                                                     k_pass1_stage's arena decode, from node_events / walk_events
 //   pass 2 per matching receipt                                                            pass2_item, receipts_get, walk_events<EMIT> (csrc/events_items.cuh)
 // against `oracle_generate_event_proof`: matching receipts, every EventProof field, the witness CID set, n_exec — and, with one
 // events / receipts block replaced by a mutated copy under the same CID (or removed), the same status at the same index.
@@ -26,7 +26,6 @@
 #include "../../ipc_filecoin_proofs_b200/csrc/walk.cuh"
 #ifndef __CUDA_ARCH__
 #define prefetch_l2(p) ((void)0)   // inline PTX: nothing to do on the host
-#define prefetch_l1(p) ((void)0)
 #endif
 #include "../../ipc_filecoin_proofs_b200/csrc/events_items.cuh"
 #include "../../oracle/oracle.h"
@@ -202,7 +201,7 @@ static bool engine(const Blocks& B, const ipcfp_tipset_desc& td, const char* sig
     }
     { uint8_t t1[32]; memset(t1, 0, 32); size_t n1 = strlen(topic1); memcpy(t1, topic1, n1 < 32 ? n1 : 32); memcpy(m.t1, t1, 32); }
     m.actor = actor; m.has_actor = has_actor ? 1 : 0;
-    // ---- pass 1 (pass1_body's per-receipt sequence)
+    // ---- pass 1 (the per-receipt arena decode of k_pass1_stage)
     const uint64_t N = td.n_receipts;
     std::vector<uint32_t> cnt(N + 1, 0), nby(N + 1, 0), match_rel;
     for (uint64_t i = lo; i < hi; i++) {
@@ -220,7 +219,7 @@ static bool engine(const Blocks& B, const ipcfp_tipset_desc& td, const char* sig
         amt_node_begin(r, bw, h);
         uint32_t nv = rd_array(r);
         WalkOut wo{0, 0, false};
-        node_events<WALK_COUNT>(r, p, h, nv, 0, m, wo, nullptr, 0);
+        node_events<WALK_COUNT>(r, p, h, nv, 0, m, wo, nullptr);
         amt_node_finish(r, h, nv, height);
         if (r.err) { report_error(&err, ST_PASS1, i, DC_DECODE, r.err); continue; }
         if (h.nl) {

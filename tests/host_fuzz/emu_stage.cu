@@ -4,7 +4,7 @@
 // host and driven exactly as the kernel drives it — prologue fills, then { wait, landed = front, any lane alive?, fill, step } —
 // for whole warps of 32 generated / mutated events-AMT root blocks laid out at random offsets of one arena, with the asynchronous
 // copies modelled ADVERSARIALLY (a copy poisons its 16 destination bytes at once and delivers only at the next wait), against the
-// arena decode sequence of pass1_body. Properties: a node the staged path takes is accepted by the arena path with the same
+// arena decode sequence the kernel falls back to. Properties: a node the staged path takes is accepted by the arena path with the same
 // (any, #proofs, #bytes); every well-formed single-node block IS taken; nothing is read outside [arena base, arena end + 512).
 //
 //   nvcc -std=c++17 -O2 -o emu_stage tests/host_fuzz/emu_stage.cu && ./emu_stage [warps] [seed]
@@ -19,7 +19,6 @@
 #include "../../ipc_filecoin_proofs_b200/csrc/ipld.cuh"
 #ifndef __CUDA_ARCH__
 #define prefetch_l2(p) ((void)0)
-#define prefetch_l1(p) ((void)0)
 #endif
 #define IPCFP_STAGE_HOST_STATS 1
 static unsigned long long g_stage_events = 0, g_stage_slow_events = 0, g_stage_iters = 0;
@@ -101,7 +100,7 @@ static std::vector<uint8_t> make_root(bool& wellformed_single) {
 }
 
 
-template <int CH, int NSLOT, int CPP, int LEAN = 0>
+template <int CH, int NSLOT, int CPP>
 static int run(uint64_t warps, uint64_t* taken_out, uint64_t* wf_out, uint64_t* slow_out) {
     using GEO = StageGeom<CH, NSLOT, CPP>;
     uint64_t taken_n = 0, wf = 0;
@@ -168,12 +167,12 @@ static int run(uint64_t warps, uint64_t* taken_out, uint64_t* wf_out, uint64_t* 
             for (uint32_t l = 0; l < 32; l++) { L[l].landed = L[l].front; alive |= L[l].state != 0; }
             if (!alive) break;
             fill();
-            for (uint32_t l = 0; l < 32; l++) { if (LEAN) L[l].step_lean(m); else L[l].step(m); }
+            for (uint32_t l = 0; l < 32; l++) L[l].step(m);
             g_stage_iters++;
             if (++guard > 100000) { fprintf(stderr, "STAGE <%d,%d,%d>: no progress (warp %llu)\n", CH, NSLOT, CPP, (unsigned long long)w); return 1; }
         }
         if (oob) { fprintf(stderr, "STAGE <%d,%d,%d>: a copy left the arena / the rings (warp %llu)\n", CH, NSLOT, CPP, (unsigned long long)w); return 1; }
-        // ---- every lane against the arena path (pass1_body's sequence)
+        // ---- every lane against the arena path (the kernel's fallback sequence)
         for (uint32_t l = 0; l < 32; l++) {
             if (!have[l]) { if (L[l].taken) { fprintf(stderr, "STAGE: a lane without a node reports a result\n"); return 1; } continue; }
             const uint8_t* p = base + 16 + off[l];
@@ -186,7 +185,7 @@ static int run(uint64_t warps, uint64_t* taken_out, uint64_t* wf_out, uint64_t* 
             amt_node_begin(r, bw, h);
             uint32_t nv = rd_array(r);
             WalkOut wa{0, 0, false};
-            node_events<WALK_COUNT>(r, p, h, nv, 0, m, wa, nullptr, 0);
+            node_events<WALK_COUNT>(r, p, h, nv, 0, m, wa, nullptr);
             amt_node_finish(r, h, nv, height);
             if (L[l].taken) {
                 taken_n++;
@@ -216,7 +215,7 @@ int main(int argc, char** argv) {
     if (argc > 3) {   // canonical-shape statistics per geometry: iterations per warp and events that left the fast path
         g_canonical = true;
         auto one = [&](const char* name, int rc) { printf("  %s: %llu warp iterations, %llu events, %llu through the arena decoder\n", name, g_stage_iters, g_stage_events, g_stage_slow_events); g_stage_iters = g_stage_events = g_stage_slow_events = 0; return rc; };
-        if (one("lean128x4x1", run<128, 4, 1, 1>(warps, &taken, &wf, &slow)) || one("lean64x8x2", run<64, 8, 2, 1>(warps, &taken, &wf, &slow)) || one("128x4x1", run<128, 4, 1>(warps, &taken, &wf, &slow)) || one("64x4x2", run<64, 4, 2>(warps, &taken, &wf, &slow)) || one("64x8x2", run<64, 8, 2>(warps, &taken, &wf, &slow)) ||
+        if (one("128x4x1", run<128, 4, 1>(warps, &taken, &wf, &slow)) || one("64x4x2", run<64, 4, 2>(warps, &taken, &wf, &slow)) || one("64x8x2", run<64, 8, 2>(warps, &taken, &wf, &slow)) ||
             one("128x4x2", run<128, 4, 2>(warps, &taken, &wf, &slow)) || one("256x2x1", run<256, 2, 1>(warps, &taken, &wf, &slow)))
             return 1;
         g_canonical = false;
@@ -224,11 +223,6 @@ int main(int argc, char** argv) {
     if (run<128, 4, 1>(warps, &taken, &wf, &slow) || run<64, 4, 2>(warps, &taken, &wf, &slow) || run<64, 8, 2>(warps, &taken, &wf, &slow) || run<128, 4, 2>(warps, &taken, &wf, &slow) ||
         run<256, 2, 1>(warps, &taken, &wf, &slow))
         return 1;
-    {   // the lean decoder of pass 1's count mode
-        const unsigned long long e0 = g_stage_events, s0 = g_stage_slow_events;
-        if (run<128, 4, 1, 1>(warps, &taken, &wf, &slow) || run<64, 8, 2, 1>(warps, &taken, &wf, &slow) || run<128, 4, 2, 1>(warps, &taken, &wf, &slow) || run<64, 4, 2, 1>(warps, &taken, &wf, &slow)) return 1;
-        printf("ok: lean decoder: %llu events, %llu of them through the arena decoder\n", g_stage_events - e0, g_stage_slow_events - s0);
-    }
     printf("ok: staged pass 1 == arena pass 1 for 5 geometries x %llu warps: %llu nodes taken by the staged path, %llu well-formed single-node blocks (all taken); %llu events, %llu of them through the arena decoder; %llu warp iterations\n",
            (unsigned long long)warps, (unsigned long long)taken, (unsigned long long)wf, g_stage_events, g_stage_slow_events, g_stage_iters);
     return 0;

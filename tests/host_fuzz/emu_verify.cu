@@ -28,7 +28,6 @@
 #include "../../ipc_filecoin_proofs_b200/csrc/walk.cuh"
 #ifndef __CUDA_ARCH__
 #define prefetch_l2(p) ((void)0)   // inline PTX: nothing to do on the host
-#define prefetch_l1(p) ((void)0)
 #endif
 #include "../../ipc_filecoin_proofs_b200/csrc/verify_items.cuh"
 #include "../../oracle/oracle.h"

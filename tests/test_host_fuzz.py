@@ -101,8 +101,8 @@ def test_event_path_emulated_on_cpu_matches_oracle():
 
 
 def test_staged_pass1_lane_logic_emulated_on_cpu():
-    """tests/host_fuzz/emu_stage.cu: the per-lane logic of the (default; IPCFP_PASS1_STAGE picks another geometry) shared-memory-staged pass-1 kernel —
-    `StageLane` / `StageWin` / `lean_stamped_event` of csrc/pass1_stage.cuh — under an adversarial model of the asynchronous fills:
+    """tests/host_fuzz/emu_stage.cu: the per-lane logic of the shared-memory-staged pass-1 kernel —
+    `StageLane` / `StageWin` / `stage_fill_lane` of csrc/pass1_stage.cuh — under an adversarial model of the asynchronous fills:
     staged decode == arena decode for every node, five ring geometries."""
     exe, env = _harness("emu_stage", with_synth=False)
     out = subprocess.run([exe, "300", "12"], capture_output=True, text=True, env=env)

@@ -28,8 +28,6 @@ def main():
     ap.add_argument("--verify", action="store_true")
     ap.add_argument("--timeline", action="store_true", help="per-step kernel / copy timeline under torch.profiler (see above)")
     ap.add_argument("--storage", type=int, default=0, help="also run N storage-slot lookups on a 1M-entry HAMT")
-    ap.add_argument("--sweep", default="", help="comma-separated pass-1 variants, e.g. MINB=8,STAGE=128x4x1,RING=128x4: every variant runs "
-                                                 "warmup+steps resident steps in THIS process; prints the median device ms of pass 1")
     args = ap.parse_args()
     import synth
     from ipc_filecoin_proofs_b200 import _abi as A
@@ -49,34 +47,6 @@ def main():
     tip = C.c_void_p()
     assert L.ipcfp_tipset_upload(st._h, C.byref(d), C.byref(tip)) == 0
     log("tipset uploaded")
-    if args.sweep:
-        import numpy as np
-        ref = None
-        for var in args.sweep.split(","):
-            for k in ("IPCFP_PASS1_STAGE", "IPCFP_PASS1_RING", "IPCFP_PASS1_MINB", "IPCFP_PASS1_TUNE", "IPCFP_PASS1_W16"):
-                os.environ.pop(k, None)
-            for kv in var.split("+"):
-                name, val = kv.split("=")
-                os.environ["IPCFP_PASS1_" + name] = val
-            p1, tot = [], []
-            sig = None
-            for k in range(args.warmup + args.steps):
-                out = C.POINTER(A.EventResultC)()
-                rc = L.ipcfp_generate_event_proof_resident(st._h, tip, C.byref(spec), 0, C.byref(out))
-                if rc != 0:
-                    log(f"variant {var}: FAILED {rc} {L.ipcfp_last_error()}")
-                    break
-                r = out.contents
-                if k >= args.warmup:
-                    p1.append(r.ms_pass1); tot.append(r.ms_total)
-                sig = (int(r.n_matching), int(r.n_proofs), int(r.witness.n_blocks), int(r.pass1_bytes))
-                L.ipcfp_event_result_free(out)
-            if ref is None:
-                ref = sig
-            print(f"SWEEP {var:24s} pass1 median {np.median(p1):.4f} ms min {np.min(p1):.4f} | step median {np.median(tot):.3f} ms | "
-                  f"result {sig} {'same' if sig == ref else 'DIFFERENT from the first variant'}", flush=True)
-        log("sweep done")
-        return
     if args.timeline:
         timeline(L, A, st, tip, spec, args.warmup, args.steps)
         return
