@@ -34,6 +34,7 @@ class SynthParams(C.Structure):
         ("shard_hi", C.c_uint64),
         ("threads", C.c_uint32),
         ("same_topic1", C.c_uint32),
+        ("event_shapes", C.c_uint32),
     ]
 
 

@@ -13,6 +13,7 @@
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <functional>
 #include <string>
 #include <thread>
@@ -266,8 +267,158 @@ static void gen_event(const Gen& g, Rng& r, uint64_t i, uint32_t j, bool forced,
     }
 }
 
+// ------------------------------------------------------------------ varied event shapes (event_shapes = 1)
+// One [flags, key, codec, value] entry of a StampedEvent.
+struct Entry { uint64_t flags; const char* key; uint64_t codec; Bytes val; };
+
+static Bytes rand_bytes(Rng& r, size_t n) {
+    Bytes b(n);
+    for (size_t k = 0; k < n; k++) b[k] = (uint8_t)r.next();
+    return b;
+}
+static Bytes bytes_of(const uint8_t* p, size_t n) { return Bytes(p, p + n); }
+
+// The spec's predicate on one event, restated from the reference: the emitter filter, then extract_evm_log (the last of duplicate
+// keys wins; `topics` selects Case A and must be a multiple of 32 bytes; Case B takes t1, t2, ... while present, each exactly
+// 32 bytes), then topic 0 == the signature hash and topic 1 == the padded topic1.
+static bool shaped_event_matches(const Gen& g, uint64_t em, const std::vector<Entry>& es) {
+    if (g.p.has_actor_filter && em != g.target_actor) return false;
+    const uint8_t* T0 = g.tp.t0[0];
+    const uint8_t* T1 = g.tp.t1[TARGET_TOPIC1_IDX];
+    static const char* tk[4] = {"t1", "t2", "t3", "t4"};
+    const Bytes* t[4] = {nullptr, nullptr, nullptr, nullptr};
+    const Bytes* topics = nullptr;
+    for (const Entry& e : es) {
+        if (!strcmp(e.key, "topics")) topics = &e.val;
+        for (int k = 0; k < 4; k++) if (!strcmp(e.key, tk[k])) t[k] = &e.val;
+    }
+    if (topics) return topics->size() % 32 == 0 && topics->size() >= 64 && !memcmp(topics->data(), T0, 32) && !memcmp(topics->data() + 32, T1, 32);
+    int lead = 0;
+    while (lead < 4 && t[lead]) {
+        if (t[lead]->size() != 32) return false;
+        lead++;
+    }
+    return lead >= 2 && !memcmp(t[0]->data(), T0, 32) && !memcmp(t[1]->data(), T1, 32);
+}
+
+// One event of the varied distribution. A forced event is an unambiguous match; every other event fails the spec, either as one
+// of the named near misses (wrong emitter under the filter, a 31-byte t2, swapped topics, the target topics only at t3/t4, Case A
+// with one topic) or as a random shape that is deflected (its effective topic 0 replaced) should it match by accident.
+static void gen_event_shaped(const Gen& g, Rng& r, bool forced, Bytes& o) {
+    const uint8_t* T0 = g.tp.t0[0];
+    const uint8_t* T1 = g.tp.t1[TARGET_TOPIC1_IDX];
+    const uint64_t ta = g.target_actor;
+    // immediate, 1-, 2-, 4- and 8-byte CBOR heads
+    const uint64_t emitters[8] = {5, 23, 24, 255, 1000 + r.next() % 16, 65536 + ta, (1ull << 40) + ta, ta};
+    uint64_t em = emitters[r.next() % 8];
+    auto topic = [&]() -> Bytes {   // a 32-byte topic from the pool the tipset's topics come from
+        uint64_t k = r.next() % 24;
+        return k < 8 ? bytes_of(g.tp.t0[k], 32) : bytes_of(g.tp.t1[k - 8], 32);
+    };
+    auto data_b = [&]() -> Bytes { return rand_bytes(r, r.next() % 3 == 0 ? 256 + r.next() % 700 : r.next() % 64); };
+    std::vector<Entry> es;
+    auto add = [&](const char* key, Bytes v) { es.push_back(Entry{3, key, 0x55, std::move(v)}); };
+    static const char* tk[4] = {"t1", "t2", "t3", "t4"};
+    if (forced) {
+        if (g.p.has_actor_filter) em = ta;
+        if (r.next() % 3 == 0) {
+            Bytes tp = bytes_of(T0, 32);
+            tp.insert(tp.end(), T1, T1 + 32);
+            for (uint64_t k = r.next() % 3; k > 0; k--) { Bytes x = topic(); tp.insert(tp.end(), x.begin(), x.end()); }
+            add("topics", tp);
+            add("data", rand_bytes(r, r.next() % 300));
+        } else {
+            add("t1", bytes_of(T0, 32));
+            add("t2", bytes_of(T1, 32));
+            for (uint64_t k = 2, nt = 2 + r.next() % 3; k < nt; k++) add(tk[k], topic());
+            if (r.next() % 4) add("d", data_b());
+        }
+    } else {
+        unsigned kind = (unsigned)(r.next() % 16);
+        if (kind == 8) {                                   // wrong emitter (a miss only under the filter; deflected otherwise)
+            if (g.p.has_actor_filter && em == ta) em = ta + 1;
+            add("t1", bytes_of(T0, 32)); add("t2", bytes_of(T1, 32)); add("d", data_b());
+        } else if (kind == 9) {                            // 31-byte t2
+            add("t1", bytes_of(T0, 32)); add("t2", bytes_of(T1, 31)); add("d", data_b());
+        } else if (kind == 10) {                           // swapped topics
+            add("t1", bytes_of(T1, 32)); add("t2", bytes_of(T0, 32)); add("d", data_b());
+        } else if (kind == 11) {                           // the target topics only at t3 / t4
+            add("t1", topic()); add("t2", topic()); add("t3", bytes_of(T0, 32)); add("t4", bytes_of(T1, 32));
+        } else if (kind == 12) {                           // Case A with one topic
+            add("topics", bytes_of(T0, 32)); add("data", rand_bytes(r, r.next() % 300));
+        } else if (kind < 4) {                             // Case A, 0..4 topics
+            Bytes tp;
+            for (uint64_t k = r.next() % 5; k > 0; k--) { Bytes x = topic(); tp.insert(tp.end(), x.begin(), x.end()); }
+            add("topics", tp);
+            add("data", rand_bytes(r, r.next() % 300));
+        } else {                                           // Case B, 1..4 topics (now and then of another length), optional d
+            for (uint64_t k = 0, nt = 1 + r.next() % 4; k < nt; k++) add(tk[k], r.next() % 16 == 0 ? rand_bytes(r, r.next() % 40) : topic());
+            if (r.next() % 4) add("d", data_b());
+        }
+    }
+    // odd flags and codecs (the reference reads neither)
+    static const uint64_t odd[8] = {0, 1, 7, 23, 24, 255, 300, 70000};
+    for (Entry& e : es) {
+        if (r.next() % 8 == 0) e.flags = odd[r.next() % 8];
+        if (r.next() % 8 == 0) e.codec = odd[r.next() % 8];
+    }
+    // an unknown key; a duplicate placed before the entry it repeats (the later one wins, so the event's meaning is kept)
+    static const char* unknown[6] = {"topic", "dat", "t5", "t0", "D", "tt1"};
+    if (r.next() % 8 == 0) {
+        size_t at = (size_t)(r.next() % (es.size() + 1));
+        es.insert(es.begin() + (long)at, Entry{3, unknown[r.next() % 6], 0x55, rand_bytes(r, r.next() % 40)});
+    }
+    if (!es.empty() && r.next() % 8 == 0) {
+        size_t at = (size_t)(r.next() % es.size());
+        Entry dup{es[at].flags, es[at].key, es[at].codec, rand_bytes(r, r.next() % 2 ? 32 : r.next() % 40)};
+        es.insert(es.begin() + (long)at, dup);
+    }
+    if (forced != shaped_event_matches(g, em, es)) {
+        if (forced) { fprintf(stderr, "synth: a forced event does not match\n"); abort(); }
+        // the effective topic 0 (of the last `topics`, else the last `t1`) becomes another signature
+        bool has_topics = false;
+        for (const Entry& e : es) has_topics |= !strcmp(e.key, "topics");
+        for (size_t k = es.size(); k-- > 0;)
+            if (!strcmp(es[k].key, has_topics ? "topics" : "t1")) { memcpy(es[k].val.data(), g.tp.t0[1], 32); break; }
+    }
+    cb_array(o, 2);
+    cb_uint(o, em);
+    cb_array(o, es.size());
+    for (const Entry& e : es) {
+        cb_array(o, 4);
+        cb_uint(o, e.flags);
+        cb_text(o, e.key);
+        cb_uint(o, e.codec);
+        cb_bytes(o, e.val.data(), e.val.size());
+    }
+}
+
+// Receipt i of the varied mode: 0..events_per_receipt events (at least one when selected).
+static ReceiptInfo gen_receipt_shaped(const Gen& g, uint64_t i, BlockSet* out, Cid* root) {
+    Rng r = rng_for(g.p.seed, DOM_RECEIPT, i);
+    ReceiptInfo ri;
+    bool sel = (r.next() % 1000000) < g.p.match_ppm;
+    int bw = (r.next() % 1000) < g.p.bw3_permille ? 3 : 5;
+    bool null_root = (r.next() % 1000) < g.p.null_root_permille;
+    ri.gas = (uint32_t)r.next();
+    const uint32_t E = g.p.events_per_receipt;
+    uint32_t n = E ? (uint32_t)(r.next() % (E + 1)) : 0;
+    if (sel && n == 0) n = 1;
+    ri.has_root = !null_root && E > 0;
+    ri.selected = sel && ri.has_root;
+    if (!ri.has_root) { memset(root->b, 0, 38); return ri; }
+    uint32_t sel_pos = n ? (uint32_t)(r.next() % n) : 0;
+    std::vector<Bytes> evs(n);
+    for (uint32_t j = 0; j < n; j++) gen_event_shaped(g, r, sel && j == sel_pos, evs[j]);
+    auto vf = [&](uint64_t k, Bytes& o) { o.insert(o.end(), evs[k].begin(), evs[k].end()); };
+    auto kf = [](int, uint64_t) { return true; };
+    *root = build_amt(n, bw, 3, vf, kf, out, 1);
+    return ri;
+}
+
 // Generates receipt i: its events AMT blocks (into `out` when non-null) and root CID.
 static ReceiptInfo gen_receipt(const Gen& g, uint64_t i, BlockSet* out, Cid* root) {
+    if (g.p.event_shapes == 1) return gen_receipt_shaped(g, i, out, root);
     Rng r = rng_for(g.p.seed, DOM_RECEIPT, i);
     ReceiptInfo ri;
     bool sel = (r.next() % 1000000) < g.p.match_ppm;

@@ -37,6 +37,9 @@ typedef struct synth_params {
                                    0,0 = everything                                          */
     uint32_t threads;           /* 0 = hardware_concurrency                                 */
     uint32_t same_topic1;       /* config 1: every event shares the target topic1           */
+    uint32_t event_shapes;      /* 0: the fixed shapes above; 1: varied events (emitter heads, topic
+                                   counts, data sizes, codecs, flags, duplicate / unknown keys,
+                                   near misses) and 0..events_per_receipt events per receipt  */
 } synth_params;
 
 typedef struct synth_tipset synth_tipset;

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from ipc_filecoin_proofs_b200 import _abi as A
-from tests.util import ShuffledTipset, assert_event_results_equal, assert_witness_equal, spec_of
+from tests.util import ShuffledTipset, assert_event_results_equal, assert_witness_equal, spec_of, synth_tipset
 
 pytestmark = pytest.mark.gpu
 
@@ -79,20 +79,30 @@ def test_event_proof_parity(api, oracle_mod, synth_mod, cfg):
     dict(n_receipts=1, events_per_receipt=1, match_ppm=1000000, dup_msgs=0, n_parents=1),
     dict(n_receipts=9, events_per_receipt=8, match_ppm=0, n_parents=3, dup_msgs=2),
     dict(n_receipts=700, events_per_receipt=300, match_ppm=20000, n_parents=1),             # bw-3 AMTs of height 2
+    # varied event shapes (synth event_shapes = 1): single-node roots over 4 KB and roots with links, events larger than pass 1's ring
+    dict(event_shapes=1, n_receipts=600, events_per_receipt=40, match_ppm=300000),
+    dict(event_shapes=1, n_receipts=500, events_per_receipt=12, match_ppm=300000, has_actor_filter=0, bw3_permille=300, null_root_permille=50),
+    dict(event_shapes=1, n_receipts=300, events_per_receipt=40, match_ppm=200000, target_actor=65536 + 7, bw3_permille=500),
+    # N on either side of the single-CTA scan of pass 1's counts (16 384)
+    dict(event_shapes=1, n_receipts=16384, events_per_receipt=6, match_ppm=60000, null_root_permille=20),
+    dict(event_shapes=1, n_receipts=16385, events_per_receipt=6, match_ppm=60000, has_actor_filter=0, n_parents=3),
 ])
 def test_event_proof_shapes(api, oracle_mod, synth_mod, kw):
     ts = synth_mod.Tipset(synth_mod.default_params(seed=99, **kw))
     exp = oracle_mod.Store.from_tipset(ts).generate_event_proof(ts, spec_of(ts))
     got = api.BlockStore.from_tipset(ts).generate_event_proof(ts, spec_of(ts))
     assert_event_results_equal(got, exp)
+    if kw.get("event_shapes"):
+        assert got.matching.tolist() == ts.selected.tolist() and len(got.proofs) == len(ts.selected) > 0
 
 
-def test_event_proof_block_order_and_alignment(api, oracle_mod, ts2):
-    exp = oracle_mod.Store.from_tipset(ts2).generate_event_proof(ts2, spec_of(ts2))
-    for misalign in (False, True):
-        sh = ShuffledTipset(ts2, seed=3, misalign=misalign)
-        got = api.BlockStore.from_tipset(sh, verify_cids=True).generate_event_proof(sh, spec_of(sh))
-        assert_event_results_equal(got, exp)
+def test_event_proof_block_order_and_alignment(api, oracle_mod, synth_mod, ts2):
+    for ts in (ts2, synth_tipset(synth_mod, "shapes")):
+        exp = oracle_mod.Store.from_tipset(ts).generate_event_proof(ts, spec_of(ts))
+        for layout in (dict(misalign=False), dict(misalign=True), dict(roots_mod128=True)):
+            sh = ShuffledTipset(ts, seed=3, **layout)
+            got = api.BlockStore.from_tipset(sh, verify_cids=True).generate_event_proof(sh, spec_of(sh))
+            assert_event_results_equal(got, exp)
 
 
 def test_skip_tx_flag(api, oracle_mod, ts2):
@@ -117,6 +127,38 @@ def test_storage_slots_parity(api, oracle_mod, ts3_small):
     for i, k in enumerate(ks[:50]):
         v = ts.storage_entry(k)[1]
         assert bytes(got.values[i][32 - len(v):]) == v
+
+
+@pytest.mark.parametrize("strict", [None, "1"])
+@pytest.mark.parametrize("k", [1000, 16384, 16385])   # one lookup per warp up to 16 384, one per thread (strict decoder) above
+def test_storage_slots_parity_lookup_counts(api, oracle_mod, ts3_small, monkeypatch, k, strict):
+    """Present, duplicate and absent keys in shuffled order, on both sides of k_read_slots' per-warp / per-thread switch, with the
+    strict HAMT decoder forced or not: found flags, raw lengths, values and witness equal the oracle's."""
+    if strict is None:
+        monkeypatch.delenv("IPCFP_HAMT_STRICT", raising=False)
+    else:
+        monkeypatch.setenv("IPCFP_HAMT_STRICT", strict)
+    ts = ts3_small
+    n = int(ts.params.hamt_entries)
+    rng = np.random.default_rng(5 + k)
+    n_absent, n_dup = k // 10, k // 20
+    ks = rng.integers(0, n, k - n_absent - n_dup - 1).tolist() + [n]
+    ks += rng.choice(ks, n_dup).tolist()                                          # duplicate keys
+    keys = [ts.storage_entry(e)[0] for e in ks] + [ts.storage_absent_key(e) for e in range(n_absent)]
+    present = np.array([True] * len(ks) + [False] * n_absent)
+    order = rng.permutation(k)
+    keys, present = [keys[i] for i in order], present[order]
+    slots = api.compute_mapping_slots(keys, [0] * len(keys))
+    slots_np = np.frombuffer(b"".join(slots), dtype=np.uint8)
+    exp = oracle_mod.Store.from_tipset(ts).read_storage_slots(ts.storage_root, slots_np)
+    got = api.BlockStore.from_tipset(ts, verify_cids=True).read_storage_slots(ts.storage_root, slots_np)
+    assert len(got.found) == k
+    assert np.array_equal(got.found, exp.found) and np.array_equal(got.raw_len, exp.raw_len) and np.array_equal(got.values, exp.values)
+    assert_witness_equal(got.witness, exp.witness)
+    assert np.array_equal(got.found.astype(bool), present)
+    for pos in np.nonzero(present)[0][:50]:
+        v = ts.storage_entry(ks[order[pos]])[1]
+        assert bytes(got.values[pos][32 - len(v):]) == v
 
 
 def test_storage_proofs_parity(api, oracle_mod, ts3_small):
@@ -437,9 +479,9 @@ def _verify_both(api, oracle_mod, w, ts, r, spec):
     return got
 
 
-@pytest.mark.parametrize("cfg", [1, 2])
+@pytest.mark.parametrize("cfg", [1, 2, "shapes", "shapes-nofilter"])
 def test_verify_event_proofs_gpu(api, oracle_mod, synth_mod, cfg):
-    ts = synth_mod.Tipset(synth_mod.config_params(cfg))
+    ts = synth_tipset(synth_mod, cfg)
     spec = spec_of(ts)
     r = api.BlockStore.from_tipset(ts, verify_cids=True).generate_event_proof(ts, spec)
     assert len(r.proofs) > 0

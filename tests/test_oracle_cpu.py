@@ -11,7 +11,7 @@ import pytest
 
 from ipc_filecoin_proofs_b200 import _abi as A
 from tests import golden_util
-from tests.util import EditedTipset, ShuffledTipset, assert_event_results_equal, dict_of, spec_of
+from tests.util import SHAPES, EditedTipset, ShuffledTipset, assert_event_results_equal, dict_of, spec_of, synth_tipset
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -52,21 +52,60 @@ def test_topic_constants(oracle_mod):
 
 
 # ------------------------------------------------------------------ synthetic data is well-formed DAG-CBOR with valid CIDs
-@pytest.mark.parametrize("cfg", [1, 2])
+@pytest.mark.parametrize("cfg", [1, 2, "shapes", "shapes-nofilter"])
 def test_synth_blocks_roundtrip_cbor2(synth_mod, cfg):
-    ts = synth_mod.Tipset(synth_mod.config_params(cfg))
+    ts = synth_tipset(synth_mod, cfg)
     for i in range(ts.n_blocks):
         b = ts.block(i)
         assert cbor2.dumps(cbor2.loads(b)) == b                       # minimal, definite-length encoding
         assert hashlib.blake2b(b, digest_size=32).digest() == bytes(ts.cids[i][6:])
         assert bytes(ts.cids[i][:6]) == bytes([0x01, 0x71, 0xa0, 0xe4, 0x02, 0x20])
         assert int(ts.offsets[i]) % 16 == 0
-    # shapes from SURVEY.md §8(a)
     import collections
     d = ts.as_dict()
-    lens = collections.Counter(len(d[bytes(ts.events_roots[i])]) for i in range(int(ts.n_receipts)))
-    assert lens.most_common(1)[0][0] == 1028   # events-AMT v3 bw5 root with 8 x 127-byte StampedEvents
+    roots = [d[bytes(ts.events_roots[i])] for i in range(int(ts.n_receipts)) if ts.has_events_root[i]]
+    if cfg in SHAPES:
+        _check_varied_shapes(ts, roots)
+    else:
+        # shapes from SURVEY.md §8(a)
+        lens = collections.Counter(len(r) for r in roots)
+        assert lens.most_common(1)[0][0] == 1028   # events-AMT v3 bw5 root with 8 x 127-byte StampedEvents
     assert oracle_mod_verify(ts)
+
+
+def _check_varied_shapes(ts, roots):
+    """The varied mode covers what it is there for: every emitter head size, Case A with 0-4 topics, Case B with 1-4 topics,
+    2-byte data length heads (59 nnnn), odd codecs and flags, duplicate and unknown keys, empty and linked AMTs, and single-node
+    roots over 4 KB that hold a forced match."""
+    seen = set()
+    linked = empty = 0
+    for raw in roots:
+        bw, height, count, node = cbor2.loads(raw)
+        linked += bool(node[1])
+        empty += count == 0
+        for em, entries in node[2]:
+            seen.add(("head", 0 if em < 24 else 1 if em < 256 else 2 if em < 65536 else 4 if em < 2 ** 32 else 8))
+            keys = [e[1] for e in entries]
+            seen.update(("key", key) for key in keys)
+            if len(set(keys)) < len(keys):
+                seen.add("duplicate")
+            if "topics" in keys:
+                seen.add(("case A topics", len(entries[keys.index("topics")][3]) // 32))
+            else:
+                seen.add(("case B topics", sum(1 for t in ("t1", "t2", "t3", "t4") if t in keys)))
+            for flags, key, codec, value in entries:
+                if flags != 3 or codec != 0x55:
+                    seen.add("odd codec or flags")
+                if len(value) >= 256:
+                    seen.add("2-byte length")
+    d = ts.as_dict()
+    big_selected = sum(1 for raw in (d[bytes(ts.events_roots[i])] for i in ts.selected.tolist()) if len(raw) > 4096 and not cbor2.loads(raw)[3][1])
+    want = {("head", h) for h in (0, 1, 2, 4, 8)} | {("case A topics", n) for n in range(5)} | {("case B topics", n) for n in range(1, 5)}
+    want |= {("key", k) for k in ("t1", "t2", "t3", "t4", "d", "topics", "data", "t5", "dat")} | {"duplicate", "odd codec or flags", "2-byte length"}
+    assert want <= seen, want - seen
+    assert empty > 0 and big_selected > 0
+    if ts.params.events_per_receipt > 32:
+        assert linked > 0 and big_selected >= 20
 
 
 def oracle_mod_verify(ts):
@@ -89,10 +128,10 @@ def test_oracle_matches_golden_storage(oracle_mod):
     golden_util.check_storage_result(z, st.generate_storage_proofs(s, specs))
 
 
-@pytest.mark.parametrize("cfg", [1, 2])
+@pytest.mark.parametrize("cfg", [1, 2, "shapes", "shapes-nofilter"])
 def test_oracle_vs_python_oracle(oracle_mod, synth_mod, cfg):
     from oracle import pyoracle as P
-    ts = synth_mod.Tipset(synth_mod.config_params(cfg))
+    ts = synth_tipset(synth_mod, cfg)
     r = oracle_mod.Store.from_tipset(ts).generate_event_proof(ts, spec_of(ts))
     pr = P.generate_event_proof(ts.as_dict(), ts, ts.event_signature, ts.topic1, ts.actor_filter)
     assert pr["matching"] == r.matching.tolist() == ts.selected.tolist()

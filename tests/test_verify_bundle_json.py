@@ -11,7 +11,7 @@ import pytest
 
 from ipc_filecoin_proofs_b200 import _abi as A
 from ipc_filecoin_proofs_b200 import bundle_json as J
-from tests.util import adversarial_tipset, spec_of
+from tests.util import adversarial_tipset, spec_of, synth_tipset
 
 pytestmark = pytest.mark.gpu
 
@@ -105,9 +105,9 @@ def unified3(api, ts3_small, oracle_mod):
     return J.dumps(J.unified_bundle(ts3_small, b))
 
 
-@pytest.mark.parametrize("cfg", [1, 2])
+@pytest.mark.parametrize("cfg", [1, 2, "shapes", "shapes-nofilter"])
 def test_canonical_event_bundles(api, synth_mod, cfg):
-    ts = synth_mod.Tipset(synth_mod.config_params(cfg))
+    ts = synth_tipset(synth_mod, cfg)
     text, r = event_text(api, ts)
     assert r.proofs
     host_text = J.dumps(J.event_bundle(ts, api.BlockStore.from_tipset(ts).generate_event_proof(ts, spec_of(ts))))

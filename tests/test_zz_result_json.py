@@ -9,7 +9,7 @@ import pytest
 
 from ipc_filecoin_proofs_b200 import _abi as A
 from ipc_filecoin_proofs_b200 import bundle_json as J
-from tests.util import EditedTipset, ShuffledTipset, spec_of
+from tests.util import EditedTipset, ShuffledTipset, spec_of, synth_tipset
 
 pytestmark = pytest.mark.gpu
 
@@ -64,9 +64,9 @@ def _check(api, ts, flags=0, resident_too=True, store=None):
     return base, want
 
 
-@pytest.mark.parametrize("cfg", [1, 2])
+@pytest.mark.parametrize("cfg", [1, 2, "shapes", "shapes-nofilter"])
 def test_json_equals_host_renderers(api, synth_mod, cfg):
-    base, _ = _check(api, synth_mod.Tipset(synth_mod.config_params(cfg)))
+    base, _ = _check(api, synth_tipset(synth_mod, cfg))
     assert base.proofs
 
 

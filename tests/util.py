@@ -28,19 +28,48 @@ def assert_witness_equal(a, b):
     assert a.blocks() == b.blocks()
 
 
-class ShuffledTipset:
-    """Same tipset with the flat block arrays permuted (the engine must not depend on block order)."""
+# Tipsets of the varied event-shape mode of the synthetic builder (event_shapes = 1), used as extra inputs next to the BASELINE
+# configs: emitters with 1- to 8-byte heads, 0-4 topics, data up to 955 bytes, odd codecs and flags, duplicate and unknown keys,
+# near misses, 0..events_per_receipt events per receipt (bit width 5: single-node roots, many over 4 KB, and roots with links).
+SHAPES = {
+    "shapes": dict(seed=41, n_receipts=600, events_per_receipt=40, match_ppm=300000),
+    "shapes-nofilter": dict(seed=42, n_receipts=600, events_per_receipt=12, match_ppm=300000, has_actor_filter=0, bw3_permille=300,
+                            null_root_permille=50),
+}
 
-    def __init__(self, ts, seed=7, misalign=False):
+
+def synth_tipset(synth_mod, cfg):
+    """The BASELINE config `cfg` (an int) or the varied-shape tipset SHAPES[cfg]."""
+    if cfg in SHAPES:
+        return synth_mod.Tipset(synth_mod.default_params(event_shapes=1, **SHAPES[cfg]))
+    return synth_mod.Tipset(synth_mod.config_params(cfg))
+
+
+class ShuffledTipset:
+    """Same tipset with the flat block arrays permuted (the engine must not depend on block order).
+    misalign: blocks start 0-6 bytes after the previous one. roots_mod128: the k-th events-root block starts at an offset ≡ k
+    (mod 128) and an events root is the last block of the blob (the other blocks 16-byte aligned)."""
+
+    def __init__(self, ts, seed=7, misalign=False, roots_mod128=False):
         rng = np.random.default_rng(seed)
         perm = rng.permutation(ts.n_blocks)
+        roots = set()
+        if roots_mod128:
+            roots = {bytes(ts.events_roots[i]) for i in range(int(ts.n_receipts)) if ts.has_events_root[i]}
+            last = max(k for k, i in enumerate(perm) if bytes(ts.cids[i]) in roots)
+            perm = np.concatenate([perm[:last], perm[last + 1:], perm[last:last + 1]])
         self._ts = ts
         lens = ts.lengths[perm]
         offs = np.zeros(ts.n_blocks, dtype=np.uint64)
         pos = 0
         chunks = []
+        kroot = 0
         for k, i in enumerate(perm):
-            pad = int(rng.integers(0, 7)) if misalign else (16 - pos % 16) % 16
+            if roots_mod128 and bytes(ts.cids[i]) in roots:
+                pad = (kroot - pos) % 128
+                kroot += 1
+            else:
+                pad = int(rng.integers(0, 7)) if misalign else (16 - pos % 16) % 16
             chunks.append(bytes(pad))
             pos += pad
             offs[k] = pos
