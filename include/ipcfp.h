@@ -242,6 +242,12 @@ typedef struct ipcfp_bundle {
     uint64_t n_event_results;
     ipcfp_event_result** events;    /* one per event spec */
     ipcfp_witness witness;          /* UnifiedProofBundle.blocks: BTreeSet<(Cid, data)> order */
+    /* IPCFP_RESULT_JSON only (NULL / 0 otherwise): the UnifiedProofBundle as JSON, byte for byte what ipcfp_bundle_to_json renders for the
+     * same call made without flags. NUL-terminated, json_len bytes without the NUL, owned by the bundle. */
+    const char* json;
+    uint64_t json_len;
+    float ms_total;                 /* device time of the whole call, milliseconds (CUDA events on the store's stream)                */
+    float ms_json;                  /* IPCFP_RESULT_JSON: device time of the rendering and its copy to the host; 0 otherwise          */
 } ipcfp_bundle;
 
 /* ------------------------------------------------------------------------------------------
@@ -295,10 +301,21 @@ ipcfp_status ipcfp_generate_storage_proofs(ipcfp_store* s, const ipcfp_tipset_de
                                            uint64_t n_specs, ipcfp_storage_result** out);
 void ipcfp_storage_result_free(ipcfp_storage_result* r);
 
-/* generate_proof_bundle (src/proofs/generator.rs:25-95). */
+/* generate_proof_bundle (src/proofs/generator.rs:25-95): the storage specs, then the event specs in order, then the union of every
+ * proof's blocks (BTreeSet<(Cid, data)>, built on the device). Equivalent to ipcfp_tipset_upload followed by
+ * ipcfp_generate_proof_bundle_resident with flags = 0. */
 ipcfp_status ipcfp_generate_proof_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs,
                                          uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
                                          ipcfp_bundle** out);
+/* The same against a tipset uploaded once with ipcfp_tipset_upload; it fails where ipcfp_generate_proof_bundle fails, with the same status
+ * and index. flags (any other bit: IPCFP_ERR_INVALID_ARG):
+ *   IPCFP_WITNESS_BY_REFERENCE  every witness of the bundle (storage->witness, each events[k]->witness and the union `witness`) comes
+ *                               by reference: blob NULL, offsets into the blob the store was created from;
+ *   IPCFP_RESULT_JSON           the bundle also carries `json`, the UnifiedProofBundle text rendered on the device (block bytes are read
+ *                               from the store, so it combines with IPCFP_WITNESS_BY_REFERENCE). One extra host synchronisation.
+ * Storage specs need a tipset uploaded with child_parent_state_root (else IPCFP_ERR_INVALID_ARG). */
+ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                  const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_bundle** out);
 void ipcfp_bundle_free(ipcfp_bundle* b);
 
 /* ------------------------------------------------------------------------------------------

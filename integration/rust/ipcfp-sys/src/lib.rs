@@ -93,7 +93,8 @@ pub struct ipcfp_bundle_verdict { pub tipset: ipcfp_tipset_desc, pub n_storage_p
                                   pub witness_bytes: u64, pub parsed_on_device: u32, pub ms_total: f32, pub ms_parse: f32, pub ms_store: f32,
                                   pub ms_verify: f32, pub _pad: u32 }
 #[repr(C)]
-pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness }
+pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
+                          pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
 
 extern "C" {
     pub fn ipcfp_last_error() -> *const c_char;
@@ -136,6 +137,8 @@ extern "C" {
     pub fn ipcfp_storage_result_free(r: *mut ipcfp_storage_result);
     pub fn ipcfp_generate_proof_bundle(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                                        especs: *const ipcfp_event_spec, n_especs: u64, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
+    pub fn ipcfp_generate_proof_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                                                especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
     pub fn ipcfp_bundle_free(b: *mut ipcfp_bundle);
 
     pub fn ipcfp_bundle_to_json(b: *const ipcfp_bundle, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;

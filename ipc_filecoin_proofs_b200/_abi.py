@@ -209,6 +209,10 @@ class BundleC(C.Structure):
         ("n_event_results", C.c_uint64),
         ("events", C.POINTER(C.POINTER(EventResultC))),
         ("witness", Witness),
+        ("json", C.c_void_p),
+        ("json_len", C.c_uint64),
+        ("ms_total", C.c_float),
+        ("ms_json", C.c_float),
     ]
 
 
@@ -400,12 +404,19 @@ class BundlePy:
     storage: StorageResultPy
     events: list
     witness: WitnessPy
+    json: str = None        # IPCFP_RESULT_JSON: the UnifiedProofBundle text rendered on the device
+    timings: dict = field(default_factory=dict)
 
 
 def bundle_from_c(b):
     st = storage_result_from_c(b.storage.contents) if b.storage else None
     ev = [event_result_from_c(b.events[i].contents) for i in range(int(b.n_event_results))]
-    return BundlePy(st, ev, witness_from_c(b.witness))
+    timings = dict(total=b.ms_total)
+    text = None
+    if b.json:
+        text = C.string_at(b.json, int(b.json_len)).decode()
+        timings["json"] = b.ms_json
+    return BundlePy(st, ev, witness_from_c(b.witness), text, timings)
 
 
 class IpcfpError(RuntimeError):

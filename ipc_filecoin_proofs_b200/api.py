@@ -44,6 +44,7 @@ EXPORTS = [
     "ipcfp_comm_unique_id", "ipcfp_comm_init", "ipcfp_comm_destroy", "ipcfp_generate_event_proof_sharded",
     "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
     "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
+    "ipcfp_generate_proof_bundle_resident",
 ]
 
 
@@ -96,6 +97,9 @@ def lib():
         L.ipcfp_generate_proof_bundle.restype = C.c_int32
         L.ipcfp_generate_proof_bundle.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                   C.POINTER(C.POINTER(A.BundleC))]
+        L.ipcfp_generate_proof_bundle_resident.restype = C.c_int32
+        L.ipcfp_generate_proof_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                           C.POINTER(C.POINTER(A.BundleC))]
         L.ipcfp_bundle_free.argtypes = [C.POINTER(A.BundleC)]
         L.ipcfp_tipset_upload.restype = C.c_int32
         L.ipcfp_tipset_upload.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(C.c_void_p)]
@@ -292,14 +296,31 @@ class BlockStore:
             lib().ipcfp_storage_result_free(out)
 
     # --- generate_proof_bundle (proofs/generator.rs:25-95)
-    def generate_proof_bundle(self, ts, storage_specs, event_specs):
+    @staticmethod
+    def _bundle_specs(storage_specs, event_specs):
         sspecs = [(s.actor_id, s.slot) if isinstance(s, StorageProofSpec) else s for s in storage_specs]
         especs = [s.as_c() if isinstance(s, EventProofSpec) else s for s in event_specs]
+        return A.make_storage_specs(sspecs), len(sspecs), (A.EventSpec * len(especs))(*especs), len(especs)
+
+    def generate_proof_bundle(self, ts, storage_specs, event_specs):
+        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
         d, keep = A.make_tipset_desc(ts)
-        sarr = A.make_storage_specs(sspecs)
-        earr = (A.EventSpec * len(especs))(*especs)
         out = C.POINTER(A.BundleC)()
-        _check(lib().ipcfp_generate_proof_bundle(self._h, C.byref(d), sarr, len(sspecs), earr, len(especs), C.byref(out)))
+        _check(lib().ipcfp_generate_proof_bundle(self._h, C.byref(d), sarr, ns, earr, ne, C.byref(out)))
+        try:
+            return A.bundle_from_c(out.contents)
+        finally:
+            lib().ipcfp_bundle_free(out)
+
+    def upload_tipset(self, ts):
+        """ipcfp_tipset_upload: the tipset's descriptor on the device, for any number of _resident calls. close() releases it."""
+        return ResidentTipset(self, ts)
+
+    def generate_proof_bundle_resident(self, tip, storage_specs, event_specs, flags=0):
+        """ipcfp_generate_proof_bundle_resident against a ResidentTipset of this store. flags: WITNESS_BY_REFERENCE, RESULT_JSON."""
+        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
+        out = C.POINTER(A.BundleC)()
+        _check(lib().ipcfp_generate_proof_bundle_resident(self._h, tip._h, sarr, ns, earr, ne, flags, C.byref(out)))
         try:
             return A.bundle_from_c(out.contents)
         finally:
@@ -308,6 +329,28 @@ class BlockStore:
     def close(self):
         if self._h:
             lib().ipcfp_store_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ResidentTipset:
+    """A tipset descriptor uploaded to a store's device (ipcfp_tipset_upload / ipcfp_tipset_free). Valid while its store lives."""
+
+    def __init__(self, store, ts):
+        d, keep = A.make_tipset_desc(ts)
+        h = C.c_void_p()
+        _check(lib().ipcfp_tipset_upload(store._h, C.byref(d), C.byref(h)))
+        self._h = h
+        self.store = store
+
+    def close(self):
+        if self._h:
+            lib().ipcfp_tipset_free(self._h)
             self._h = None
 
     def __del__(self):

@@ -1,8 +1,6 @@
 // capi.cu — the extern "C" surface declared in include/ipcfp.h.
 #include <atomic>
 #include <cstring>
-#include <map>
-#include <set>
 
 #include "engine.cuh"
 #include "prims.cuh"
@@ -118,12 +116,97 @@ void merge_witness_cids(int device, const void* gathered, const uint64_t* counts
 
 // ------------------------------------------------------------------------------------------ bundle
 struct BundleBox {
-    ipcfp_bundle r;
+    ipcfp_bundle r;   // must stay first
     std::vector<ipcfp_event_result*> ev;
-    std::vector<uint8_t> cids, blob;
-    std::vector<uint64_t> offsets;
-    std::vector<uint32_t> lengths;
+    WitnessOut wit;   // the union
+    PinnedArray json;
+    ~BundleBox() {
+        if (r.storage) storage_result_free(r.storage);
+        for (auto* e : ev) event_result_free(e);
+    }
 };
+struct TimingEvent {
+    cudaEvent_t e = nullptr;
+    TimingEvent() { IPCFP_CUDA(cudaEventCreate(&e)); }
+    ~TimingEvent() { if (e) cudaEventDestroy(e); }
+};
+
+#define IPCFP_BUNDLE_FLAGS (IPCFP_WITNESS_BY_REFERENCE | IPCFP_RESULT_JSON)
+
+// generate_proof_bundle (proofs/generator.rs:25-95) against a device-resident tipset: the storage specs in one batch, then every event
+// spec in order, then the BTreeSet<(Cid, data)> union of every proof's blocks on the device (witness_union: OR of the lists' rank bits,
+// one compaction) and, with IPCFP_RESULT_JSON, the UnifiedProofBundle text rendered from device memory.
+static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                           const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags) {
+    if (flags & ~(uint32_t)IPCFP_BUNDLE_FLAGS) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a proof bundle");
+    if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
+    st->use();
+    const bool by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
+    cudaStream_t stream = st->stream;
+    TimingEvent t0, t1, j0, j1;
+    IPCFP_CUDA(cudaEventRecord(t0.e, stream));
+    std::unique_ptr<BundleBox> box(new BundleBox());
+    memset(&box->r, 0, sizeof box->r);
+    std::vector<const WitnessOut*> lists;
+    if (n_sspecs) {
+        if (!td.has_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+        box->r.storage = generate_storage_proofs(st, td.child_cid, td.child_state_root, sspecs, n_sspecs, by_ref);
+        lists.push_back(&storage_result_witness(box->r.storage));
+    }
+    for (uint64_t i = 0; i < n_especs; i++) {
+        box->ev.push_back(generate_event_proof(st, nullptr, td, &especs[i], flags & IPCFP_WITNESS_BY_REFERENCE, false, 0, 0, 1, 0));
+        lists.push_back(&event_result_witness(box->ev.back()));
+    }
+    witness_union(st, lists, box->wit, by_ref);
+
+    if (flags & IPCFP_RESULT_JSON) {
+        IPCFP_CUDA(cudaEventRecord(j0.e, stream));
+        // the records' inputs in ONE upload: storage proofs, every spec's EventProofs with their topics / data offsets rebased into one
+        // concatenated data blob, the tipset CIDs the records repeat
+        const uint64_t ns = box->r.storage ? box->r.storage->n_proofs : 0;
+        uint64_t np = 0, nb = 0;
+        for (auto* e : box->ev) { np += e->n_proofs; nb += e->data_blob_size; }
+        auto up16 = [](uint64_t x) { return (x + 15) & ~15ull; };
+        const uint64_t o_ev = up16(ns * sizeof(ipcfp_storage_proof)), o_blob = o_ev + up16(np * sizeof(ipcfp_event_proof)),
+                       o_cids = o_blob + up16(nb + 16), size = o_cids + 38ull * (2 + td.n_parents);
+        PinnedArray stage(st->pool, size);
+        uint8_t* h = stage.as<uint8_t>();
+        if (ns) memcpy(h, box->r.storage->proofs, ns * sizeof(ipcfp_storage_proof));
+        ipcfp_event_proof* hp = (ipcfp_event_proof*)(h + o_ev);
+        uint64_t k = 0, base = 0;
+        for (auto* e : box->ev) {
+            for (uint64_t q = 0; q < e->n_proofs; q++, k++) {
+                hp[k] = e->proofs[q];
+                hp[k].data_off += base;
+                hp[k].topics_off += base;
+            }
+            if (e->data_blob_size) memcpy(h + o_blob + base, e->data_blob, e->data_blob_size);
+            base += e->data_blob_size;
+        }
+        memcpy(h + o_cids, td.child_cid, 38);
+        memcpy(h + o_cids + 38, td.child_state_root, 38);
+        if (td.n_parents) memcpy(h + o_cids + 76, td.parent_cids.data(), 38ull * td.n_parents);
+        AsyncBuf<uint8_t> d(size, stream);
+        IPCFP_CUDA(cudaMemcpyAsync(d.p, h, size, cudaMemcpyHostToDevice, stream));
+        UnifiedJsonInputs ji{(const ipcfp_storage_proof*)d.p, ns, (const ipcfp_event_proof*)(d.p + o_ev), np, d.p + o_blob,
+                             box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n, td.parent_epoch, td.child_epoch, td.n_parents,
+                             d.p + o_cids + 76, d.p + o_cids, d.p + o_cids + 38};
+        box->r.json_len = render_unified_json(st, ji, box->json);
+        IPCFP_CUDA(cudaEventRecord(j1.e, stream));
+    }
+    IPCFP_CUDA(cudaEventRecord(t1.e, stream));
+    IPCFP_CUDA(cudaStreamSynchronize(stream));
+    box->r.n_event_results = box->ev.size();
+    box->r.events = box->ev.data();
+    box->wit.fill(box->r.witness);
+    float ms;
+    IPCFP_CUDA(cudaEventElapsedTime(&ms, t0.e, t1.e)); box->r.ms_total = ms;
+    if (flags & IPCFP_RESULT_JSON) {
+        box->r.json = box->json.as<char>();
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, j0.e, j1.e)); box->r.ms_json = ms;
+    }
+    return &box.release()->r;
+}
 
 }  // namespace ipcfp
 
@@ -137,7 +220,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_json_* | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }
@@ -266,69 +349,33 @@ ipcfp_status ipcfp_generate_storage_proofs(ipcfp_store* s, const ipcfp_tipset_de
     return guard([&] {
         if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
-        *out = generate_storage_proofs(reinterpret_cast<Store*>(s), t, specs, n);
+        if (!t) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+        *out = generate_storage_proofs(reinterpret_cast<Store*>(s), t->child_cid, t->child_parent_state_root, specs, n);
     });
 }
 void ipcfp_storage_result_free(ipcfp_storage_result* r) { if (r) storage_result_free(r); }
 
-// generate_proof_bundle (proofs/generator.rs:25-95): storage specs first, then event specs, then the
-// BTreeSet<(Cid, Vec<u8>)> union of every proof's blocks. The union is a merge of already sorted,
-// already materialised witness lists (host bookkeeping; no block is decoded or hashed here).
+// generate_proof_bundle (proofs/generator.rs:25-95): the tipset uploaded, then the resident call's body without flags
 ipcfp_status ipcfp_generate_proof_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                          const ipcfp_event_spec* especs, uint64_t n_especs, ipcfp_bundle** out) {
     return guard([&] {
         if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
         Store* st = reinterpret_cast<Store*>(s);
-        std::unique_ptr<BundleBox> box(new BundleBox());
-        memset(&box->r, 0, sizeof box->r);
-        struct Cleanup { BundleBox* b; bool armed = true; ~Cleanup() { if (armed) { if (b->r.storage) storage_result_free(b->r.storage); for (auto* e : b->ev) event_result_free(e); } } } cl{box.get()};
-        std::vector<const ipcfp_witness*> lists;
-        if (n_sspecs) { box->r.storage = generate_storage_proofs(st, t, sspecs, n_sspecs); lists.push_back(&box->r.storage->witness); }
-        if (n_especs) {
-            TipsetDev td;
-            tipset_upload(st, t, td);
-            for (uint64_t i = 0; i < n_especs; i++) {
-                box->ev.push_back(generate_event_proof(st, t, td, &especs[i], 0, false, 0, 0, 1, 0));
-                lists.push_back(&box->ev.back()->witness);
-            }
-        }
-        // k-way merge of sorted lists keyed by the store's CID order: reuse the order already
-        // established on the device — equal CIDs are byte-identical, lists are individually sorted
-        // by the same comparator, so a merge by (class rank, digest) bytes is exact.
-        auto key_of = [&](const uint8_t* cid) {
-            std::array<uint8_t, 39> k{};
-            uint32_t rank = 0xff;
-            for (size_t c = 0; c < st->class_prefix.size(); c++) if (!memcmp(cid, st->class_prefix[c].data(), 6)) rank = st->class_rank[c];
-            k[0] = (uint8_t)rank;
-            memcpy(k.data() + 1, cid + 6, 32);
-            return k;
-        };
-        std::map<std::array<uint8_t, 39>, std::pair<const ipcfp_witness*, uint64_t>> uni;
-        for (auto* w : lists) for (uint64_t i = 0; i < w->n_blocks; i++) uni.emplace(key_of(w->cids + 38 * i), std::make_pair(w, i));
-        for (auto& kv : uni) {
-            const ipcfp_witness* w = kv.second.first;
-            uint64_t i = kv.second.second;
-            box->cids.insert(box->cids.end(), w->cids + 38 * i, w->cids + 38 * i + 38);
-            box->offsets.push_back(box->blob.size());
-            box->lengths.push_back(w->lengths[i]);
-            box->blob.insert(box->blob.end(), w->blob + w->offsets[i], w->blob + w->offsets[i] + w->lengths[i]);
-        }
-        box->r.n_event_results = box->ev.size();
-        box->r.events = box->ev.data();
-        box->r.witness.n_blocks = uni.size(); box->r.witness.cids = box->cids.data(); box->r.witness.offsets = box->offsets.data(); box->r.witness.lengths = box->lengths.data();
-        box->r.witness.blob = box->blob.data(); box->r.witness.blob_size = box->blob.size();
-        cl.armed = false;
-        *out = &box.release()->r;
+        TipsetDev td;
+        tipset_upload(st, t, td);
+        *out = generate_proof_bundle(st, td, sspecs, n_sspecs, especs, n_especs, 0);
     });
 }
-void ipcfp_bundle_free(ipcfp_bundle* b) {
-    if (!b) return;
-    BundleBox* box = reinterpret_cast<BundleBox*>(b);
-    if (box->r.storage) storage_result_free(box->r.storage);
-    for (auto* e : box->ev) event_result_free(e);
-    delete box;
+ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                  const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_bundle** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = generate_proof_bundle(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, especs, n_especs, flags);
+    });
 }
+void ipcfp_bundle_free(ipcfp_bundle* b) { delete reinterpret_cast<BundleBox*>(b); }
 
 ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
                                        uint64_t blob_size, const ipcfp_event_spec* filter, uint8_t* results) {

@@ -138,6 +138,8 @@ ipcfp_bundle_verdict* verify_bundle_json(const char* json, uint64_t len, int dev
                                          ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter);
 void bundle_verdict_free(ipcfp_bundle_verdict* v);
 void event_result_free(ipcfp_event_result* r);
+struct WitnessOut;
+const WitnessOut& event_result_witness(const ipcfp_event_result* r);   // the witness of a generate_event_proof result, device copies included
 void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n);
 void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
                         uint64_t* n_out);
@@ -198,8 +200,11 @@ void exec_fetch(int device, const void* seg, uint64_t nseg, uint64_t pos0, const
 // storage.cu
 ipcfp_slot_result* read_storage_slots(Store* s, const uint8_t* root, const uint8_t* slots, uint64_t k);
 void slot_result_free(ipcfp_slot_result* r);
-ipcfp_storage_result* generate_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* specs, uint64_t n);
+// child_cid / state_root: the child block's CID and its header's parent_state_root (38 bytes each, host memory)
+ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid, const uint8_t* state_root, const ipcfp_storage_spec* specs, uint64_t n,
+                                              bool by_ref = false);
 void storage_result_free(ipcfp_storage_result* r);
+const WitnessOut& storage_result_witness(const ipcfp_storage_result* r);
 
 // witness.cu — materialise a witness bitmap into a sorted ipcfp_witness (host, pinned)
 struct WitnessOut {
@@ -235,7 +240,10 @@ struct WitnessBuilder {
     void finish_start(uint64_t mB, uint64_t bytesB, WitnessOut& out, bool want_sorted_idx = false);   // … the same without the join: everything enqueued
     void finish_join(WitnessOut& out);                                              // … wait for both streams
 };
-void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out);
+void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out, bool by_ref = false);
+// the union of witness lists of this store (the BTreeSet<(Cid, data)> of generate_proof_bundle): every entry's block marks its rank in a
+// fresh bitmap (block indices from WitnessOut::idx_dev), which is then materialised as one witness, in `Cid` order
+void witness_union(Store* s, const std::vector<const WitnessOut*>& lists, WitnessOut& out, bool by_ref);
 
 // json.cu — IPCFP_RESULT_JSON: the EventProofBundle text of one call from what is on the device after k_witness_emit (all pointers device)
 struct JsonInputs {
@@ -253,6 +261,23 @@ struct JsonInputs {
 // enqueues on the store's stream, synchronises it once (the exact length), enqueues the rendering and the copy into `out` (pinned,
 // NUL-terminated; the text is there once the stream has drained); returns the length of the text
 uint64_t render_event_json(Store* s, const JsonInputs& in, PinnedArray& out);
+// the UnifiedProofBundle text of ipcfp_generate_proof_bundle_resident (all pointers device); the same steps as render_event_json
+struct UnifiedJsonInputs {
+    const ipcfp_storage_proof* storage;   // n_storage StorageProofs
+    uint64_t n_storage;
+    const ipcfp_event_proof* proofs;      // n_proofs EventProofs of every spec, in spec order (no skipped slot)
+    uint64_t n_proofs;
+    const uint8_t* blob;                  // topics / data bytes the proofs index
+    const uint8_t* cids;                  // m*38, the union's sorted CIDs
+    const uint32_t* idx;                  // m, block index of every union entry
+    uint64_t m;
+    int64_t parent_epoch, child_epoch;
+    uint32_t n_parents;
+    const uint8_t* parent_cids;           // n_parents*38
+    const uint8_t* child_cid;             // 38
+    const uint8_t* state_root;            // 38 (read only when n_storage > 0)
+};
+uint64_t render_unified_json(Store* s, const UnifiedJsonInputs& in, PinnedArray& out);
 // ord[0..m) = the permutation that sorts the blocks idx[0..m) in `Cid` Ord (stable); runs on the store's stream (ingest: the ranks)
 size_t sort_by_cid_ws_bytes(uint64_t m);
 void sort_by_cid(Store* s, const uint32_t* idx_dev, uint32_t* ord, uint64_t m, void* workspace);

@@ -859,6 +859,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
 }
 
 void event_result_free(ipcfp_event_result* r) { delete reinterpret_cast<EventResultBox*>(r); }
+const WitnessOut& event_result_witness(const ipcfp_event_result* r) { return reinterpret_cast<const EventResultBox*>(r)->wit; }
 
 void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n) {
     uint64_t m = r->witness.n_blocks;

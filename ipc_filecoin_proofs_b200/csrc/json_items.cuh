@@ -1,7 +1,9 @@
 // json_items.cuh — per-item device functions of the EventProofBundle JSON renderer (IPCFP_RESULT_JSON, csrc/json.cu): the exact length
 // and the text of one EventProof record and of one ProofBlock record, byte for byte what csrc/bundle_json.cpp writes
 // (ipcfp_event_result_to_json; serde_json of src/proofs/events/bundle.rs:5-30, src/proofs/common/bundle.rs:10-26). They live in a header
-// so that tests/host_fuzz/emu_json.cu runs the very same code on the CPU against bundle_json.cpp.
+// so that tests/host_fuzz/emu_json.cu runs the very same code on the CPU against bundle_json.cpp. The StorageProof record and the
+// UnifiedProofBundle framing (ipcfp_generate_proof_bundle_resident with IPCFP_RESULT_JSON) are checked the same way by
+// tests/host_fuzz/emu_json_unified.cu against ipcfp_bundle_to_json.
 //
 // The bundle is laid out as
 //   {"proofs":  S P0  S P1 …  ],"blocks":  S B0  S B1 …  ]}
@@ -158,6 +160,35 @@ __device__ __forceinline__ void json_block_write(char* o, bool first, const uint
     if (lane == 0) { char* e = d + 4ull * ng; e[0] = '"'; e[1] = '}'; }
 }
 
+// ---- one StorageProof (storage/bundle.rs:5-14) of a UnifiedProofBundle, field order and spelling as bundle_json.cpp::storage_proofs_json
+struct JsonStorageCtx {
+    int64_t child_epoch;
+    const uint8_t* child_cid;    // 38
+    const uint8_t* state_root;   // 38: the child header's parent_state_root
+};
+template <class S> __device__ __forceinline__ void json_storage_record(S& s, const JsonStorageCtx& c, const ipcfp_storage_proof& p) {
+    s.lit("{\"child_epoch\":"); s.i64(c.child_epoch);
+    s.lit(",\"child_block_cid\":"); s.cid_str(c.child_cid);
+    s.lit(",\"parent_state_root\":"); s.cid_str(c.state_root);
+    s.lit(",\"actor_id\":"); s.u64(p.actor_id);
+    s.lit(",\"actor_state_cid\":"); s.cid_str(p.actor_state_cid);
+    s.lit(",\"storage_root\":"); s.cid_str(p.storage_root);
+    s.lit(",\"slot\":"); s.hex0x(p.slot, 32);
+    s.lit(",\"value\":"); s.hex0x(p.value, 32);
+    s.ch('}');
+}
+// separator included
+__device__ __forceinline__ uint64_t json_storage_len(const JsonStorageCtx& c, const ipcfp_storage_proof& p) {
+    JsonCount n;
+    json_storage_record(n, c, p);
+    return 1 + n.n;
+}
+__device__ __forceinline__ void json_storage_write(char* o, bool first, const JsonStorageCtx& c, const ipcfp_storage_proof& p) {
+    JsonWrite w{o};
+    w.ch(first ? '[' : ',');
+    json_storage_record(w, c, p);
+}
+
 // ---- framing. P, Q: summed lengths of the proof and block lists (separators included). Total length of the bundle:
 __host__ __device__ __forceinline__ uint64_t json_total_len(uint64_t P, uint64_t Q) {
     return JSON_PROOFS_HEAD + (P ? P : 1) + 1 + JSON_BLOCKS_HEAD + (Q ? Q : 1) + 2;
@@ -172,6 +203,28 @@ __device__ __forceinline__ void json_frame_write(char* o, uint64_t P, uint64_t Q
     w.lit("],\"blocks\":");
     if (!Q) w.ch('[');
     w.o = o + json_blocks_at(P) + (Q ? Q : 1);
+    w.lit("]}");
+}
+
+// ---- UnifiedProofBundle framing (common/bundle.rs:37-45): {"storage_proofs": S ,"event_proofs": P ,"blocks": Q }, each list laid out as
+// above. S, P, Q: summed lengths of the three lists (separators included).
+#define JSON_STORAGE_HEAD 18u   // {"storage_proofs":
+#define JSON_EVENTS_HEAD 16u    // ,"event_proofs":
+__host__ __device__ __forceinline__ uint64_t json_u_events_at(uint64_t S) { return JSON_STORAGE_HEAD + (S ? S : 1) + 1 + JSON_EVENTS_HEAD; }
+__host__ __device__ __forceinline__ uint64_t json_u_blocks_at(uint64_t S, uint64_t P) { return json_u_events_at(S) + (P ? P : 1) + 1 + JSON_BLOCKS_HEAD; }
+__host__ __device__ __forceinline__ uint64_t json_u_total_len(uint64_t S, uint64_t P, uint64_t Q) { return json_u_blocks_at(S, P) + (Q ? Q : 1) + 2; }
+// everything of the text that is not a record (one thread)
+__device__ __forceinline__ void json_u_frame_write(char* o, uint64_t S, uint64_t P, uint64_t Q) {
+    JsonWrite w{o};
+    w.lit("{\"storage_proofs\":");
+    if (!S) w.ch('[');
+    w.o = o + JSON_STORAGE_HEAD + (S ? S : 1);
+    w.lit("],\"event_proofs\":");
+    if (!P) w.ch('[');
+    w.o = o + json_u_events_at(S) + (P ? P : 1);
+    w.lit("],\"blocks\":");
+    if (!Q) w.ch('[');
+    w.o = o + json_u_blocks_at(S, P) + (Q ? Q : 1);
     w.lit("]}");
 }
 

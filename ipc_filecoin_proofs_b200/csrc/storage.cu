@@ -146,9 +146,10 @@ struct StorageResultBox {
     std::vector<uint64_t> spec_off;
     std::vector<uint32_t> spec_idx;
 };
-ipcfp_storage_result* generate_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* specs, uint64_t n) {
+ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid, const uint8_t* state_root, const ipcfp_storage_spec* specs, uint64_t n,
+                                              bool by_ref) {
     s->use();
-    if (!t || !t->child_cid || !t->child_parent_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+    if (!child_cid || !state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
     if (n && !specs) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
@@ -160,8 +161,8 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const ipcfp_tipset_desc*
     AsyncBuf<ipcfp_storage_proof> d_out(n + 1, st);
     AsyncBuf<uint32_t> d_rec(n * REC_CAP + 8, st), d_recn(n + 8, st), wbits((s->n + 31) / 32 + 8, st);
     wbits.zero();
-    IPCFP_CUDA(cudaMemcpyAsync(d_in.p, t->child_cid, 38, cudaMemcpyHostToDevice, st));
-    IPCFP_CUDA(cudaMemcpyAsync(d_in.p + 64, t->child_parent_state_root, 38, cudaMemcpyHostToDevice, st));
+    IPCFP_CUDA(cudaMemcpyAsync(d_in.p, child_cid, 38, cudaMemcpyHostToDevice, st));
+    IPCFP_CUDA(cudaMemcpyAsync(d_in.p + 64, state_root, 38, cudaMemcpyHostToDevice, st));
     if (n) IPCFP_CUDA(cudaMemcpyAsync(d_specs.p, specs, n * sizeof(ipcfp_storage_spec), cudaMemcpyHostToDevice, st));
     StorageArgs a;
     a.store = s->view; a.child_cid = d_in.p; a.state_root_json = d_in.p + 64; a.specs = d_specs.p; a.n = n; a.out = d_out.p;
@@ -179,7 +180,7 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const ipcfp_tipset_desc*
         IPCFP_CUDA(cudaMemcpyAsync(rec.p, d_rec.p, n * REC_CAP * 4, cudaMemcpyDeviceToHost, st));
         IPCFP_CUDA(cudaMemcpyAsync(recn.p, d_recn.p, n * 4, cudaMemcpyDeviceToHost, st));
     }
-    materialize_witness(s, wbits.p, box->wit);
+    materialize_witness(s, wbits.p, box->wit, by_ref);
     // per-spec Vec<ProofBlock>: map recorded block indices to positions in the sorted union
     PinnedArray& sorted_idx = box->wit.sorted_idx;
     IPCFP_CUDA(cudaEventRecord(s->ev[1], st));
@@ -205,5 +206,6 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const ipcfp_tipset_desc*
     return &box.release()->r;
 }
 void storage_result_free(ipcfp_storage_result* r) { delete reinterpret_cast<StorageResultBox*>(r); }
+const WitnessOut& storage_result_witness(const ipcfp_storage_result* r) { return reinterpret_cast<const StorageResultBox*>(r)->wit; }
 
 }  // namespace ipcfp

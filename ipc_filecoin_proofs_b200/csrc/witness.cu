@@ -318,14 +318,33 @@ void WitnessBuilder::finish_join(WitnessOut& out) {
     out.blob = std::move(host_blob);
 }
 
-// single-phase convenience (storage path): everything at once
-void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out) {
+// single-phase convenience (storage path, bundle union): everything at once
+void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out, bool by_ref) {
     WitnessBuilder wb(s);
+    wb.by_ref = by_ref;
     wb.snapshot(wbits_dev);
     publish_words(s, 8, 2);
     IPCFP_CUDA(cudaStreamSynchronize(s->stream));
     wb.start_copy(s->host_words.p[8], s->host_words.p[9], s->host_words.p[8], s->host_words.p[9]);   // one part
     wb.finish(0, 0, out, true);
+}
+
+// bit rank_of[idx[i]] of the union bitmap for every entry of one witness list (lists overlap: atomicOr)
+__global__ void k_union_mark(const uint32_t* __restrict__ idx, uint64_t m, const uint32_t* __restrict__ rank_of, uint32_t* bits) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint32_t r = rank_of[idx[i]];
+    atomicOr(bits + (r >> 5), 1u << (r & 31));
+}
+// Every entry's block is the one its lookup marked (equal CIDs resolve to one block of the store), so equal CIDs of different lists set one
+// bit, and reading the bitmap in bit order is `Cid` order for any number of CID prefixes.
+void witness_union(Store* s, const std::vector<const WitnessOut*>& lists, WitnessOut& out, bool by_ref) {
+    cudaStream_t st = s->stream;
+    AsyncBuf<uint32_t> bits((s->n + 31) / 32 + 8, st);
+    bits.zero();
+    for (const WitnessOut* w : lists)
+        if (w->n) { k_union_mark<<<div_up(w->n, 256), 256, 0, st>>>(w->idx_dev.p, w->n, s->rank_of.p, bits.p); IPCFP_LAUNCH_CHECK(); }
+    materialize_witness(s, bits.p, out, by_ref);
 }
 
 }  // namespace ipcfp
