@@ -52,6 +52,7 @@ struct PinnedArray {
 struct Store {
     int device = 0;
     cudaStream_t stream = nullptr, stream2 = nullptr;
+    unsigned walk_grid = 0;               // CTAs of the persistent message-AMT walk kernels (from their occupancy, set on first use)
     uint64_t n = 0, blob_size = 0;
     DevBuf<uint8_t> arena;
     DevBuf<uint64_t> offsets;

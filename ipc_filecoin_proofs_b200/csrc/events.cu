@@ -17,6 +17,8 @@
 #include <cstring>
 
 #include <chrono>
+#include <cstddef>
+#include <cooperative_groups.h>
 #include "engine.cuh"
 #include "hashes.cuh"
 #include "ipld.cuh"
@@ -27,6 +29,7 @@
 #include "rawcid.cuh"
 
 namespace ipcfp {
+namespace cg = cooperative_groups;
 
 // ------------------------------------------------------------------------------------------ pass 1 / pass 2 kernels (per-receipt code: events_items.cuh)
 // Pass 1 is k_pass1_stage (pass1_stage.cuh).
@@ -53,6 +56,18 @@ __global__ void __launch_bounds__(128) k_pass2(Pass2Args a) {
 
 // ------------------------------------------------------------------------------------------ setup + message AMT walk
 #define IPCFP_MAX_PARENTS 64
+static_assert(2 * IPCFP_MAX_PARENTS <= DENSE_MAX_AMTS, "the dense plan's tables hold every message AMT");
+// What k_setup leaves for the host and the walk, in one device block. The head (everything before the tables) reaches the host
+// in one publish (host words PRO_HOST_WORD ..); the tables stay on the device.
+struct Prologue {
+    uint32_t misc[64 + 2 * IPCFP_MAX_PARENTS];   // [0] receipts-root block, [1] a base-witness CID is missing, [2] any_skip (pass 2), [64 + k] height of AMT k
+    uint64_t amt_count[2 * IPCFP_MAX_PARENTS];   // root.count of AMT k
+    uint64_t t0[4];                              // keccak256(event signature), the Matcher's t0
+    DenseTables plan;                            // the dense walk's plan: ok, rounds, nraw, then the tables
+};
+#define PRO_HOST_WORD 24
+static constexpr uint32_t PRO_HEAD_WORDS = (uint32_t)((offsetof(Prologue, plan) + offsetof(DenseTables, per_amt)) / 8);
+static_assert(PRO_HOST_WORD + PRO_HEAD_WORDS <= 300, "the prologue's head must not reach the sharded protocol's host words");
 struct SetupArgs {
     StoreView store;
     uint32_t n_parents;
@@ -66,42 +81,66 @@ struct SetupArgs {
     unsigned long long* err;
     unsigned long long* txerr;     // message-AMT fault word (tx_err_key)
     // outputs
-    uint32_t* receipts_root_blk;
+    Prologue* pro;
     uint32_t* f_blk; uint32_t* f_meta; uint64_t* f_base;  // initial frontier: one item per message AMT
     unsigned long long* f_count;
-    uint32_t* amt_height;   // per AMT
-    uint64_t* amt_count;    // per AMT (root.count)
-    uint32_t* missing_base; // flag: a base-witness CID is not in the store (→ materialize error)
     const uint8_t* sig;     // event signature bytes (zero padded to a multiple of 8) and the Matcher whose t0 this kernel fills
     uint32_t sig_len;
     Matcher* matcher;
+    // plan_dense: also plan the dense walk (unsharded calls) into pro->plan, against these limits
+    uint32_t plan_dense;
+    uint64_t frontier_cap, max_raw;
 };
+
+// Amtv0::<MessageReceipt>::load(&receipts_root, &rec_receipts) (events/generator.rs:195-196), root validated
+__device__ __forceinline__ void setup_receipts_root(const SetupArgs& a) {
+    const StoreView& s = a.store;
+    int32_t rb = store_lookup(s, a.receipts_root);
+    if (rb < 0) { report_error(a.err, ST_RECEIPTS_ROOT, 0, DC_MISSING, 0); return; }
+    witness_mark(s, a.wbits, (uint32_t)rb);
+    a.pro->misc[0] = (uint32_t)rb;
+    uint32_t len;
+    const uint8_t* p = store_block(s, (uint32_t)rb, len);
+    Rd r(p, len);
+    uint32_t bw, h;
+    uint64_t cnt;
+    amt_root_begin(r, 0, bw, h, cnt);
+    AmtNodeHdr hd;
+    amt_node_begin(r, 3, hd);
+    uint32_t nv = rd_array(r);
+    for (uint32_t v = 0; v < nv && !r.err; v++) parse_receipt(r);
+    amt_node_finish(r, hd, nv, h);
+    if (r.err) report_error(a.err, ST_RECEIPTS_ROOT, 0, DC_DECODE, r.err);
+}
 
 // One-CTA prologue, the independent pieces on different warps so their dependent lookups overlap:
 //   thread 0        Amtv0::<MessageReceipt>::load(&receipts_root) (events/generator.rs:195-196), root validated
 //   threads 32..95  one parent each: TxMeta → BLS / SECP AMT roots (seeds the walk frontier, AMT ordinal 2b + k)
 //   thread 96       keccak256(event_signature) → Matcher.t0 (EventMatcher::new, events/generator.rs:30-35)
 //   threads 128..   base witness marks (parent headers, child header, receipts root, TxMeta blocks)
+//   thread 0, last  (plan_dense) the dense walk's plan from the roots' heights and counts, once every piece above is done
 // Errors go through the atomicMin error word, so the one reported is the one the sequential order meets first.
 __global__ void __launch_bounds__(256) k_setup(SetupArgs a) {
     const StoreView& s = a.store;
     const uint32_t t = threadIdx.x, P = a.n_parents;
+    uint32_t* const amt_height = a.pro->misc + 64;
+    uint64_t* const amt_count = a.pro->amt_count;
     if (t >= 128 && !a.skip_tx) {
         for (uint32_t i = t - 128; i < 2 * P + 2; i += 128) {
             const uint8_t* cid = i < P ? a.parent_cids + 38 * i : (i == P ? a.child_cid : (i == P + 1 ? a.receipts_root : a.txmeta_cids + 38 * (i - P - 2)));
             int32_t b = store_lookup(s, cid);
-            if (b < 0) *a.missing_base = 1; else witness_mark(s, a.wbits, (uint32_t)b);
+            if (b < 0) a.pro->misc[1] = 1; else witness_mark(s, a.wbits, (uint32_t)b);
         }
     }
     if (t == 96) {
         Digest d;
         keccak256(a.sig, a.sig_len, d);
-        a.matcher->t0[0] = d.w[0]; a.matcher->t0[1] = d.w[1]; a.matcher->t0[2] = d.w[2]; a.matcher->t0[3] = d.w[3];
+        for (int k = 0; k < 4; k++) a.matcher->t0[k] = a.pro->t0[k] = d.w[k];
     }
     // TxMeta + message AMT roots (needed for the execution order even when skip_tx). An AMT whose root cannot be loaded keeps
     // a sentinel seed (height / count 0): the walk goes on for the others, and the fault the reference meets FIRST wins the word
     if (t >= 32 && t < 96) for (uint32_t b = t - 32; b < P; b += 64) {
-        for (uint32_t k = 0; k < 2; k++) { a.f_meta[2 * b + k] = AMT_SENTINEL; a.f_blk[2 * b + k] = 0; a.f_base[2 * b + k] = 0; a.amt_height[2 * b + k] = 0; a.amt_count[2 * b + k] = 0; }
+        for (uint32_t k = 0; k < 2; k++) { a.f_meta[2 * b + k] = AMT_SENTINEL; a.f_blk[2 * b + k] = 0; a.f_base[2 * b + k] = 0; amt_height[2 * b + k] = 0; amt_count[2 * b + k] = 0; }
         int32_t tb = store_lookup(s, a.txmeta_cids + 38 * b);
         if (tb < 0) { report_tx_error(a.txerr, 3 * b, 0, 31, DC_MISSING, 0); continue; }
         if (!a.skip_tx) witness_mark(s, a.wbits, (uint32_t)tb);
@@ -127,30 +166,30 @@ __global__ void __launch_bounds__(256) k_setup(SetupArgs a) {
             a.f_blk[amt] = (uint32_t)rb;
             a.f_meta[amt] = make_meta(amt, 1, h);
             a.f_base[amt] = 0;
-            a.amt_height[amt] = h;
-            a.amt_count[amt] = cnt;
+            amt_height[amt] = h;
+            amt_count[amt] = cnt;
         }
     }
+    if (t == 0) {
+        *a.f_count = 2 * P;
+        if (!a.skip_receipts) setup_receipts_root(a);
+    }
+    if (!a.plan_dense) return;
+    __syncthreads();   // heights, counts and every fault of the pieces above are in place
     if (t != 0) return;
-    *a.f_count = 2 * P;
-    if (a.skip_receipts) return;
-    // Amtv0::<MessageReceipt>::load(&receipts_root, &rec_receipts) (events/generator.rs:195-196)
-    int32_t rb = store_lookup(s, a.receipts_root);
-    if (rb < 0) { report_error(a.err, ST_RECEIPTS_ROOT, 0, DC_MISSING, 0); return; }
-    witness_mark(s, a.wbits, (uint32_t)rb);
-    *a.receipts_root_blk = (uint32_t)rb;
-    uint32_t len;
-    const uint8_t* p = store_block(s, (uint32_t)rb, len);
-    Rd r(p, len);
-    uint32_t bw, h;
-    uint64_t cnt;
-    amt_root_begin(r, 0, bw, h, cnt);
-    AmtNodeHdr hd;
-    amt_node_begin(r, 3, hd);
-    uint32_t nv = rd_array(r);
-    for (uint32_t v = 0; v < nv && !r.err; v++) parse_receipt(r);
-    amt_node_finish(r, hd, nv, h);
-    if (r.err) report_error(a.err, ST_RECEIPTS_ROOT, 0, DC_DECODE, r.err);
+    // the whole message list (unsharded): every AMT's range is [0, ∞). The ranges are passed in the slots of per_amt that dense_plan
+    // overwrites with the clipped range of the same AMT (it reads each before it writes it).
+    const uint32_t namt = 2 * P;
+    DenseTables& pl = a.pro->plan;
+    for (uint32_t k = 0; k < namt; k++) { pl.per_amt[2ull * namt + k] = 0; pl.per_amt[3ull * namt + k] = UINT64_MAX; }
+    uint32_t rounds;
+    uint64_t nraw;
+    const bool ok = dense_plan(namt, amt_height, amt_count, pl.per_amt + 2ull * namt, pl.per_amt + 3ull * namt, a.frontier_cap, a.max_raw, sizeof(DenseTables),
+                               pl.fofs, pl.ftot, pl.per_amt, &rounds, &nraw);
+    const bool fault = *(volatile unsigned long long*)a.err != IPCFP_NO_ERROR || *(volatile unsigned long long*)a.txerr != IPCFP_NO_ERROR;
+    pl.rounds = rounds;
+    pl.nraw = nraw;
+    pl.ok = ok && !fault;   // a prologue fault: the general walk finds the fault the reference meets first
 }
 
 // ---- message-AMT walk, general form: kernels (per-item code: walk.cuh) --------------------------------------
@@ -225,17 +264,36 @@ __global__ void __launch_bounds__(TOP_CAP) k_amt_top(ExpandArgs a0, Frontier pin
     }
 }
 
-// n_rounds == 1: any grid. n_rounds > 1: ONE CTA walks several small levels back to back (barrier between levels).
-__global__ void __launch_bounds__(1024) k_amt_dense(DenseArgs a, uint32_t first_round, uint32_t n_rounds) {
-    for (uint32_t rr = 0; rr < n_rounds; rr++) {
-        const uint32_t round = first_round + rr;
-        if (*(volatile uint32_t*)a.fail) return;        // same value in every thread: written before the previous barrier / launch
-        const Frontier in = (round & 1) ? a.pong : a.ping, out = (round & 1) ? a.ping : a.pong;
-        const uint64_t n8 = (uint64_t)a.ftot[round] * 8;
-        for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n8; g += (uint64_t)gridDim.x * blockDim.x)
-            amt_item_dense(a, in, out, round, (uint32_t)(g >> 3), (uint32_t)g & 7);
-        if (n_rounds > 1) { __threadfence(); __syncthreads(); }
+// The dense walk (amt_item_dense, walk.cuh) over the plan in a.tables, in two launches: k_amt_dense walks rounds 0 .. rounds-2 as ONE
+// persistent cooperative grid with grid.sync() between rounds, k_amt_dense_leaf the last round. A level marks the blocks of the children
+// it resolves, so after the first launch every message-AMT block is recorded; the leaf round only writes the raw message list.
+// A plan that is not ok raises `fail` (the host then takes the general walk).
+#define DENSE_THREADS 256
+__global__ void __launch_bounds__(DENSE_THREADS) k_amt_dense(DenseArgs a) {
+    const DenseTables& tb = *a.tables;
+    if (!tb.ok) { if (blockIdx.x == 0 && threadIdx.x == 0) *a.fail = 1; return; }   // the same in every thread: no one waits in grid.sync
+    cg::grid_group grid = cg::this_grid();
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint32_t round = 0; round + 1 < tb.rounds; round++) {
+        // `fail` may rise while the round runs: a thread that sees it skips its items but still meets every grid.sync
+        if (!*(volatile uint32_t*)a.fail) {
+            const Frontier in = (round & 1) ? a.pong : a.ping, out = (round & 1) ? a.ping : a.pong;
+            const uint64_t n8 = (uint64_t)tb.ftot[round] * 8;
+            for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n8; g += stride)
+                amt_item_dense(a, in, out, round, (uint32_t)(g >> 3), (uint32_t)g & 7);
+        }
+        if (round + 2 < tb.rounds) grid.sync();
     }
+}
+__global__ void __launch_bounds__(DENSE_THREADS) k_amt_dense_leaf(DenseArgs a) {
+    const DenseTables& tb = *a.tables;
+    if (!tb.ok) { if (blockIdx.x == 0 && threadIdx.x == 0) *a.fail = 1; return; }
+    if (*(volatile uint32_t*)a.fail) return;
+    const uint32_t round = tb.rounds - 1;
+    const Frontier in = (round & 1) ? a.pong : a.ping, out = (round & 1) ? a.ping : a.pong;
+    const uint64_t n8 = (uint64_t)tb.ftot[round] * 8;
+    for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n8; g += (uint64_t)gridDim.x * blockDim.x)
+        amt_item_dense(a, in, out, round, (uint32_t)(g >> 3), (uint32_t)g & 7);
 }
 
 // first-seen dedup of the raw execution list (events/utils.rs:56-91): hash set keyed by the full
@@ -442,94 +500,119 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     // ---- witness bitmap + setup
     AsyncBuf<uint32_t> wbits((nblk + 31) / 32 + 8, st);
     wbits.zero();
-    const uint32_t namt_max = 2 * td.n_parents;
+    const uint32_t namt = 2 * td.n_parents;   // k_setup seeds one frontier item per message AMT
     const uint64_t cap = 4 * nblk + 1024;
     AsyncBuf<uint32_t> fA_blk(cap, st), fA_meta(cap, st), fB_blk(cap, st), fB_meta(cap, st);
     AsyncBuf<uint64_t> fA_base(cap, st), fB_base(cap, st);
-    AsyncBuf<uint32_t> misc(64 + 2 * IPCFP_MAX_PARENTS, st);
-    AsyncBuf<uint64_t> amt_count(2 * IPCFP_MAX_PARENTS, st);
-    misc.zero();
+    AsyncBuf<Prologue> pro(1, st);
+    pro.zero();
+    uint32_t* const misc = &pro.p->misc[0];
+    const uint32_t frontier_cap = (uint32_t)std::min<uint64_t>(cap, 0xffffffffull);
+    // Every message of a parent block is executed, so no message AMT counts more values than there are receipts: a dense walk of an
+    // unsharded call writes at most n_parents × n_receipts entries (a plan above that goes to the general walk).
+    const uint64_t max_raw_dev = std::min<uint64_t>(8ull * cap, (uint64_t)td.n_parents * td.n_receipts + 1024);
+    const bool force_general = getenv("IPCFP_BFS_GENERAL") != nullptr;   // read per call: tests toggle it
+    // Unsharded calls plan the dense walk on the device (k_setup) and read the prologue back only together with the witness
+    // snapshot's counts. A sharded call needs its share's length on the host before its walk (early H0, below), and the
+    // execution-order-only mode keeps its own sequence: both read the prologue back first (host synchronisation 1).
+    const bool plan_on_device = !sharded && !exo && !force_general;
     SetupArgs sa;
     sa.store = s->view; sa.n_parents = td.n_parents;
     sa.parent_cids = d_cids; sa.txmeta_cids = d_cids + 38ull * td.n_parents;
     sa.child_cid = d_cids + 76ull * td.n_parents; sa.receipts_root = sa.child_cid + 38;
     sa.skip_tx = skip_tx; sa.skip_receipts = exo ? 1 : 0; sa.wbits = wbits.p; sa.err = dw; sa.txerr = dw + 15;
-    sa.receipts_root_blk = misc.p; sa.missing_base = misc.p + 1; sa.amt_height = misc.p + 64;
+    sa.pro = pro.p;
     sa.f_blk = fA_blk.p; sa.f_meta = fA_meta.p; sa.f_base = fA_base.p; sa.f_count = dw + 1;
-    sa.amt_count = amt_count.p;
     sa.sig = d_sig; sa.sig_len = (uint32_t)siglen; sa.matcher = d_matcher;
+    sa.plan_dense = plan_on_device ? 1 : 0; sa.frontier_cap = frontier_cap; sa.max_raw = max_raw_dev;
     k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaMemcpyAsync(hw + 400, d_matcher, 32, cudaMemcpyDeviceToHost, st));   // t0 → hw[400..404)
-    IPCFP_CUDA(cudaMemcpyAsync(hw + 24, misc.p, (64 + 2 * IPCFP_MAX_PARENTS) * 4, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaMemcpyAsync(hw + 128, amt_count.p, 2 * IPCFP_MAX_PARENTS * 8, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 16 * 8, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    // A fault seen by the prologue (TxMeta / AMT root / receipts root) is NOT thrown yet: the reference walks the message AMTs
-    // before it loads the receipts root, and a fault inside an earlier AMT precedes a missing later root — walk first (general
-    // kernels: they cope with the sentinel seeds), then report the first one in the reference's order.
-    const bool early_fault = hw[0] != IPCFP_NO_ERROR || hw[15] != IPCFP_NO_ERROR;
-    memcpy(mh.t0, hw + 400, 32);
-    const uint32_t* misc_h = (const uint32_t*)(hw + 24);
-    const uint32_t receipts_root_blk = misc_h[0];
-    const bool missing_base = misc_h[1] != 0;
-    uint32_t namt = (uint32_t)hw[1];
-    uint32_t last_round = 0;
-    for (uint32_t k = 0; k < namt && k < namt_max; k++) last_round = std::max(last_round, misc_h[64 + k]);
-
-    // ---- message AMT BFS (recording + raw execution list)
     IPCFP_CUDA(cudaEventRecord(s->ev[1], st));
+
+    // the prologue's head as the host reads it (host words PRO_HOST_WORD ..) once publish_prologue and a synchronisation have run
+    const Prologue* ph = (const Prologue*)(hw + PRO_HOST_WORD);
+    auto publish_prologue = [&]() { publish_words_from(s, pro.p, PRO_HOST_WORD, PRO_HEAD_WORDS); };
+    bool early_fault = false, missing_base = false;
+    uint32_t receipts_root_blk = 0, last_round = 0;
     // share of the concatenated ("raw") message list this call walks: everything, or — sharded —
     // [Nraw*lo/N, Nraw*hi/N) expressed as one index range per AMT
     std::vector<uint64_t> h_rng(4 * IPCFP_MAX_PARENTS, 0);
-    const uint64_t nraw_total = shard_amt_ranges(namt, (const uint64_t*)(hw + 128), sharded, lo, hi, td.n_receipts, h_rng.data(),
-                                                 h_rng.data() + 2 * IPCFP_MAX_PARENTS);
+    uint64_t nraw_total = 0;
+    auto read_prologue = [&]() {   // hw[0] / hw[15]: the fault words as the prologue left them
+        early_fault = hw[0] != IPCFP_NO_ERROR || hw[15] != IPCFP_NO_ERROR;
+        memcpy(mh.t0, ph->t0, 32);
+        receipts_root_blk = ph->misc[0];
+        missing_base = ph->misc[1] != 0;
+        last_round = 0;
+        for (uint32_t k = 0; k < namt; k++) last_round = std::max(last_round, ph->misc[64 + k]);
+        nraw_total = shard_amt_ranges(namt, ph->amt_count, sharded, lo, hi, td.n_receipts, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS);
+    };
+
+    // ---- message AMT BFS (recording + raw execution list)
     AsyncBuf<uint32_t> counts(cap + 1024, st);
     AsyncBuf<uint64_t> out_off(cap + 1024, st), scratch(scan_scratch_elems(std::max<uint64_t>(cap, N) + 64) + 64, st);
     unsigned long long *ccount = dw + 1, *ncount = dw + 2, *total_dev = dw + 13;
-    const uint32_t frontier_cap = (uint32_t)std::min<uint64_t>(cap, 0xffffffffull);
     AsyncBuf<RawCid> exec_raw;
     uint64_t raw_cap = 0;
 
-    // ---- (a) dense walk: plan the level layout on the host (see k_amt_dense)
-    const bool force_general = getenv("IPCFP_BFS_GENERAL") != nullptr;   // read per call: tests toggle it
+    // ---- (a) dense walk (see k_amt_dense): planned by k_setup, or here
     DensePlan plan;
-    if (namt > 0 && namt <= namt_max && !force_general && !early_fault)
-        plan = make_dense_plan(namt, misc_h + 64, (const uint64_t*)(hw + 128), h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS, frontier_cap, 8ull * cap,
-                               STAGE_TABLES);
-    AsyncBuf<uint8_t> d_tables;
+    if (!plan_on_device) {
+        publish_words(s, 0, 16);
+        publish_prologue();
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        // A fault seen by the prologue (TxMeta / AMT root / receipts root) is NOT thrown yet: the reference walks the message AMTs
+        // before it loads the receipts root, and a fault inside an earlier AMT precedes a missing later root — walk first (general
+        // kernels: they cope with the sentinel seeds), then report the first one in the reference's order.
+        read_prologue();
+        if (namt > 0 && !force_general && !early_fault)
+            plan = make_dense_plan(namt, ph->misc + 64, ph->amt_count, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS, frontier_cap, 8ull * cap,
+                                   sizeof(DenseTables));
+    }
     AsyncBuf<uint64_t> d_foff;
     AsyncBuf<uint32_t> d_flen;
-    auto run_dense = [&]() {
-        // tables: per_amt (u64) | fofs (u32) | ftot (u32) through the pinned staging block
-        const size_t nb_amt = plan.per_amt.size() * 8, nb_fofs = plan.fofs.size() * 4, nb_ftot = plan.ftot.size() * 4;
-        uint8_t* ht = s->stage.as<uint8_t>() + tables_off;
-        memcpy(ht, plan.per_amt.data(), nb_amt);
-        memcpy(ht + nb_amt, plan.fofs.data(), nb_fofs);
-        memcpy(ht + nb_amt + nb_fofs, plan.ftot.data(), nb_ftot);
-        d_tables.alloc(nb_amt + nb_fofs + nb_ftot + 64, st);
-        IPCFP_CUDA(cudaMemcpyAsync(d_tables.p, ht, nb_amt + nb_fofs + nb_ftot, cudaMemcpyHostToDevice, st));
-        raw_cap = plan.nraw;
+    DenseArgs da;
+    memset(&da, 0, sizeof da);
+    auto run_dense = [&]() {   // rounds 0 .. rounds-2; run_dense_leaf enqueues the last one
+        if (!plan_on_device) {   // the host's plan goes where k_setup writes it for unsharded calls
+            static_assert(sizeof(DenseTables) <= STAGE_TABLES, "the dense plan must fit its staging slot");
+            DenseTables* ht = (DenseTables*)(s->stage.as<uint8_t>() + tables_off);
+            memset(ht, 0, sizeof *ht);
+            ht->ok = 1; ht->rounds = plan.rounds; ht->nraw = plan.nraw;
+            std::copy(plan.per_amt.begin(), plan.per_amt.end(), ht->per_amt);
+            std::copy(plan.fofs.begin(), plan.fofs.end(), ht->fofs);
+            std::copy(plan.ftot.begin(), plan.ftot.end(), ht->ftot);
+            IPCFP_CUDA(cudaMemcpyAsync(&pro.p->plan, ht, sizeof(DenseTables), cudaMemcpyHostToDevice, st));
+        }
+        raw_cap = plan_on_device ? max_raw_dev : plan.nraw;
         exec_raw.alloc(raw_cap + 64, st);
-        exec_raw.zero();   // pool memory is not zeroed: an entry the walk failed to write must never look like a message CID
-        DenseArgs da;
+        // a dense walk that succeeds writes every entry of [0, nraw), and the host reads none of it otherwise. A sharded call's early
+        // exchange reads the list before the host knows whether the walk succeeded: there an entry the walk did not write must never
+        // look like a message CID.
+        if (!plan_on_device) exec_raw.zero();
+        const DenseTables* tb = &pro.p->plan;
         da.store = s->view;
         da.ping = Frontier{fA_blk.p, fA_meta.p, fA_base.p}; da.pong = Frontier{fB_blk.p, fB_meta.p, fB_base.p};
         da.vals = exec_raw.p;
-        const uint64_t* pa = (const uint64_t*)d_tables.p;
-        da.vbase = pa; da.cnt = pa + namt; da.lo = pa + 2ull * namt; da.hi = pa + 3ull * namt;
-        da.fofs = (const uint32_t*)(d_tables.p + nb_amt); da.ftot = (const uint32_t*)(d_tables.p + nb_amt + nb_fofs);
+        da.tables = tb;
+        da.vbase = tb->per_amt; da.cnt = tb->per_amt + namt; da.lo = tb->per_amt + 2ull * namt; da.hi = tb->per_amt + 3ull * namt;
+        da.fofs = tb->fofs; da.ftot = tb->ftot;
         da.namt = namt; da.record = skip_tx ? 0 : 1; da.wbits = wbits.p; da.fail = (uint32_t*)(dw + 14);
+        // frontier items of a round ≥ 1: an AMT holding c values has at most c/8 + 1 nodes on any level
         uint64_t fmax = 1;
-        for (uint32_t r = 0; r < plan.rounds; r++) fmax = std::max<uint64_t>(fmax, plan.ftot[r]);
+        if (plan_on_device) fmax = max_raw_dev / 8 + namt + 8;
+        else for (uint32_t r = 0; r < plan.rounds; r++) fmax = std::max<uint64_t>(fmax, plan.ftot[r]);
         d_foff.alloc(2 * fmax + 8, st); d_flen.alloc(2 * fmax + 8, st);
         da.f_off[0] = d_foff.p; da.f_off[1] = d_foff.p + fmax; da.f_len[0] = d_flen.p; da.f_len[1] = d_flen.p + fmax;
-        uint32_t top = 0;
-        while (top < plan.rounds && plan.ftot[top] <= 1024) top++;
-        if (top) { k_amt_dense<<<1, 1024, 0, st>>>(da, 0, top); IPCFP_LAUNCH_CHECK(); }
-        for (uint32_t r = top; r < plan.rounds; r++) {
-            k_amt_dense<<<div_up((uint64_t)plan.ftot[r] * 8, 256), 256, 0, st>>>(da, r, 1); IPCFP_LAUNCH_CHECK();
+        if (!s->walk_grid) {   // the persistent grid: every CTA of it resident at once
+            int per_sm = 0, sms = 0;
+            IPCFP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_amt_dense, DENSE_THREADS, 0));
+            IPCFP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device));
+            s->walk_grid = (unsigned)std::max(1, per_sm * sms);
         }
+        void* args[] = {&da};
+        IPCFP_CUDA(cudaLaunchCooperativeKernel((const void*)k_amt_dense, s->walk_grid, DENSE_THREADS, args, 0, st)); IPCFP_LAUNCH_CHECK();
     };
+    auto run_dense_leaf = [&]() { k_amt_dense_leaf<<<s->walk_grid, DENSE_THREADS, 0, st>>>(da); IPCFP_LAUNCH_CHECK(); };
 
     // ---- (b) general walk: count → scan → expand per level, any AMT shape, exact errors
     AsyncBuf<uint64_t> d_rng;
@@ -577,8 +660,8 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         }
         // *ccount now holds the number of raw execution entries (k_amt_top leaves it in place as well).
     };
-    bool dense_used = plan.ok;
-    if (dense_used) run_dense(); else run_general();
+    bool dense_used = plan_on_device || plan.ok;   // device plan: whether it is ok is known at the next synchronisation
+    if (dense_used) { run_dense(); run_dense_leaf(); } else run_general();
     IPCFP_CUDA(cudaEventRecord(s->ev[9], st));   // the raw message list of this call is complete (cross-shard exchange waits for it)
     bool xch_early = false;
     if (xch) {
@@ -597,8 +680,10 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     wbuild.by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
     if (!exo) wbuild.snapshot(wbits.p);
     publish_words(s, 0, 18);   // error word, frontier counters (dw[1]/dw[2]), witness counts (dw[8], dw[9]), dense-walk flag (dw[14]), gather split (dw[16], dw[17])
+    if (plan_on_device) publish_prologue();
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (dense_used && hw[14] != 0) {   // the AMTs are not what the dense walk assumes: redo the walk with the general kernels
+    if (plan_on_device) read_prologue();
+    if (dense_used && hw[14] != 0) {   // the AMTs are not what the dense walk assumes (or its plan was not ok): redo the walk with the general kernels
         dense_used = false;
         k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();   // re-seed the frontier (same outputs as before)
         run_general();
@@ -613,7 +698,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         if (!xch) throw Error(IPCFP_ERR_UNSUPPORTED, "unsupported input (message list longer than the walk's capacity)");
         pend_tx = std::min<uint64_t>(pend_tx, tx_err_key(IPCFP_TX_EIDX_NONE, 0, 0, DC_UNSUPPORTED, 1));
     }
-    uint64_t nraw = dense_used ? plan.nraw : std::min<uint64_t>(hw[ccount_idx], raw_cap);
+    uint64_t nraw = dense_used ? (plan_on_device ? ph->plan.nraw : plan.nraw) : std::min<uint64_t>(hw[ccount_idx], raw_cap);
     // early mode: the exchange that is running was fed the PLANNED slice; if the dense walk gave up, the list was rewritten underneath it
     bool xch_stale = xch_early && (!dense_used || nraw != plan.nraw);
     if (xch && !xch_early && (pend_tx != IPCFP_NO_ERROR || pend_err != IPCFP_NO_ERROR)) {
@@ -685,7 +770,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     memset(&box->r, 0, sizeof box->r);
     AsyncBuf<ipcfp_event_proof> d_proofs(n_proofs + 1, st);
     AsyncBuf<uint8_t> d_blob(n_bytes + 16, st);
-    uint32_t* any_skip_dev = misc.p + 2;
+    uint32_t* any_skip_dev = misc + 2;
     if (M) {
         Pass2Args p2;
         p2.store = s->view; p2.store_dev = s->view_dev.p; p2.m_dev = d_matcher; p2.m = mh; p2.events_roots = td.events_roots.p; p2.lo = lo; p2.match_rel = match_rel.p; p2.n_match = M;
@@ -709,7 +794,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     // blocks recorded by pass 2 (receipt paths + events AMTs of the matches): the late part of the witness
     wbuild.finish_enqueue(wbits.p);
     publish_words(s, 0, 20);
-    publish_words_from(s, misc.p, 20, 2);   // misc[2] = any_skip (32-bit words 0..3 land in hw[20..21])
+    publish_words_from(s, misc, 20, 2);   // misc[2] = any_skip (32-bit words 0..3 land in hw[20..21])
     IPCFP_CUDA(cudaStreamSynchronize(st));
     note_errors(hw);
     // base-witness CIDs (parent headers, child header, TxMeta) are only dereferenced by WitnessCollector::materialize

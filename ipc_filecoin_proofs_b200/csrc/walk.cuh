@@ -142,6 +142,7 @@ __device__ __forceinline__ void amt_item_expand(const ExpandArgs& a, uint64_t t,
 // the number of raw entries is known to the host up front. Any surprise (a bitmap that differs, a decode error,
 // a missing block) only raises `fail`: the host then re-walks with the general count → scan → expand kernels
 // above, which handle sparse AMTs and produce the error the reference's sequential walk would report.
+struct DenseTables;
 struct DenseArgs {
     StoreView store;
     Frontier ping, pong;     // round r reads (r even ? ping : pong) and writes the other
@@ -157,6 +158,7 @@ struct DenseArgs {
     uint32_t* fail;
     uint64_t* f_off[2];      // where each frontier item's block is (arena offset, length), by round parity — rounds ≥ 1
     uint32_t* f_len[2];
+    const DenseTables* tables;   // the kernels of events.cu read the plan's ok flag and round count here
 };
 // Eight lanes per node. The walk only has to DETECT anything unusual, not name it, so instead of the sequential
 // strict decoder the node is matched against the one byte layout a bw-3 node the strict decoder accepts can have:
@@ -250,7 +252,70 @@ inline uint64_t shard_amt_ranges(uint32_t namt, const uint64_t* cnts, bool shard
 }
 
 // Level layout of the dense walk (see k_amt_dense): per round and AMT the first frontier slot, per AMT the first value slot.
-// ok == false: the geometry is not one the dense walk takes (the caller uses the general walk).
+// One implementation for both sides: k_setup plans unsharded calls on the device, the host plans sharded ones (and the CPU
+// emulations in tests/host_fuzz). Tables have the fixed capacity below, laid out with stride namt:
+//   fofs[r * namt + k]   first frontier position of AMT k in round r
+//   ftot[r]              frontier items of round r
+//   per_amt              vbase[namt] | cnt[namt] | lo[namt] | hi[namt]
+// Returns ok; false: the geometry is not one the dense walk takes (the caller uses the general walk).
+#define DENSE_MAX_AMTS 128     // 2 message AMTs per parent block, IPCFP_MAX_PARENTS = 64
+#define DENSE_MAX_ROUNDS 21    // heights up to 20
+__host__ __device__ inline bool dense_plan(uint32_t namt, const uint32_t* heights, const uint64_t* cnts, const uint64_t* range_lo, const uint64_t* range_hi,
+                                           uint64_t frontier_cap, uint64_t max_raw, size_t max_table_bytes, uint32_t* fofs, uint32_t* ftot,
+                                           uint64_t* per_amt, uint32_t* rounds_out, uint64_t* nraw_out) {
+    *rounds_out = 0; *nraw_out = 0;
+    bool ok = namt > 0 && namt <= DENSE_MAX_AMTS;
+    uint32_t last_round = 0;
+    // a root whose count exceeds what its height can hold (8^(height+1)) is NOT dense by construction: every per-node check of
+    // amt_item_dense would pass on a completely full tree while count promises more values than exist — the general walk
+    // (which never trusts count) takes those
+    for (uint32_t k = 0; ok && k < namt; k++) {
+        ok = heights[k] <= 20 && cnts[k] <= (1ull << 40) && cnts[k] <= (1ull << (3 * (heights[k] + 1)));
+        last_round = heights[k] > last_round ? heights[k] : last_round;
+    }
+    if (!ok) return false;
+    const uint32_t rounds = last_round + 1;
+    uint64_t vb = 0;
+    for (uint32_t k = 0; k < namt; k++) {
+        const uint64_t c = cnts[k];
+        const uint64_t l = range_lo[k] < c ? range_lo[k] : c;
+        const uint64_t hc = range_hi[k] < c ? range_hi[k] : c, h = hc > l ? hc : l;
+        // an EMPTY share strictly inside an AMT (a shard without a single message): the general walk still follows the
+        // path to that position (its range test is "child begins before hi and ends after lo"); leave that corner to it
+        if (l == h && l > 0) ok = false;
+        per_amt[k] = vb; per_amt[namt + k] = c; per_amt[2ull * namt + k] = l; per_amt[3ull * namt + k] = h;
+        vb += h - l;
+    }
+    for (uint32_t r = 0; ok && r < rounds; r++) {
+        uint64_t run = 0;
+        for (uint32_t k = 0; k < namt; k++) {
+            fofs[(size_t)r * namt + k] = (uint32_t)run;
+            const uint32_t hk = heights[k];
+            if (r > hk) continue;                              // this AMT is shallower: already finished
+            const uint64_t l = per_amt[2ull * namt + k], h = per_amt[3ull * namt + k];
+            const uint32_t sh = 3 * (hk - r + 1);              // a node of this round spans 2^sh indices
+            uint64_t nodes = r == 0 ? 1 : (l < h ? (sh >= 64 ? 1 : ((h - 1) >> sh) - (l >> sh) + 1) : 0);
+            run += nodes;
+            if (run > frontier_cap) { ok = false; break; }
+        }
+        ftot[r] = (uint32_t)run;
+    }
+    const size_t tbytes = (size_t)rounds * namt * 4 + (size_t)rounds * 4 + 4ull * namt * 8 + 64;
+    if (vb > max_raw || tbytes > max_table_bytes) ok = false;
+    *rounds_out = rounds; *nraw_out = vb;
+    return ok;
+}
+
+// a plan as the walk kernels read it from device memory (k_setup writes it, or the host uploads it)
+struct DenseTables {
+    uint32_t ok, rounds;
+    uint64_t nraw;
+    uint64_t per_amt[4 * DENSE_MAX_AMTS];
+    uint32_t fofs[DENSE_MAX_ROUNDS * DENSE_MAX_AMTS];
+    uint32_t ftot[DENSE_MAX_ROUNDS];
+};
+
+// the same plan in host vectors
 struct DensePlan {
     bool ok = false;
     uint32_t rounds = 0;
@@ -261,49 +326,13 @@ struct DensePlan {
 inline DensePlan make_dense_plan(uint32_t namt, const uint32_t* heights, const uint64_t* cnts, const uint64_t* range_lo, const uint64_t* range_hi,
                                  uint64_t frontier_cap, uint64_t max_raw, size_t max_table_bytes) {
     DensePlan plan;
-    bool ok = namt > 0;
-    uint32_t last_round = 0;
-    // a root whose count exceeds what its height can hold (8^(height+1)) is NOT dense by construction: every per-node check of
-    // amt_item_dense would pass on a completely full tree while count promises more values than exist — the general walk
-    // (which never trusts count) takes those
-    for (uint32_t k = 0; ok && k < namt; k++) {
-        ok = heights[k] <= 20 && cnts[k] <= (1ull << 40) && cnts[k] <= (1ull << (3 * (heights[k] + 1)));
-        last_round = std::max(last_round, heights[k]);
-    }
-    if (ok) {
-        plan.rounds = last_round + 1;
-        plan.fofs.assign((size_t)plan.rounds * namt, 0);
-        plan.ftot.assign(plan.rounds, 0);
-        plan.per_amt.assign(4ull * namt, 0);
-        uint64_t vb = 0;
-        for (uint32_t k = 0; k < namt; k++) {
-            const uint64_t c = cnts[k];
-            const uint64_t l = std::min(range_lo[k], c), h = std::max(l, std::min(range_hi[k], c));
-            // an EMPTY share strictly inside an AMT (a shard without a single message): the general walk still follows the
-            // path to that position (its range test is "child begins before hi and ends after lo"); leave that corner to it
-            if (l == h && l > 0) ok = false;
-            plan.per_amt[k] = vb; plan.per_amt[namt + k] = c; plan.per_amt[2ull * namt + k] = l; plan.per_amt[3ull * namt + k] = h;
-            vb += h - l;
-        }
-        plan.nraw = vb;
-        for (uint32_t r = 0; ok && r < plan.rounds; r++) {
-            uint64_t run = 0;
-            for (uint32_t k = 0; k < namt; k++) {
-                plan.fofs[(size_t)r * namt + k] = (uint32_t)run;
-                const uint32_t hk = heights[k];
-                if (r > hk) continue;                              // this AMT is shallower: already finished
-                const uint64_t l = plan.per_amt[2ull * namt + k], h = plan.per_amt[3ull * namt + k];
-                const uint32_t sh = 3 * (hk - r + 1);              // a node of this round spans 2^sh indices
-                uint64_t nodes = r == 0 ? 1 : (l < h ? (sh >= 64 ? 1 : ((h - 1) >> sh) - (l >> sh) + 1) : 0);
-                run += nodes;
-                if (run > frontier_cap) { ok = false; break; }
-            }
-            plan.ftot[r] = (uint32_t)run;
-        }
-        const size_t tbytes = plan.fofs.size() * 4 + plan.ftot.size() * 4 + plan.per_amt.size() * 8 + 64;
-        if (plan.nraw > max_raw || tbytes > max_table_bytes) ok = false;
-    }
-    plan.ok = ok;
+    plan.fofs.assign((size_t)DENSE_MAX_ROUNDS * namt, 0);
+    plan.ftot.assign(DENSE_MAX_ROUNDS, 0);
+    plan.per_amt.assign(4ull * namt, 0);
+    plan.ok = dense_plan(namt, heights, cnts, range_lo, range_hi, frontier_cap, max_raw, max_table_bytes, plan.fofs.data(), plan.ftot.data(),
+                         plan.per_amt.data(), &plan.rounds, &plan.nraw);
+    plan.fofs.resize((size_t)plan.rounds * namt);
+    plan.ftot.resize(plan.rounds);
     return plan;
 }
 
