@@ -10,7 +10,13 @@
 
 namespace ipcfp {
 
-#define REC_CAP 192
+// Distinct blocks one storage proof can record, on the longest path the decode contract (DESIGN.md §3) accepts: the child header and the
+// StateRoot; the actors HAMT at width 5, whose level k reads hash bits [5k, 5k + 5) and so has at most ⌊256/5⌋ = 51 levels; the EVM
+// state; the contract-state block (A1–B2; for C it is the HAMT root itself); a storage HAMT at width 1, at most 256 levels. Wider
+// storage HAMTs are shallower (⌊256/bw⌋ ≤ 256). 2 + 51 + 1 + 1 + 256 = 311, rounded up to a multiple of 32 words.
+#define REC_FIXED_BLOCKS 4          // header, StateRoot, EVM state, contract-state block
+#define REC_CAP 320
+static_assert(REC_CAP >= REC_FIXED_BLOCKS + 256 / 5 + 256 / 1, "a storage proof's recorder must hold the longest accepted path");
 
 // RecordingBlockStore of one proof: per-thread list (for the per-spec Vec<ProofBlock>) + union bitmap
 struct Recorder {
@@ -25,7 +31,7 @@ struct Recorder {
         if (wbits) witness_mark_rank(wbits, rank_of ? rank_of[blk] : blk);   // (the verifiers walk without recording)
         if (!list) return;
         for (uint32_t i = 0; i < n; i++) if (list[i] == blk) return;
-        if (n < REC_CAP) list[n++] = blk; else overflow = true;
+        if (n < REC_CAP) list[n++] = blk; else overflow = true;   // guard only: no accepted input records more than REC_CAP blocks
     }
 };
 struct Fail { uint32_t code; uint32_t detail; };
