@@ -264,6 +264,49 @@ __global__ void __launch_bounds__(TOP_CAP) k_amt_top(ExpandArgs a0, Frontier pin
     }
 }
 
+// The message-AMT fault word ranks a fault by the first index below it in 44 bits (tx_err_key). In an AMT of height ≥ 14 indices
+// reach 8^15 = 2^45 (and wrap past 2^64 at height 21), so two faults of one AMT can tie on that field, or compare wrongly, and the
+// level decides. When the word names a node fault in such an AMT, this kernel (one thread, error path only) walks that AMT in order
+// as Amt::for_each does and overwrites the word with the first fault it meets. Its TxMeta and root header decoded (the word names a
+// node fault), so only the nodes are checked.
+#define TX_KEY_EXACT_HEIGHT 13   // 8^(13+1) = 2^42: every index of an AMT up to this height fits the key's 44-bit base
+__global__ void k_amt_first_fault(StoreView s, const uint8_t* txmeta_cids, uint32_t amt, unsigned long long* word) {
+    const uint32_t eidx = 3 * (amt >> 1) + 1 + (amt & 1);
+    uint32_t len;
+    const uint8_t* p = store_block(s, (uint32_t)store_lookup(s, txmeta_cids + 38 * (amt >> 1)), len);
+    Rd rt(p, len);
+    rd_array_exact(rt, 2);
+    const uint32_t c0 = rd_cid(rt), c1 = rd_cid(rt);
+    uint32_t blk[DENSE_MAX_ROUNDS + 1], next[DENSE_MAX_ROUNDS + 1];   // per depth: the node's block and the next slot to visit
+    blk[0] = (uint32_t)store_lookup(s, p + ((amt & 1) ? c1 : c0));
+    next[0] = 0;
+    uint32_t height = 0;
+    for (int d = 0; d >= 0;) {
+        const uint8_t* q = store_block(s, blk[d], len);
+        Rd r(q, len);
+        if (d == 0) { uint32_t bw; uint64_t c; amt_root_begin(r, 0, bw, height, c); }
+        const uint32_t level = height - (uint32_t)d;
+        AmtNodeHdr h;
+        amt_node_begin(r, 3, h);
+        if (next[d] == 0) {   // entering the node: the whole node is decoded (values included), as the reference's load does
+            const uint32_t nv = rd_array(r);
+            for (uint32_t v = 0; v < nv && !r.err; v++) (void)rd_cid(r);
+            amt_node_finish(r, h, nv, level);
+            if (r.err) { *word = tx_err_key(eidx, 0, level, DC_DECODE, r.err); return; }
+        }
+        const uint32_t bm8 = (uint32_t)h.bm.b0 & 0xffu & ~((1u << next[d]) - 1u);
+        if (!h.nl || !bm8 || next[d] >= 8) { d--; continue; }
+        const uint32_t slot = (uint32_t)__ffs(bm8) - 1;
+        next[d] = slot + 1;
+        const uint32_t rank = (uint32_t)__popc((uint32_t)h.bm.b0 & ((1u << slot) - 1u));
+        const int32_t child = store_lookup(s, q + h.links_off + 43 * rank + 5);
+        if (child < 0) { *word = tx_err_key(eidx, 0, level - 1, DC_MISSING, 0); return; }
+        d++;
+        blk[d] = (uint32_t)child;
+        next[d] = 0;
+    }
+}
+
 // The dense walk (amt_item_dense, walk.cuh) over the plan in a.tables, in two launches: k_amt_dense walks rounds 0 .. rounds-2 as ONE
 // persistent cooperative grid with grid.sync() between rounds, k_amt_dense_leaf the last round. A level marks the blocks of the children
 // it resolves, so after the first launch every message-AMT block is recorded; the leaf round only writes the raw message list.
@@ -614,51 +657,86 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     };
     auto run_dense_leaf = [&]() { k_amt_dense_leaf<<<s->walk_grid, DENSE_THREADS, 0, st>>>(da); IPCFP_LAUNCH_CHECK(); };
 
-    // ---- (b) general walk: count → scan → expand per level, any AMT shape, exact errors
+    // ---- (b) general walk: count → scan → expand per level, any AMT shape, exact errors. It is the fallback, and it sizes every
+    // buffer by what it walks rather than by the store: each parent block's AMTs are walked on their own, so parents that share their
+    // messages need a frontier per parent while the store holds those nodes once. Below the fused rounds it synchronises once per level
+    // and allocates that level's output from the exact total its scan computed.
     AsyncBuf<uint64_t> d_rng;
+    AsyncBuf<uint32_t> g_blk[2], g_meta[2];
+    AsyncBuf<uint64_t> g_base[2];
+    auto ensure_scratch = [&](uint64_t n) {   // scan scratch for n items
+        if (scratch.n < scan_scratch_elems(n + 64) + 64) scratch.alloc(scan_scratch_elems(n + 64) + 64, st);
+    };
     auto run_general = [&]() {
         d_rng.alloc(4 * IPCFP_MAX_PARENTS, st);
         IPCFP_CUDA(cudaMemcpyAsync(d_rng.p, h_rng.data(), h_rng.size() * 8, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        Frontier fcur{fA_blk.p, fA_meta.p, fA_base.p}, fnxt{fB_blk.p, fB_meta.p, fB_base.p};
+        auto ensure_g = [&](int i, uint64_t n) {
+            if (g_blk[i].n < n) { g_blk[i].alloc(n, st); g_meta[i].alloc(n, st); g_base[i].alloc(n, st); }
+        };
+        auto gview = [&](int i) { return Frontier{g_blk[i].p, g_meta[i].p, g_base[i].p}; };
+        // the fused rounds' last output can be 8 × TOP_CAP items however small the store is: both ping-pong buffers hold that much,
+        // and the seeds k_setup wrote move into the first
+        ensure_g(0, 8 * TOP_CAP); ensure_g(1, 8 * TOP_CAP);
+        IPCFP_CUDA(cudaMemcpyAsync(g_blk[0].p, fA_blk.p, namt * 4ull, cudaMemcpyDeviceToDevice, st));
+        IPCFP_CUDA(cudaMemcpyAsync(g_meta[0].p, fA_meta.p, namt * 4ull, cudaMemcpyDeviceToDevice, st));
+        IPCFP_CUDA(cudaMemcpyAsync(g_base[0].p, fA_base.p, namt * 8ull, cudaMemcpyDeviceToDevice, st));
+        int cur = 0;   // g buffer holding the frontier of `round`
         ccount = dw + 1; ncount = dw + 2;
         ExpandArgs ea;
         ea.store = s->view; ea.last_round = last_round; ea.record = skip_tx ? 0 : 1; ea.wbits = wbits.p; ea.err = dw + 15;
-        ea.vals = nullptr; ea.cap = frontier_cap;
+        ea.vals = nullptr; ea.cap = 8 * TOP_CAP;
         ea.rlo = d_rng.p; ea.rhi = d_rng.p + 2 * IPCFP_MAX_PARENTS;
-        // static frontier bound per round: namt * 8^round
-        auto bound_of = [&](uint32_t round) { uint64_t b = namt; for (uint32_t k = 0; k < round && b <= cap; k++) b *= 8; return std::min<uint64_t>(b, cap); };
-        auto alloc_vals = [&]() {
-            raw_cap = std::min<uint64_t>(bound_of(last_round) * 8, 8 * cap);
+        auto alloc_vals = [&](uint64_t n) {
+            raw_cap = n;
             exec_raw.alloc(raw_cap + 64, st);
             exec_raw.zero();
             ea.vals = exec_raw.p;
         };
-        // fused single-CTA rounds while the static bound fits one CTA
+        // fused single-CTA rounds while the static frontier bound namt · 8^round fits one CTA
+        auto bound_of = [&](uint32_t round) { uint64_t b = namt; for (uint32_t k = 0; k < round && b <= TOP_CAP; k++) b *= 8; return b; };
         uint32_t top_rounds = 0;
         while (top_rounds <= last_round && bound_of(top_rounds) <= TOP_CAP) top_rounds++;
         uint32_t round = 0;
         if (top_rounds) {
-            if (top_rounds > last_round) alloc_vals();  // the last round is inside the fused kernel
+            if (top_rounds > last_round) alloc_vals(bound_of(last_round) * 8);  // the last round is inside the fused kernel
             ExpandArgs a0 = ea;
-            a0.in = fcur; a0.in_count = ccount; a0.out = fnxt; a0.round = 0; a0.out_off = out_off.p;
-            k_amt_top<<<1, TOP_CAP, 0, st>>>(a0, fcur, fnxt, ccount, 0, top_rounds, out_off.p); IPCFP_LAUNCH_CHECK();
-            if (top_rounds & 1) std::swap(fcur, fnxt);
+            a0.in = gview(0); a0.in_count = ccount; a0.out = gview(1); a0.round = 0; a0.out_off = out_off.p;
+            k_amt_top<<<1, TOP_CAP, 0, st>>>(a0, gview(0), gview(1), ccount, 0, top_rounds, out_off.p); IPCFP_LAUNCH_CHECK();
+            cur = top_rounds & 1;
             round = top_rounds;
         }
+        if (round > last_round) return;   // *ccount holds the number of raw execution entries
+        publish_words(s, (uint32_t)(ccount - dw), 1);
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        uint64_t items = hw[ccount - dw];
         for (; round <= last_round; round++) {
-            uint64_t items = bound_of(round);
-            if (round == last_round) alloc_vals();
-            unsigned grid = div_up(std::max<uint64_t>(items, 1), 128);
-            k_amt_count<<<grid, 128, 0, st>>>(s->view, fcur, ccount, round, last_round, ea.cap, counts.p, ea.rlo, ea.rhi); IPCFP_LAUNCH_CHECK();
-            exclusive_scan_u32(counts.p, out_off.p, (uint64_t)grid * 128, (uint64_t*)total_dev, scratch.p, st);
+            const uint64_t slots = (uint64_t)div_up(std::max<uint64_t>(items, 1), 128) * 128;
+            if (counts.n < slots) { counts.alloc(slots, st); out_off.alloc(slots, st); }
+            ensure_scratch(slots);
+            k_amt_count<<<(unsigned)(slots / 128), 128, 0, st>>>(s->view, gview(cur), ccount, round, last_round, (uint32_t)items, counts.p, ea.rlo, ea.rhi);
+            IPCFP_LAUNCH_CHECK();
+            exclusive_scan_u32(counts.p, out_off.p, slots, (uint64_t*)total_dev, scratch.p, st);
+            publish_words(s, (uint32_t)(total_dev - dw), 1);
+            IPCFP_CUDA(cudaStreamSynchronize(st));
+            const uint64_t total = hw[total_dev - dw];
+            if (round == last_round) alloc_vals(total);   // before `a` copies ea.vals
             ExpandArgs a = ea;
-            a.in = fcur; a.in_count = ccount; a.out = fnxt; a.round = round; a.out_off = out_off.p;
+            a.in = gview(cur); a.in_count = ccount; a.round = round; a.out_off = out_off.p; a.out = gview(cur ^ 1);
+            a.cap = (uint32_t)items;   // clamps the input count; every output position is below `total`
+            if (round < last_round) {
+                // a level of 2^32 nodes is 64 GB of frontier alone: device memory runs out before this refuses anything
+                if (std::max(total, items) >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "message-AMT walk: a level of 2^32 nodes or more");
+                ensure_g(cur ^ 1, std::max(total, items) + 1);
+                a.out = gview(cur ^ 1);
+                a.cap = (uint32_t)(std::max(total, items) + 1);
+                cur ^= 1;
+            }
             k_amt_expand<<<div_up(std::max<uint64_t>(items, 1) * 8, 128), 128, 0, st>>>(a, counts.p, ncount, total_dev); IPCFP_LAUNCH_CHECK();
-            std::swap(fcur, fnxt);
             std::swap(ccount, ncount);
+            items = total;
         }
-        // *ccount now holds the number of raw execution entries (k_amt_top leaves it in place as well).
+        // *ccount now holds the number of raw execution entries.
     };
     bool dense_used = plan_on_device || plan.ok;   // device plan: whether it is ok is known at the next synchronisation
     if (dense_used) { run_dense(); run_dense_leaf(); } else run_general();
@@ -693,6 +771,19 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         IPCFP_CUDA(cudaStreamSynchronize(st));
     }
     const uint32_t ccount_idx = (uint32_t)(ccount - dw);
+    if (!sharded && hw[15] != IPCFP_NO_ERROR) {
+        // a node fault (level < 31) in a message AMT tall enough for its indices to outgrow the key: resolve it in order
+        const uint64_t key = hw[15];
+        const uint32_t eidx = (uint32_t)(key >> 56), level = 31u - ((uint32_t)(key >> 7) & 31u);
+        if (eidx != IPCFP_TX_EIDX_NONE && eidx % 3 != 0 && level < 31) {
+            const uint32_t amt = 2 * (eidx / 3) + eidx % 3 - 1;
+            if (ph->misc[64 + amt] > TX_KEY_EXACT_HEIGHT) {
+                k_amt_first_fault<<<1, 1, 0, st>>>(s->view, sa.txmeta_cids, amt, dw + 15); IPCFP_LAUNCH_CHECK();
+                publish_words(s, 15, 1);
+                IPCFP_CUDA(cudaStreamSynchronize(st));
+            }
+        }
+    }
     note_errors(hw);
     if (!dense_used && hw[ccount_idx] > raw_cap) {
         if (!xch) throw Error(IPCFP_ERR_UNSUPPORTED, "unsupported input (message list longer than the walk's capacity)");
@@ -717,6 +808,9 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
     unsigned long long* n_exec_dev = dw + 3;
     if (sharded) IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));   // execution order is resolved across ranks by the caller
     else if (nraw) {
+        // positions in the list are 32-bit (dedup table, exec_idx): 2^32 entries are 160 GB of message CIDs, past device memory
+        if (nraw >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "message list of 2^32 entries or more");
+        ensure_scratch((nraw + 31) / 32);   // the general walk's list can outgrow the scratch sized for the store and the receipts
         uint64_t slots = 64;
         while (slots < 2 * nraw) slots <<= 1;
         AsyncBuf<unsigned long long> dtab(slots, st);

@@ -18,7 +18,8 @@ __device__ __forceinline__ uint32_t make_meta(uint32_t amt, uint32_t is_root, ui
 struct Frontier { uint32_t* blk; uint32_t* meta; uint64_t* base; };
 
 // slots (children, or values at level 0) of a node at `base` whose index range intersects [rlo, rhi):
-// the share of the message AMTs a shard walks (all ones when not sharded)
+// the share of the message AMTs a shard walks (all ones when not sharded). rhi = 2^64 − 1 is unbounded: an index that
+// saturates there (the top of a height-21 AMT) still belongs to the call that owns the AMT's tail.
 __device__ __forceinline__ uint32_t slot_mask(uint64_t base, uint32_t level, uint64_t rlo, uint64_t rhi) {
     uint64_t sub = pow_sat(3, level);
     uint32_t m = 0;
@@ -27,7 +28,7 @@ __device__ __forceinline__ uint32_t slot_mask(uint64_t base, uint32_t level, uin
         uint64_t off = sub == ~0ull ? (sl ? ~0ull : 0) : sub * sl;
         uint64_t cb = base + off < base ? ~0ull : base + off;
         uint64_t ce = cb + sub < cb ? ~0ull : cb + sub;
-        if (cb < rhi && ce > rlo) m |= 1u << sl;
+        if ((rhi == ~0ull || cb < rhi) && ce > rlo) m |= 1u << sl;
     }
     return m;
 }

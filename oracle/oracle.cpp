@@ -438,14 +438,14 @@ template <class V> struct Amt {
         const uint32_t width = 1u << bw;
         if (nd.leaf) {
             for (uint32_t i = 0; i < width; i++)
-                if (nd.vals.size() && nd.vals[i] && base + i >= lo && base + i < hi) f(base + i, *nd.vals[i]);
+                if (nd.vals.size() && nd.vals[i] && base + i >= lo && (hi == UINT64_MAX || base + i < hi)) f(base + i, *nd.vals[i]);
             return;
         }
         uint64_t sub = pow_sat((uint64_t)bw, h);
         for (uint32_t i = 0; i < width; i++) {
             if (!nd.links[i]) continue;
             uint64_t a = base + (uint64_t)i * sub, b = (sub == UINT64_MAX) ? UINT64_MAX : a + sub;
-            if (!(a < hi && b > lo)) continue;
+            if (!((hi == UINT64_MAX || a < hi) && b > lo)) continue;   // hi = 2^64 − 1: unbounded (the engine's slot_mask)
             AmtNode<V> ch = load_node(*nd.links[i], h - 1);
             for_each_range_node(ch, h - 1, a, lo, hi, f);
         }

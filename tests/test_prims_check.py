@@ -22,13 +22,12 @@ def _nvflags():
 
 
 @pytest.fixture(scope="module")
-def prims_check_exe():
+def prims_check_exe(tmp_path_factory):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
-    build = os.path.join(ROOT, "tests", "gpu_prims", "_build")
-    os.makedirs(build, exist_ok=True)
-    exe = os.path.join(build, "prims_check")
+    # built outside the source tree, which may be read-only
+    exe = str(tmp_path_factory.mktemp("prims_check") / "prims_check")
     cc = subprocess.run([nvcc, *_nvflags(), "-o", exe, SRC, PRIMS], cwd=ROOT, capture_output=True, text=True)
     assert cc.returncode == 0, cc.stderr[-3000:]
     return exe
