@@ -4,7 +4,7 @@ NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CSRC      := ipc_filecoin_proofs_b200/csrc
 NVFLAGS   := -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr
-CU_SRCS   := $(CSRC)/store.cu $(CSRC)/events.cu $(CSRC)/storage.cu $(CSRC)/witness.cu $(CSRC)/prims.cu $(CSRC)/parallel.cu $(CSRC)/verify.cu $(CSRC)/json.cu $(CSRC)/json_parse.cu $(CSRC)/capi.cu
+CU_SRCS   := $(CSRC)/store.cu $(CSRC)/events.cu $(CSRC)/storage.cu $(CSRC)/witness.cu $(CSRC)/prims.cu $(CSRC)/parallel.cu $(CSRC)/verify.cu $(CSRC)/json.cu $(CSRC)/json_parse.cu $(CSRC)/rpc_json.cu $(CSRC)/capi.cu
 CU_OBJS   := $(CU_SRCS:.cu=.o)
 CU_HDRS   := $(wildcard $(CSRC)/*.cuh) include/ipcfp.h
 LIB       := ipc_filecoin_proofs_b200/libipcfp.so
@@ -18,7 +18,10 @@ $(CSRC)/%.o: $(CSRC)/%.cu $(CU_HDRS) Makefile
 $(CSRC)/bundle_json.o: $(CSRC)/bundle_json.cpp include/ipcfp.h
 	$(CXX) -O2 -std=c++17 -fPIC -c $< -o $@
 
-$(CSRC)/bundle_parse.o: $(CSRC)/bundle_parse.cpp include/ipcfp.h
+$(CSRC)/bundle_parse.o: $(CSRC)/bundle_parse.cpp $(CSRC)/json_value.h include/ipcfp.h
+	$(CXX) -O2 -std=c++17 -fPIC -c $< -o $@
+
+$(CSRC)/rpc_parse.o: $(CSRC)/rpc_parse.cpp $(CSRC)/json_value.h include/ipcfp.h
 	$(CXX) -O2 -std=c++17 -fPIC -c $< -o $@
 
 # HIDE_INTERNALS=1 links with csrc/exports.map: only ipcfp_* stay in the dynamic symbol table (what a C-ABI library should export).
@@ -29,8 +32,10 @@ LIB_LDFLAGS := -Xlinker --version-script=$(CSRC)/exports.map
 endif
 LIB_OUT ?= $(LIB)
 
-$(LIB_OUT): $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o $(CSRC)/exports.map
-	$(NVCC) -shared -gencode arch=compute_90a,code=sm_90a $(LIB_LDFLAGS) -o $@ $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o -lcudart -ldl
+HOST_OBJS := $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o $(CSRC)/rpc_parse.o
+
+$(LIB_OUT): $(CU_OBJS) $(HOST_OBJS) $(CSRC)/exports.map
+	$(NVCC) -shared -gencode arch=compute_90a,code=sm_90a $(LIB_LDFLAGS) -o $@ $(CU_OBJS) $(HOST_OBJS) -lcudart -ldl
 
 synth/libipcfp_synth.so: synth/synth.cpp synth/synth.h synth/cpu_crypto.h
 	$(CXX) -O2 -std=c++17 -fPIC -shared -pthread -o $@ synth/synth.cpp
@@ -39,10 +44,10 @@ oracle/liboracle.so: oracle/oracle.cpp oracle/oracle.h synth/cpu_crypto.h includ
 	$(CXX) -O2 -std=c++17 -fPIC -shared -pthread -o $@ oracle/oracle.cpp
 
 clean:
-	rm -f $(CU_OBJS) $(CSRC)/bundle_json.o $(CSRC)/bundle_parse.o $(LIB) synth/libipcfp_synth.so oracle/liboracle.so
+	rm -f $(CU_OBJS) $(HOST_OBJS) $(LIB) synth/libipcfp_synth.so oracle/liboracle.so
 
 # The host-compiled device headers (tests/host_fuzz) and the JSON parser under AddressSanitizer + UBSan (DESIGN.md §7.12)
 sanitize:
-	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py -q
+	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py tests/test_rpc_json_host.py -q
 
 .PHONY: all clean sanitize

@@ -290,6 +290,60 @@ ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tip
  * CUDA events or order their own device work after the engine's. */
 void* ipcfp_store_stream(ipcfp_store* s);
 
+/* ------------------------------------------------------------------------------------------
+ * The tipset straight from the Lotus JSON-RPC results (src/client/types.rs:11-58): `parent` and `child` are the `result` values of
+ * ChainGetTipSetByHeight (ApiTipset), `receipts` the `result` of ChainGetParentReceipts (Vec<ApiReceipt>) — the values only, not the
+ * {"jsonrpc",…} envelope. Not NUL-terminated: each text is exactly its length in bytes.
+ *
+ * ipcfp_tipset_desc_from_json (host C++, no device) reads them as serde_json::from_str does, then builds the descriptor as
+ * extract_child_info / collect_base_witness / find_matching_events do (events/generator.rs:112-145, :199-211):
+ *   parent_epoch / child_epoch       parent.Height / child.Height
+ *   parent_cids / parent_txmeta_cids parent.Cids[i]["/"] / parent.Blocks[i].Messages["/"]
+ *   child_cid                        child.Cids[0]["/"]
+ *   receipts_root                    child.Blocks[0].ParentMessageReceipts["/"]
+ *   child_parent_state_root          child.Blocks[0].ParentStateRoot["/"]
+ *   events_roots / has_events_root   receipts[i].EventsRoot["/"]; a missing or null EventsRoot is None (38 zero bytes, flag 0)
+ * serde's derive rules: PascalCase keys, compared after unescaping; unknown keys are skipped (their values must still be valid JSON);
+ * a repeated known key is an error. Required: ApiTipset {Cids, Blocks, Height}, ApiBlockHeader {Miner, Parents, ParentStateRoot,
+ * ParentMessageReceipts, Messages, Height}, ApiReceipt {ExitCode (u32), Return (string, never decoded), GasUsed (u64)}, CIDMap {"/"}.
+ * Integers are plain JSON integers in range ("-0", "1.0", "1e3" are not).
+ * Documented deviation: serde's derive also accepts a struct written as a JSON array of its fields; Lotus never writes that form, and
+ * it is refused here with IPCFP_ERR_UNSUPPORTED.
+ * Statuses: malformed JSON, a wrong type, a missing or repeated field, an integer out of range, an invalid CID string →
+ * IPCFP_ERR_INVALID_ARG; a valid CID that is not a 38-byte binary CID or not spelled "b…" (base32) → IPCFP_ERR_UNSUPPORTED (the rule of
+ * ipcfp_bundle_from_json); an empty child Cids or Blocks → IPCFP_ERR_INVALID_ARG (the reference panics on the index); parent Cids and
+ * Blocks of different lengths → IPCFP_ERR_UNSUPPORTED (the descriptor has one n_parents). The texts are checked in the order parent,
+ * child, receipts; within an ApiTipset the structure first, then its CIDs. ipcfp_last_error_index() is the receipt's position for a
+ * fault inside one element of the list (its JSON, its fields, its CID), UINT64_MAX for any other fault (the list's brackets and commas,
+ * trailing bytes, the tipset texts). *out is released with ipcfp_parsed_tipset_free.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ipcfp_parsed_tipset {
+    ipcfp_tipset_desc desc;   /* its arrays are owned by the object */
+} ipcfp_parsed_tipset;
+ipcfp_status ipcfp_tipset_desc_from_json(const char* parent, uint64_t parent_len, const char* child, uint64_t child_len, const char* receipts,
+                                         uint64_t receipts_len, ipcfp_parsed_tipset** out);
+void ipcfp_parsed_tipset_free(ipcfp_parsed_tipset* p);
+/* The same texts straight to a device-resident tipset, for every _resident / _sharded call. The result, status and index are in every
+ * case those of ipcfp_tipset_desc_from_json followed by ipcfp_tipset_upload. The two ApiTipset texts are read on the host. The receipt
+ * list is parsed on the device when it is in canonical form — no whitespace, every element exactly
+ *   {"ExitCode":<u32>,"Return":"<base64 characters and '='>","GasUsed":<u64>,"EventsRoot":null|{"/":"b<61 base32 characters>"}}
+ * — with the events roots written straight into the tipset's device arrays. Any other text (whitespace, other key orders, unknown or
+ * missing keys, escapes, other CID spellings, texts of 4 GiB or more, and every invalid text) goes through ipcfp_tipset_desc_from_json
+ * instead. ipcfp_tipset_describe tells which path ran. */
+ipcfp_status ipcfp_tipset_upload_json(ipcfp_store* s, const char* parent, uint64_t parent_len, const char* child, uint64_t child_len,
+                                      const char* receipts, uint64_t receipts_len, ipcfp_tipset** out);
+/* Read a resident tipset back: its descriptor — the host copies it holds; with with_events_roots != 0 also events_roots /
+ * has_events_root, copied back from the device on the first such request (else those two are NULL) — which the host renderers and the
+ * verifiers take, and how it was built. Pointers stay valid until ipcfp_tipset_free. */
+typedef struct ipcfp_tipset_info {
+    ipcfp_tipset_desc desc;
+    uint32_t parsed_on_device;   /* 1: the receipt list was parsed on the device; 0: ipcfp_tipset_upload or the host parser     */
+    float ms_parse;              /* ipcfp_tipset_upload_json: wall time of the receipt list's parse, its copy to the device included; 0 otherwise */
+    float ms_kernels;            /* device parse only: time of its kernels (CUDA events on the store's stream); 0 otherwise     */
+    uint32_t _pad;
+} ipcfp_tipset_info;
+ipcfp_status ipcfp_tipset_describe(ipcfp_tipset* t, int with_events_roots, ipcfp_tipset_info* out);
+
 /* read_storage_slot (src/proofs/storage/decode.rs:36-97), batched over k slot keys against one
  * contract_state root, with a RecordingBlockStore-equivalent witness. */
 ipcfp_status ipcfp_read_storage_slots(ipcfp_store* s, const uint8_t contract_state_root[IPCFP_CID_LEN],

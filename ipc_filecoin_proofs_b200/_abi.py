@@ -151,6 +151,47 @@ class ParsedBundleC(C.Structure):
     ]
 
 
+class ParsedTipsetC(C.Structure):
+    """ipcfp_parsed_tipset (ipcfp_tipset_desc_from_json)."""
+    _fields_ = [("desc", TipsetDesc)]
+
+
+class TipsetInfoC(C.Structure):
+    """ipcfp_tipset_info (ipcfp_tipset_describe)."""
+    _fields_ = [("desc", TipsetDesc), ("parsed_on_device", C.c_uint32), ("ms_parse", C.c_float), ("ms_kernels", C.c_float),
+                ("_pad", C.c_uint32)]
+
+
+@dataclass
+class TipsetInfoPy:
+    """A tipset descriptor read back from the C ABI, with the attribute names of synth.Tipset (so make_tipset_desc takes it)."""
+    parent_epoch: int
+    child_epoch: int
+    n_parents: int
+    parent_cids: np.ndarray          # (n_parents, 38)
+    parent_txmeta_cids: np.ndarray   # (n_parents, 38)
+    child_cid: np.ndarray            # (38,)
+    receipts_root: np.ndarray        # (38,)
+    parent_state_root: np.ndarray    # (38,) or None
+    n_receipts: int
+    events_roots: np.ndarray         # (n_receipts, 38), or None when not read back
+    has_events_root: np.ndarray      # (n_receipts,), or None when not read back
+    parsed_on_device: bool = False
+    ms_parse: float = 0.0
+    ms_kernels: float = 0.0
+
+
+def tipset_info_from_c(d, parsed_on_device=0, ms_parse=0.0, ms_kernels=0.0):
+    P, N = int(d.n_parents), int(d.n_receipts)
+    roots = _arr(d.events_roots, N * CID_LEN, np.uint8).reshape(N, CID_LEN) if d.events_roots or not N else None
+    has = _arr(d.has_events_root, N, np.uint8) if d.has_events_root or not N else None
+    return TipsetInfoPy(int(d.parent_epoch), int(d.child_epoch), P, _arr(d.parent_cids, P * CID_LEN, np.uint8).reshape(P, CID_LEN),
+                        _arr(d.parent_txmeta_cids, P * CID_LEN, np.uint8).reshape(P, CID_LEN), _arr(d.child_cid, CID_LEN, np.uint8),
+                        _arr(d.receipts_root, CID_LEN, np.uint8),
+                        _arr(d.child_parent_state_root, CID_LEN, np.uint8) if d.child_parent_state_root else None, N, roots, has,
+                        bool(parsed_on_device), float(ms_parse), float(ms_kernels))
+
+
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
 TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
 

@@ -44,7 +44,8 @@ EXPORTS = [
     "ipcfp_comm_unique_id", "ipcfp_comm_init", "ipcfp_comm_destroy", "ipcfp_generate_event_proof_sharded",
     "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
     "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
-    "ipcfp_generate_proof_bundle_resident",
+    "ipcfp_generate_proof_bundle_resident", "ipcfp_tipset_desc_from_json", "ipcfp_parsed_tipset_free", "ipcfp_tipset_upload_json",
+    "ipcfp_tipset_describe",
 ]
 
 
@@ -147,6 +148,15 @@ def lib():
         L.ipcfp_verify_bundle_json.argtypes = [C.c_char_p, C.c_uint64, C.c_int, A.TrustedParentFn, A.TrustedChildFn, C.c_void_p, C.c_void_p,
                                                C.POINTER(C.POINTER(A.BundleVerdictC))]
         L.ipcfp_bundle_verdict_free.argtypes = [C.POINTER(A.BundleVerdictC)]
+        L.ipcfp_tipset_desc_from_json.restype = C.c_int32
+        L.ipcfp_tipset_desc_from_json.argtypes = [C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64,
+                                                  C.POINTER(C.POINTER(A.ParsedTipsetC))]
+        L.ipcfp_parsed_tipset_free.argtypes = [C.POINTER(A.ParsedTipsetC)]
+        L.ipcfp_tipset_upload_json.restype = C.c_int32
+        L.ipcfp_tipset_upload_json.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64,
+                                               C.POINTER(C.c_void_p)]
+        L.ipcfp_tipset_describe.restype = C.c_int32
+        L.ipcfp_tipset_describe.argtypes = [C.c_void_p, C.c_int, C.POINTER(A.TipsetInfoC)]
         _lib = L
     return _lib
 
@@ -316,6 +326,15 @@ class BlockStore:
         """ipcfp_tipset_upload: the tipset's descriptor on the device, for any number of _resident calls. close() releases it."""
         return ResidentTipset(self, ts)
 
+    def upload_tipset_json(self, parent_text, child_text, receipts_text):
+        """ipcfp_tipset_upload_json: the tipset straight from the Lotus JSON-RPC results — the ApiTipset of the parent and of the child
+        (ChainGetTipSetByHeight) and the receipt list (ChainGetParentReceipts), each the `result` value as str or bytes. The receipt list is
+        parsed on the device when it is canonical. Returns a ResidentTipset; failures raise IpcfpError (status, receipt index)."""
+        p, c, r = (_text(x) for x in (parent_text, child_text, receipts_text))
+        h = C.c_void_p()
+        _check(lib().ipcfp_tipset_upload_json(self._h, p, len(p), c, len(c), r, len(r), C.byref(h)))
+        return ResidentTipset(self, None, h)
+
     def generate_proof_bundle_resident(self, tip, storage_specs, event_specs, flags=0):
         """ipcfp_generate_proof_bundle_resident against a ResidentTipset of this store. flags: WITNESS_BY_REFERENCE, RESULT_JSON."""
         sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
@@ -341,12 +360,20 @@ class BlockStore:
 class ResidentTipset:
     """A tipset descriptor uploaded to a store's device (ipcfp_tipset_upload / ipcfp_tipset_free). Valid while its store lives."""
 
-    def __init__(self, store, ts):
-        d, keep = A.make_tipset_desc(ts)
-        h = C.c_void_p()
-        _check(lib().ipcfp_tipset_upload(store._h, C.byref(d), C.byref(h)))
-        self._h = h
+    def __init__(self, store, ts, handle=None):
+        if handle is None:
+            d, keep = A.make_tipset_desc(ts)
+            handle = C.c_void_p()
+            _check(lib().ipcfp_tipset_upload(store._h, C.byref(d), C.byref(handle)))
+        self._h = handle
         self.store = store
+
+    def describe(self, with_events_roots=True):
+        """ipcfp_tipset_describe → A.TipsetInfoPy: the descriptor the tipset holds (events roots copied back from the device when asked),
+        which path parsed its receipt list and how long that took."""
+        info = A.TipsetInfoC()
+        _check(lib().ipcfp_tipset_describe(self._h, 1 if with_events_roots else 0, C.byref(info)))
+        return A.tipset_info_from_c(info.desc, info.parsed_on_device, info.ms_parse, info.ms_kernels)
 
     def close(self):
         if self._h:
@@ -358,6 +385,23 @@ class ResidentTipset:
             self.close()
         except Exception:
             pass
+
+
+def _text(x):
+    return x.encode() if isinstance(x, str) else x if isinstance(x, bytes) else bytes(x)
+
+
+def tipset_desc_from_json(parent_text, child_text, receipts_text):
+    """ipcfp_tipset_desc_from_json (host parser, no device): the descriptor of the Lotus JSON-RPC texts as an A.TipsetInfoPy. Failures raise
+    IpcfpError with the status and the receipt index (UINT64_MAX outside the receipt list's elements)."""
+    p, c, r = (_text(x) for x in (parent_text, child_text, receipts_text))
+    out = C.POINTER(A.ParsedTipsetC)()
+    L = lib()
+    _check(L.ipcfp_tipset_desc_from_json(p, len(p), c, len(c), r, len(r), C.byref(out)))
+    try:
+        return A.tipset_info_from_c(out.contents.desc)
+    finally:
+        L.ipcfp_parsed_tipset_free(out)
 
 
 def _to_json(fn, obj_ptr, ts):

@@ -220,7 +220,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }
@@ -317,6 +317,24 @@ ipcfp_status ipcfp_tipset_upload(ipcfp_store* s, const ipcfp_tipset_desc* t, ipc
     });
 }
 void ipcfp_tipset_free(ipcfp_tipset* t) { delete reinterpret_cast<TipsetDev*>(t); }
+ipcfp_status ipcfp_tipset_upload_json(ipcfp_store* s, const char* parent, uint64_t parent_len, const char* child, uint64_t child_len,
+                                      const char* receipts, uint64_t receipts_len, ipcfp_tipset** out) {
+    return guard([&] {
+        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        Store* st = reinterpret_cast<Store*>(s);
+        std::unique_ptr<TipsetDev> td(new TipsetDev());
+        tipset_upload_json(st, parent, parent_len, child, child_len, receipts, receipts_len, *td);
+        IPCFP_CUDA(cudaStreamSynchronize(st->stream));
+        *out = reinterpret_cast<ipcfp_tipset*>(td.release());
+    });
+}
+ipcfp_status ipcfp_tipset_describe(ipcfp_tipset* t, int with_events_roots, ipcfp_tipset_info* out) {
+    return guard([&] {
+        if (!t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        tipset_describe(*reinterpret_cast<TipsetDev*>(t), with_events_roots != 0, out);
+    });
+}
 ipcfp_status ipcfp_generate_event_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, uint32_t flags,
                                                  ipcfp_event_result** out) {
     return guard([&] {

@@ -87,6 +87,12 @@ struct TipsetDev {
     uint64_t n_receipts = 0;
     DevBuf<uint8_t> events_roots;  // n*38
     DevBuf<uint8_t> has_root;      // n
+    int device = 0;
+    // ipcfp_tipset_upload_json: which path parsed the receipt list and its wall time; ipcfp_tipset_describe: the host copies of the
+    // receipt arrays (made on its first request)
+    bool parsed_on_device = false;
+    float ms_parse = 0.f, ms_kernels = 0.f;
+    std::vector<uint8_t> host_roots, host_has;
 };
 
 struct ScopedStatus;  // capi.cu
@@ -117,6 +123,10 @@ void publish_words_on(Store* s, cudaStream_t stream, const void* src_dev, uint32
 
 // events.cu
 void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td);
+// rpc_json.cu — ipcfp_tipset_upload_json / ipcfp_tipset_describe
+void tipset_upload_json(Store* s, const char* parent, uint64_t parent_len, const char* child, uint64_t child_len, const char* receipts,
+                        uint64_t receipts_len, TipsetDev& td);
+void tipset_describe(TipsetDev& td, bool with_roots, ipcfp_tipset_info* out);
 // the reconstructed execution order of a tipset on the device (reconstruct_execution_order, events/utils.rs:16-30): exec[i] = exec_raw[exec_idx[i]]
 struct ExecOrderOut {
     uint64_t n_exec = 0, nraw = 0;

@@ -443,6 +443,7 @@ void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td) {
     if (t->n_parents > IPCFP_MAX_PARENTS) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
     if (t->n_receipts >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^32 receipts");
     if (t->n_receipts && (!t->events_roots || !t->has_events_root)) throw Error(IPCFP_ERR_INVALID_ARG, "events roots missing");
+    td.device = s->device;
     td.parent_epoch = t->parent_epoch; td.child_epoch = t->child_epoch; td.n_parents = t->n_parents;
     td.parent_cids.assign(t->parent_cids, t->parent_cids + 38ull * t->n_parents);
     td.txmeta_cids.assign(t->parent_txmeta_cids, t->parent_txmeta_cids + 38ull * t->n_parents);
