@@ -154,7 +154,7 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
         lists.push_back(&storage_result_witness(box->r.storage));
     }
     for (uint64_t i = 0; i < n_especs; i++) {
-        box->ev.push_back(generate_event_proof(st, nullptr, td, &especs[i], flags & IPCFP_WITNESS_BY_REFERENCE, false, 0, 0, 1, 0));
+        box->ev.push_back(generate_event_proof(st, td, &especs[i], flags & IPCFP_WITNESS_BY_REFERENCE, false, 0, 0));
         lists.push_back(&event_result_witness(box->ev.back()));
     }
     witness_union(st, lists, box->wit, by_ref);
@@ -289,7 +289,7 @@ ipcfp_status ipcfp_generate_event_proof(ipcfp_store* s, const ipcfp_tipset_desc*
         Store* st = reinterpret_cast<Store*>(s);
         TipsetDev td;
         tipset_upload(st, t, td);
-        *out = generate_event_proof(st, t, td, spec, flags, false, 0, 0, 1, 0);
+        *out = generate_event_proof(st, td, spec, flags, false, 0, 0);
     });
 }
 ipcfp_status ipcfp_generate_event_proof_shard(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_spec* spec, uint64_t lo, uint64_t hi,
@@ -300,7 +300,7 @@ ipcfp_status ipcfp_generate_event_proof_shard(ipcfp_store* s, const ipcfp_tipset
         Store* st = reinterpret_cast<Store*>(s);
         TipsetDev td;
         tipset_upload(st, t, td);
-        *out = generate_event_proof(st, t, td, spec, flags, true, lo, hi, world_size, rank);
+        *out = generate_event_proof(st, td, spec, flags, true, lo, hi);
     });
 }
 void ipcfp_event_result_free(ipcfp_event_result* r) { if (r) event_result_free(r); }
@@ -340,7 +340,7 @@ ipcfp_status ipcfp_generate_event_proof_resident(ipcfp_store* s, ipcfp_tipset* t
     return guard([&] {
         if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), nullptr, *reinterpret_cast<TipsetDev*>(t), spec, flags, false, 0, 0, 1, 0);
+        *out = generate_event_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), spec, flags, false, 0, 0);
     });
 }
 ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, uint64_t lo, uint64_t hi,
@@ -348,7 +348,7 @@ ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tip
     return guard([&] {
         if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), nullptr, *reinterpret_cast<TipsetDev*>(t), spec, flags, true, lo, hi, world_size, rank);
+        *out = generate_event_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), spec, flags, true, lo, hi);
     });
 }
 void* ipcfp_store_stream(ipcfp_store* s) { return s ? (void*)reinterpret_cast<Store*>(s)->stream : nullptr; }
@@ -444,7 +444,7 @@ ipcfp_status ipcfp_generate_event_proof_sharded(ipcfp_comm* c, ipcfp_store* s, i
         TipsetDev& td = *reinterpret_cast<TipsetDev*>(t);
         for (uint32_t k = 0; k < W; k++) if (bounds[k] > bounds[k + 1]) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must ascend");
         if (bounds[0] != 0 || bounds[W] != td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must cover [0, n_receipts)");
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), nullptr, td, spec, flags, true, bounds[r], bounds[r + 1], W, r, cm);
+        *out = generate_event_proof(reinterpret_cast<Store*>(s), td, spec, flags, true, bounds[r], bounds[r + 1], cm);
     });
 }
 

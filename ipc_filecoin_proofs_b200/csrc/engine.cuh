@@ -49,6 +49,71 @@ struct PinnedArray {
     template <class T> T* as() const { return (T*)p; }
 };
 
+// ---- The store's counter words and events
+// dev_words: one slot per counter or fault word a kernel writes. host_words[0, DW_COUNT) mirror them at the same index
+// (publish_words(s, first, n) with first + n <= DW_COUNT); the host-only regions behind the mirror receive other device data.
+enum DevWord : uint32_t {
+    DW_ERR = 0,                            // first error key (report_error)
+    DW_FRONTIER_A = 1, DW_FRONTIER_B = 2,  // general walk: frontier counters (ping / pong); k_setup seeds A
+    DW_UNKNOWN_CLASSES = 1,                // store ingest: CIDs of no known class
+    DW_FIRST_BAD = 2,                      // store ingest: first block whose CID does not match its bytes
+    DW_N_EXEC = 3,
+    DW_STATS = 4,                          // 4 / 5: nodes / bytes pass 1 (or the slot lookup) read
+    DW_N_MATCH = 6,
+    DW_N_PROOFS = 7,
+    DW_WIT_A = 8, DW_WIT_A_BYTES = 9,      // witness snapshot: blocks, padded bytes
+    DW_WIT_B = 10, DW_WIT_B_BYTES = 11,    // late witness blocks, padded bytes
+    DW_BLOB_BYTES = 12,                    // topics / data bytes of the proofs
+    DW_LEVEL_TOTAL = 13,                   // general walk: the level's exact total
+    DW_DENSE_FAIL = 14,                    // the dense walk gave up
+    DW_TX_ERR = 15,                        // message-AMT fault key (tx_err_key)
+    DW_SPLIT_IDX = 16, DW_SPLIT_BYTES = 17,  // witness gather split: blocks and bytes of the first part
+    DW_UNION_SIZE = 18,                    // sharded: size of the replicated witness union
+    DW_EXEC_CHECK = 19,                    // sharded: error key of the exec.get check
+    DW_JSON_TOTAL0 = 24, DW_JSON_TOTAL1 = 25, DW_JSON_OVERFLOW = 26, DW_JSON_TOTAL2 = 27,
+    DW_COUNT = 64
+};
+constexpr uint32_t MAX_WORLD = 255;   // ranks of one sharded call
+// Host-only regions of host_words, each right behind the previous one. The sizes of types defined in a .cu file are asserted there.
+constexpr uint32_t HW_PROLOGUE_WORDS = 230;                                   // events.cu: the head of Prologue
+constexpr uint32_t HW_JSON_TOTALS_WORDS = DW_JSON_TOTAL2 - DW_JSON_TOTAL0 + 1;  // json.cu: list totals and overflow flag
+constexpr uint32_t HW_ANY_SKIP_WORDS = 2;                                     // events.cu: Prologue::misc[0..3], misc[2] = any_skip
+constexpr uint32_t HW_PARKED_KEY_WORDS = 1;                                   // verify.cu: the TxMeta check's error key
+constexpr uint32_t HW_EXCHANGE_WORDS = 2;                                     // parallel.cu: exchange overflow flag, n_exec
+constexpr uint32_t HW_UNION_PARTS_WORDS = 2 * MAX_WORLD;                      // parallel.cu: [partition size, overflow] per rank
+constexpr uint32_t HW_JP_META_WORDS = 17;                                     // json_parse.cu: JpMeta
+constexpr uint32_t HW_RJ_META_WORDS = 2;                                      // rpc_json.cu: RjMeta
+enum HostWord : uint32_t {
+    HW_PROLOGUE = DW_COUNT,
+    HW_JSON_TOTALS = HW_PROLOGUE + HW_PROLOGUE_WORDS,
+    HW_ANY_SKIP = HW_JSON_TOTALS + HW_JSON_TOTALS_WORDS,
+    HW_PARKED_KEY = HW_ANY_SKIP + HW_ANY_SKIP_WORDS,
+    HW_EXCH_OVERFLOW = HW_PARKED_KEY + HW_PARKED_KEY_WORDS, HW_EXCH_N_EXEC = HW_EXCH_OVERFLOW + 1,
+    HW_UNION_PARTS = HW_EXCH_OVERFLOW + HW_EXCHANGE_WORDS,
+    HW_JP_META = HW_UNION_PARTS + HW_UNION_PARTS_WORDS,
+    HW_RJ_META = HW_JP_META + HW_JP_META_WORDS,
+    HW_END = HW_RJ_META + HW_RJ_META_WORDS
+};
+constexpr uint32_t HW_COUNT = 1024;
+static_assert(DW_JSON_TOTAL2 < DW_COUNT, "a mirrored slot never reaches a host-only region (they start at DW_COUNT)");
+static_assert(HW_EXCH_N_EXEC < HW_UNION_PARTS, "the exchange words fit their region");
+static_assert(HW_END <= HW_COUNT, "the host-only regions fit the mapped words");
+// Store::ev: the event-proof step's timeline. storage.cu gives slots 1..3 meanings of its own.
+enum StoreEvent : uint32_t {
+    EV_BEGIN = 0,
+    EV_SETUP = 1, EV_STORAGE_END = 1,
+    EV_EXEC_ORDER = 2, EV_LOOKUP_BEGIN = 2,   // execution order done (walk, snapshot, dedup)
+    EV_PASS1 = 3, EV_LOOKUP_END = 3,
+    EV_PASS2 = 4,
+    EV_END = 5,
+    EV_WITNESS_SORTED = 6,   // the sorted witness CID list exists on the device (also: the first gather part, for its D2H)
+    EV_BLOB_COPIED = 7,      // the witness blob's D2H is done (side stream)
+    EV_GATHER_B = 8,         // the second gather part, for its D2H
+    EV_RAW_LIST = 9,         // the raw message list of the call is complete (the cross-shard exchange waits for it)
+    EV_JSON_BEGIN = 10, EV_JSON_END = 11,
+    EV_COUNT = 12
+};
+
 struct Store {
     int device = 0;
     cudaStream_t stream = nullptr, stream2 = nullptr;
@@ -69,10 +134,10 @@ struct Store {
     uint64_t first_bad = UINT64_MAX;
     std::shared_ptr<PinnedPool> pool;
     // small persistent scratch
-    DevBuf<unsigned long long> dev_words;  // [0] error word, [1..] counters
-    PinnedBuf<uint64_t> host_words;
+    DevBuf<unsigned long long> dev_words;  // DW_COUNT slots (DevWord)
+    PinnedBuf<uint64_t> host_words;        // HW_COUNT mapped words (HostWord)
     PinnedArray stage;                     // pinned staging (from the process-wide pool) for small per-call uploads: spec, tipset CIDs, walk tables
-    cudaEvent_t ev[12] = {};
+    cudaEvent_t ev[EV_COUNT] = {};
     ~Store();
     void use() const { IPCFP_CUDA(cudaSetDevice(device)); }
 };
@@ -115,11 +180,10 @@ Store* store_shell(int device);   // stream, events, counters; no block yet
 void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev);
 void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws);
 void store_verify_all(Store* s);
-// counters dev_words[first, first+count) → host_words (same indices) through mapped host memory: a tiny kernel
-// instead of a D2H copy, so the read-back never queues behind a large copy on the copy engine
-void publish_words(Store* s, uint32_t first, uint32_t count);
-void publish_words_from(Store* s, const void* src_dev, uint32_t dst_first, uint32_t n_words);
-void publish_words_on(Store* s, cudaStream_t stream, const void* src_dev, uint32_t dst_first, uint32_t n_words);   // the same on another stream
+// n_words device words at src_dev (null: the mirrored dev_words[dst_first ..]) → host_words[dst_first ..) through mapped host memory,
+// on `stream` (null: the store's stream): a tiny kernel instead of a D2H copy, so the read-back never queues behind a large copy on
+// the copy engine
+void publish_words(Store* s, uint32_t dst_first, uint32_t n_words, const void* src_dev = nullptr, cudaStream_t stream = nullptr);
 
 // events.cu
 void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td);
@@ -133,9 +197,8 @@ struct ExecOrderOut {
     AsyncBuf<RawCid> exec_raw;
     AsyncBuf<uint32_t> exec_idx;
 };
-ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags,
-                                         bool sharded, uint64_t lo, uint64_t hi, uint32_t world, uint32_t rank, Comm* comm = nullptr,
-                                         ExecOrderOut* exo = nullptr);
+ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
+                                         Comm* comm = nullptr, ExecOrderOut* exo = nullptr);
 // verify.cu — batched verifiers over a witness store
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
                          const ipcfp_event_spec* filter, uint8_t* results);
@@ -162,7 +225,7 @@ void comm_destroy(Comm* c);
 uint32_t comm_world(const Comm* c);
 uint32_t comm_rank(const Comm* c);
 // One sharded generate_event_proof call's share of the protocol (see the banner in parallel.cu). generate_event_proof drives it:
-//   agree_slices → start_exchange → positions_for → agree_results → fetch_and_patch → witness_union
+//   agree_early or agree_slices → start_exchange → positions_for → agree_results → fetch_and_patch → witness_union → finish → fill_result
 struct ShardExchange {
     Comm* c;
     Store* s;
@@ -180,29 +243,39 @@ struct ShardExchange {
     // P / F
     uint64_t M = 0;
     const uint32_t* match_rel_dev = nullptr;
+    unsigned long long* n_exec_out = nullptr;
     // H0 / H2 (global values, identical on every rank)
     uint64_t g_tx = ~0ull, g_err = ~0ull;
     bool g_missing_base = false, g_overflow = false, g_stale = false;
     uint64_t M_max = 0, nw_max = 0, M_total = 0, proofs_total = 0;
     std::vector<uint64_t> nw_all;
+    // W
+    bool full_union = false;
+    const uint8_t* wit_cids = nullptr;
+    uint64_t wit_n = 0;
+    uint8_t* union_dev = nullptr;
     ShardExchange(Comm* comm, Store* store, uint64_t lo_, uint64_t hi_);
     void agree_early(bool can_promise, uint64_t planned_nseg, uint64_t nraw_total);
     void agree_slices(uint64_t tx_key, uint64_t err_key, uint64_t nseg_);
-    void start_exchange(const void* seg_dev, cudaEvent_t seg_ready);
-    void positions_for(cudaStream_t st, const uint32_t* match_rel, uint64_t n_match, unsigned long long* n_exec_out);
-    void agree_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, uint64_t exch_overflow, bool stale);
-    void fetch_and_patch(cudaStream_t st, ipcfp_event_proof* proofs_dev, uint64_t n_proofs);
-    void witness_union(cudaStream_t st, const uint8_t* cids_dev, uint64_t n_local, uint8_t** out_dev, uint64_t* n_out_dev_word);
-    // the same union left distributed: this rank's partition (sorted) in *out_dev; every rank's [partition size, overflow flag] lands in
-    // the store's mapped words [host_word_first, +2·world) with the next sync of `st`. Any overflow flag set: repeat with
-    // union_piece_cap(true).
-    uint64_t union_piece_cap(bool cannot_overflow) const;
-    void witness_union_partitioned(cudaStream_t st, const uint8_t* cids_dev, uint64_t n_local, uint64_t cap, uint8_t** out_dev, uint32_t host_word_first);
-    void timings(float* ms_exchange, float* ms_fetch, float* ms_union) const;   // after the call's final sync
+    void start_exchange(const void* seg_dev);   // behind EV_RAW_LIST
+    void positions_for(const uint32_t* match_rel, uint64_t n_match, unsigned long long* n_exec_out_);
+    // H2 after the engine stream's pass-2 synchronisation; true: every shard goes on. A stale early promise repeats H0, X, P and H2.
+    bool agree_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, bool stale, const void* seg_dev,
+                       uint64_t nseg_);
+    void fetch_and_patch(ipcfp_event_proof* proofs_dev, uint64_t n_proofs, void* proofs_host);
+    void witness_union(const uint8_t* cids_dev, uint64_t n_local, bool full);   // behind EV_WITNESS_SORTED
+    void finish();                                                             // joins both protocol streams (the union's retry included)
+    void fill_result(ipcfp_event_result& r) const;
     void trace_timeline(cudaEvent_t origin, const char* engine_part) const;
-    cudaStream_t stream() const;            // the exchange stream
-    cudaStream_t union_stream() const;      // the witness union's own stream (its communicator is independent of the exchange's)
-    uint64_t host_word(uint32_t i) const;   // the store's mapped words: 300 = exchange overflow flag, 301 = n_exec (valid after the sync that follows positions_for)
+private:
+    void gather_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, uint64_t exch_overflow, bool stale);
+    void patch(ipcfp_event_proof* proofs_dev, uint64_t n_proofs);
+    void union_replicated(uint64_t* n_out_dev_word);
+    // the union left distributed: this rank's partition (sorted) in union_dev; every rank's [partition size, overflow flag] lands in
+    // host words HW_UNION_PARTS with the next sync of the union stream. Any overflow flag set: repeat with union_piece_cap(true).
+    uint64_t union_piece_cap(bool cannot_overflow) const;
+    void union_partitioned(uint64_t cap);
+    void timings(float* ms_exchange, float* ms_fetch, float* ms_union) const;   // after the call's final sync
 };
 void exec_bucketize(int device, const void* seg, uint64_t nseg, uint64_t pos0, uint32_t world, uint64_t cap, void* send, uint64_t* counts_host);
 void exec_dedup(int device, const void* recv, const uint64_t* counts, uint32_t world, uint64_t cap, uint64_t* dup_dev, uint64_t cap_out, uint64_t* n_dup);

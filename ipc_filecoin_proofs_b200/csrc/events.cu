@@ -18,6 +18,7 @@
 
 #include <chrono>
 #include <cstddef>
+#include <optional>
 #include <cooperative_groups.h>
 #include "engine.cuh"
 #include "hashes.cuh"
@@ -34,14 +35,6 @@ namespace cg = cooperative_groups;
 // ------------------------------------------------------------------------------------------ pass 1 / pass 2 kernels (per-receipt code: events_items.cuh)
 // Pass 1 is k_pass1_stage (pass1_stage.cuh).
 
-// exec.get(i) for every matching receipt against the GLOBAL execution order length (sharded calls: the order spans shards)
-__global__ void k_check_exec(const uint32_t* __restrict__ match_rel, uint64_t n_match, uint64_t lo, const unsigned long long* __restrict__ n_exec,
-                             unsigned long long* err) {
-    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n_match) return;
-    const uint64_t i = lo + match_rel[t];
-    if (i >= *n_exec) report_error(err, ST_PASS2, i, 0 /* DC_MISSING_EXEC, ranked before every other code at the same receipt */, 0);
-}
 // a.per_warp: one matching receipt per WARP (lane 0 walks). A matching receipt is a chain of dependent accesses (hash probe → record →
 // strict decode of a 349–413 B node, 7 levels at 1 M receipts, then its events AMT), and 32 lanes on 32 different paths execute that
 // chain serialised by divergence: ≈ 1 000 matches in 8 CTAs keep 8 of the GPU's 132 SMs busy. One warp per match is the shape
@@ -58,16 +51,16 @@ __global__ void __launch_bounds__(128) k_pass2(Pass2Args a) {
 #define IPCFP_MAX_PARENTS 64
 static_assert(2 * IPCFP_MAX_PARENTS <= DENSE_MAX_AMTS, "the dense plan's tables hold every message AMT");
 // What k_setup leaves for the host and the walk, in one device block. The head (everything before the tables) reaches the host
-// in one publish (host words PRO_HOST_WORD ..); the tables stay on the device.
+// in one publish (host words HW_PROLOGUE ..); the tables stay on the device.
 struct Prologue {
     uint32_t misc[64 + 2 * IPCFP_MAX_PARENTS];   // [0] receipts-root block, [1] a base-witness CID is missing, [2] any_skip (pass 2), [64 + k] height of AMT k
     uint64_t amt_count[2 * IPCFP_MAX_PARENTS];   // root.count of AMT k
     uint64_t t0[4];                              // keccak256(event signature), the Matcher's t0
     DenseTables plan;                            // the dense walk's plan: ok, rounds, nraw, then the tables
 };
-#define PRO_HOST_WORD 24
 static constexpr uint32_t PRO_HEAD_WORDS = (uint32_t)((offsetof(Prologue, plan) + offsetof(DenseTables, per_amt)) / 8);
-static_assert(PRO_HOST_WORD + PRO_HEAD_WORDS <= 300, "the prologue's head must not reach the sharded protocol's host words");
+static_assert(PRO_HEAD_WORDS <= HW_PROLOGUE_WORDS, "the prologue's head fits its host words (HW_PROLOGUE)");
+static_assert(offsetof(Prologue, misc) == 0 && 3 * sizeof(uint32_t) <= HW_ANY_SKIP_WORDS * 8, "misc[2] (any_skip) fits its host words (HW_ANY_SKIP)");
 struct SetupArgs {
     StoreView store;
     uint32_t n_parents;
@@ -430,10 +423,11 @@ static void throw_tx_error(uint64_t key) {
     if (eidx != IPCFP_TX_EIDX_NONE && eidx % 3 == 0 && code == DC_MISSING) out_index = eidx / 3;   // missing TxMeta of parent b
     throw Error(st, std::string(what) + " in message AMTs (detail " + std::to_string(detail) + ")", out_index);
 }
-// the failure the reference's sequential order meets first: message-AMT stage before everything else
-static void check_device_errors(const uint64_t* hw) {
-    if (hw[15] != IPCFP_NO_ERROR) throw_tx_error(hw[15]);
-    if (hw[0] != IPCFP_NO_ERROR) throw_device_error(hw[0]);
+// the failure the reference's sequential order meets first: message-AMT stage before everything else, a missing base-witness block last
+static void throw_first(uint64_t tx_key, uint64_t err_key, bool missing_base = false) {
+    if (tx_key != IPCFP_NO_ERROR) throw_tx_error(tx_key);
+    if (err_key != IPCFP_NO_ERROR) throw_device_error(err_key);
+    if (missing_base) throw Error(IPCFP_ERR_MISSING_BLOCK, "missing block (base witness CID not in the store)");
 }
 
 void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td) {
@@ -460,75 +454,167 @@ void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td) {
     }
 }
 
-ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*/, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags,
-                                         bool sharded, uint64_t lo, uint64_t hi, uint32_t world, uint32_t rank, Comm* comm, ExecOrderOut* exo) {
-    s->use();
-    cudaStream_t st = s->stream;
-    const auto t_enter = std::chrono::steady_clock::now();
-    static thread_local std::chrono::steady_clock::time_point t_last_exit = t_enter;
-    if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
-    // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
-    if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
-    if (!sharded) { lo = 0; hi = td.n_receipts; }
-    if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
-    const uint64_t N = hi - lo;
-    const uint64_t nblk = s->n;
-    const bool skip_tx = (flags & IPCFP_SCAN_SKIP_TX_AMTS) != 0;
-    // comm != nullptr: this call is one shard of a multi-GPU call and runs the cross-shard protocol itself (parallel.cu). Failures
-    // are then not thrown where they are seen: every rank keeps taking part in the collectives and all ranks fail together, with
-    // the error the reference's sequential order meets first across ALL shards.
+namespace {
+static constexpr size_t STAGE_TABLES = 32768;   // second half of the store's staging block: dense-walk tables
+
+// One generate_event_proof call: its arguments, its state and buffers, and its phases, which generate_event_proof runs in order.
+// comm != nullptr: this call is one shard of a multi-GPU call and runs the cross-shard protocol itself (parallel.cu). Failures are then
+// not thrown where they are seen: every rank keeps taking part in the collectives and all ranks fail together, with the error the
+// reference's sequential order meets first across ALL shards.
+// Host synchronisations, per mode:
+//   unsharded         snapshot_and_sync after the walk (again after a dense walk that gave up; once more for k_amt_first_fault),
+//                     pass1, pass2, read_back's witness join (IPCFP_RESULT_JSON: render_event_json's one before it), fill
+//   IPCFP_BFS_GENERAL, sharded, execution-order only: walk reads the prologue back first; run_general synchronises after its range
+//                     upload, after the fused rounds and once per level below them
+//   execution-order only: walk, snapshot_and_sync, then dedup reads n_exec back and the call ends
+//   sharded over NCCL: besides, every H0 / H2 gather, ShardExchange::agree_results and finish, a late H0 that fails, and fill's copy of
+//                     the union partition (IPCFP_SHARDED_UNION_TO_HOST)
+struct EventCall {
+    Store* s;
+    cudaStream_t st;
+    TipsetDev& td;
+    const ipcfp_event_spec* spec;
+    uint32_t flags;
+    bool sharded;
+    uint64_t lo, hi;
+    Comm* comm;
+    ExecOrderOut* exo;
+    std::chrono::steady_clock::time_point t_enter;
+    uint64_t N = 0, nblk = 0;
+    bool skip_tx = false;
     std::unique_ptr<ShardExchange> xch;
-    if (comm) {
-        if (!sharded) throw Error(IPCFP_ERR_INVALID_ARG, "communicator given for an unsharded call");
-        if (s->class_prefix.size() > 1) throw Error(IPCFP_ERR_UNSUPPORTED, "sharded calls need a store with one CID prefix");
-        xch.reset(new ShardExchange(comm, s, lo, hi));
-    }
     uint64_t pend_tx = IPCFP_NO_ERROR, pend_err = IPCFP_NO_ERROR;   // first failure seen so far (xch mode)
-    auto note_errors = [&](const uint64_t* hwp) {
-        if (!xch) { check_device_errors(hwp); return; }
-        pend_tx = std::min<uint64_t>(pend_tx, hwp[15]);
-        pend_err = std::min<uint64_t>(pend_err, hwp[0]);
-    };
-    auto throw_global = [&](uint64_t gtx, uint64_t gerr, bool gmissing) {
-        if (gtx != IPCFP_NO_ERROR) throw_tx_error(gtx);
-        if (gerr != IPCFP_NO_ERROR) throw_device_error(gerr);
-        if (gmissing) throw Error(IPCFP_ERR_MISSING_BLOCK, "missing block (base witness CID not in the store)");
-    };
-    unsigned long long* dw = s->dev_words.p;  // [0] err, [1..] counters
-    uint64_t* hw = s->host_words.p;
-
-    IPCFP_CUDA(cudaEventRecord(s->ev[0], st));
-    IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
-    IPCFP_CUDA(cudaMemsetAsync(dw + 1, 0, 40 * 8, st));
-    IPCFP_CUDA(cudaMemsetAsync(dw + 15, 0xff, 8, st));   // message-AMT fault word
-
-    // ---- matcher
+    unsigned long long* dw;
+    uint64_t* hw;
+    // stage
     Matcher mh;
-    memset(&mh, 0, sizeof mh);
-    {
-        size_t n1 = strlen(spec->topic_1);
-        uint8_t t1[32];
-        memset(t1, 0, 32);
-        memcpy(t1, spec->topic_1, n1 < 32 ? n1 : 32);  // ascii_to_bytes32 (evm.rs:72-78)
-        memcpy(mh.t1, t1, 32);
-        mh.actor = spec->actor_id_filter;
-        mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
+    size_t siglen = 0, tables_off = 0;
+    AsyncBuf<uint8_t> small;
+    uint8_t *d_sig = nullptr, *d_cids = nullptr;
+    Matcher* d_matcher = nullptr;
+    // setup
+    AsyncBuf<uint32_t> wbits;
+    uint32_t namt = 0;
+    uint64_t cap = 0;
+    AsyncBuf<uint32_t> fA_blk, fA_meta, fB_blk, fB_meta;
+    AsyncBuf<uint64_t> fA_base, fB_base;
+    AsyncBuf<Prologue> pro;
+    uint32_t* misc = nullptr;
+    uint32_t frontier_cap = 0;
+    uint64_t max_raw_dev = 0;
+    bool force_general = false, plan_on_device = false;
+    SetupArgs sa;
+    // walk
+    const Prologue* ph;   // the prologue's head as the host reads it, once publish_prologue and a synchronisation have run
+    bool early_fault = false, missing_base = false;
+    uint32_t receipts_root_blk = 0, last_round = 0;
+    // share of the concatenated ("raw") message list this call walks: everything, or — sharded — [Nraw*lo/N, Nraw*hi/N) expressed as
+    // one index range per AMT
+    std::vector<uint64_t> h_rng = std::vector<uint64_t>(4 * IPCFP_MAX_PARENTS, 0);
+    uint64_t nraw_total = 0;
+    AsyncBuf<uint32_t> counts;
+    AsyncBuf<uint64_t> out_off, scratch;
+    unsigned long long *ccount = nullptr, *ncount = nullptr, *total_dev = nullptr;
+    AsyncBuf<RawCid> exec_raw;
+    uint64_t raw_cap = 0;
+    DensePlan plan;
+    AsyncBuf<uint64_t> d_foff;
+    AsyncBuf<uint32_t> d_flen;
+    DenseArgs da;
+    AsyncBuf<uint64_t> d_rng;
+    AsyncBuf<uint32_t> g_blk[2], g_meta[2];
+    AsyncBuf<uint64_t> g_base[2];
+    bool dense_used = false, xch_early = false;
+    std::optional<WitnessBuilder> wbuild;
+    uint64_t nraw = 0;
+    bool xch_stale = false;
+    // dedup
+    AsyncBuf<uint32_t> exec_idx, keep_bits;
+    unsigned long long* n_exec_dev = nullptr;
+    // pass 1
+    AsyncBuf<uint32_t> match_bits, cnt, nby;
+    AsyncBuf<uint64_t> pbase, bbase;
+    AsyncBuf<uint32_t> match_rel;
+    AsyncBuf<uint64_t> wp3;
+    uint64_t n_exec = 0, M = 0, pass1_nodes = 0, pass1_bytes = 0, n_proofs = 0, n_bytes = 0;
+    // pass 2 and the result
+    std::unique_ptr<EventResultBox> box;
+    AsyncBuf<ipcfp_event_proof> d_proofs;
+    AsyncBuf<uint8_t> d_blob;
+    uint64_t mB = 0;
+    bool any_skip = false;
+    PinnedArray rel;
+    uint64_t json_len = 0;
+
+    EventCall(Store* s_, TipsetDev& td_, const ipcfp_event_spec* spec_, uint32_t flags_, bool sharded_, uint64_t lo_, uint64_t hi_, Comm* comm_,
+              ExecOrderOut* exo_)
+        : s(s_), st(s_->stream), td(td_), spec(spec_), flags(flags_), sharded(sharded_), lo(lo_), hi(hi_), comm(comm_), exo(exo_),
+          dw(s_->dev_words.p), hw(s_->host_words.p), ph((const Prologue*)(s_->host_words.p + HW_PROLOGUE)) {}
+
+    void note_errors() {   // the fault words as the last publish left them
+        if (!xch) { throw_first(hw[DW_TX_ERR], hw[DW_ERR]); return; }
+        pend_tx = std::min<uint64_t>(pend_tx, hw[DW_TX_ERR]);
+        pend_err = std::min<uint64_t>(pend_err, hw[DW_ERR]);
     }
-    // spec + tipset CIDs go up in ONE copy from the store's pinned staging block (no host sync):
-    //   [0,1024) Matcher (t0 is filled in on the device) | signature, zero padded | parent, TxMeta, child, receipts-root CIDs
-    const size_t siglen = strlen(spec->event_signature);
-    const size_t sig_cap = (siglen + 64) & ~(size_t)63;
-    const size_t cids_bytes = 38ull * (2 * td.n_parents + 2);
-    const size_t small_bytes = 1024 + sig_cap + cids_bytes + 64;
-    static_assert(sizeof(Matcher) <= 1024, "Matcher must fit its staging slot");
-    const size_t STAGE_TABLES = 32768;                    // second half of the staging block: dense-walk tables
-    const size_t tables_off = std::max<size_t>(STAGE_TABLES, (small_bytes + 63) & ~(size_t)63);
-    if (!s->stage.p || s->stage.cap < tables_off + STAGE_TABLES) s->stage = PinnedArray(s->pool, tables_off + STAGE_TABLES);
-    AsyncBuf<uint8_t> small(small_bytes, st);
-    uint8_t* d_sig = small.p + 1024;                       // 8-byte aligned
-    uint8_t* d_cids = small.p + 1024 + sig_cap;
-    Matcher* d_matcher = (Matcher*)small.p;
-    {
+    void publish_prologue() { publish_words(s, HW_PROLOGUE, PRO_HEAD_WORDS, pro.p); }
+    void read_prologue() {   // the fault words as the prologue left them, and its head
+        early_fault = hw[DW_ERR] != IPCFP_NO_ERROR || hw[DW_TX_ERR] != IPCFP_NO_ERROR;
+        memcpy(mh.t0, ph->t0, 32);
+        receipts_root_blk = ph->misc[0];
+        missing_base = ph->misc[1] != 0;
+        last_round = 0;
+        for (uint32_t k = 0; k < namt; k++) last_round = std::max(last_round, ph->misc[64 + k]);
+        nraw_total = shard_amt_ranges(namt, ph->amt_count, sharded, lo, hi, td.n_receipts, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS);
+    }
+    void ensure_scratch(uint64_t n) {   // scan scratch for n items
+        if (scratch.n < scan_scratch_elems(n + 64) + 64) scratch.alloc(scan_scratch_elems(n + 64) + 64, st);
+    }
+
+    // ---- checks, and the spec + tipset CIDs up in ONE copy from the store's pinned staging block (no host sync)
+    void stage() {
+        s->use();
+        t_enter = std::chrono::steady_clock::now();
+        if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+        // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
+        if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
+        if (!sharded) { lo = 0; hi = td.n_receipts; }
+        if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
+        N = hi - lo;
+        nblk = s->n;
+        skip_tx = (flags & IPCFP_SCAN_SKIP_TX_AMTS) != 0;
+        if (comm) {
+            if (!sharded) throw Error(IPCFP_ERR_INVALID_ARG, "communicator given for an unsharded call");
+            if (s->class_prefix.size() > 1) throw Error(IPCFP_ERR_UNSUPPORTED, "sharded calls need a store with one CID prefix");
+            xch.reset(new ShardExchange(comm, s, lo, hi));
+        }
+
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
+        IPCFP_CUDA(cudaMemsetAsync(dw + DW_ERR, 0xff, 8, st));
+        IPCFP_CUDA(cudaMemsetAsync(dw + DW_FRONTIER_A, 0, 40 * 8, st));   // the 40 counters behind the error word
+        IPCFP_CUDA(cudaMemsetAsync(dw + DW_TX_ERR, 0xff, 8, st));
+
+        memset(&mh, 0, sizeof mh);
+        {
+            size_t n1 = strlen(spec->topic_1);
+            uint8_t t1[32];
+            memset(t1, 0, 32);
+            memcpy(t1, spec->topic_1, n1 < 32 ? n1 : 32);  // ascii_to_bytes32 (evm.rs:72-78)
+            memcpy(mh.t1, t1, 32);
+            mh.actor = spec->actor_id_filter;
+            mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
+        }
+        //   [0,1024) Matcher (t0 is filled in on the device) | signature, zero padded | parent, TxMeta, child, receipts-root CIDs
+        siglen = strlen(spec->event_signature);
+        const size_t sig_cap = (siglen + 64) & ~(size_t)63;
+        const size_t cids_bytes = 38ull * (2 * td.n_parents + 2);
+        const size_t small_bytes = 1024 + sig_cap + cids_bytes + 64;
+        static_assert(sizeof(Matcher) <= 1024, "Matcher must fit its staging slot");
+        tables_off = std::max<size_t>(STAGE_TABLES, (small_bytes + 63) & ~(size_t)63);
+        if (!s->stage.p || s->stage.cap < tables_off + STAGE_TABLES) s->stage = PinnedArray(s->pool, tables_off + STAGE_TABLES);
+        small.alloc(small_bytes, st);
+        d_sig = small.p + 1024;                       // 8-byte aligned
+        d_cids = small.p + 1024 + sig_cap;
+        d_matcher = (Matcher*)small.p;
         uint8_t* hs = s->stage.as<uint8_t>();
         memset(hs, 0, small_bytes);
         memcpy(hs, &mh, sizeof(Matcher));
@@ -541,82 +627,62 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         IPCFP_CUDA(cudaMemcpyAsync(small.p, hs, small_bytes, cudaMemcpyHostToDevice, st));
     }
 
-    // ---- witness bitmap + setup
-    AsyncBuf<uint32_t> wbits((nblk + 31) / 32 + 8, st);
-    wbits.zero();
-    const uint32_t namt = 2 * td.n_parents;   // k_setup seeds one frontier item per message AMT
-    const uint64_t cap = 4 * nblk + 1024;
-    AsyncBuf<uint32_t> fA_blk(cap, st), fA_meta(cap, st), fB_blk(cap, st), fB_meta(cap, st);
-    AsyncBuf<uint64_t> fA_base(cap, st), fB_base(cap, st);
-    AsyncBuf<Prologue> pro(1, st);
-    pro.zero();
-    uint32_t* const misc = &pro.p->misc[0];
-    const uint32_t frontier_cap = (uint32_t)std::min<uint64_t>(cap, 0xffffffffull);
-    // Every message of a parent block is executed, so no message AMT counts more values than there are receipts: a dense walk of an
-    // unsharded call writes at most n_parents × n_receipts entries (a plan above that goes to the general walk).
-    const uint64_t max_raw_dev = std::min<uint64_t>(8ull * cap, (uint64_t)td.n_parents * td.n_receipts + 1024);
-    const bool force_general = getenv("IPCFP_BFS_GENERAL") != nullptr;   // read per call: tests toggle it
-    // Unsharded calls plan the dense walk on the device (k_setup) and read the prologue back only together with the witness
-    // snapshot's counts. A sharded call needs its share's length on the host before its walk (early H0, below), and the
-    // execution-order-only mode keeps its own sequence: both read the prologue back first (host synchronisation 1).
-    const bool plan_on_device = !sharded && !exo && !force_general;
-    SetupArgs sa;
-    sa.store = s->view; sa.n_parents = td.n_parents;
-    sa.parent_cids = d_cids; sa.txmeta_cids = d_cids + 38ull * td.n_parents;
-    sa.child_cid = d_cids + 76ull * td.n_parents; sa.receipts_root = sa.child_cid + 38;
-    sa.skip_tx = skip_tx; sa.skip_receipts = exo ? 1 : 0; sa.wbits = wbits.p; sa.err = dw; sa.txerr = dw + 15;
-    sa.pro = pro.p;
-    sa.f_blk = fA_blk.p; sa.f_meta = fA_meta.p; sa.f_base = fA_base.p; sa.f_count = dw + 1;
-    sa.sig = d_sig; sa.sig_len = (uint32_t)siglen; sa.matcher = d_matcher;
-    sa.plan_dense = plan_on_device ? 1 : 0; sa.frontier_cap = frontier_cap; sa.max_raw = max_raw_dev;
-    k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaEventRecord(s->ev[1], st));
-
-    // the prologue's head as the host reads it (host words PRO_HOST_WORD ..) once publish_prologue and a synchronisation have run
-    const Prologue* ph = (const Prologue*)(hw + PRO_HOST_WORD);
-    auto publish_prologue = [&]() { publish_words_from(s, pro.p, PRO_HOST_WORD, PRO_HEAD_WORDS); };
-    bool early_fault = false, missing_base = false;
-    uint32_t receipts_root_blk = 0, last_round = 0;
-    // share of the concatenated ("raw") message list this call walks: everything, or — sharded —
-    // [Nraw*lo/N, Nraw*hi/N) expressed as one index range per AMT
-    std::vector<uint64_t> h_rng(4 * IPCFP_MAX_PARENTS, 0);
-    uint64_t nraw_total = 0;
-    auto read_prologue = [&]() {   // hw[0] / hw[15]: the fault words as the prologue left them
-        early_fault = hw[0] != IPCFP_NO_ERROR || hw[15] != IPCFP_NO_ERROR;
-        memcpy(mh.t0, ph->t0, 32);
-        receipts_root_blk = ph->misc[0];
-        missing_base = ph->misc[1] != 0;
-        last_round = 0;
-        for (uint32_t k = 0; k < namt; k++) last_round = std::max(last_round, ph->misc[64 + k]);
-        nraw_total = shard_amt_ranges(namt, ph->amt_count, sharded, lo, hi, td.n_receipts, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS);
-    };
-
-    // ---- message AMT BFS (recording + raw execution list)
-    AsyncBuf<uint32_t> counts(cap + 1024, st);
-    AsyncBuf<uint64_t> out_off(cap + 1024, st), scratch(scan_scratch_elems(std::max<uint64_t>(cap, N) + 64) + 64, st);
-    unsigned long long *ccount = dw + 1, *ncount = dw + 2, *total_dev = dw + 13;
-    AsyncBuf<RawCid> exec_raw;
-    uint64_t raw_cap = 0;
-
-    // ---- (a) dense walk (see k_amt_dense): planned by k_setup, or here
-    DensePlan plan;
-    if (!plan_on_device) {
-        publish_words(s, 0, 16);
-        publish_prologue();
-        IPCFP_CUDA(cudaStreamSynchronize(st));
-        // A fault seen by the prologue (TxMeta / AMT root / receipts root) is NOT thrown yet: the reference walks the message AMTs
-        // before it loads the receipts root, and a fault inside an earlier AMT precedes a missing later root — walk first (general
-        // kernels: they cope with the sentinel seeds), then report the first one in the reference's order.
-        read_prologue();
-        if (namt > 0 && !force_general && !early_fault)
-            plan = make_dense_plan(namt, ph->misc + 64, ph->amt_count, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS, frontier_cap, 8ull * cap,
-                                   sizeof(DenseTables));
+    // ---- witness bitmap + k_setup
+    void setup() {
+        wbits.alloc((nblk + 31) / 32 + 8, st);
+        wbits.zero();
+        namt = 2 * td.n_parents;   // k_setup seeds one frontier item per message AMT
+        cap = 4 * nblk + 1024;
+        fA_blk.alloc(cap, st); fA_meta.alloc(cap, st); fB_blk.alloc(cap, st); fB_meta.alloc(cap, st);
+        fA_base.alloc(cap, st); fB_base.alloc(cap, st);
+        pro.alloc(1, st);
+        pro.zero();
+        misc = &pro.p->misc[0];
+        frontier_cap = (uint32_t)std::min<uint64_t>(cap, 0xffffffffull);
+        // Every message of a parent block is executed, so no message AMT counts more values than there are receipts: a dense walk of an
+        // unsharded call writes at most n_parents × n_receipts entries (a plan above that goes to the general walk).
+        max_raw_dev = std::min<uint64_t>(8ull * cap, (uint64_t)td.n_parents * td.n_receipts + 1024);
+        force_general = getenv("IPCFP_BFS_GENERAL") != nullptr;   // read per call: tests toggle it
+        // Unsharded calls plan the dense walk on the device (k_setup) and read the prologue back only together with the witness
+        // snapshot's counts. A sharded call needs its share's length on the host before its walk (early H0, below), and the
+        // execution-order-only mode keeps its own sequence: both read the prologue back first (host synchronisation 1).
+        plan_on_device = !sharded && !exo && !force_general;
+        sa.store = s->view; sa.n_parents = td.n_parents;
+        sa.parent_cids = d_cids; sa.txmeta_cids = d_cids + 38ull * td.n_parents;
+        sa.child_cid = d_cids + 76ull * td.n_parents; sa.receipts_root = sa.child_cid + 38;
+        sa.skip_tx = skip_tx; sa.skip_receipts = exo ? 1 : 0; sa.wbits = wbits.p; sa.err = dw + DW_ERR; sa.txerr = dw + DW_TX_ERR;
+        sa.pro = pro.p;
+        sa.f_blk = fA_blk.p; sa.f_meta = fA_meta.p; sa.f_base = fA_base.p; sa.f_count = dw + DW_FRONTIER_A;
+        sa.sig = d_sig; sa.sig_len = (uint32_t)siglen; sa.matcher = d_matcher;
+        sa.plan_dense = plan_on_device ? 1 : 0; sa.frontier_cap = frontier_cap; sa.max_raw = max_raw_dev;
+        k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_SETUP], st));
     }
-    AsyncBuf<uint64_t> d_foff;
-    AsyncBuf<uint32_t> d_flen;
-    DenseArgs da;
-    memset(&da, 0, sizeof da);
-    auto run_dense = [&]() {   // rounds 0 .. rounds-2; run_dense_leaf enqueues the last one
+
+    // ---- message AMT walk (recording + raw execution list): dense if the plan holds, else general
+    void walk() {
+        counts.alloc(cap + 1024, st);
+        out_off.alloc(cap + 1024, st); scratch.alloc(scan_scratch_elems(std::max<uint64_t>(cap, N) + 64) + 64, st);
+        ccount = dw + DW_FRONTIER_A; ncount = dw + DW_FRONTIER_B; total_dev = dw + DW_LEVEL_TOTAL;
+        if (!plan_on_device) {   // the dense walk planned here
+            publish_words(s, 0, DW_TX_ERR + 1);
+            publish_prologue();
+            IPCFP_CUDA(cudaStreamSynchronize(st));
+            // A fault seen by the prologue (TxMeta / AMT root / receipts root) is NOT thrown yet: the reference walks the message AMTs
+            // before it loads the receipts root, and a fault inside an earlier AMT precedes a missing later root — walk first (general
+            // kernels: they cope with the sentinel seeds), then report the first one in the reference's order.
+            read_prologue();
+            if (namt > 0 && !force_general && !early_fault)
+                plan = make_dense_plan(namt, ph->misc + 64, ph->amt_count, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS, frontier_cap, 8ull * cap,
+                                       sizeof(DenseTables));
+        }
+        memset(&da, 0, sizeof da);
+        dense_used = plan_on_device || plan.ok;   // device plan: whether it is ok is known at the next synchronisation
+        if (dense_used) run_dense(); else run_general();
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_RAW_LIST], st));
+    }
+    // (a) the dense walk (see k_amt_dense): rounds 0 .. rounds-2 in one cooperative launch, then the leaf round
+    void run_dense() {
         if (!plan_on_device) {   // the host's plan goes where k_setup writes it for unsharded calls
             static_assert(sizeof(DenseTables) <= STAGE_TABLES, "the dense plan must fit its staging slot");
             DenseTables* ht = (DenseTables*)(s->stage.as<uint8_t>() + tables_off);
@@ -640,7 +706,7 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         da.tables = tb;
         da.vbase = tb->per_amt; da.cnt = tb->per_amt + namt; da.lo = tb->per_amt + 2ull * namt; da.hi = tb->per_amt + 3ull * namt;
         da.fofs = tb->fofs; da.ftot = tb->ftot;
-        da.namt = namt; da.record = skip_tx ? 0 : 1; da.wbits = wbits.p; da.fail = (uint32_t*)(dw + 14);
+        da.namt = namt; da.record = skip_tx ? 0 : 1; da.wbits = wbits.p; da.fail = (uint32_t*)(dw + DW_DENSE_FAIL);
         // frontier items of a round ≥ 1: an AMT holding c values has at most c/8 + 1 nodes on any level
         uint64_t fmax = 1;
         if (plan_on_device) fmax = max_raw_dev / 8 + namt + 8;
@@ -655,20 +721,13 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         }
         void* args[] = {&da};
         IPCFP_CUDA(cudaLaunchCooperativeKernel((const void*)k_amt_dense, s->walk_grid, DENSE_THREADS, args, 0, st)); IPCFP_LAUNCH_CHECK();
-    };
-    auto run_dense_leaf = [&]() { k_amt_dense_leaf<<<s->walk_grid, DENSE_THREADS, 0, st>>>(da); IPCFP_LAUNCH_CHECK(); };
-
-    // ---- (b) general walk: count → scan → expand per level, any AMT shape, exact errors. It is the fallback, and it sizes every
+        k_amt_dense_leaf<<<s->walk_grid, DENSE_THREADS, 0, st>>>(da); IPCFP_LAUNCH_CHECK();
+    }
+    // (b) the general walk: count → scan → expand per level, any AMT shape, exact errors. It is the fallback, and it sizes every
     // buffer by what it walks rather than by the store: each parent block's AMTs are walked on their own, so parents that share their
     // messages need a frontier per parent while the store holds those nodes once. Below the fused rounds it synchronises once per level
     // and allocates that level's output from the exact total its scan computed.
-    AsyncBuf<uint64_t> d_rng;
-    AsyncBuf<uint32_t> g_blk[2], g_meta[2];
-    AsyncBuf<uint64_t> g_base[2];
-    auto ensure_scratch = [&](uint64_t n) {   // scan scratch for n items
-        if (scratch.n < scan_scratch_elems(n + 64) + 64) scratch.alloc(scan_scratch_elems(n + 64) + 64, st);
-    };
-    auto run_general = [&]() {
+    void run_general() {
         d_rng.alloc(4 * IPCFP_MAX_PARENTS, st);
         IPCFP_CUDA(cudaMemcpyAsync(d_rng.p, h_rng.data(), h_rng.size() * 8, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));
@@ -683,9 +742,9 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
         IPCFP_CUDA(cudaMemcpyAsync(g_meta[0].p, fA_meta.p, namt * 4ull, cudaMemcpyDeviceToDevice, st));
         IPCFP_CUDA(cudaMemcpyAsync(g_base[0].p, fA_base.p, namt * 8ull, cudaMemcpyDeviceToDevice, st));
         int cur = 0;   // g buffer holding the frontier of `round`
-        ccount = dw + 1; ncount = dw + 2;
+        ccount = dw + DW_FRONTIER_A; ncount = dw + DW_FRONTIER_B;
         ExpandArgs ea;
-        ea.store = s->view; ea.last_round = last_round; ea.record = skip_tx ? 0 : 1; ea.wbits = wbits.p; ea.err = dw + 15;
+        ea.store = s->view; ea.last_round = last_round; ea.record = skip_tx ? 0 : 1; ea.wbits = wbits.p; ea.err = dw + DW_TX_ERR;
         ea.vals = nullptr; ea.cap = 8 * TOP_CAP;
         ea.rlo = d_rng.p; ea.rhi = d_rng.p + 2 * IPCFP_MAX_PARENTS;
         auto alloc_vals = [&](uint64_t n) {
@@ -718,9 +777,9 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
             k_amt_count<<<(unsigned)(slots / 128), 128, 0, st>>>(s->view, gview(cur), ccount, round, last_round, (uint32_t)items, counts.p, ea.rlo, ea.rhi);
             IPCFP_LAUNCH_CHECK();
             exclusive_scan_u32(counts.p, out_off.p, slots, (uint64_t*)total_dev, scratch.p, st);
-            publish_words(s, (uint32_t)(total_dev - dw), 1);
+            publish_words(s, DW_LEVEL_TOTAL, 1);
             IPCFP_CUDA(cudaStreamSynchronize(st));
-            const uint64_t total = hw[total_dev - dw];
+            const uint64_t total = hw[DW_LEVEL_TOTAL];
             if (round == last_round) alloc_vals(total);   // before `a` copies ea.vals
             ExpandArgs a = ea;
             a.in = gview(cur); a.in_count = ccount; a.round = round; a.out_off = out_off.p; a.out = gview(cur ^ 1);
@@ -738,304 +797,269 @@ ipcfp_event_result* generate_event_proof(Store* s, const ipcfp_tipset_desc* /*t*
             items = total;
         }
         // *ccount now holds the number of raw execution entries.
-    };
-    bool dense_used = plan_on_device || plan.ok;   // device plan: whether it is ok is known at the next synchronisation
-    if (dense_used) { run_dense(); run_dense_leaf(); } else run_general();
-    IPCFP_CUDA(cudaEventRecord(s->ev[9], st));   // the raw message list of this call is complete (cross-shard exchange waits for it)
-    bool xch_early = false;
-    if (xch) {
-        // EARLY H0: with dense message AMTs the length of this shard's slice is known from the roots alone (plan.nraw), so the peers can
-        // agree on the slices while the walk is still running and the whole execution-order exchange goes onto the (high-priority)
-        // exchange stream right behind it — it then runs under the witness snapshot, the host's sync and pass 1 instead of after them.
-        // A shard that cannot promise its slice yet (sparse AMTs → general walk, a fault in the prologue) says so and EVERY shard takes
-        // the late path below; a promise that turns out wrong (the dense walk raised its flag) is repaired after pass 2 (`stale`).
-        xch->agree_early(plan.ok && !early_fault, plan.ok ? plan.nraw : 0, nraw_total);
-        xch_early = xch->all_early;
-        if (xch_early) xch->start_exchange(exec_raw.p, s->ev[9]);
     }
-    // Witness snapshot: base witness + every message-AMT block are final at this point — start moving
-    // them to the host while pass 1 / pass 2 run (witness.cu).
-    WitnessBuilder wbuild(s);
-    wbuild.by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
-    if (!exo) wbuild.snapshot(wbits.p);
-    publish_words(s, 0, 18);   // error word, frontier counters (dw[1]/dw[2]), witness counts (dw[8], dw[9]), dense-walk flag (dw[14]), gather split (dw[16], dw[17])
-    if (plan_on_device) publish_prologue();
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (plan_on_device) read_prologue();
-    if (dense_used && hw[14] != 0) {   // the AMTs are not what the dense walk assumes (or its plan was not ok): redo the walk with the general kernels
-        dense_used = false;
-        k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();   // re-seed the frontier (same outputs as before)
-        run_general();
-        IPCFP_CUDA(cudaEventRecord(s->ev[9], st));
-        if (!exo) wbuild.snapshot(wbits.p);
-        publish_words(s, 0, 18);
+    // Witness snapshot: base witness + every message-AMT block are final at this point — start moving them to the host while pass 1 /
+    // pass 2 run (witness.cu). Publishes the error word, frontier counters, witness counts, dense-walk flag and gather split.
+    void snapshot_and_sync(bool with_prologue) {
+        if (!exo) wbuild->snapshot(wbits.p);
+        publish_words(s, 0, DW_SPLIT_BYTES + 1);
+        if (with_prologue) publish_prologue();
         IPCFP_CUDA(cudaStreamSynchronize(st));
+        if (with_prologue) read_prologue();
     }
-    const uint32_t ccount_idx = (uint32_t)(ccount - dw);
-    if (!sharded && hw[15] != IPCFP_NO_ERROR) {
-        // a node fault (level < 31) in a message AMT tall enough for its indices to outgrow the key: resolve it in order
-        const uint64_t key = hw[15];
-        const uint32_t eidx = (uint32_t)(key >> 56), level = 31u - ((uint32_t)(key >> 7) & 31u);
-        if (eidx != IPCFP_TX_EIDX_NONE && eidx % 3 != 0 && level < 31) {
-            const uint32_t amt = 2 * (eidx / 3) + eidx % 3 - 1;
-            if (ph->misc[64 + amt] > TX_KEY_EXACT_HEIGHT) {
-                k_amt_first_fault<<<1, 1, 0, st>>>(s->view, sa.txmeta_cids, amt, dw + 15); IPCFP_LAUNCH_CHECK();
-                publish_words(s, 15, 1);
-                IPCFP_CUDA(cudaStreamSynchronize(st));
+
+    // ---- after the walk: early H0, snapshot, the dense fallback, the first fault of a tall AMT, the capacity check, late H0
+    void settle_walk() {
+        if (xch) {
+            // EARLY H0: with dense message AMTs the length of this shard's slice is known from the roots alone (plan.nraw), so the peers can
+            // agree on the slices while the walk is still running and the whole execution-order exchange goes onto the (high-priority)
+            // exchange stream right behind it — it then runs under the witness snapshot, the host's sync and pass 1 instead of after them.
+            // A shard that cannot promise its slice yet (sparse AMTs → general walk, a fault in the prologue) says so and EVERY shard takes
+            // the late path below; a promise that turns out wrong (the dense walk raised its flag) is repaired after pass 2 (`stale`).
+            xch->agree_early(plan.ok && !early_fault, plan.ok ? plan.nraw : 0, nraw_total);
+            xch_early = xch->all_early;
+            if (xch_early) xch->start_exchange(exec_raw.p);
+        }
+        wbuild.emplace(s);
+        wbuild->by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
+        snapshot_and_sync(plan_on_device);
+        if (dense_used && hw[DW_DENSE_FAIL] != 0) {   // the AMTs are not what the dense walk assumes (or its plan was not ok): redo the walk with the general kernels
+            dense_used = false;
+            k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();   // re-seed the frontier (same outputs as before)
+            run_general();
+            IPCFP_CUDA(cudaEventRecord(s->ev[EV_RAW_LIST], st));
+            snapshot_and_sync(false);
+        }
+        const uint32_t ccount_idx = (uint32_t)(ccount - dw);
+        if (!sharded && hw[DW_TX_ERR] != IPCFP_NO_ERROR) {
+            // a node fault (level < 31) in a message AMT tall enough for its indices to outgrow the key: resolve it in order
+            const uint64_t key = hw[DW_TX_ERR];
+            const uint32_t eidx = (uint32_t)(key >> 56), level = 31u - ((uint32_t)(key >> 7) & 31u);
+            if (eidx != IPCFP_TX_EIDX_NONE && eidx % 3 != 0 && level < 31) {
+                const uint32_t amt = 2 * (eidx / 3) + eidx % 3 - 1;
+                if (ph->misc[64 + amt] > TX_KEY_EXACT_HEIGHT) {
+                    k_amt_first_fault<<<1, 1, 0, st>>>(s->view, sa.txmeta_cids, amt, dw + DW_TX_ERR); IPCFP_LAUNCH_CHECK();
+                    publish_words(s, DW_TX_ERR, 1);
+                    IPCFP_CUDA(cudaStreamSynchronize(st));
+                }
             }
         }
+        note_errors();
+        if (!dense_used && hw[ccount_idx] > raw_cap) {
+            if (!xch) throw Error(IPCFP_ERR_UNSUPPORTED, "unsupported input (message list longer than the walk's capacity)");
+            pend_tx = std::min<uint64_t>(pend_tx, tx_err_key(IPCFP_TX_EIDX_NONE, 0, 0, DC_UNSUPPORTED, 1));
+        }
+        nraw = dense_used ? (plan_on_device ? ph->plan.nraw : plan.nraw) : std::min<uint64_t>(hw[ccount_idx], raw_cap);
+        // early mode: the exchange that is running was fed the PLANNED slice; if the dense walk gave up, the list was rewritten underneath it
+        xch_stale = xch_early && (!dense_used || nraw != plan.nraw);
+        if (xch && !xch_early && (pend_tx != IPCFP_NO_ERROR || pend_err != IPCFP_NO_ERROR)) {
+            // this shard has no message list: tell the peers (H0), then fail — with the first error over ALL shards, like them
+            xch->agree_slices(pend_tx, pend_err, 0);
+            throw_first(xch->g_tx, xch->g_err);
+        }
+        if (!exo) wbuild->start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_SPLIT_IDX], hw[DW_SPLIT_BYTES]);
+        if (xch && !xch_early) {
+            // LATE H0 (some shard could not promise its slice before its walk was over): agree on the slices now and start the exchange
+            xch->agree_slices(IPCFP_NO_ERROR, IPCFP_NO_ERROR, nraw);
+            if (!xch->peers_ok) { IPCFP_CUDA(cudaStreamSynchronize(st)); throw_first(xch->g_tx, xch->g_err); }
+            xch->start_exchange(exec_raw.p);
+        }
     }
-    note_errors(hw);
-    if (!dense_used && hw[ccount_idx] > raw_cap) {
-        if (!xch) throw Error(IPCFP_ERR_UNSUPPORTED, "unsupported input (message list longer than the walk's capacity)");
-        pend_tx = std::min<uint64_t>(pend_tx, tx_err_key(IPCFP_TX_EIDX_NONE, 0, 0, DC_UNSUPPORTED, 1));
-    }
-    uint64_t nraw = dense_used ? (plan_on_device ? ph->plan.nraw : plan.nraw) : std::min<uint64_t>(hw[ccount_idx], raw_cap);
-    // early mode: the exchange that is running was fed the PLANNED slice; if the dense walk gave up, the list was rewritten underneath it
-    bool xch_stale = xch_early && (!dense_used || nraw != plan.nraw);
-    if (xch && !xch_early && (pend_tx != IPCFP_NO_ERROR || pend_err != IPCFP_NO_ERROR)) {
-        // this shard has no message list: tell the peers (H0), then fail — with the first error over ALL shards, like them
-        xch->agree_slices(pend_tx, pend_err, 0);
-        throw_global(xch->g_tx, xch->g_err, false);
-    }
-    if (!exo) wbuild.start_copy(hw[8], hw[9], hw[16], hw[17]);
-    if (xch && !xch_early) {
-        // LATE H0 (some shard could not promise its slice before its walk was over): agree on the slices now and start the exchange
-        xch->agree_slices(IPCFP_NO_ERROR, IPCFP_NO_ERROR, nraw);
-        if (!xch->peers_ok) { IPCFP_CUDA(cudaStreamSynchronize(st)); throw_global(xch->g_tx, xch->g_err, false); }
-        xch->start_exchange(exec_raw.p, s->ev[9]);
-    }
-    AsyncBuf<uint32_t> exec_idx(nraw + 32, st), keep_bits((nraw + 31) / 32 + 8, st);
-    unsigned long long* n_exec_dev = dw + 3;
-    if (sharded) IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));   // execution order is resolved across ranks by the caller
-    else if (nraw) {
-        // positions in the list are 32-bit (dedup table, exec_idx): 2^32 entries are 160 GB of message CIDs, past device memory
-        if (nraw >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "message list of 2^32 entries or more");
-        ensure_scratch((nraw + 31) / 32);   // the general walk's list can outgrow the scratch sized for the store and the receipts
-        uint64_t slots = 64;
-        while (slots < 2 * nraw) slots <<= 1;
-        AsyncBuf<unsigned long long> dtab(slots, st);
-        dtab.zero();
-        k_dedup_insert<<<div_up(nraw, 256), 256, 0, st>>>(exec_raw.p, nraw, dtab.p, slots - 1); IPCFP_LAUNCH_CHECK();
-        k_dedup_flags<<<div_up((nraw + 31) / 32 * 32, 256), 256, 0, st>>>(exec_raw.p, nraw, dtab.p, slots - 1, keep_bits.p); IPCFP_LAUNCH_CHECK();
-        AsyncBuf<uint64_t> wp2((nraw + 31) / 32 + 8, st);
-        bitmap_to_indices(keep_bits.p, nraw, exec_idx.p, (uint64_t*)n_exec_dev, wp2.p, scratch.p, st);
-    } else IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));
-    IPCFP_CUDA(cudaEventRecord(s->ev[2], st));
-    if (exo) {
+
+    // ---- first-seen dedup of the raw list: the execution order. False: execution-order-only mode, which ends here
+    bool dedup() {
+        exec_idx.alloc(nraw + 32, st); keep_bits.alloc((nraw + 31) / 32 + 8, st);
+        n_exec_dev = dw + DW_N_EXEC;
+        if (sharded) IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));   // execution order is resolved across ranks by the caller
+        else if (nraw) {
+            // positions in the list are 32-bit (dedup table, exec_idx): 2^32 entries are 160 GB of message CIDs, past device memory
+            if (nraw >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "message list of 2^32 entries or more");
+            ensure_scratch((nraw + 31) / 32);   // the general walk's list can outgrow the scratch sized for the store and the receipts
+            uint64_t slots = 64;
+            while (slots < 2 * nraw) slots <<= 1;
+            AsyncBuf<unsigned long long> dtab(slots, st);
+            dtab.zero();
+            k_dedup_insert<<<div_up(nraw, 256), 256, 0, st>>>(exec_raw.p, nraw, dtab.p, slots - 1); IPCFP_LAUNCH_CHECK();
+            k_dedup_flags<<<div_up((nraw + 31) / 32 * 32, 256), 256, 0, st>>>(exec_raw.p, nraw, dtab.p, slots - 1, keep_bits.p); IPCFP_LAUNCH_CHECK();
+            AsyncBuf<uint64_t> wp2((nraw + 31) / 32 + 8, st);
+            bitmap_to_indices(keep_bits.p, nraw, exec_idx.p, (uint64_t*)n_exec_dev, wp2.p, scratch.p, st);
+        } else IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_EXEC_ORDER], st));
+        if (!exo) return true;
         // execution-order-only mode (the batched verifier, verify.cu): hand the order over and stop before the scan
-        publish_words(s, 3, 1);
+        publish_words(s, DW_N_EXEC, 1);
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        exo->n_exec = hw[3];
+        exo->n_exec = hw[DW_N_EXEC];
         exo->nraw = nraw;
         exo->exec_raw = std::move(exec_raw);
         exo->exec_idx = std::move(exec_idx);
-        return nullptr;
+        return false;
     }
 
-    // ---- PASS 1
-    AsyncBuf<uint32_t> match_bits((N + 31) / 32 + 8, st), cnt(N + 8, st), nby(N + 8, st);
-    AsyncBuf<uint64_t> pbase(N + 8, st), bbase(N + 8, st);
-    Pass1Args p1;
-    p1.store = s->view; p1.store_dev = s->view_dev.p; p1.m_dev = d_matcher; p1.m = mh; p1.events_roots = td.events_roots.p; p1.has_root = td.has_root.p; p1.lo = lo; p1.hi = hi;
-    p1.match_bits = match_bits.p; p1.cnt = cnt.p; p1.nbytes = nby.p; p1.err = dw; p1.stats = dw + 4;
-    if (N) {
-        // 4 warps per CTA, 3 CTAs per SM; every lane has a ring of 4 chunks of 128 bytes, one chunk filled per pass (pass1_stage.cuh)
-        const int smem = 4 * StageGeom<128, 4, 1>::WARP_BYTES;
-        IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        k_pass1_stage<128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
+    // ---- pass 1: matching receipts, per-receipt proof counts and bytes
+    void pass1() {
+        match_bits.alloc((N + 31) / 32 + 8, st); cnt.alloc(N + 8, st); nby.alloc(N + 8, st);
+        pbase.alloc(N + 8, st); bbase.alloc(N + 8, st);
+        Pass1Args p1;
+        p1.store = s->view; p1.store_dev = s->view_dev.p; p1.m_dev = d_matcher; p1.m = mh; p1.events_roots = td.events_roots.p; p1.has_root = td.has_root.p; p1.lo = lo; p1.hi = hi;
+        p1.match_bits = match_bits.p; p1.cnt = cnt.p; p1.nbytes = nby.p; p1.err = dw + DW_ERR; p1.stats = dw + DW_STATS;
+        if (N) {
+            // 4 warps per CTA, 3 CTAs per SM; every lane has a ring of 4 chunks of 128 bytes, one chunk filled per pass (pass1_stage.cuh)
+            const int smem = 4 * StageGeom<128, 4, 1>::WARP_BYTES;
+            IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            k_pass1_stage<128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
+        }
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS1], st));
+        match_rel.alloc(N + 32, st);
+        wp3.alloc((N + 31) / 32 + 8, st);
+        bitmap_to_indices(match_bits.p, (N + 31) / 32 * 32, match_rel.p, (uint64_t*)(dw + DW_N_MATCH), wp3.p, scratch.p, st);
+        exclusive_scan_u32(cnt.p, pbase.p, N, (uint64_t*)(dw + DW_N_PROOFS), scratch.p, st);
+        exclusive_scan_u32(nby.p, bbase.p, N, (uint64_t*)(dw + DW_BLOB_BYTES), scratch.p, st);
+        publish_words(s, 0, DW_TX_ERR + 1);
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        note_errors();
+        n_exec = hw[DW_N_EXEC];
+        M = hw[DW_N_MATCH];
+        pass1_nodes = hw[DW_STATS]; pass1_bytes = hw[DW_STATS + 1];
+        n_proofs = hw[DW_N_PROOFS]; n_bytes = hw[DW_BLOB_BYTES];
     }
-    IPCFP_CUDA(cudaEventRecord(s->ev[3], st));
-    AsyncBuf<uint32_t> match_rel(N + 32, st);
-    AsyncBuf<uint64_t> wp3((N + 31) / 32 + 8, st);
-    unsigned long long* n_match_dev = dw + 6;
-    bitmap_to_indices(match_bits.p, (N + 31) / 32 * 32, match_rel.p, (uint64_t*)n_match_dev, wp3.p, scratch.p, st);
-    exclusive_scan_u32(cnt.p, pbase.p, N, (uint64_t*)(dw + 7), scratch.p, st);
-    exclusive_scan_u32(nby.p, bbase.p, N, (uint64_t*)(dw + 12), scratch.p, st);
-    publish_words(s, 0, 16);
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    note_errors(hw);
-    uint64_t n_exec = hw[3];
-    const uint64_t M = hw[6];
-    const uint64_t pass1_nodes = hw[4], pass1_bytes = hw[5];
-    uint64_t n_proofs = hw[7], n_bytes = hw[12];
 
-    // ---- PASS 2
-    std::unique_ptr<EventResultBox> box(new EventResultBox());
-    memset(&box->r, 0, sizeof box->r);
-    AsyncBuf<ipcfp_event_proof> d_proofs(n_proofs + 1, st);
-    AsyncBuf<uint8_t> d_blob(n_bytes + 16, st);
-    uint32_t* any_skip_dev = misc + 2;
-    if (M) {
-        Pass2Args p2;
-        p2.store = s->view; p2.store_dev = s->view_dev.p; p2.m_dev = d_matcher; p2.m = mh; p2.events_roots = td.events_roots.p; p2.lo = lo; p2.match_rel = match_rel.p; p2.n_match = M;
-        p2.receipts_root_blk = receipts_root_blk; p2.exec_cids = exec_raw.p; p2.exec_idx = exec_idx.p; p2.n_exec = n_exec_dev;
-        p2.wbits = wbits.p; p2.err = dw; p2.cnt = cnt.p; p2.proof_base = pbase.p; p2.byte_base = bbase.p;
-        p2.proofs = d_proofs.p; p2.blob = d_blob.p; p2.any_skip = any_skip_dev; p2.resolve_msg = sharded ? 0 : 1;
-        p2.per_warp = (M <= 16384 && !getenv("IPCFP_PASS2_PER_THREAD")) ? 1 : 0;
-        k_pass2<<<div_up(p2.per_warp ? M * 32 : M, 128), 128, 0, st>>>(p2); IPCFP_LAUNCH_CHECK();
+    // ---- pass 2: receipts-AMT paths, events walks, EventProofs; the late witness blocks
+    void pass2() {
+        box.reset(new EventResultBox());
+        memset(&box->r, 0, sizeof box->r);
+        d_proofs.alloc(n_proofs + 1, st);
+        d_blob.alloc(n_bytes + 16, st);
+        if (M) {
+            Pass2Args p2;
+            p2.store = s->view; p2.store_dev = s->view_dev.p; p2.m_dev = d_matcher; p2.m = mh; p2.events_roots = td.events_roots.p; p2.lo = lo; p2.match_rel = match_rel.p; p2.n_match = M;
+            p2.receipts_root_blk = receipts_root_blk; p2.exec_cids = exec_raw.p; p2.exec_idx = exec_idx.p; p2.n_exec = n_exec_dev;
+            p2.wbits = wbits.p; p2.err = dw + DW_ERR; p2.cnt = cnt.p; p2.proof_base = pbase.p; p2.byte_base = bbase.p;
+            p2.proofs = d_proofs.p; p2.blob = d_blob.p; p2.any_skip = misc + 2; p2.resolve_msg = sharded ? 0 : 1;
+            p2.per_warp = (M <= 16384 && !getenv("IPCFP_PASS2_PER_THREAD")) ? 1 : 0;
+            k_pass2<<<div_up(p2.per_warp ? M * 32 : M, 128), 128, 0, st>>>(p2); IPCFP_LAUNCH_CHECK();
+        }
+        // pass 2 did not wait for the cross-shard exchange; now that both are done: P (parallel.cu)
+        if (xch) xch->positions_for(match_rel.p, M, n_exec_dev);
+        // blocks recorded by pass 2 (receipt paths + events AMTs of the matches): the late part of the witness
+        wbuild->finish_enqueue(wbits.p);
+        publish_words(s, 0, DW_EXEC_CHECK + 1);
+        publish_words(s, HW_ANY_SKIP, HW_ANY_SKIP_WORDS, misc);
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        note_errors();
+        // base-witness CIDs (parent headers, child header, TxMeta) are only dereferenced by WitnessCollector::materialize
+        // (common/witness.rs:43-56, events/generator.rs:104), i.e. AFTER every receipts-root / pass-1 / pass-2 failure
+        if (!xch && missing_base && !skip_tx) throw_first(IPCFP_NO_ERROR, IPCFP_NO_ERROR, true);
+        mB = hw[DW_WIT_B];
+        any_skip = ((const uint32_t*)(hw + HW_ANY_SKIP))[2] != 0;
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS2], st));
     }
-    if (xch) {
-        // pass 2 did not wait for the cross-shard exchange; now that both are done: the global n_exec, the raw positions of this rank's
-        // matches, and exec.get(i) of events/generator.rs:244-246 for every match — it PRECEDES r_amt.get(i) in the reference, so at the
-        // same receipt it outranks whatever pass 2 reported (code 0 sorts first in the error word)
-        // (all of it on the EXCHANGE stream, behind the exchange: the engine stream goes on with the witness and never waits for a peer)
-        cudaStream_t sx = xch->stream();
-        xch->positions_for(sx, match_rel.p, M, n_exec_dev);
-        IPCFP_CUDA(cudaMemsetAsync(dw + 19, 0xff, 8, sx));   // the check has its own word: it may have to be repeated (stale exchange)
-        if (M) { k_check_exec<<<div_up(M, 128), 128, 0, sx>>>(match_rel.p, M, lo, n_exec_dev, dw + 19); IPCFP_LAUNCH_CHECK(); }
-        publish_words_on(s, sx, dw + 19, 19, 1);
-    }
-    // blocks recorded by pass 2 (receipt paths + events AMTs of the matches): the late part of the witness
-    wbuild.finish_enqueue(wbits.p);
-    publish_words(s, 0, 20);
-    publish_words_from(s, misc, 20, 2);   // misc[2] = any_skip (32-bit words 0..3 land in hw[20..21])
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    note_errors(hw);
-    // base-witness CIDs (parent headers, child header, TxMeta) are only dereferenced by WitnessCollector::materialize
-    // (common/witness.rs:43-56, events/generator.rs:104), i.e. AFTER every receipts-root / pass-1 / pass-2 failure
-    if (!xch && missing_base && !skip_tx) throw Error(IPCFP_ERR_MISSING_BLOCK, "missing block (base witness CID not in the store)");
-    const uint64_t mB = hw[10];
-    const bool any_skip = ((const uint32_t*)(hw + 20))[2] != 0;
-    IPCFP_CUDA(cudaEventRecord(s->ev[4], st));
 
-    // ---- results to the host
-    box->matching = PinnedArray(s->pool, (M + 1) * 8);
-    box->proofs = PinnedArray(s->pool, (n_proofs + 1) * sizeof(ipcfp_event_proof));
-    box->blob = PinnedArray(s->pool, n_bytes + 16);
-    PinnedArray rel(s->pool, (M + 1) * 4);
-    if (M) IPCFP_CUDA(cudaMemcpyAsync(rel.p, match_rel.p, M * 4, cudaMemcpyDeviceToHost, st));
-    if (n_proofs && !xch) IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_proofs.p, n_proofs * sizeof(ipcfp_event_proof), cudaMemcpyDeviceToHost, st));
-    if (n_bytes) IPCFP_CUDA(cudaMemcpyAsync(box->blob.p, d_blob.p, n_bytes, cudaMemcpyDeviceToHost, st));
-
-    // ---- witness: late blocks, sort in Cid order, index arrays (engine stream; the sharded protocol's tail runs beside it)
-    wbuild.finish_start(mB, hw[11], box->wit);
-    uint8_t* union_dev = nullptr;
-    if (xch) {
-        cudaStream_t sx = xch->stream();
-        // H2: how far did every shard get. All ranks continue or fail together, naming the same first error. (The host waits for its
-        // peers here while its own GPU sorts the witness.)
-        IPCFP_CUDA(cudaStreamSynchronize(sx));
-        uint64_t pend_chk = hw[19];
-        xch->agree_results(pend_tx, std::min(pend_err, pend_chk), missing_base && !skip_tx, n_proofs, hw[8] + mB, xch->host_word(300), xch_stale);
-        if (xch->g_stale && xch->g_tx == IPCFP_NO_ERROR) {
-            // some shard's early promise was wrong: its slice differs from what the running exchange used. Every shard repeats the
-            // exchange with the slices as they really are (late H0), then the positions, the exec.get check and H2.
-            xch->agree_slices(pend_tx, pend_err, nraw);
-            if (xch->peers_ok) {
-                xch->start_exchange(exec_raw.p, s->ev[9]);
-                xch->positions_for(sx, match_rel.p, M, n_exec_dev);
-                IPCFP_CUDA(cudaMemsetAsync(dw + 19, 0xff, 8, sx));
-                if (M) { k_check_exec<<<div_up(M, 128), 128, 0, sx>>>(match_rel.p, M, lo, n_exec_dev, dw + 19); IPCFP_LAUNCH_CHECK(); }
-                publish_words_on(s, sx, dw + 19, 19, 1);
-                IPCFP_CUDA(cudaStreamSynchronize(sx));
-                pend_chk = hw[19];
+    // ---- results to the host; the witness's late blocks, Cid order and index arrays (engine stream); the sharded tail beside it; JSON
+    void read_back() {
+        box->matching = PinnedArray(s->pool, (M + 1) * 8);
+        box->proofs = PinnedArray(s->pool, (n_proofs + 1) * sizeof(ipcfp_event_proof));
+        box->blob = PinnedArray(s->pool, n_bytes + 16);
+        rel = PinnedArray(s->pool, (M + 1) * 4);
+        if (M) IPCFP_CUDA(cudaMemcpyAsync(rel.p, match_rel.p, M * 4, cudaMemcpyDeviceToHost, st));
+        if (n_proofs && !xch) IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_proofs.p, n_proofs * sizeof(ipcfp_event_proof), cudaMemcpyDeviceToHost, st));
+        if (n_bytes) IPCFP_CUDA(cudaMemcpyAsync(box->blob.p, d_blob.p, n_bytes, cudaMemcpyDeviceToHost, st));
+        wbuild->finish_start(mB, hw[DW_WIT_B_BYTES], box->wit);
+        if (xch) {
+            if (!xch->agree_results(pend_tx, pend_err, missing_base && !skip_tx, n_proofs, hw[DW_WIT_A] + mB, xch_stale, exec_raw.p, nraw)) {
+                wbuild->finish_join(box->wit);   // nothing of this call may be in flight when its buffers go
+                throw_first(xch->g_tx, xch->g_err, xch->g_missing_base);
+                throw Error(IPCFP_ERR_UNSUPPORTED, "execution-order exchange: bucket overflow (skewed CID hash distribution)");
             }
-            xch->agree_results(pend_tx, std::min(pend_err, pend_chk), missing_base && !skip_tx, n_proofs, hw[8] + mB, xch->host_word(300), false);
+            xch->fetch_and_patch(d_proofs.p, n_proofs, box->proofs.p);
+            xch->witness_union(box->wit.cids_dev.p, box->wit.n, (flags & IPCFP_SHARDED_UNION_FULL) != 0);
         }
-        if (xch->g_tx != IPCFP_NO_ERROR || xch->g_err != IPCFP_NO_ERROR || xch->g_missing_base || xch->g_overflow) {
-            wbuild.finish_join(box->wit);   // nothing of this call may be in flight when its buffers go
-            throw_global(xch->g_tx, xch->g_err, xch->g_missing_base);
-            throw Error(IPCFP_ERR_UNSUPPORTED, "execution-order exchange: bucket overflow (skewed CID hash distribution)");
+        // IPCFP_RESULT_JSON: render the bundle from the device copies (json.cu) while the witness blob copy, if any, is still on the wire
+        if (flags & IPCFP_RESULT_JSON) {
+            IPCFP_CUDA(cudaEventRecord(s->ev[EV_JSON_BEGIN], st));
+            JsonInputs ji{d_proofs.p, n_proofs, d_blob.p, box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n,
+                          td.parent_epoch, td.child_epoch, td.n_parents, sa.parent_cids, sa.child_cid};
+            json_len = render_event_json(s, ji, box->json);
+            IPCFP_CUDA(cudaEventRecord(s->ev[EV_JSON_END], st));
         }
-        n_exec = xch->host_word(301);
-        // EventProof.message_cid = exec[exec_index], fetched from the shards that hold them (pass 2 is complete: the host synchronised on it)
-        xch->fetch_and_patch(sx, d_proofs.p, n_proofs);
-        if (n_proofs) IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_proofs.p, n_proofs * sizeof(ipcfp_event_proof), cudaMemcpyDeviceToHost, sx));
-        // union of the shards' witness CID sets as soon as this shard's sorted list exists (event after k_witness_emit), on its own
-        // stream and communicator: it runs beside the message-CID fetch
-        cudaStream_t sw = xch->union_stream();
-        IPCFP_CUDA(cudaStreamWaitEvent(sw, s->ev[6], 0));
-        if (flags & IPCFP_SHARDED_UNION_FULL) {
-            xch->witness_union(sw, box->wit.cids_dev.p, box->wit.n, &union_dev, (uint64_t*)(dw + 18));
-            publish_words_on(s, sw, dw + 18, 18, 1);
-        } else xch->witness_union_partitioned(sw, box->wit.cids_dev.p, box->wit.n, xch->union_piece_cap(false), &union_dev, 320);   // [size, overflow] per rank → hw[320 ..)
+        wbuild->finish_join(box->wit);
+        if (xch) xch->finish();
     }
-    // IPCFP_RESULT_JSON: render the bundle from the device copies (json.cu) while the witness blob copy, if any, is still on the wire
-    uint64_t json_len = 0;
-    if (flags & IPCFP_RESULT_JSON) {
-        IPCFP_CUDA(cudaEventRecord(s->ev[10], st));
-        JsonInputs ji{d_proofs.p, n_proofs, d_blob.p, box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n,
-                      td.parent_epoch, td.child_epoch, td.n_parents, sa.parent_cids, sa.child_cid};
-        json_len = render_event_json(s, ji, box->json);
-        IPCFP_CUDA(cudaEventRecord(s->ev[11], st));
-    }
-    wbuild.finish_join(box->wit);
-    if (xch) {
-        IPCFP_CUDA(cudaStreamSynchronize(xch->stream()));
-        IPCFP_CUDA(cudaStreamSynchronize(xch->union_stream()));
-        if (!(flags & IPCFP_SHARDED_UNION_FULL)) {
-            bool overflow = false;
-            for (uint32_t q = 0; q < world; q++) overflow |= hw[320 + 2 * q + 1] != 0;
-            if (overflow) {   // a piece did not fit its slot on some rank (every rank sees the same words): once more with slots that cannot overflow
-                xch->witness_union_partitioned(xch->union_stream(), box->wit.cids_dev.p, box->wit.n, xch->union_piece_cap(true), &union_dev, 320);
-                IPCFP_CUDA(cudaStreamSynchronize(xch->union_stream()));
-            }
+
+    // ---- the result
+    ipcfp_event_result* fill() {
+        static thread_local std::chrono::steady_clock::time_point t_last_exit = t_enter;
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_END], st));
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        {
+            uint64_t* mo = box->matching.as<uint64_t>();
+            const uint32_t* rp = rel.as<uint32_t>();
+            for (uint64_t k = 0; k < M; k++) mo[k] = lo + rp[k];
         }
-    }
-    IPCFP_CUDA(cudaEventRecord(s->ev[5], st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    {
-        uint64_t* mo = box->matching.as<uint64_t>();
-        const uint32_t* rp = rel.as<uint32_t>();
-        for (uint64_t k = 0; k < M; k++) mo[k] = lo + rp[k];
-    }
-    if (any_skip) {  // receipts the AMT does not hold (`continue` at :249-251): compact their reserved slots away
-        ipcfp_event_proof* pp = box->proofs.as<ipcfp_event_proof>();
-        uint64_t w = 0;
-        for (uint64_t k = 0; k < n_proofs; k++) if (pp[k].exec_index != UINT64_MAX) pp[w++] = pp[k];
-        n_proofs = w;
-    }
-    ipcfp_event_result& r = box->r;
-    r.n_matching = M; r.matching_indices = box->matching.as<uint64_t>();
-    r.n_proofs = n_proofs; r.proofs = box->proofs.as<ipcfp_event_proof>();
-    r.data_blob = box->blob.as<uint8_t>(); r.data_blob_size = n_bytes;
-    box->wit.fill(r.witness);
-    r.n_exec = n_exec;
-    float ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[0], s->ev[5])); r.ms_total = ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[1], s->ev[2])); r.ms_txamt = ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[2], s->ev[3])); r.ms_pass1 = ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[3], s->ev[4])); r.ms_pass2 = ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[4], s->ev[5])); r.ms_witness = ms;
-    r.pass1_bytes = pass1_bytes; r.pass1_nodes = pass1_nodes;
-    if (flags & IPCFP_RESULT_JSON) {
-        r.json = box->json.as<char>(); r.json_len = json_len;
-        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[10], s->ev[11])); r.ms_json = ms;
-    }
-    r.shard_raw_total = nraw_total;
-    if (sharded) { r.n_exec = 0; r.shard_exec_count = nraw; box->shard_exec = std::move(exec_raw); r.shard_exec_dev = box->shard_exec.p; }
-    if (xch) {
+        if (any_skip) {  // receipts the AMT does not hold (`continue` at :249-251): compact their reserved slots away
+            ipcfp_event_proof* pp = box->proofs.as<ipcfp_event_proof>();
+            uint64_t w = 0;
+            for (uint64_t k = 0; k < n_proofs; k++) if (pp[k].exec_index != UINT64_MAX) pp[w++] = pp[k];
+            n_proofs = w;
+        }
+        ipcfp_event_result& r = box->r;
+        r.n_matching = M; r.matching_indices = box->matching.as<uint64_t>();
+        r.n_proofs = n_proofs; r.proofs = box->proofs.as<ipcfp_event_proof>();
+        r.data_blob = box->blob.as<uint8_t>(); r.data_blob_size = n_bytes;
+        box->wit.fill(r.witness);
         r.n_exec = n_exec;
-        r.union_cids_dev = union_dev;
-        if (flags & IPCFP_SHARDED_UNION_FULL) { r.n_union_cids = r.n_union_part = hw[18]; r.union_part_first = 0; }
-        else {
-            r.n_union_cids = 0;
-            for (uint32_t q = 0; q < world; q++) { if (q == rank) r.union_part_first = r.n_union_cids; r.n_union_cids += hw[320 + 2 * q]; }
-            r.n_union_part = hw[320 + 2 * rank];
+        float ms;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_BEGIN], s->ev[EV_END])); r.ms_total = ms;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_SETUP], s->ev[EV_EXEC_ORDER])); r.ms_txamt = ms;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_EXEC_ORDER], s->ev[EV_PASS1])); r.ms_pass1 = ms;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_PASS1], s->ev[EV_PASS2])); r.ms_pass2 = ms;
+        IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_PASS2], s->ev[EV_END])); r.ms_witness = ms;
+        r.pass1_bytes = pass1_bytes; r.pass1_nodes = pass1_nodes;
+        if (flags & IPCFP_RESULT_JSON) {
+            r.json = box->json.as<char>(); r.json_len = json_len;
+            IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_JSON_BEGIN], s->ev[EV_JSON_END])); r.ms_json = ms;
         }
-        r.total_matching = xch->M_total; r.total_proofs = xch->proofs_total;
-        xch->timings(&r.ms_exchange, &r.ms_fetch, &r.ms_union);
-        if (getenv("IPCFP_XCH_TRACE")) {
-            float t[6]; char buf[384];
-            const int evs[6] = {2, 3, 4, 6, 7, 5};   // walk+snapshot done, pass 1 done, pass 2 done, sorted CID list, 51 MB copy done, end
-            for (int i = 0; i < 6; i++) cudaEventElapsedTime(&t[i], s->ev[0], s->ev[evs[i]]);
-            const auto t_now = std::chrono::steady_clock::now();
-            const double host_call = std::chrono::duration<double, std::milli>(t_now - t_enter).count();
-            const double host_gap = std::chrono::duration<double, std::milli>(t_enter - t_last_exit).count();
-            snprintf(buf, sizeof buf, "host: gap since last call %.3f, in call %.3f | walk %.3f pass1 %.3f pass2 %.3f sorted %.3f blobD2H %.3f end %.3f", host_gap, host_call,
-                     t[0], t[1], t[2], t[3], t[4], t[5]);
-            t_last_exit = std::chrono::steady_clock::now();
-            xch->trace_timeline(s->ev[0], buf);
+        r.shard_raw_total = nraw_total;
+        if (sharded) { r.n_exec = 0; r.shard_exec_count = nraw; box->shard_exec = std::move(exec_raw); r.shard_exec_dev = box->shard_exec.p; }
+        if (xch) {
+            xch->fill_result(r);
+            if (getenv("IPCFP_XCH_TRACE")) {
+                float t[6]; char buf[384];
+                // walk+snapshot done, pass 1 done, pass 2 done, sorted CID list, 51 MB copy done, end
+                const int evs[6] = {EV_EXEC_ORDER, EV_PASS1, EV_PASS2, EV_WITNESS_SORTED, EV_BLOB_COPIED, EV_END};
+                for (int i = 0; i < 6; i++) cudaEventElapsedTime(&t[i], s->ev[EV_BEGIN], s->ev[evs[i]]);
+                const auto t_now = std::chrono::steady_clock::now();
+                const double host_call = std::chrono::duration<double, std::milli>(t_now - t_enter).count();
+                const double host_gap = std::chrono::duration<double, std::milli>(t_enter - t_last_exit).count();
+                snprintf(buf, sizeof buf, "host: gap since last call %.3f, in call %.3f | walk %.3f pass1 %.3f pass2 %.3f sorted %.3f blobD2H %.3f end %.3f", host_gap, host_call,
+                         t[0], t[1], t[2], t[3], t[4], t[5]);
+                t_last_exit = std::chrono::steady_clock::now();
+                xch->trace_timeline(s->ev[EV_BEGIN], buf);
+            }
+            if (flags & IPCFP_SHARDED_UNION_TO_HOST) {
+                box->union_host = PinnedArray(s->pool, r.n_union_part * 38 + 64);
+                if (r.n_union_part) IPCFP_CUDA(cudaMemcpyAsync(box->union_host.p, r.union_cids_dev, r.n_union_part * 38, cudaMemcpyDeviceToHost, st));
+                IPCFP_CUDA(cudaStreamSynchronize(st));
+                r.union_cids = box->union_host.as<uint8_t>();
+            }
         }
-        if (flags & IPCFP_SHARDED_UNION_TO_HOST) {
-            box->union_host = PinnedArray(s->pool, r.n_union_part * 38 + 64);
-            if (r.n_union_part) IPCFP_CUDA(cudaMemcpyAsync(box->union_host.p, union_dev, r.n_union_part * 38, cudaMemcpyDeviceToHost, st));
-            IPCFP_CUDA(cudaStreamSynchronize(st));
-            r.union_cids = box->union_host.as<uint8_t>();
-        }
+        return &box.release()->r;
     }
-    return &box.release()->r;
+};
+}  // namespace
+
+ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
+                                         Comm* comm, ExecOrderOut* exo) {
+    EventCall c(s, td, spec, flags, sharded, lo, hi, comm, exo);
+    c.stage();
+    c.setup();
+    c.walk();
+    c.settle_walk();
+    if (!c.dedup()) return nullptr;
+    c.pass1();
+    c.pass2();
+    c.read_back();
+    return c.fill();
 }
 
 void event_result_free(ipcfp_event_result* r) { delete reinterpret_cast<EventResultBox*>(r); }

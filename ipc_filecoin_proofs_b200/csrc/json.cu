@@ -64,9 +64,9 @@ __global__ void __launch_bounds__(256) k_json_blocks(const uint8_t* __restrict__
 }
 
 // The steps both renderers share. A text is made of up to three lists of records; per list the caller enqueues the record lengths into
-// lens (the overflow flag is dev_words[26], cleared by the constructor), then offsets() scans every list and reads the list totals back
+// lens (the overflow flag is DW_JSON_OVERFLOW, cleared by the constructor), then offsets() scans every list and reads the list totals back
 // in the one host synchronisation of JSON mode, and copy_out() copies the written text into pinned host memory.
-// dev_words [24] [25] [27]: list totals, [26]: overflow flag → host words 200..203.
+// DW_JSON_TOTAL0..2: list totals → host words HW_JSON_TOTALS.
 namespace {
 struct JsonLists {
     static constexpr int MAXL = 3;
@@ -89,16 +89,16 @@ struct JsonLists {
         scratch.alloc(scan_scratch_elems(mx + 1) + 8, st);
         IPCFP_CUDA(cudaMemsetAsync(overflow(), 0, 8, st));
     }
-    unsigned long long* overflow() const { return s->dev_words.p + 26; }
+    unsigned long long* overflow() const { return s->dev_words.p + DW_JSON_OVERFLOW; }
     void offsets() {
-        static const int word[MAXL] = {24, 25, 27};
+        static const int word[MAXL] = {DW_JSON_TOTAL0, DW_JSON_TOTAL1, DW_JSON_TOTAL2};
         unsigned long long* dw = s->dev_words.p;
         for (int k = 0; k < nl; k++) exclusive_scan_u32(lens[k].p, offs[k].p, n[k], (uint64_t*)(dw + word[k]), scratch.p, st);
-        publish_words_from(s, dw + 24, 200, 4);
+        publish_words(s, HW_JSON_TOTALS, HW_JSON_TOTALS_WORDS, dw + DW_JSON_TOTAL0);
         IPCFP_CUDA(cudaStreamSynchronize(st));   // the exact length of the text: JSON mode's one host synchronisation
         const uint64_t* hw = s->host_words.p;
-        if (hw[202]) throw Error(IPCFP_ERR_UNSUPPORTED, "a record of the JSON bundle is longer than 4 GiB");
-        for (int k = 0; k < nl; k++) total[k] = hw[200 + word[k] - 24];
+        if (hw[HW_JSON_TOTALS + DW_JSON_OVERFLOW - DW_JSON_TOTAL0]) throw Error(IPCFP_ERR_UNSUPPORTED, "a record of the JSON bundle is longer than 4 GiB");
+        for (int k = 0; k < nl; k++) total[k] = hw[HW_JSON_TOTALS + word[k] - DW_JSON_TOTAL0];
     }
     void copy_out(const char* d_text, uint64_t len, PinnedArray& out) const {
         out = PinnedArray(s->pool, len + 1);

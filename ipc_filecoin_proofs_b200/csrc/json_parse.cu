@@ -34,7 +34,7 @@ struct JpMeta {
     unsigned long long witness_bytes;
     unsigned long long e_total, b_total;
 };
-static const uint32_t JP_HOST_WORD = 500;   // the meta words land in the store's pinned host words from here on
+static_assert(sizeof(JpMeta) <= HW_JP_META_WORDS * 8, "the meta words fit their host words (HW_JP_META)");
 
 __global__ void __launch_bounds__(256) k_jp_mark(const char* __restrict__ t, uint64_t len, uint32_t* bits, uint64_t nwords) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -212,7 +212,7 @@ static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, in
     k_jp_records<<<div_up(cap * 32, 128), 128, 0, st>>>(d_text.p, len, pos.p, cap, meta.p, elen.p, blen.p); IPCFP_LAUNCH_CHECK();
     exclusive_scan_u32(elen.p, eoff.p, cap, (uint64_t*)&meta.p->e_total, scratch.p, st);
     exclusive_scan_u32(blen.p, boff.p, cap, (uint64_t*)&meta.p->b_total, scratch.p, st);
-    uint64_t* hm = s->host_words.p + JP_HOST_WORD;
+    uint64_t* hm = s->host_words.p + HW_JP_META;
     IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, sizeof(JpMeta), cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 1
     JpMeta m;

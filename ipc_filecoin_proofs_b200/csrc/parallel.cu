@@ -635,6 +635,14 @@ __global__ void k_part_pack(const RawCid* __restrict__ list, uint64_t n, uint32_
 __global__ void k_part_counts(const RawCid* __restrict__ recv, uint32_t world, uint64_t cap, uint64_t* counts) {
     for (uint32_t r = threadIdx.x; r < world; r += blockDim.x) counts[r] = recv[(uint64_t)r * (cap + 1)].w[0];
 }
+// exec.get(i) for every matching receipt against the GLOBAL execution order length (sharded calls: the order spans shards)
+__global__ void k_check_exec(const uint32_t* __restrict__ match_rel, uint64_t n_match, uint64_t lo, const unsigned long long* __restrict__ n_exec,
+                             unsigned long long* err) {
+    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_match) return;
+    const uint64_t i = lo + match_rel[t];
+    if (i >= *n_exec) report_error(err, ST_PASS2, i, 0 /* DC_MISSING_EXEC, ranked before every other code at the same receipt */, 0);
+}
 }  // namespace ipcfp
 
 // ------------------------------------------------------------------------------------------ host side of the protocol
@@ -664,12 +672,9 @@ static void run_all_gather_host(Comm* c, const uint64_t* mine, uint32_t k, uint6
     (void)all;
 }
 
-uint64_t ShardExchange::host_word(uint32_t i) const { return s->host_words.p[i]; }
-cudaStream_t ShardExchange::stream() const { return c->sx; }
-cudaStream_t ShardExchange::union_stream() const { return c->sw; }
 ShardExchange::ShardExchange(Comm* comm, Store* store, uint64_t lo_, uint64_t hi_) : c(comm), s(store), lo(lo_), hi(hi_) {
     if (c->device != s->device) throw Error(IPCFP_ERR_INVALID_ARG, "communicator and store are bound to different devices");
-    if (c->world > 255) throw Error(IPCFP_ERR_UNSUPPORTED, "world too large");
+    if (c->world > MAX_WORLD) throw Error(IPCFP_ERR_UNSUPPORTED, "world too large");
 }
 
 // EARLY H0: can every shard promise the length of its slice already (dense message AMTs: known from the roots), and do all shards see the
@@ -720,12 +725,12 @@ void ShardExchange::agree_slices(uint64_t tx_key, uint64_t err_key, uint64_t nse
 }
 
 // X: bucketize → all-to-all → dedup → duplicate bitmap → all-reduce, all on the exchange stream (runs underneath pass 1)
-void ShardExchange::start_exchange(const void* seg_dev, cudaEvent_t seg_ready) {
+void ShardExchange::start_exchange(const void* seg_dev) {
     NcclApi* n = nccl_api();
     const uint32_t W = c->world;
     cudaStream_t sx = c->sx;
     seg = (const RawCid*)seg_dev;
-    IPCFP_CUDA(cudaStreamWaitEvent(sx, seg_ready, 0));
+    IPCFP_CUDA(cudaStreamWaitEvent(sx, s->ev[EV_RAW_LIST], 0));
     IPCFP_CUDA(cudaEventRecord(c->tm[0], sx));
     cap = max_nseg / W + max_nseg / (4 * W) + 1024;
     const uint64_t segbytes = XSEG_HDR + cap * 48;
@@ -782,11 +787,15 @@ void ShardExchange::start_exchange(const void* seg_dev, cudaEvent_t seg_ready) {
     overflow_dev = overflow;
 }
 
-// P: before pass 2 — the global n_exec for the "Missing message at index" check, raw positions of this rank's matches
-void ShardExchange::positions_for(cudaStream_t st, const uint32_t* match_rel, uint64_t n_match, unsigned long long* n_exec_out) {
+// P: the global n_exec, raw positions of this rank's matches, and exec.get(i) of events/generator.rs:244-246 for every match — it
+// PRECEDES r_amt.get(i) in the reference, so at the same receipt it outranks whatever pass 2 reported (code 0 sorts first in the error
+// word). All of it on the exchange stream behind X: the engine stream goes on with the witness and never waits for a peer.
+void ShardExchange::positions_for(const uint32_t* match_rel, uint64_t n_match, unsigned long long* n_exec_out_) {
+    cudaStream_t st = c->sx;
+    n_exec_out = n_exec_out_;
     IPCFP_CUDA(cudaStreamWaitEvent(st, c->ev_a, 0));
     IPCFP_CUDA(cudaMemcpyAsync(n_exec_out, n_exec_dev, 8, cudaMemcpyDeviceToDevice, st));
-    publish_words_on(s, st, overflow_dev, 300, 2);   // host_words[300] = exchange overflow flag, [301] = n_exec: read after the next sync of that stream
+    publish_words(s, HW_EXCH_OVERFLOW, HW_EXCHANGE_WORDS, overflow_dev, st);   // overflow flag, n_exec: read after the next sync of that stream
     M = n_match;
     c->req.ensure(n_match + 64);
     if (n_match) {
@@ -794,10 +803,36 @@ void ShardExchange::positions_for(cudaStream_t st, const uint32_t* match_rel, ui
         IPCFP_LAUNCH_CHECK();
     }
     match_rel_dev = match_rel;
+    unsigned long long* chk = s->dev_words.p + DW_EXEC_CHECK;   // the check has its own word: it may have to be repeated (stale exchange)
+    IPCFP_CUDA(cudaMemsetAsync(chk, 0xff, 8, st));
+    if (n_match) { k_check_exec<<<div_up(n_match, 128), 128, 0, st>>>(match_rel, n_match, lo, n_exec_out, chk); IPCFP_LAUNCH_CHECK(); }
+    publish_words(s, DW_EXEC_CHECK, 1, nullptr, st);
 }
 
-// H2: every rank reports how far it got; all ranks continue or fail TOGETHER, with the same (first) error
-void ShardExchange::agree_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, uint64_t exch_overflow, bool stale) {
+// H2 (the host waits for its peers here while its own GPU sorts the witness). All ranks continue or fail together, naming the same first
+// error. When some shard's early promise was wrong, its slice differs from what the running exchange used: every shard repeats the
+// exchange with the slices as they really are (late H0), then the positions, the exec.get check and H2.
+bool ShardExchange::agree_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, bool stale, const void* seg_dev,
+                                  uint64_t nseg_) {
+    const uint64_t* hw = s->host_words.p;
+    IPCFP_CUDA(cudaStreamSynchronize(c->sx));
+    uint64_t pend_chk = hw[DW_EXEC_CHECK];
+    gather_results(tx_key, std::min(err_key, pend_chk), missing_base, n_proofs, n_witness, hw[HW_EXCH_OVERFLOW], stale);
+    if (g_stale && g_tx == IPCFP_NO_ERROR) {
+        agree_slices(tx_key, err_key, nseg_);
+        if (peers_ok) {
+            start_exchange(seg_dev);
+            positions_for(match_rel_dev, M, n_exec_out);
+            IPCFP_CUDA(cudaStreamSynchronize(c->sx));
+            pend_chk = hw[DW_EXEC_CHECK];
+        }
+        gather_results(tx_key, std::min(err_key, pend_chk), missing_base, n_proofs, n_witness, hw[HW_EXCH_OVERFLOW], false);
+    }
+    return g_tx == IPCFP_NO_ERROR && g_err == IPCFP_NO_ERROR && !g_missing_base && !g_overflow;
+}
+
+// every rank reports how far it got; the global values are the same on every rank
+void ShardExchange::gather_results(uint64_t tx_key, uint64_t err_key, bool missing_base, uint64_t n_proofs, uint64_t n_witness, uint64_t exch_overflow, bool stale) {
     const uint32_t W = c->world;
     uint64_t mine[8] = {tx_key, err_key, missing_base ? 1ull : 0ull, M, n_proofs, n_witness, exch_overflow, stale ? 1ull : 0ull};
     uint64_t* all = c->host.p;
@@ -818,8 +853,15 @@ void ShardExchange::agree_results(uint64_t tx_key, uint64_t err_key, bool missin
     }
 }
 
-// F: positions wanted by every rank → the owners answer → EventProof.message_cid of this rank's proofs
-void ShardExchange::fetch_and_patch(cudaStream_t st, ipcfp_event_proof* proofs_dev, uint64_t n_proofs) {
+// F: positions wanted by every rank → the owners answer → EventProof.message_cid of this rank's proofs (pass 2 is complete: the host
+// synchronised on it) → proofs_host
+void ShardExchange::fetch_and_patch(ipcfp_event_proof* proofs_dev, uint64_t n_proofs, void* proofs_host) {
+    cudaStream_t st = c->sx;
+    patch(proofs_dev, n_proofs);
+    if (n_proofs) IPCFP_CUDA(cudaMemcpyAsync(proofs_host, proofs_dev, n_proofs * sizeof(ipcfp_event_proof), cudaMemcpyDeviceToHost, st));
+}
+void ShardExchange::patch(ipcfp_event_proof* proofs_dev, uint64_t n_proofs) {
+    cudaStream_t st = c->sx;
     IPCFP_CUDA(cudaEventRecord(c->tm[2], st));
     IPCFP_CUDA(cudaEventRecord(c->tm[3], st));
     if (M_max == 0) return;
@@ -843,8 +885,46 @@ void ShardExchange::fetch_and_patch(cudaStream_t st, ipcfp_event_proof* proofs_d
     IPCFP_CUDA(cudaEventRecord(c->tm[3], st));
 }
 
-// W: union of the per-shard sorted witness CID lists (BTreeSet union of common/witness.rs:24-40) on every rank
-void ShardExchange::witness_union(cudaStream_t st, const uint8_t* cids_dev, uint64_t n_local, uint8_t** out_dev, uint64_t* n_out_dev_word) {
+// W: the union of the shards' witness CID sets as soon as this shard's sorted list exists (event after k_witness_emit), on its own
+// stream and communicator: it runs beside the message-CID fetch
+void ShardExchange::witness_union(const uint8_t* cids_dev, uint64_t n_local, bool full) {
+    cudaStream_t sw = c->sw;
+    full_union = full; wit_cids = cids_dev; wit_n = n_local;
+    IPCFP_CUDA(cudaStreamWaitEvent(sw, s->ev[EV_WITNESS_SORTED], 0));
+    if (full) {
+        union_replicated((uint64_t*)(s->dev_words.p + DW_UNION_SIZE));
+        publish_words(s, DW_UNION_SIZE, 1, nullptr, sw);
+    } else union_partitioned(union_piece_cap(false));
+}
+void ShardExchange::finish() {
+    IPCFP_CUDA(cudaStreamSynchronize(c->sx));
+    IPCFP_CUDA(cudaStreamSynchronize(c->sw));
+    if (full_union) return;
+    bool overflow = false;
+    for (uint32_t q = 0; q < c->world; q++) overflow |= s->host_words.p[HW_UNION_PARTS + 2 * q + 1] != 0;
+    if (overflow) {   // a piece did not fit its slot on some rank (every rank sees the same words): once more with slots that cannot overflow
+        union_partitioned(union_piece_cap(true));
+        IPCFP_CUDA(cudaStreamSynchronize(c->sw));
+    }
+}
+void ShardExchange::fill_result(ipcfp_event_result& r) const {
+    const uint64_t* hw = s->host_words.p;
+    r.n_exec = hw[HW_EXCH_N_EXEC];
+    r.union_cids_dev = union_dev;
+    if (full_union) { r.n_union_cids = r.n_union_part = hw[DW_UNION_SIZE]; r.union_part_first = 0; }
+    else {
+        r.n_union_cids = 0;
+        for (uint32_t q = 0; q < c->world; q++) { if (q == c->rank) r.union_part_first = r.n_union_cids; r.n_union_cids += hw[HW_UNION_PARTS + 2 * q]; }
+        r.n_union_part = hw[HW_UNION_PARTS + 2 * c->rank];
+    }
+    r.total_matching = M_total; r.total_proofs = proofs_total;
+    timings(&r.ms_exchange, &r.ms_fetch, &r.ms_union);
+}
+// union of the per-shard sorted witness CID lists (BTreeSet union of common/witness.rs:24-40) on every rank
+void ShardExchange::union_replicated(uint64_t* n_out_dev_word) {
+    const uint8_t* cids_dev = wit_cids;
+    const uint64_t n_local = wit_n;
+    cudaStream_t st = c->sw;
     NcclApi* n = nccl_api();
     const uint32_t W = c->world;
     IPCFP_CUDA(cudaEventRecord(c->tm[4], st));
@@ -870,7 +950,7 @@ void ShardExchange::witness_union(cudaStream_t st, const uint8_t* cids_dev, uint
     unsigned long long* n_union = c->words2.p + 3000;
     exclusive_scan_u32(c->flags.p, c->fscan.p, total_listed, (uint64_t*)n_union, c->scan_tmp.p, st);
     k_merge_emit38<<<g, 256, 0, st>>>((const RawCid*)c->gather.p, counts, W, capw, c->pos_of.p, c->flags.p, c->fscan.p, c->merged.p); IPCFP_LAUNCH_CHECK();
-    *out_dev = c->merged.p;
+    union_dev = c->merged.p;
     IPCFP_CUDA(cudaMemcpyAsync(n_out_dev_word, n_union, 8, cudaMemcpyDeviceToDevice, st));
     IPCFP_CUDA(cudaEventRecord(c->tm[5], st));
 }
@@ -888,7 +968,10 @@ uint64_t ShardExchange::union_piece_cap(bool cannot_overflow) const {
     if (const char* e = getenv("IPCFP_UNION_CAP")) return (uint64_t)std::max(1, atoi(e));   // tests: force the overflow path
     return std::min<uint64_t>(nw_max + 1, 2 * ((nw_max + W - 1) / W) + 1024);
 }
-void ShardExchange::witness_union_partitioned(cudaStream_t st, const uint8_t* cids_dev, uint64_t n_local, uint64_t cap, uint8_t** out_dev, uint32_t host_word_first) {
+void ShardExchange::union_partitioned(uint64_t cap) {
+    const uint8_t* cids_dev = wit_cids;
+    const uint64_t n_local = wit_n;
+    cudaStream_t st = c->sw;
     NcclApi* n = nccl_api();
     const uint32_t W = c->world, me = c->rank;
     IPCFP_CUDA(cudaEventRecord(c->tm[4], st));
@@ -925,10 +1008,10 @@ void ShardExchange::witness_union_partitioned(cudaStream_t st, const uint8_t* ci
     k_merge_rank<<<g, 256, 0, st>>>(lists, (const uint64_t*)col_d, W, stride, c->starts.p, c->pos_of.p, c->flags.p, b0, nb); IPCFP_LAUNCH_CHECK();
     exclusive_scan_u32(c->flags.p, c->fscan.p, total_cap, (uint64_t*)mine_d, c->scan_tmp.p, st);
     k_merge_emit38<<<g, 256, 0, st>>>(lists, (const uint64_t*)col_d, W, stride, c->pos_of.p, c->flags.p, c->fscan.p, c->merged.p); IPCFP_LAUNCH_CHECK();
-    // [partition size, overflow] of all ranks → the store's mapped words [host_word_first, +2·world): read after the caller's next sync of this stream
+    // [partition size, overflow] of all ranks → the store's mapped words HW_UNION_PARTS: read after the next sync of this stream
     IPCFP_NCCL(n->AllGather(mine_d, all_d, 2, ncclUint64, c->cw, st));
-    publish_words_on(s, st, all_d, host_word_first, 2 * W);
-    *out_dev = c->merged.p;
+    publish_words(s, HW_UNION_PARTS, 2 * W, all_d, st);
+    union_dev = c->merged.p;
     IPCFP_CUDA(cudaEventRecord(c->tm[5], st));
 }
 void ShardExchange::timings(float* ms_exchange, float* ms_fetch, float* ms_union) const {

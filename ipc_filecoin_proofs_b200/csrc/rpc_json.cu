@@ -23,7 +23,7 @@ struct RjMeta {
     unsigned long long defer;   // non-zero: not canonical
     unsigned long long n;       // record starts
 };
-static const uint32_t RJ_HOST_WORD = 600;   // the meta words land in the store's pinned host words from here on
+static_assert(sizeof(RjMeta) <= HW_RJ_META_WORDS * 8, "the meta words fit their host words (HW_RJ_META)");
 
 __global__ void __launch_bounds__(256) k_rj_mark(const char* __restrict__ t, uint64_t len, uint32_t* bits, uint64_t nwords, RjMeta* meta) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -67,14 +67,14 @@ static bool receipts_on_device(Store* s, const char* text, uint64_t len, TipsetD
     // straight from the caller's pageable memory: the driver's own pipelined staging beat a copy through two pinned chunks of the pool
     // (8 MB each, filled by one host thread): the whole parse of the 142 MB list of 1 M receipts took 22 ms against 28 ms on an H100 host
     IPCFP_CUDA(cudaMemcpyAsync(d_text.p, text, len, cudaMemcpyHostToDevice, st));
-    cudaEvent_t ev[4] = {};
-    struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int k = 0; k < 4; k++) if (e[k]) cudaEventDestroy(e[k]); } } g{ev};
-    for (auto& e : ev) IPCFP_CUDA(cudaEventCreate(&e));
-    IPCFP_CUDA(cudaEventRecord(ev[0], st));
+    cudaEvent_t tm[4] = {};
+    struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int k = 0; k < 4; k++) if (e[k]) cudaEventDestroy(e[k]); } } g{tm};
+    for (auto& e : tm) IPCFP_CUDA(cudaEventCreate(&e));
+    IPCFP_CUDA(cudaEventRecord(tm[0], st));
     k_rj_mark<<<div_up(nwords, 256), 256, 0, st>>>(d_text.p, len, bits.p, nwords, meta.p); IPCFP_LAUNCH_CHECK();
     bitmap_to_indices(bits.p, len, pos.p, (uint64_t*)&meta.p->n, word_prefix.p, scratch.p, st);
-    IPCFP_CUDA(cudaEventRecord(ev[1], st));
-    uint64_t* hm = s->host_words.p + RJ_HOST_WORD;
+    IPCFP_CUDA(cudaEventRecord(tm[1], st));
+    uint64_t* hm = s->host_words.p + HW_RJ_META;
     IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, sizeof(RjMeta), cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 1
     const uint64_t n = hm[1];
@@ -82,14 +82,14 @@ static bool receipts_on_device(Store* s, const char* text, uint64_t len, TipsetD
     td.n_receipts = n;
     td.events_roots.alloc(n * 38 + 64);
     td.has_root.alloc(n + 64);
-    IPCFP_CUDA(cudaEventRecord(ev[2], st));
+    IPCFP_CUDA(cudaEventRecord(tm[2], st));
     k_rj_records<<<div_up(n, 128), 128, 0, st>>>(d_text.p, len, pos.p, n, td.events_roots.p, td.has_root.p, meta.p); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaEventRecord(ev[3], st));
+    IPCFP_CUDA(cudaEventRecord(tm[3], st));
     IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 2
     float a, b;
-    IPCFP_CUDA(cudaEventElapsedTime(&a, ev[0], ev[1]));
-    IPCFP_CUDA(cudaEventElapsedTime(&b, ev[2], ev[3]));
+    IPCFP_CUDA(cudaEventElapsedTime(&a, tm[0], tm[1]));
+    IPCFP_CUDA(cudaEventElapsedTime(&b, tm[2], tm[3]));
     td.ms_kernels = a + b;
     return hm[0] == 0;
 }

@@ -90,7 +90,7 @@ ipcfp_slot_result* read_storage_slots(Store* s, const uint8_t* root, const uint8
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
     uint64_t* hw = s->host_words.p;
-    IPCFP_CUDA(cudaEventRecord(s->ev[0], st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
     AsyncBuf<uint8_t> d_in(64 + 32 * k, st), d_found(k + 8, st), d_vals(32 * k + 32, st);
     AsyncBuf<uint32_t> d_len(k + 8, st), wbits((s->n + 31) / 32 + 8, st);
@@ -102,17 +102,17 @@ ipcfp_slot_result* read_storage_slots(Store* s, const uint8_t* root, const uint8
     if (k) IPCFP_CUDA(cudaMemcpyAsync(d_in.p + 64, slots, 32 * k, cudaMemcpyHostToDevice, st));
     SlotArgs a;
     a.store = s->view; a.root_cid = d_in.p; a.slots = d_in.p + 64; a.n = k; a.found = d_found.p; a.raw_len = d_len.p; a.values = d_vals.p;
-    a.wbits = wbits.p; a.err = dw; a.stats = dw + 4; a.strict_only = getenv("IPCFP_HAMT_STRICT") ? 1 : 0;
-    IPCFP_CUDA(cudaMemsetAsync(dw + 4, 0, 16, st));
-    IPCFP_CUDA(cudaEventRecord(s->ev[2], st));
+    a.wbits = wbits.p; a.err = dw; a.stats = dw + DW_STATS; a.strict_only = getenv("IPCFP_HAMT_STRICT") ? 1 : 0;
+    IPCFP_CUDA(cudaMemsetAsync(dw + DW_STATS, 0, 16, st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_LOOKUP_BEGIN], st));
     a.per_warp = k <= 16384 ? 1 : 0;
     if (!a.per_warp) a.strict_only = 1;
     if (k) { k_read_slots<<<div_up(a.per_warp ? k * 32 : k, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK(); }
-    IPCFP_CUDA(cudaEventRecord(s->ev[3], st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_LOOKUP_END], st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 6 * 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (hw[0] != IPCFP_NO_ERROR) throw_storage_error(hw[0]);
-    const uint64_t stat_nodes = hw[4], stat_bytes = hw[5];
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_storage_error(hw[DW_ERR]);
+    const uint64_t stat_nodes = hw[DW_STATS], stat_bytes = hw[DW_STATS + 1];
     std::unique_ptr<SlotResultBox> box(new SlotResultBox());
     memset(&box->r, 0, sizeof box->r);
     box->found = PinnedArray(s->pool, k + 8);
@@ -124,14 +124,14 @@ ipcfp_slot_result* read_storage_slots(Store* s, const uint8_t* root, const uint8
         IPCFP_CUDA(cudaMemcpyAsync(box->values.p, d_vals.p, k * 32, cudaMemcpyDeviceToHost, st));
     }
     materialize_witness(s, wbits.p, box->wit);
-    IPCFP_CUDA(cudaEventRecord(s->ev[1], st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_STORAGE_END], st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
     box->r.n = k; box->r.found = box->found.as<uint8_t>(); box->r.raw_len = box->raw_len.as<uint32_t>(); box->r.values = box->values.as<uint8_t>();
     box->wit.fill(box->r.witness);
     float ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[0], s->ev[1]));
+    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_BEGIN], s->ev[EV_STORAGE_END]));
     box->r.ms_total = ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[2], s->ev[3]));
+    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_LOOKUP_BEGIN], s->ev[EV_LOOKUP_END]));
     box->r.ms_lookup = ms;
     box->r.lookup_nodes = stat_nodes;
     box->r.lookup_bytes = stat_bytes + 32 * k;
@@ -154,7 +154,7 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
     uint64_t* hw = s->host_words.p;
-    IPCFP_CUDA(cudaEventRecord(s->ev[0], st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
     AsyncBuf<uint8_t> d_in(128, st);
     AsyncBuf<ipcfp_storage_spec> d_specs(n + 1, st);
@@ -170,7 +170,7 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
     if (n) { k_storage_proofs<<<div_up(n * 32, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK(); }
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (hw[0] != IPCFP_NO_ERROR) throw_storage_error(hw[0]);
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_storage_error(hw[DW_ERR]);
     std::unique_ptr<StorageResultBox> box(new StorageResultBox());
     memset(&box->r, 0, sizeof box->r);
     box->proofs = PinnedArray(s->pool, (n + 1) * sizeof(ipcfp_storage_proof));
@@ -183,7 +183,7 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
     materialize_witness(s, wbits.p, box->wit, by_ref);
     // per-spec Vec<ProofBlock>: map recorded block indices to positions in the sorted union
     PinnedArray& sorted_idx = box->wit.sorted_idx;
-    IPCFP_CUDA(cudaEventRecord(s->ev[1], st));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_STORAGE_END], st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
     std::map<uint32_t, uint32_t> pos;
     for (uint64_t i = 0; i < box->wit.n; i++) pos[sorted_idx.as<uint32_t>()[i]] = (uint32_t)i;
@@ -201,7 +201,7 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
     box->r.spec_witness_offsets = box->spec_off.data();
     box->r.spec_witness_index = box->spec_idx.data();
     float ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[0], s->ev[1]));
+    IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_BEGIN], s->ev[EV_STORAGE_END]));
     box->r.ms_total = ms;
     return &box.release()->r;
 }

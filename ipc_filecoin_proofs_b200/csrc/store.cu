@@ -242,17 +242,9 @@ __global__ void k_publish(const unsigned long long* __restrict__ src, unsigned l
     if (i < n) dst[i] = src[i];
     __threadfence_system();
 }
-void publish_words(Store* s, uint32_t first, uint32_t count) {
-    k_publish<<<div_up(count, 64), 64, 0, s->stream>>>(s->dev_words.p + first, (unsigned long long*)s->host_words.dev + first, count);
-    IPCFP_LAUNCH_CHECK();
-}
-void publish_words_from(Store* s, const void* src_dev, uint32_t dst_first, uint32_t n_words) {
-    k_publish<<<div_up(n_words, 64), 64, 0, s->stream>>>((const unsigned long long*)src_dev, (unsigned long long*)s->host_words.dev + dst_first, n_words);
-    IPCFP_LAUNCH_CHECK();
-}
-
-void publish_words_on(Store* s, cudaStream_t stream, const void* src_dev, uint32_t dst_first, uint32_t n_words) {
-    k_publish<<<div_up(n_words, 64), 64, 0, stream>>>((const unsigned long long*)src_dev, (unsigned long long*)s->host_words.dev + dst_first, n_words);
+void publish_words(Store* s, uint32_t dst_first, uint32_t n_words, const void* src_dev, cudaStream_t stream) {
+    const unsigned long long* src = src_dev ? (const unsigned long long*)src_dev : s->dev_words.p + dst_first;
+    k_publish<<<div_up(n_words, 64), 64, 0, stream ? stream : s->stream>>>(src, (unsigned long long*)s->host_words.dev + dst_first, n_words);
     IPCFP_LAUNCH_CHECK();
 }
 
@@ -320,13 +312,13 @@ Store* store_shell(int device) {
     IPCFP_CUDA(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
     for (auto& e : s->ev) IPCFP_CUDA(cudaEventCreate(&e));
     cudaStream_t st = s->stream;
-    s->dev_words.alloc_pooled(64);
-    host_words_take(device, s->host_words, 1024);
+    s->dev_words.alloc_pooled(DW_COUNT);
+    host_words_take(device, s->host_words, HW_COUNT);
     {
         cudaMemPool_t mp;
         if (cudaDeviceGetDefaultMemPool(&mp, device) == cudaSuccess) { uint64_t thr = UINT64_MAX; cudaMemPoolSetAttribute(mp, cudaMemPoolAttrReleaseThreshold, &thr); }
     }
-    IPCFP_CUDA(cudaMemsetAsync(s->dev_words.p, 0, 64 * 8, st));
+    IPCFP_CUDA(cudaMemsetAsync(s->dev_words.p, 0, DW_COUNT * 8, st));
     return s.release();
 }
 
@@ -362,13 +354,13 @@ void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, co
     for (int attempt = 0; attempt < 2 && n; attempt++) {
         compute_class_ranks(s);
         fill_view(s);
-        unsigned long long* unknown = s->dev_words.p + 1;
+        unsigned long long* unknown = s->dev_words.p + DW_UNKNOWN_CLASSES;
         IPCFP_CUDA(cudaMemsetAsync(unknown, 0, 8, st));
         k_extract_digests<<<div_up(n, 256), 256, 0, st>>>(cids_dev, (uint32_t)n, s->view, s->digests.p, s->cls.p, unknown);
         IPCFP_LAUNCH_CHECK();
-        IPCFP_CUDA(cudaMemcpyAsync(s->host_words.p, unknown, 8, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaMemcpyAsync(s->host_words.p + DW_UNKNOWN_CLASSES, unknown, 8, cudaMemcpyDeviceToHost, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        if (s->host_words.p[0] == 0) break;
+        if (s->host_words.p[DW_UNKNOWN_CLASSES] == 0) break;
         if (attempt == 1) throw Error(IPCFP_ERR_UNSUPPORTED, "internal: CID classes unresolved");
         // rare path: several CID prefixes in one store — enumerate them on the host
         std::vector<uint8_t> back;
@@ -418,12 +410,12 @@ static uint32_t blake2b_class_mask(const Store* s) {
 // IPCFP_STORE_VERIFY_CIDS over every block of a store whose blocks are all on the device already; synchronises, sets first_bad
 void store_verify_all(Store* s) {
     cudaStream_t st = s->stream;
-    unsigned long long* bad = s->dev_words.p + 2;
+    unsigned long long* bad = s->dev_words.p + DW_FIRST_BAD;
     IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
     if (s->n) { k_verify_cids<<<div_up(s->n, 128), 128, 0, st>>>(s->view, 0, (uint32_t)s->n, blake2b_class_mask(s), bad); IPCFP_LAUNCH_CHECK(); }
-    publish_words(s, 2, 1);
+    publish_words(s, DW_FIRST_BAD, 1);
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    s->first_bad = s->host_words.p[2];
+    s->first_bad = s->host_words.p[DW_FIRST_BAD];
 }
 
 Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size, uint64_t n,
@@ -481,16 +473,16 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
     store_index(s.get(), cids_dev.p, cids, cids, sort_ws);
     if (verify) {
         const uint32_t mask = blake2b_class_mask(s.get());
-        unsigned long long* bad = s->dev_words.p + 2;
+        unsigned long long* bad = s->dev_words.p + DW_FIRST_BAD;
         IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
         for (size_t k = 0; k < chunks.size(); k++) {   // chunk k is checked while chunk k+1 is on the wire
             const Chunk& c = chunks[k];
             IPCFP_CUDA(cudaStreamWaitEvent(st, chunk_ev[k], 0));
             if (c.b1 > c.b0) { k_verify_cids<<<div_up(c.b1 - c.b0, 128), 128, 0, st>>>(s->view, (uint32_t)c.b0, (uint32_t)c.b1, mask, bad); IPCFP_LAUNCH_CHECK(); }
         }
-        publish_words(s.get(), 2, 1);
+        publish_words(s.get(), DW_FIRST_BAD, 1);
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        s->first_bad = s->host_words.p[2];  // reported by the C ABI as IPCFP_ERR_CID_MISMATCH (handle stays valid)
+        s->first_bad = s->host_words.p[DW_FIRST_BAD];  // reported by the C ABI as IPCFP_ERR_CID_MISMATCH (handle stays valid)
     } else {
         // the blob must have landed before anything reads blocks
         IPCFP_CUDA(cudaStreamWaitEvent(st, chunk_ev.back(), 0));

@@ -89,7 +89,7 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
     IPCFP_CUDA(cudaMemcpyAsync(h_flags, d_flags.p, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (hw[0] != IPCFP_NO_ERROR) throw_verify_error(hw[0]);
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
     ExecOrderOut exo;
     if (h_flags[0]) {
         // collect_exec_list(verify_txmeta = true) once for the whole batch: TxMeta recompute, then the engine's own message-AMT walk
@@ -108,11 +108,11 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         memset(&dummy, 0, sizeof dummy);
         dummy.event_signature = "";
         dummy.topic_1 = "";
-        IPCFP_CUDA(cudaMemcpyAsync(hw + 40, dw, 8, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaMemcpyAsync(hw + HW_PARKED_KEY, dw, 8, cudaMemcpyDeviceToHost, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        const uint64_t tx_key = hw[40];
+        const uint64_t tx_key = hw[HW_PARKED_KEY];
         try {
-            (void)generate_event_proof(s, nullptr, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, 1, 0, nullptr, &exo);
+            (void)generate_event_proof(s, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, nullptr, &exo);
         } catch (Error& e) {
             e.index = 0;   // failures of the walk surface at the first proof, like everything that depends on the tipset only
             throw;
@@ -149,7 +149,7 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
     IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (hw[0] != IPCFP_NO_ERROR) throw_verify_error(hw[0]);
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
 }
 
 // ------------------------------------------------------------------------------------------ storage
@@ -187,7 +187,7 @@ void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp
     IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (hw[0] != IPCFP_NO_ERROR) throw_verify_error(hw[0]);
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
 }
 
 }  // namespace ipcfp

@@ -197,7 +197,7 @@ WitnessBuilder::WitnessBuilder(Store* store) : s(store) {
     scratch.alloc(scan_scratch_elems(std::max<uint64_t>(nwords, n)) + 8, st);
 }
 
-// where to split the snapshot gather: dev_words[16] = number of blocks in the first part, [17] = their padded bytes
+// where to split the snapshot gather: DW_SPLIT_IDX = number of blocks in the first part, DW_SPLIT_BYTES = their padded bytes
 __global__ void k_chunk_bounds(const uint64_t* __restrict__ offs, const unsigned long long* count, const unsigned long long* total, unsigned long long* out) {
     const uint64_t m = *count;
     uint64_t ia = m / 8;
@@ -211,15 +211,15 @@ __global__ void k_padded_lengths_dev(const uint32_t* __restrict__ idx, const uns
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_max) out[i] = i < *count ? (lengths[bar[idx[i]]] + 15u) & ~15u : 0u;
 }
-// enqueue: bitmap → idx[0..mA), padded offsets; totals land in dev_words[8] (mA) and [9] (bytesA) — the caller
+// enqueue: bitmap → idx[0..mA), padded offsets; totals land in DW_WIT_A (mA) and DW_WIT_A_BYTES (bytesA) — the caller
 // publishes both and syncs ONCE before start_copy
 void WitnessBuilder::snapshot(const uint32_t* wbits) {
     unsigned long long* dw = s->dev_words.p;
     IPCFP_CUDA(cudaMemcpyAsync(bitsA.p, wbits, nwords * 4, cudaMemcpyDeviceToDevice, st));
-    bitmap_to_indices(bitsA.p, s->n, idx.p, (uint64_t*)(dw + 8), word_prefix.p, scratch.p, st);
-    if (s->n) { k_padded_lengths_dev<<<div_up(s->n, 256), 256, 0, st>>>(idx.p, dw + 8, s->n, s->lengths.p, s->block_at_rank.p, plen.p); IPCFP_LAUNCH_CHECK(); }
-    exclusive_scan_u32(plen.p, offs.p, s->n, (uint64_t*)(dw + 9), scratch.p, st);
-    k_chunk_bounds<<<1, 1, 0, st>>>(offs.p, dw + 8, dw + 9, dw + 16); IPCFP_LAUNCH_CHECK();
+    bitmap_to_indices(bitsA.p, s->n, idx.p, (uint64_t*)(dw + DW_WIT_A), word_prefix.p, scratch.p, st);
+    if (s->n) { k_padded_lengths_dev<<<div_up(s->n, 256), 256, 0, st>>>(idx.p, dw + DW_WIT_A, s->n, s->lengths.p, s->block_at_rank.p, plen.p); IPCFP_LAUNCH_CHECK(); }
+    exclusive_scan_u32(plen.p, offs.p, s->n, (uint64_t*)(dw + DW_WIT_A_BYTES), scratch.p, st);
+    k_chunk_bounds<<<1, 1, 0, st>>>(offs.p, dw + DW_WIT_A, dw + DW_WIT_A_BYTES, dw + DW_SPLIT_IDX); IPCFP_LAUNCH_CHECK();
     have_snapshot = true;
 }
 // host knows mA and bytesA: gather (main stream, two parts), D2H on the side stream as soon as each part is there
@@ -228,7 +228,7 @@ void WitnessBuilder::start_copy(uint64_t mA_, uint64_t bytesA_, uint64_t split_i
     bytesA = bytesA_;
     if (by_ref) {   // nothing to gather or copy: the index arrays are all the host gets (finish_start)
         bytesA = 0;
-        IPCFP_CUDA(cudaEventRecord(s->ev[7], st2));
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_BLOB_COPIED], st2));
         return;
     }
     host_cap = bytesA + bytesA / 8 + (8u << 20);
@@ -237,27 +237,27 @@ void WitnessBuilder::start_copy(uint64_t mA_, uint64_t bytesA_, uint64_t split_i
     dblobA.alloc(bytesA + 64, st);
     const uint64_t ia = std::min(split_idx, mA), ba = ia == mA ? bytesA : std::min(split_bytes, bytesA);
     if (ia) { k_witness_copy<<<div_up(ia * 32, 256), 256, 0, st>>>(idx.p, ia, s->view, offs.p, dblobA.p); IPCFP_LAUNCH_CHECK(); }
-    IPCFP_CUDA(cudaEventRecord(s->ev[6], st));
-    IPCFP_CUDA(cudaStreamWaitEvent(st2, s->ev[6], 0));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_WITNESS_SORTED], st));
+    IPCFP_CUDA(cudaStreamWaitEvent(st2, s->ev[EV_WITNESS_SORTED], 0));
     if (ba) IPCFP_CUDA(cudaMemcpyAsync(host_blob.p, dblobA.p, ba, cudaMemcpyDeviceToHost, st2));
     if (mA > ia) {
         k_witness_copy<<<div_up((mA - ia) * 32, 256), 256, 0, st>>>(idx.p + ia, mA - ia, s->view, offs.p + ia, dblobA.p); IPCFP_LAUNCH_CHECK();
-        IPCFP_CUDA(cudaEventRecord(s->ev[8], st));
-        IPCFP_CUDA(cudaStreamWaitEvent(st2, s->ev[8], 0));
+        IPCFP_CUDA(cudaEventRecord(s->ev[EV_GATHER_B], st));
+        IPCFP_CUDA(cudaStreamWaitEvent(st2, s->ev[EV_GATHER_B], 0));
         if (bytesA > ba) IPCFP_CUDA(cudaMemcpyAsync((uint8_t*)host_blob.p + ba, dblobA.p + ba, bytesA - ba, cudaMemcpyDeviceToHost, st2));
     }
-    IPCFP_CUDA(cudaEventRecord(s->ev[7], st2));
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_BLOB_COPIED], st2));
 }
-// enqueue: B = bits & ~A → idx[mA..mA+mB); totals in dev_words[10] (mB)
+// enqueue: B = bits & ~A → idx[mA..mA+mB); totals in DW_WIT_B (mB)
 void WitnessBuilder::finish_enqueue(const uint32_t* wbits) {
     unsigned long long* dw = s->dev_words.p;
     bitsB.alloc(nwords + 8, st);
     k_andnot<<<div_up(nwords ? nwords : 1, 256), 256, 0, st>>>(wbits, bitsA.p, bitsB.p, nwords); IPCFP_LAUNCH_CHECK();
-    bitmap_to_indices(bitsB.p, s->n, idx.p + mA, (uint64_t*)(dw + 10), word_prefixB.p, scratch.p, st);
+    bitmap_to_indices(bitsB.p, s->n, idx.p + mA, (uint64_t*)(dw + DW_WIT_B), word_prefixB.p, scratch.p, st);
     // their padded bytes, so that the host learns both numbers with the caller's next synchronisation
-    IPCFP_CUDA(cudaMemsetAsync(dw + 11, 0, 8, st));
+    IPCFP_CUDA(cudaMemsetAsync(dw + DW_WIT_B_BYTES, 0, 8, st));
     const uint64_t bound = s->n > mA ? s->n - mA : 0;
-    if (bound) { k_sum_padded_dev<<<div_up(bound, 256), 256, 0, st>>>(idx.p + mA, dw + 10, bound, s->lengths.p, s->block_at_rank.p, dw + 11); IPCFP_LAUNCH_CHECK(); }
+    if (bound) { k_sum_padded_dev<<<div_up(bound, 256), 256, 0, st>>>(idx.p + mA, dw + DW_WIT_B, bound, s->lengths.p, s->block_at_rank.p, dw + DW_WIT_B_BYTES); IPCFP_LAUNCH_CHECK(); }
 }
 void WitnessBuilder::finish(uint64_t mB_, uint64_t bytesB_, WitnessOut& out, bool want_sorted_idx) {
     finish_start(mB_, bytesB_, out, want_sorted_idx);
@@ -271,7 +271,7 @@ void WitnessBuilder::finish_start(uint64_t mB_, uint64_t bytesB_, WitnessOut& ou
     if (by_ref) { bytesB = 0; mB_ = 0; }   // (mB stays: the late entries are still listed; only their bytes are not gathered)
     if (mB_) {
         k_padded_lengths<<<div_up(mB, 256), 256, 0, st>>>(idx.p + mA, mB, s->lengths.p, s->block_at_rank.p, plen.p); IPCFP_LAUNCH_CHECK();
-        exclusive_scan_u32(plen.p, offs.p + mA, mB, (uint64_t*)(dw + 11), scratch.p, st);
+        exclusive_scan_u32(plen.p, offs.p + mA, mB, (uint64_t*)(dw + DW_WIT_B_BYTES), scratch.p, st);
     }
     if (bytesA + bytesB > host_cap) {  // rare: more late blocks than the slack — move to a bigger buffer
         IPCFP_CUDA(cudaStreamSynchronize(st2));
@@ -294,7 +294,7 @@ void WitnessBuilder::finish_start(uint64_t mB_, uint64_t bytesB_, WitnessOut& ou
                                                        d_lens.p, d_idx.p, by_ref ? 1 : 0);
         IPCFP_LAUNCH_CHECK();
     }
-    IPCFP_CUDA(cudaEventRecord(s->ev[6], st));   // the sorted CID list exists on the device (the multi-GPU union waits for this, not for the copies below)
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_WITNESS_SORTED], st));   // the sorted CID list exists on the device (the multi-GPU union waits for this, not for the copies below)
     out.n = m;
     out.blob_size = bytesA + bytesB;
     out.cids = PinnedArray(s->pool, m * 38 + 64);
@@ -312,7 +312,7 @@ void WitnessBuilder::finish_start(uint64_t mB_, uint64_t bytesB_, WitnessOut& ou
     dblobB_keep = std::move(dblobB);
 }
 void WitnessBuilder::finish_join(WitnessOut& out) {
-    IPCFP_CUDA(cudaStreamWaitEvent(st, s->ev[7], 0));  // the big copy on the side stream
+    IPCFP_CUDA(cudaStreamWaitEvent(st, s->ev[EV_BLOB_COPIED], 0));  // the big copy on the side stream
     IPCFP_CUDA(cudaStreamSynchronize(st));
     IPCFP_CUDA(cudaStreamSynchronize(st2));
     out.blob = std::move(host_blob);
@@ -323,9 +323,10 @@ void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out, b
     WitnessBuilder wb(s);
     wb.by_ref = by_ref;
     wb.snapshot(wbits_dev);
-    publish_words(s, 8, 2);
+    publish_words(s, DW_WIT_A, 2);
     IPCFP_CUDA(cudaStreamSynchronize(s->stream));
-    wb.start_copy(s->host_words.p[8], s->host_words.p[9], s->host_words.p[8], s->host_words.p[9]);   // one part
+    const uint64_t* hw = s->host_words.p;
+    wb.start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_WIT_A], hw[DW_WIT_A_BYTES]);   // one part
     wb.finish(0, 0, out, true);
 }
 
