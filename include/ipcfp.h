@@ -344,6 +344,49 @@ typedef struct ipcfp_tipset_info {
 } ipcfp_tipset_info;
 ipcfp_status ipcfp_tipset_describe(ipcfp_tipset* t, int with_events_roots, ipcfp_tipset_info* out);
 
+/* ------------------------------------------------------------------------------------------
+ * The block store straight from Filecoin.ChainReadObj JSON-RPC responses (src/client/blockstore.rs:20-28). The caller fetches block i
+ * as request i: Filecoin.ChainReadObj([{"/": <CID i>}]) with "id": i, and hands over the response texts exactly as received — each text
+ * one JSON-RPC 2.0 response object or a batch (an array of them), not NUL-terminated, the responses in any order, spread over any number
+ * of texts. Each response object has "jsonrpc":"2.0", "id" (a JSON integer, 0 <= id < n_blocks) and exactly one of "result" (a string:
+ * standard base64 with padding and zero unused bits — the block's bytes) and "error" (any JSON value). Unknown members are skipped; a
+ * repeated member is an error; JSON escapes in strings are undone before decoding.
+ *
+ * ipcfp_blocks_from_rpc_json (host C++, no device) returns the blocks in request order: blocks.cids is a copy of `cids` (n_blocks*38),
+ * block i sits at blocks.offsets[i] (16-aligned, ascending), blocks.lengths[i] bytes long, in blocks.blob. Checks, in this order:
+ *   1. texts in order, elements in order: a malformed text, an element that breaks the rules above, an id out of range or invalid base64 →
+ *      IPCFP_ERR_INVALID_ARG, index = the element's position counted over all texts (a text that does not start with '[' after
+ *      whitespace is one element); a fault outside every element (brackets, commas, trailing bytes) → index UINT64_MAX;
+ *   2. the smallest id that does not appear exactly once → IPCFP_ERR_INVALID_ARG, index = that id;
+ *   3. the smallest id answered with an "error" → IPCFP_ERR_MISSING_BLOCK, index = that id.
+ * *out is released with ipcfp_parsed_blocks_free.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ipcfp_parsed_blocks {
+    ipcfp_witness blocks;   /* host arrays owned by the object; block i = request i */
+} ipcfp_parsed_blocks;
+ipcfp_status ipcfp_blocks_from_rpc_json(const uint8_t* cids /* n_blocks*38 */, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens,
+                                        uint64_t n_texts, ipcfp_parsed_blocks** out);
+void ipcfp_parsed_blocks_free(ipcfp_parsed_blocks* p);
+/* The same texts straight to a new block store. The store, status and index are in every case those of ipcfp_blocks_from_rpc_json
+ * followed by ipcfp_store_create(blocks.cids, blocks.offsets, blocks.lengths, blocks.blob, blocks.blob_size, n_blocks, device, flags):
+ * block i of the store is the block of request i, so ipcfp_store_first_bad_block and every index are request ids. The bytes come from
+ * an RPC node: pass IPCFP_STORE_VERIFY_CIDS, which checks every block against its CID (IPCFP_ERR_CID_MISMATCH at the request id; *out is
+ * then set, as with ipcfp_store_create). Texts in canonical form are parsed on the device, the base64 decoded straight into the store's
+ * arena — each text either one element or "[" elements joined by "," "]", no whitespace, every element exactly
+ *   {"jsonrpc":"2.0","result":"<base64>","id":<decimal, no leading zeros>}
+ * and all texts together under 4 GiB. Any other input (whitespace, other member orders, escapes, error responses, repeated or missing ids,
+ * and every invalid text) goes through ipcfp_blocks_from_rpc_json instead, with the same result.
+ * Such a store has no caller blob for by-reference offsets to point into: every generate call on it with IPCFP_WITNESS_BY_REFERENCE
+ * returns IPCFP_ERR_UNSUPPORTED (IPCFP_RESULT_JSON reads the store itself and works). info (may be NULL): which path ran and its times. */
+typedef struct ipcfp_store_json_info {
+    uint32_t parsed_on_device;   /* 1: the device parsed the texts; 0: ipcfp_blocks_from_rpc_json did                                 */
+    float ms_parse;              /* wall time until the blocks were in the store's arena (copy of the texts included), before the index  */
+    float ms_kernels;            /* device parse only: time of its kernels (CUDA events on the store's stream); 0 otherwise                */
+    uint32_t _pad;
+} ipcfp_store_json_info;
+ipcfp_status ipcfp_store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts,
+                                         int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info);
+
 /* read_storage_slot (src/proofs/storage/decode.rs:36-97), batched over k slot keys against one
  * contract_state root, with a RecordingBlockStore-equivalent witness. */
 ipcfp_status ipcfp_read_storage_slots(ipcfp_store* s, const uint8_t contract_state_root[IPCFP_CID_LEN],

@@ -98,6 +98,10 @@ pub struct ipcfp_parsed_tipset { pub desc: ipcfp_tipset_desc }
 pub struct ipcfp_tipset_info { pub desc: ipcfp_tipset_desc, pub parsed_on_device: u32, pub ms_parse: f32, pub ms_kernels: f32,
                                pub _pad: u32 }
 #[repr(C)]
+pub struct ipcfp_parsed_blocks { pub blocks: ipcfp_witness }
+#[repr(C)]
+pub struct ipcfp_store_json_info { pub parsed_on_device: u32, pub ms_parse: f32, pub ms_kernels: f32, pub _pad: u32 }
+#[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
                           pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
 
@@ -134,6 +138,11 @@ extern "C" {
     pub fn ipcfp_tipset_upload_json(s: *mut ipcfp_store, parent: *const c_char, parent_len: u64, child: *const c_char, child_len: u64,
                                     receipts: *const c_char, receipts_len: u64, out: *mut *mut ipcfp_tipset) -> ipcfp_status;
     pub fn ipcfp_tipset_describe(t: *mut ipcfp_tipset, with_events_roots: c_int, out: *mut ipcfp_tipset_info) -> ipcfp_status;
+    pub fn ipcfp_blocks_from_rpc_json(cids: *const u8, n_blocks: u64, texts: *const *const c_char, text_lens: *const u64, n_texts: u64,
+                                      out: *mut *mut ipcfp_parsed_blocks) -> ipcfp_status;
+    pub fn ipcfp_parsed_blocks_free(p: *mut ipcfp_parsed_blocks);
+    pub fn ipcfp_store_create_rpc_json(cids: *const u8, n_blocks: u64, texts: *const *const c_char, text_lens: *const u64, n_texts: u64,
+                                       device: c_int, flags: u32, out: *mut *mut ipcfp_store, info: *mut ipcfp_store_json_info) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, spec: *const ipcfp_event_spec, flags: u32,
                                                out: *mut *mut ipcfp_event_result) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_shard(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, spec: *const ipcfp_event_spec, lo: u64, hi: u64,

@@ -192,6 +192,24 @@ def tipset_info_from_c(d, parsed_on_device=0, ms_parse=0.0, ms_kernels=0.0):
                         bool(parsed_on_device), float(ms_parse), float(ms_kernels))
 
 
+class ParsedBlocksC(C.Structure):
+    """ipcfp_parsed_blocks (ipcfp_blocks_from_rpc_json)."""
+    _fields_ = [("blocks", Witness)]
+
+
+class StoreJsonInfoC(C.Structure):
+    """ipcfp_store_json_info (ipcfp_store_create_rpc_json)."""
+    _fields_ = [("parsed_on_device", C.c_uint32), ("ms_parse", C.c_float), ("ms_kernels", C.c_float), ("_pad", C.c_uint32)]
+
+
+@dataclass
+class StoreJsonInfoPy:
+    """How ipcfp_store_create_rpc_json built a store: the path that parsed the texts and its times."""
+    parsed_on_device: bool
+    ms_parse: float
+    ms_kernels: float
+
+
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
 TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
 

@@ -45,7 +45,7 @@ EXPORTS = [
     "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
     "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
     "ipcfp_generate_proof_bundle_resident", "ipcfp_tipset_desc_from_json", "ipcfp_parsed_tipset_free", "ipcfp_tipset_upload_json",
-    "ipcfp_tipset_describe",
+    "ipcfp_tipset_describe", "ipcfp_blocks_from_rpc_json", "ipcfp_parsed_blocks_free", "ipcfp_store_create_rpc_json",
 ]
 
 
@@ -157,6 +157,13 @@ def lib():
                                                C.POINTER(C.c_void_p)]
         L.ipcfp_tipset_describe.restype = C.c_int32
         L.ipcfp_tipset_describe.argtypes = [C.c_void_p, C.c_int, C.POINTER(A.TipsetInfoC)]
+        L.ipcfp_blocks_from_rpc_json.restype = C.c_int32
+        L.ipcfp_blocks_from_rpc_json.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_uint64,
+                                                 C.POINTER(C.POINTER(A.ParsedBlocksC))]
+        L.ipcfp_parsed_blocks_free.argtypes = [C.POINTER(A.ParsedBlocksC)]
+        L.ipcfp_store_create_rpc_json.restype = C.c_int32
+        L.ipcfp_store_create_rpc_json.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_uint64, C.c_int,
+                                                  C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(A.StoreJsonInfoC)]
         _lib = L
     return _lib
 
@@ -243,6 +250,30 @@ class BlockStore:
     @classmethod
     def from_tipset(cls, ts, device=0, verify_cids=False):
         return cls(ts.cids, ts.offsets, ts.lengths, ts.blob, device, verify_cids)
+
+    @classmethod
+    def from_rpc_json(cls, cids, texts, device=0, verify_cids=False):
+        """ipcfp_store_create_rpc_json: the store straight from Filecoin.ChainReadObj responses. cids: (n, 38) — request i asks for CID i
+        with "id": i; texts: the response texts as received (str or bytes), each one response object or a batch. Canonical texts are
+        parsed on the device. `.json_info` tells which path ran. Failures raise IpcfpError (status, request id or response position) with
+        `.first_bad_block` as BlockStore() sets it. Pass verify_cids=True for bytes from an RPC node."""
+        cids = np.ascontiguousarray(cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+        arr, lens, keep = _text_array(texts)
+        self = cls.__new__(cls)
+        self.n_blocks, self.device, self._h = len(cids), device, None
+        h, info = C.c_void_p(), A.StoreJsonInfoC()
+        st = lib().ipcfp_store_create_rpc_json(cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep), device,
+                                               A.STORE_VERIFY_CIDS if verify_cids else 0, C.byref(h), C.byref(info))
+        self._h = h
+        self.json_info = A.StoreJsonInfoPy(bool(info.parsed_on_device), float(info.ms_parse), float(info.ms_kernels))
+        if st != A.OK:
+            bad = lib().ipcfp_store_first_bad_block(h) if h else None
+            msg, idx = lib().ipcfp_last_error().decode(errors="replace"), lib().ipcfp_last_error_index()
+            self.close()
+            e = A.IpcfpError(st, msg, idx)
+            e.first_bad_block = bad
+            raise e
+        return self
 
     def get(self, cid):
         cid = _u8(cid)
@@ -389,6 +420,28 @@ class ResidentTipset:
 
 def _text(x):
     return x.encode() if isinstance(x, str) else x if isinstance(x, bytes) else bytes(x)
+
+
+def _text_array(texts):
+    """texts (str or bytes each) → (char** array, u64 length array, the bytes objects they point into)."""
+    keep = [_text(t) for t in texts]
+    arr = (C.c_char_p * max(len(keep), 1))(*keep)
+    lens = (C.c_uint64 * max(len(keep), 1))(*[len(t) for t in keep])
+    return arr, lens, keep
+
+
+def blocks_from_rpc_json(cids, texts):
+    """ipcfp_blocks_from_rpc_json (host parser, no device): the blocks of Filecoin.ChainReadObj responses in request order, as an
+    A.WitnessPy (cids, 16-aligned offsets, lengths, blob). Failures raise IpcfpError with the status and the index include/ipcfp.h gives."""
+    cids = np.ascontiguousarray(cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+    arr, lens, keep = _text_array(texts)
+    out = C.POINTER(A.ParsedBlocksC)()
+    L = lib()
+    _check(L.ipcfp_blocks_from_rpc_json(cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep), C.byref(out)))
+    try:
+        return A.witness_from_c(out.contents.blocks)
+    finally:
+        L.ipcfp_parsed_blocks_free(out)
 
 
 def tipset_desc_from_json(parent_text, child_text, receipts_text):

@@ -140,6 +140,8 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
                                            const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags) {
     if (flags & ~(uint32_t)IPCFP_BUNDLE_FLAGS) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a proof bundle");
     if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
+    if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !st->caller_blob)
+        throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_WITNESS_BY_REFERENCE needs a store made from a caller's blob (ipcfp_store_create)");
     st->use();
     const bool by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
     cudaStream_t stream = st->stream;
@@ -220,7 +222,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* k_rb_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }
@@ -245,6 +247,18 @@ ipcfp_status ipcfp_store_create(const uint8_t* cids, const uint64_t* offsets, co
         *out = nullptr;
         Store* s = store_create(cids, offsets, lengths, blob, blob_size, n_blocks, device, flags);
         *out = reinterpret_cast<ipcfp_store*>(s);
+        if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
+    });
+}
+ipcfp_status ipcfp_store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts,
+                                         int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info) {
+    return guard([&] {
+        if (!out) throw Error(IPCFP_ERR_INVALID_ARG, "null out");
+        *out = nullptr;
+        ipcfp_store_json_info si;
+        Store* s = store_create_rpc_json(cids, n_blocks, texts, text_lens, n_texts, device, flags, si);
+        *out = reinterpret_cast<ipcfp_store*>(s);
+        if (info) *info = si;
         if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
     });
 }

@@ -83,6 +83,7 @@ constexpr uint32_t HW_EXCHANGE_WORDS = 2;                                     //
 constexpr uint32_t HW_UNION_PARTS_WORDS = 2 * MAX_WORLD;                      // parallel.cu: [partition size, overflow] per rank
 constexpr uint32_t HW_JP_META_WORDS = 17;                                     // json_parse.cu: JpMeta
 constexpr uint32_t HW_RJ_META_WORDS = 2;                                      // rpc_json.cu: RjMeta
+constexpr uint32_t HW_RB_META_WORDS = 4;                                      // rpc_blocks.cu: RbMeta
 enum HostWord : uint32_t {
     HW_PROLOGUE = DW_COUNT,
     HW_JSON_TOTALS = HW_PROLOGUE + HW_PROLOGUE_WORDS,
@@ -92,7 +93,8 @@ enum HostWord : uint32_t {
     HW_UNION_PARTS = HW_EXCH_OVERFLOW + HW_EXCHANGE_WORDS,
     HW_JP_META = HW_UNION_PARTS + HW_UNION_PARTS_WORDS,
     HW_RJ_META = HW_JP_META + HW_JP_META_WORDS,
-    HW_END = HW_RJ_META + HW_RJ_META_WORDS
+    HW_RB_META = HW_RJ_META + HW_RJ_META_WORDS,
+    HW_END = HW_RB_META + HW_RB_META_WORDS
 };
 constexpr uint32_t HW_COUNT = 1024;
 static_assert(DW_JSON_TOTAL2 < DW_COUNT, "a mirrored slot never reaches a host-only region (they start at DW_COUNT)");
@@ -132,6 +134,7 @@ struct Store {
     std::vector<std::array<uint8_t, 6>> class_prefix;  // distinct CID prefixes in this store
     std::vector<uint32_t> class_rank;                  // rank of each class in `Cid` Ord
     uint64_t first_bad = UINT64_MAX;
+    bool caller_blob = true;   // false: made from JSON-RPC texts (rpc_blocks.cu), no caller blob for IPCFP_WITNESS_BY_REFERENCE offsets
     std::shared_ptr<PinnedPool> pool;
     // small persistent scratch
     DevBuf<unsigned long long> dev_words;  // DW_COUNT slots (DevWord)
@@ -180,6 +183,9 @@ Store* store_shell(int device);   // stream, events, counters; no block yet
 void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev);
 void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws);
 void store_verify_all(Store* s);
+// rpc_blocks.cu — ipcfp_store_create_rpc_json (info: which path ran, its times)
+Store* store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts, int device,
+                             uint32_t flags, ipcfp_store_json_info& info);
 // n_words device words at src_dev (null: the mirrored dev_words[dst_first ..]) → host_words[dst_first ..) through mapped host memory,
 // on `stream` (null: the store's stream): a tiny kernel instead of a D2H copy, so the read-back never queues behind a large copy on
 // the copy engine

@@ -577,6 +577,8 @@ struct EventCall {
         if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
         // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
         if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
+        if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !s->caller_blob)
+            throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_WITNESS_BY_REFERENCE needs a store made from a caller's blob (ipcfp_store_create)");
         if (!sharded) { lo = 0; hi = td.n_receipts; }
         if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
         N = hi - lo;

@@ -207,17 +207,9 @@ struct JpBlock {
     uint64_t data_at, n_chars;   // the base64 characters
     uint32_t pads, len;          // '=' count, decoded length
 };
-JP_FN bool jp_block_head(const char* t, uint64_t at, uint64_t end, JpBlock& b, uint8_t* cid_out) {
-    JpCur c{t, at, end};
-    if (!c.lit("{\"cid\":[")) return false;
-    for (int k = 0; k < IPCFP_CID_LEN; k++) {
-        uint64_t v;
-        if ((k && !c.lit(",")) || !c.u64(v) || v > 255) return false;
-        if (cid_out) cid_out[k] = (uint8_t)v;
-    }
-    if (!c.lit("],\"data\":\"") || end - c.p < 2 || t[end - 2] != '"' || t[end - 1] != '}') return false;
-    b.data_at = c.p;
-    b.n_chars = end - 2 - c.p;
+// the base64 string of b.n_chars characters at b.data_at: its length, padding and zero unused bits; sets pads and len. The characters
+// before the padding are left to jp_block_char_ok.
+JP_FN bool jp_b64_span(const char* t, JpBlock& b) {
     if (b.n_chars & 3) return false;
     const char* d = t + b.data_at;
     const uint64_t n = b.n_chars;
@@ -230,6 +222,19 @@ JP_FN bool jp_block_head(const char* t, uint64_t at, uint64_t end, JpBlock& b, u
     if (len > 0xffffffffull) return false;
     b.len = (uint32_t)len;
     return true;
+}
+JP_FN bool jp_block_head(const char* t, uint64_t at, uint64_t end, JpBlock& b, uint8_t* cid_out) {
+    JpCur c{t, at, end};
+    if (!c.lit("{\"cid\":[")) return false;
+    for (int k = 0; k < IPCFP_CID_LEN; k++) {
+        uint64_t v;
+        if ((k && !c.lit(",")) || !c.u64(v) || v > 255) return false;
+        if (cid_out) cid_out[k] = (uint8_t)v;
+    }
+    if (!c.lit("],\"data\":\"") || end - c.p < 2 || t[end - 2] != '"' || t[end - 1] != '}') return false;
+    b.data_at = c.p;
+    b.n_chars = end - 2 - c.p;
+    return jp_b64_span(t, b);
 }
 // data character k (k < n_chars - pads) is a base64 digit: what jp_block_head leaves to the lanes
 JP_FN bool jp_block_char_ok(const char* t, const JpBlock& b, uint64_t k) { return jp_b64(t[b.data_at + k]) >= 0; }

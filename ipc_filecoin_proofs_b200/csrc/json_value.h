@@ -1,4 +1,4 @@
-// json_value.h — the JSON value parser of the host-side readers (csrc/bundle_parse.cpp, csrc/rpc_parse.cpp): a DOM of the text in
+// json_value.h — the JSON value parser of the host-side readers (csrc/bundle_parse.cpp, csrc/rpc_parse.cpp, csrc/rpc_blocks_parse.cpp): a DOM of the text in
 // serde_json's grammar (RFC 8259, escapes decoded, number literals kept as text) and the field readers the readers share. Plain C++,
 // built with g++; every reader includes it into its own anonymous namespace. A failed field read throws Fail with its status.
 #pragma once
@@ -200,6 +200,27 @@ void cid_of_string(const std::string& s, uint8_t out[IPCFP_CID_LEN]) {
     if (acc != 0) bad();   // non-zero padding bits
     if (raw.size() != IPCFP_CID_LEN) bad(IPCFP_ERR_UNSUPPORTED);
     memcpy(out, raw.data(), IPCFP_CID_LEN);
+}
+void unbase64(const std::string& s, std::vector<uint8_t>& out) {   // standard alphabet, padding required (base64::STANDARD)
+    if (s.size() % 4) bad();
+    auto d = [](char c) -> uint32_t {
+        return c >= 'A' && c <= 'Z' ? (uint32_t)(c - 'A') : c >= 'a' && c <= 'z' ? (uint32_t)(c - 'a' + 26) : c >= '0' && c <= '9' ? (uint32_t)(c - '0' + 52)
+               : c == '+' ? 62u : c == '/' ? 63u : 99u;
+    };
+    for (size_t i = 0; i < s.size(); i += 4) {
+        const bool last = i + 4 == s.size();
+        uint32_t a = d(s[i]), b = d(s[i + 1]);
+        if (a == 99 || b == 99) bad();
+        const bool p3 = s[i + 3] == '=', p2 = s[i + 2] == '=';
+        if ((p2 || p3) && !last) bad();
+        if (p2 && !p3) bad();
+        uint32_t c = p2 ? 0 : d(s[i + 2]), e = p3 ? 0 : d(s[i + 3]);
+        if (c == 99 || e == 99) bad();
+        uint32_t v = (a << 18) | (b << 12) | (c << 6) | e;
+        out.push_back((uint8_t)(v >> 16));
+        if (!p2) out.push_back((uint8_t)(v >> 8)); else if (b & 15) bad();          // canonical: unused bits are zero
+        if (!p3) out.push_back((uint8_t)v); else if (!p2 && (c & 3)) bad();
+    }
 }
 
 }  // namespace
