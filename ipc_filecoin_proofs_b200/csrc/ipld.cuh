@@ -128,7 +128,7 @@ __device__ __forceinline__ void amt_root_begin(Rd& r, int version, uint32_t& bw,
         bw = r.err ? 3 : (uint32_t)b;
     }
     uint64_t h = rd_uint(r);
-    if (!r.err && h * bw > 64) rd_fail(r, CE_AMT);
+    if (!r.err && (h > 64 || (uint32_t)h * bw > 64)) rd_fail(r, CE_AMT);   // height·bw ≤ 64; the 64-bit product would wrap (h ≥ 2^61)
     height = r.err ? 0 : (uint32_t)h;
     count = rd_uint(r);
 }

@@ -386,7 +386,7 @@ template <class V> struct Amt {
             a.bw = (int)bw;
         }
         uint64_t h = d.uint();
-        if (h * (uint64_t)a.bw > 64) fail_decode("amt: height exceeds maximum");
+        if (h > 64 || h * (uint64_t)a.bw > 64) fail_decode("amt: height exceeds maximum");   // height·bw ≤ 64; the product alone would wrap
         a.height = (uint32_t)h;
         a.count = d.uint();
         a.root = decode_amt_node<V>(d, a.bw, a.height);

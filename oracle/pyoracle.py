@@ -123,6 +123,8 @@ class Amt:
             self.height, self.count, self.root = r
         else:
             self.bw, self.height, self.count, self.root = r
+        if not 1 <= self.bw <= 8 or self.height * self.bw > 64:
+            raise ValueError("amt: bit width %d, height %d" % (self.bw, self.height))
         self.rec = rec
 
     def _expand(self, node):

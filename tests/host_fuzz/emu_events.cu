@@ -353,7 +353,102 @@ static int compare_shard(const Blocks& B, const ipcfp_tipset_desc& td, const cha
     return 0;
 }
 
+// ---- hand-built events-AMT roots: one whose height·bw wraps modulo 2^64 (bw 5, height 0x3333333333333334 over a chain of 70
+// one-link nodes: refused at the root, and walk_events must not follow the chain), and the deepest legal walk (bw 1, height 64, one
+// value at 2^64 − 2: 65 frames of walk_events). Under AddressSanitizer a walk deeper than its frame stack is a report.
+static void put_head(std::vector<uint8_t>& o, uint32_t major, uint64_t n) {
+    if (n < 24) { o.push_back((uint8_t)(major << 5 | n)); return; }
+    int sz = n < 0x100 ? 1 : n < 0x10000 ? 2 : n < 0x100000000ull ? 4 : 8;
+    o.push_back((uint8_t)(major << 5 | (sz == 1 ? 24 : sz == 2 ? 25 : sz == 4 ? 26 : 27)));
+    for (int k = sz - 1; k >= 0; k--) o.push_back((uint8_t)(n >> (8 * k)));
+}
+static std::vector<uint8_t> put_block(Blocks& B, const std::vector<uint8_t>& b) {
+    static const uint8_t prefix[6] = {0x01, 0x71, 0xa0, 0xe4, 0x02, 0x20};
+    std::vector<uint8_t> cid(prefix, prefix + 6);
+    uint64_t x = 0x9E3779B97F4A7C15ull * (B.n + 1);
+    for (int k = 0; k < 32; k++) { x ^= x >> 29; x *= 0xBF58476D1CE4E5B9ull; cid.push_back((uint8_t)(x >> 56)); }
+    while (B.blob.size() % 16) B.blob.push_back(0);
+    B.cids.insert(B.cids.end(), cid.begin(), cid.end());
+    B.offs.push_back(B.blob.size());
+    B.lens.push_back((uint32_t)b.size());
+    B.blob.insert(B.blob.end(), b.begin(), b.end());
+    B.n++;
+    return cid;
+}
+static std::vector<uint8_t> amt_node(uint32_t bw, uint32_t slot, const std::vector<uint8_t>* link, const std::vector<uint8_t>* value) {
+    std::vector<uint8_t> o{0x83};
+    const uint32_t blen = bw <= 3 ? 1u : (1u << (bw - 3));
+    put_head(o, 2, blen);
+    for (uint32_t k = 0; k < blen; k++) o.push_back((link || value) && slot / 8 == k ? (uint8_t)(1u << (slot % 8)) : 0);
+    o.push_back(link ? 0x81 : 0x80);
+    if (link) { o.insert(o.end(), {0xd8, 0x2a, 0x58, 0x27, 0x00}); o.insert(o.end(), link->begin(), link->end()); }
+    o.push_back(value ? 0x81 : 0x80);
+    if (value) o.insert(o.end(), value->begin(), value->end());
+    return o;
+}
+static std::vector<uint8_t> amt_root(uint32_t bw, uint64_t height, const std::vector<uint8_t>& node) {
+    std::vector<uint8_t> o{0x84};
+    put_head(o, 0, bw); put_head(o, 0, height); put_head(o, 0, 1);
+    o.insert(o.end(), node.begin(), node.end());
+    return o;
+}
+static int hand_built_roots() {
+    Matcher m;
+    memset(&m, 0, sizeof m);
+    std::vector<uint8_t> ev{0x82, 0x19, 0x03, 0xe9, 0x82};   // [1001, [t1 = 32 × 0x11, t2 = 32 × 0x22]]
+    for (uint8_t t : {(uint8_t)0x11, (uint8_t)0x22}) {
+        ev.insert(ev.end(), {0x84, 0x03, 0x62, 't', (uint8_t)(t == 0x11 ? '1' : '2'), 0x18, 0x55, 0x58, 0x20});
+        ev.insert(ev.end(), 32, t);
+    }
+    memset(m.t0, 0x11, 32); memset(m.t1, 0x22, 32);
+    // the wrapping height
+    Blocks B;
+    B.n = 0;
+    std::vector<uint8_t> c = put_block(B, amt_node(5, 0, nullptr, nullptr));
+    for (int d = 0; d < 70; d++) c = put_block(B, amt_node(5, 0, &c, nullptr));
+    put_block(B, amt_root(5, 0x3333333333333334ull, amt_node(5, 0, &c, nullptr)));
+    // the deepest legal walk: 2^64 − 2 takes slot 0 at height 64, slot 1 at 63 … 1, slot 0 at the leaf
+    c = put_block(B, amt_node(1, 0, nullptr, &ev));
+    for (int lvl = 1; lvl <= 63; lvl++) c = put_block(B, amt_node(1, 1, &c, nullptr));
+    put_block(B, amt_root(1, 64, amt_node(1, 0, &c, nullptr)));
+    B.blob.resize(B.blob.size() + 64, 0);
+    HostStore hs(B.cids.data(), B.offs.data(), B.lens.data(), B.blob.data(), B.blob.size(), B.n);
+    const StoreView& sv = hs.view;
+    const uint32_t wrap_root = 71, deep_root = (uint32_t)B.n - 1;
+    {
+        uint32_t len, bw, height;
+        uint64_t cnt;
+        const uint8_t* p = store_block(sv, wrap_root, len);
+        WalkOut wo{0, 0, false};
+        uint32_t detail = 0;
+        uint32_t rc = walk_events<WALK_COUNT>(&sv, wrap_root, &m, nullptr, wo, nullptr, &detail);   // first: a walk down the chain overflows
+        if (rc != DC_DECODE) { fprintf(stderr, "HAND-BUILT: walk of the wrapping root returned %u, not a decode error\n", rc); return 1; }
+        Rd r(p, len);
+        amt_root_begin(r, 3, bw, height, cnt);
+        if (!r.err) { fprintf(stderr, "HAND-BUILT: root of height 0x3333333333333334 at bit width 5 decoded\n"); return 1; }
+    }
+    {
+        WalkOut wo{0, 0, false};
+        uint32_t detail = 0;
+        uint32_t rc = walk_events<WALK_COUNT>(&sv, deep_root, &m, nullptr, wo, nullptr, &detail);
+        if (rc || wo.nproofs != 1) { fprintf(stderr, "HAND-BUILT: deepest walk returned %u with %u proofs\n", rc, wo.nproofs); return 1; }
+        ipcfp_event_proof q[1];
+        std::vector<uint8_t> blob(wo.nbytes + 16);
+        EmitCtx ec;
+        memset(&ec, 0, sizeof ec);
+        ec.proofs = q; ec.blob = blob.data(); ec.blob_off = 0; ec.exec_index = 3;
+        wo = WalkOut{0, 0, false};
+        rc = walk_events<WALK_EMIT>(&sv, deep_root, &m, nullptr, wo, &ec, &detail);
+        if (rc || wo.nproofs != 1 || q[0].event_index != 0xFFFFFFFFFFFFFFFEull || q[0].emitter != 1001) {
+            fprintf(stderr, "HAND-BUILT: deepest walk emitted event index %llx\n", (unsigned long long)q[0].event_index);
+            return 1;
+        }
+    }
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    if (hand_built_roots()) return 1;
     uint64_t cases = argc > 1 ? strtoull(argv[1], nullptr, 10) : 10;
     uint64_t muts = argc > 2 ? strtoull(argv[2], nullptr, 10) : 60;
     rs = argc > 3 ? strtoull(argv[3], nullptr, 10) : 0xE7E47ull;
@@ -466,5 +561,6 @@ int main(int argc, char** argv) {
     }
     printf("ok: event path on the CPU == oracle for %llu tipsets: %llu runs equal in every field, %llu runs failing identically, %llu of them through the general walk (one run in three carries two independent faults)\n",
            (unsigned long long)cases, (unsigned long long)n_ok, (unsigned long long)n_err, (unsigned long long)n_skip);
+    printf("ok: hand-built roots: a height whose product with the bit width wraps is refused, the 65-frame walk emits index 2^64 - 2\n");
     return 0;
 }

@@ -95,6 +95,7 @@ def test_event_path_emulated_on_cpu_matches_oracle():
     out = subprocess.run([exe, "24", "120", "5"], capture_output=True, text=True, env=env)
     assert out.returncode == 0, out.stderr[-3000:]
     assert out.stdout.startswith("ok: event path on the CPU == oracle for 24 tipsets"), out.stdout
+    assert "ok: hand-built roots" in out.stdout, out.stdout
     runs_ok, runs_err = int(out.stdout.split(":")[2].split()[0]), int(out.stdout.split("field,")[1].split()[0])
     general = int(out.stdout.split("identically,")[1].split()[0])
     assert runs_ok > 200 and runs_err > 1000 and general > 100, out.stdout
@@ -119,6 +120,7 @@ def test_event_path_emulation_under_sanitizers():
     out = subprocess.run([exe, "10", "60", "31"], capture_output=True, text=True, env=env)
     assert out.returncode == 0, (out.stdout + out.stderr)[-4000:]
     assert out.stdout.startswith("ok: event path on the CPU == oracle for 10 tipsets"), out.stdout
+    assert "ok: hand-built roots" in out.stdout, out.stdout   # a root whose height wraps, the 65-frame walk (emu_events.cu)
     assert "runtime error" not in out.stderr and "AddressSanitizer" not in out.stderr, out.stderr[-4000:]
 
 
