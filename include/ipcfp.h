@@ -416,6 +416,35 @@ ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* 
 void ipcfp_bundle_free(ipcfp_bundle* b);
 
 /* ------------------------------------------------------------------------------------------
+ * Fetch planning: which blocks to request before ipcfp_generate_proof_bundle_resident can run on a store that does not hold them all.
+ * N(S) is the set of blocks the generators of that call would get for this tipset and these specs, as far as decoding the blocks
+ * already in the store S finds them (the rules are DESIGN.md §2, "Fetch planning"); the plan is M(S) = N(S) \ S. Each call is one
+ * round: fetch the plan's CIDs, build a store from the blocks held so far plus the new ones, upload the tipset to it and call again.
+ * Once a plan is empty, ipcfp_generate_proof_bundle_resident on the store gives what it gives on a store with every block: the same
+ * bundle, or the same status and index. The planner itself never returns IPCFP_ERR_MISSING_BLOCK or IPCFP_ERR_DECODE; a block that
+ * does not decode only has no children here. Any flag bit, or storage specs against a tipset without child_parent_state_root, is
+ * IPCFP_ERR_INVALID_ARG. An empty store works (every root is missing). *out is released with ipcfp_fetch_plan_free.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct ipcfp_fetch_plan {
+    uint64_t n_missing;
+    const uint8_t* cids;   /* n_missing*38: M(S), unique, in `Cid` order, none of them in the store */
+    uint64_t n_needed;     /* blocks of N(S) present in the store                                   */
+    uint32_t n_levels;     /* frontier levels of the AMT walk on the device                          */
+    float ms_total;        /* CUDA events on the store's stream                                      */
+} ipcfp_fetch_plan;
+ipcfp_status ipcfp_plan_fetch_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                       const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out);
+/* ipcfp_tipset_upload, then ipcfp_plan_fetch_resident */
+ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                              const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out);
+void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p);
+/* The round as one Filecoin.ChainReadObj batch: request k asks for plan->cids[k] with "id": first_id + k, compact JSON
+ *   [{"jsonrpc":"2.0","method":"Filecoin.ChainReadObj","params":[{"/":"b…"}],"id":<first_id + k>},…]
+ * With first_id = the number of blocks already held, the responses go straight to ipcfp_store_create_rpc_json with
+ * cids = (blocks already held) ++ plan->cids. Host-side rendering: no device is needed. *out is released with ipcfp_json_free. */
+ipcfp_status ipcfp_fetch_plan_to_rpc_json(const ipcfp_fetch_plan* p, uint64_t first_id, char** out, uint64_t* out_len);
+
+/* ------------------------------------------------------------------------------------------
  * Wire format (src/proofs/common/bundle.rs:10-45, src/proofs/events/bundle.rs:5-30, src/proofs/storage/bundle.rs:5-14): the JSON
  * `serde_json::to_string` gives for UnifiedProofBundle / EventProofBundle — struct field order, compact, CIDs as "bafy2bzace…"
  * strings, "0x" lower-case hex, base64 block data (ProofBlock.cid as the byte array cid 0.11's Serialize emits). t supplies the

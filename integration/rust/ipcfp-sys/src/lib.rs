@@ -102,6 +102,8 @@ pub struct ipcfp_parsed_blocks { pub blocks: ipcfp_witness }
 #[repr(C)]
 pub struct ipcfp_store_json_info { pub parsed_on_device: u32, pub ms_parse: f32, pub ms_kernels: f32, pub _pad: u32 }
 #[repr(C)]
+pub struct ipcfp_fetch_plan { pub n_missing: u64, pub cids: *const u8, pub n_needed: u64, pub n_levels: u32, pub ms_total: f32 }
+#[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
                           pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
 
@@ -160,6 +162,12 @@ extern "C" {
     pub fn ipcfp_generate_proof_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                                                 especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
     pub fn ipcfp_bundle_free(b: *mut ipcfp_bundle);
+    pub fn ipcfp_plan_fetch_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                                     especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_plan_fetch(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                            especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_fetch_plan_free(p: *mut ipcfp_fetch_plan);
+    pub fn ipcfp_fetch_plan_to_rpc_json(p: *const ipcfp_fetch_plan, first_id: u64, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
 
     pub fn ipcfp_bundle_to_json(b: *const ipcfp_bundle, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_event_result_to_json(r: *const ipcfp_event_result, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;

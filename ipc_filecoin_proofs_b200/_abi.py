@@ -210,6 +210,27 @@ class StoreJsonInfoPy:
     ms_kernels: float
 
 
+class FetchPlanC(C.Structure):
+    """ipcfp_fetch_plan (ipcfp_plan_fetch_resident)."""
+    _fields_ = [("n_missing", C.c_uint64), ("cids", C.POINTER(C.c_uint8)), ("n_needed", C.c_uint64), ("n_levels", C.c_uint32),
+                ("ms_total", C.c_float)]
+
+
+@dataclass
+class FetchPlanPy:
+    """One round of fetch planning: the CIDs the store lacks ((n, 38), `Cid` order), how many needed blocks it holds, the device walk's
+    levels and its time."""
+    cids: np.ndarray
+    n_needed: int
+    n_levels: int
+    ms_total: float
+
+
+def fetch_plan_from_c(p):
+    cids = np.ctypeslib.as_array(p.cids, shape=(p.n_missing * CID_LEN,)).copy() if p.n_missing else np.zeros(0, np.uint8)
+    return FetchPlanPy(cids.reshape(-1, CID_LEN), int(p.n_needed), int(p.n_levels), float(p.ms_total))
+
+
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
 TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
 

@@ -46,6 +46,7 @@ EXPORTS = [
     "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
     "ipcfp_generate_proof_bundle_resident", "ipcfp_tipset_desc_from_json", "ipcfp_parsed_tipset_free", "ipcfp_tipset_upload_json",
     "ipcfp_tipset_describe", "ipcfp_blocks_from_rpc_json", "ipcfp_parsed_blocks_free", "ipcfp_store_create_rpc_json",
+    "ipcfp_plan_fetch_resident", "ipcfp_plan_fetch", "ipcfp_fetch_plan_free", "ipcfp_fetch_plan_to_rpc_json",
 ]
 
 
@@ -164,6 +165,15 @@ def lib():
         L.ipcfp_store_create_rpc_json.restype = C.c_int32
         L.ipcfp_store_create_rpc_json.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_uint64, C.c_int,
                                                   C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(A.StoreJsonInfoC)]
+        L.ipcfp_plan_fetch_resident.restype = C.c_int32
+        L.ipcfp_plan_fetch_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                C.POINTER(C.POINTER(A.FetchPlanC))]
+        L.ipcfp_plan_fetch.restype = C.c_int32
+        L.ipcfp_plan_fetch.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
+                                       C.POINTER(C.POINTER(A.FetchPlanC))]
+        L.ipcfp_fetch_plan_free.argtypes = [C.POINTER(A.FetchPlanC)]
+        L.ipcfp_fetch_plan_to_rpc_json.restype = C.c_int32
+        L.ipcfp_fetch_plan_to_rpc_json.argtypes = [C.POINTER(A.FetchPlanC), C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         _lib = L
     return _lib
 
@@ -376,6 +386,17 @@ class BlockStore:
         finally:
             lib().ipcfp_bundle_free(out)
 
+    def plan_fetch(self, tip, storage_specs, event_specs, flags=0):
+        """ipcfp_plan_fetch_resident → A.FetchPlanPy: the CIDs this store lacks of the blocks generate_proof_bundle_resident(tip,
+        storage_specs, event_specs) would read, as far as the blocks it holds tell (one round; see fetch_until_complete)."""
+        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
+        out = C.POINTER(A.FetchPlanC)()
+        _check(lib().ipcfp_plan_fetch_resident(self._h, tip._h, sarr, ns, earr, ne, flags, C.byref(out)))
+        try:
+            return A.fetch_plan_from_c(out.contents)
+        finally:
+            lib().ipcfp_fetch_plan_free(out)
+
     def close(self):
         if self._h:
             lib().ipcfp_store_destroy(self._h)
@@ -442,6 +463,54 @@ def blocks_from_rpc_json(cids, texts):
         return A.witness_from_c(out.contents.blocks)
     finally:
         L.ipcfp_parsed_blocks_free(out)
+
+
+def fetch_plan_to_rpc_json(cids, first_id=0):
+    """ipcfp_fetch_plan_to_rpc_json: one Filecoin.ChainReadObj batch (bytes) asking for cids ((n, 38)) with ids first_id + k."""
+    cids = np.ascontiguousarray(cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+    p = A.FetchPlanC(len(cids), cids.ctypes.data_as(C.POINTER(C.c_uint8)) if cids.size else None, 0, 0, 0.0)
+    out, ln = C.c_void_p(), C.c_uint64()
+    _check(lib().ipcfp_fetch_plan_to_rpc_json(C.byref(p), first_id, C.byref(out), C.byref(ln)))
+    try:
+        return C.string_at(out.value, ln.value)
+    finally:
+        lib().ipcfp_json_free(out)
+
+
+@dataclass
+class FetchRound:
+    """One round of fetch_until_complete: the CIDs requested, the plan's device time, the wall time of the store rebuild after it."""
+    cids: np.ndarray
+    ms_plan: float
+    ms_rebuild: float
+
+
+def fetch_until_complete(fetch, upload_tipset, storage_specs, event_specs, device=0, verify_cids=True, max_rounds=10000):
+    """Plans and fetches rounds until the store holds every block a proof bundle needs (include/ipcfp.h, "Fetch planning").
+
+    fetch(cids, first_id) asks for cids ((k, 38)) and returns the Filecoin.ChainReadObj response texts (request j has "id": first_id + j;
+    fetch_plan_to_rpc_json(cids, first_id) is that request); upload_tipset(store) returns the store's ResidentTipset (upload_tipset or
+    upload_tipset_json). Starts from an empty store; each round rebuilds it with BlockStore.from_rpc_json over every response so far.
+    Returns (store, tipset, rounds, cids, texts): the complete store, its tipset, the FetchRounds, and the CIDs and texts it was built
+    from."""
+    import time
+    all_cids, texts, rounds = np.zeros((0, A.CID_LEN), np.uint8), [], []
+    store = BlockStore(all_cids, np.zeros(0, np.uint64), np.zeros(0, np.uint32), np.zeros(0, np.uint8), device=device)
+    tip = upload_tipset(store)
+    for _ in range(max_rounds):
+        plan = store.plan_fetch(tip, storage_specs, event_specs)
+        if not len(plan.cids):
+            return store, tip, rounds, all_cids, texts
+        got = fetch(plan.cids, len(all_cids))
+        texts += [got] if isinstance(got, (bytes, str)) else list(got)
+        all_cids = np.concatenate([all_cids, plan.cids])
+        t0 = time.perf_counter()
+        tip.close()
+        store.close()
+        store = BlockStore.from_rpc_json(all_cids, texts, device=device, verify_cids=verify_cids)
+        tip = upload_tipset(store)
+        rounds.append(FetchRound(plan.cids, plan.ms_total, (time.perf_counter() - t0) * 1e3))
+    raise RuntimeError("fetch_until_complete: no fixed point after %d rounds" % max_rounds)
 
 
 def tipset_desc_from_json(parent_text, child_text, receipts_text):

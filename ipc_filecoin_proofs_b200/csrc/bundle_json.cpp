@@ -145,5 +145,23 @@ ipcfp_status ipcfp_event_result_to_json(const ipcfp_event_result* r, const ipcfp
     return *out ? IPCFP_OK : IPCFP_ERR_INVALID_ARG;
 }
 void ipcfp_json_free(char* p) { free(p); }
+// one Filecoin.ChainReadObj request per CID of the plan, in plan order, ids first_id + k
+ipcfp_status ipcfp_fetch_plan_to_rpc_json(const ipcfp_fetch_plan* p, uint64_t first_id, char** out, uint64_t* out_len) {
+    if (!p || !out || (p->n_missing && !p->cids)) return IPCFP_ERR_INVALID_ARG;
+    std::string o;
+    o.reserve(2 + p->n_missing * 140);
+    o.push_back('[');
+    for (uint64_t k = 0; k < p->n_missing; k++) {
+        if (k) o.push_back(',');
+        o += "{\"jsonrpc\":\"2.0\",\"method\":\"Filecoin.ChainReadObj\",\"params\":[{\"/\":";
+        cid_string(o, p->cids + 38 * k);
+        o += "}],\"id\":";
+        num(o, first_id + k);
+        o.push_back('}');
+    }
+    o.push_back(']');
+    *out = dup_out(o, out_len);
+    return *out ? IPCFP_OK : IPCFP_ERR_INVALID_ARG;
+}
 
 }  // extern "C"

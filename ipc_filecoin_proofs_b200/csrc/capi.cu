@@ -80,15 +80,20 @@ void merge_witness_cids(int device, const void* gathered, const uint64_t* counts
     // The order is the raw byte order of the 38 bytes, which is `Cid` Ord only among CIDs that share one prefix (the varint
     // multihash code does not sort bytewise): lists with several prefixes are refused, like the sharded call refuses such stores.
     check_device(device);
+    *n_out = 0;
+    *n_out = sort_unique_cids(nullptr, gathered, counts, world, cap, out, cap_out, nullptr);
+}
+
+uint64_t sort_unique_cids(cudaStream_t st, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
+                          uint64_t* mixed) {
     std::vector<uint64_t> seg(world + 1, 0);
     for (uint32_t r = 0; r < world; r++) { if (counts[r] > cap) throw Error(IPCFP_ERR_INVALID_ARG, "count exceeds segment capacity"); seg[r + 1] = seg[r] + counts[r]; }
     uint64_t total = seg[world];
-    *n_out = 0;
-    if (!total) return;
+    if (mixed) *mixed = UINT64_MAX;
+    if (!total) return 0;
     uint32_t r0 = 0;
     while (!counts[r0]) r0++;
     const uint8_t* first = (const uint8_t*)gathered + 38ull * r0 * cap;
-    cudaStream_t st = nullptr;
     AsyncBuf<uint64_t> d_seg(world + 1, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_seg.p, seg.data(), (world + 1) * 8, cudaMemcpyHostToDevice, st));
     AsyncBuf<uint32_t> keys(total, st), vals(total, st), ka(total, st), va(total, st), bits((total + 31) / 32 + 8, st), pos(total + 32, st);
@@ -106,12 +111,13 @@ void merge_witness_cids(int device, const void* gathered, const uint64_t* counts
     uint64_t h[2] = {0, 0};
     IPCFP_CUDA(cudaMemcpyAsync(h, cnt.p, 16, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (h[1] != UINT64_MAX) throw Error(IPCFP_ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", h[1]);
+    if (mixed) *mixed = h[1];
+    else if (h[1] != UINT64_MAX) throw Error(IPCFP_ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", h[1]);
     const uint64_t n = h[0];
     if (n > cap_out) throw Error(IPCFP_ERR_INVALID_ARG, "output buffer too small for the merged witness CID list");
     k_merge_emit<<<div_up(n, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, pos.p, n, (uint8_t*)out); IPCFP_LAUNCH_CHECK();
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    *n_out = n;
+    return n;
 }
 
 // ------------------------------------------------------------------------------------------ bundle
@@ -129,6 +135,18 @@ struct TimingEvent {
     cudaEvent_t e = nullptr;
     TimingEvent() { IPCFP_CUDA(cudaEventCreate(&e)); }
     ~TimingEvent() { if (e) cudaEventDestroy(e); }
+};
+
+struct FetchPlanBox {
+    ipcfp_fetch_plan r;   // must stay first
+    FetchPlan plan;
+    void fill() {
+        r.n_missing = plan.cids.size() / 38;
+        r.cids = plan.cids.data();
+        r.n_needed = plan.n_needed;
+        r.n_levels = plan.n_levels;
+        r.ms_total = plan.ms_total;
+    }
 };
 
 #define IPCFP_BUNDLE_FLAGS (IPCFP_WITNESS_BY_REFERENCE | IPCFP_RESULT_JSON)
@@ -408,6 +426,35 @@ ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* 
     });
 }
 void ipcfp_bundle_free(ipcfp_bundle* b) { delete reinterpret_cast<BundleBox*>(b); }
+
+ipcfp_status ipcfp_plan_fetch_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                       const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+        plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, especs, n_especs, box->plan);
+        box->fill();
+        *out = &box.release()->r;
+    });
+}
+ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                              const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out) {
+    return guard([&] {
+        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+        Store* st = reinterpret_cast<Store*>(s);
+        TipsetDev td;
+        tipset_upload(st, t, td);
+        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+        plan_fetch(st, td, sspecs, n_sspecs, especs, n_especs, box->plan);
+        box->fill();
+        *out = &box.release()->r;
+    });
+}
+void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }
 
 ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
                                        uint64_t blob_size, const ipcfp_event_spec* filter, uint8_t* results) {

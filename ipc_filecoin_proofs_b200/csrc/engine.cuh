@@ -223,6 +223,20 @@ const WitnessOut& event_result_witness(const ipcfp_event_result* r);   // the wi
 void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n);
 void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
                         uint64_t* n_out);
+// capi.cu: the body of merge_witness_cids on stream st (the raw byte order of the 38 bytes, duplicates removed, into out); returns the
+// count. mixed == nullptr: several CID prefixes are refused as merge_witness_cids refuses them; else *mixed = the first position whose
+// prefix differs from the first entry's (UINT64_MAX: none) and the list is sorted all the same.
+uint64_t sort_unique_cids(cudaStream_t st, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
+                          uint64_t* mixed);
+// plan.cu — ipcfp_plan_fetch_resident: the CIDs of N(S) \ S for the generators of a proof bundle (DESIGN.md §2, "Fetch planning")
+struct FetchPlan {
+    std::vector<uint8_t> cids;   // n*38, `Cid` order
+    uint64_t n_needed = 0;
+    uint32_t n_levels = 0;
+    float ms_total = 0.f;
+};
+void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
+                FetchPlan& out);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);

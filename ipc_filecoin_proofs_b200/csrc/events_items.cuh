@@ -125,8 +125,10 @@ struct Pass1Args {
 };
 
 // ------------------------------------------------------------------------------------------ receipts AMT
-// Amtv0<Receipt>::get(i) with recording (events/generator.rs:249). 1 = Some, 0 = None, <0 = -DevCode.
-static __device__ int receipts_get(const StoreView& s, uint32_t root_blk, uint64_t i, uint32_t* wbits, uint32_t* detail) {
+// Amtv0<Receipt>::get(i) with recording (events/generator.rs:249). 1 = Some, 0 = None, <0 = -DevCode. missing (may be null): on
+// -DC_MISSING, the CID of the node that is not in the store (the fetch planner reads it; plan.cu).
+static __device__ int receipts_get(const StoreView& s, uint32_t root_blk, uint64_t i, uint32_t* wbits, uint32_t* detail,
+                                   const uint8_t** missing = nullptr) {
     uint32_t len;
     const uint8_t* p = store_block(s, root_blk, len);
     Rd r(p, len);
@@ -151,7 +153,7 @@ static __device__ int receipts_get(const StoreView& s, uint32_t root_blk, uint64
         if (!bm_test(h.bm, idx)) return 0;
         uint32_t k = bm_rank(h.bm, idx);
         int32_t child = store_lookup(s, p + h.links_off + 43 * k + 5);
-        if (child < 0) { *detail = 0; return -(int)DC_MISSING; }
+        if (child < 0) { *detail = 0; if (missing) *missing = p + h.links_off + 43 * k + 5; return -(int)DC_MISSING; }
         witness_mark(s, wbits, (uint32_t)child);
         p = store_block(s, (uint32_t)child, len);
         r = Rd(p, len);

@@ -27,6 +27,7 @@ struct Recorder {
     uint32_t hamt_nodes = 0, hamt_bytes = 0;   // HAMT nodes decoded through this recorder and their bytes (measurement: K5's algorithmic bytes)
     bool strict_only = false;                  // A/B switch (IPCFP_HAMT_STRICT=1): skip the fast node decoder
     const uint32_t* rank_of = nullptr;         // StoreView::rank_of (witness bitmaps are indexed by Cid rank); nullptr = identity
+    const uint8_t* missing = nullptr;          // the CID of the last get that found no block (the fetch planner reads it; plan.cu)
     __device__ void note(uint32_t blk) {
         if (wbits) witness_mark_rank(wbits, rank_of ? rank_of[blk] : blk);   // (the verifiers walk without recording)
         if (!list) return;
@@ -41,7 +42,7 @@ struct Fail { uint32_t code; uint32_t detail; };
 // the CID before forwarding; a missing block never reaches the witness because the call fails)
 __device__ __forceinline__ int32_t rec_get(const StoreView& s, Recorder& rec, const uint8_t* cid38) {
     int32_t b = store_lookup(s, cid38);
-    if (b >= 0) rec.note((uint32_t)b);
+    if (b >= 0) rec.note((uint32_t)b); else rec.missing = cid38;
     return b;
 }
 
