@@ -114,6 +114,16 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         try {
             (void)generate_event_proof(s, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, nullptr, &exo);
         } catch (Error& e) {
+            // collect_exec_list takes the parents in order and checks parent k's TxMeta CID before it walks parent k's two message AMTs.
+            // The walk's fault key names the parent it met (eidx / 3: its TxMeta, BLS or SECP AMT); a mismatching TxMeta of an earlier
+            // parent, or of the same one (its TxMeta loaded and decoded, so the fault is in one of its AMTs), is met first.
+            if (tx_key != IPCFP_NO_ERROR) {
+                IPCFP_CUDA(cudaMemcpyAsync(hw + DW_TX_ERR, dw + DW_TX_ERR, 8, cudaMemcpyDeviceToHost, st));
+                IPCFP_CUDA(cudaStreamSynchronize(st));
+                const uint64_t walk_key = hw[DW_TX_ERR];
+                const uint32_t eidx = (uint32_t)(walk_key >> 56);
+                if (walk_key == IPCFP_NO_ERROR || eidx == IPCFP_TX_EIDX_NONE || (uint32_t)(tx_key & 0xff) <= eidx / 3) throw_verify_error(tx_key);
+            }
             e.index = 0;   // failures of the walk surface at the first proof, like everything that depends on the tipset only
             throw;
         }

@@ -1399,6 +1399,8 @@ ipcfp_status oracle_verify_event_proofs(const ipcfp_witness* w, const ipcfp_tips
             HeaderLite child = decode_header(child_raw);
             if (child.parents != ts.parent_cids) continue;
             if (child.height != ts.child_epoch) continue;
+            // parent_tipset_cids[0] of an empty list panics in the reference: a decode error here, as in the engine
+            if (ts.parent_cids.empty()) throw Err(IPCFP_ERR_DECODE, "child header and tipset name no parent", pi);
             Bytes ph_raw;
             if (!bs.get(ts.parent_cids[0], ph_raw)) throw Err(IPCFP_ERR_MISSING_BLOCK, "missing parent header in witness", pi);
             HeaderLite ph = decode_header(ph_raw);

@@ -83,7 +83,7 @@ static void fail_key(Verdict& v, uint64_t key) {   // csrc/verify.cu throw_verif
 
 // ------------------------------------------------------------------------------------------ event proofs: verify.cu's verify_event_proofs, item by item
 static Verdict engine_events(const Blocks& W, const ipcfp_tipset_desc& td, const std::vector<ipcfp_event_proof>& proofs, const std::vector<uint8_t>& blob,
-                             const Matcher* filter, bool* txmeta_fault) {
+                             const Matcher* filter) {
     Verdict v;
     const uint64_t n = proofs.size();
     v.results.assign(n, 0);
@@ -110,16 +110,27 @@ static Verdict engine_events(const Blocks& W, const ipcfp_tipset_desc& td, const
         unsigned long long txerr = IPCFP_NO_ERROR;
         for (uint32_t k = 0; k < P; k++) verify_txmeta_item(hs.view, d_tx, k, &txerr);
         // the execution order: every BLS / SECP message AMT of every parent, first occurrence wins (events/utils.rs:48-94). The engine
-        // runs its own walk + dedup kernels here (emulated elsewhere); a failure of that walk fails the call at proof 0.
+        // runs its own walk + dedup kernels here (emulated elsewhere); a failure of that walk fails the call at proof 0. Its fault key
+        // names the parent it met, which is the first parent whose prefix of the parent list fails to walk. verify.cu ranks a TxMeta
+        // mismatch at that parent or an earlier one first (the reference checks parent k's TxMeta before it walks parent k's AMTs).
         ipcfp_tipset_desc t2 = td;
         t2.parent_txmeta_cids = d_tx;
         oracle_store* os = oracle_store_create(W.cids.data(), W.offs.data(), W.lens.data(), W.blob.data(), W.n);
         std::vector<uint8_t> raw(38ull * 400000);
         uint64_t nraw = 0;
-        const ipcfp_status st = oracle_message_list(os, &t2, raw.data(), raw.size() / 38, &nraw);
+        ipcfp_status st = oracle_message_list(os, &t2, raw.data(), raw.size() / 38, &nraw);
+        uint32_t walk_parent = P;
+        if (st != IPCFP_OK) {
+            for (uint32_t k = 1; k <= P && walk_parent == P; k++) {
+                t2.n_parents = k;
+                uint64_t nk = 0;
+                if (oracle_message_list(os, &t2, raw.data(), raw.size() / 38, &nk) != IPCFP_OK) walk_parent = k - 1;
+            }
+            t2.n_parents = P;
+        }
         oracle_store_destroy(os);
+        if (txerr != IPCFP_NO_ERROR && (st == IPCFP_OK || (uint32_t)(txerr & 0xff) <= walk_parent)) { fail_key(v, txerr); return v; }
         if (st != IPCFP_OK) { v.status = st; v.index = 0; return v; }
-        if (txerr != IPCFP_NO_ERROR) { fail_key(v, txerr); *txmeta_fault = true; return v; }
         std::unordered_map<std::string, uint32_t> seen;
         exec_raw.resize(nraw);
         for (uint64_t k = 0; k < nraw; k++) {
@@ -166,9 +177,9 @@ static Verdict oracle_events(const Blocks& W, const ipcfp_tipset_desc& td, const
     return v;
 }
 
-static int compare(const char* what, const Verdict& e, const Verdict& o, bool loose_status, uint64_t* n_ok, uint64_t* n_err) {
+static int compare(const char* what, const Verdict& e, const Verdict& o, uint64_t* n_ok, uint64_t* n_err) {
     if (o.status != IPCFP_OK || e.status != IPCFP_OK) {
-        const bool same = loose_status ? (e.status != IPCFP_OK && o.status != IPCFP_OK) : (e.status == o.status && e.index == o.index);
+        const bool same = e.status == o.status && e.index == o.index;
         if (!same) { fprintf(stderr, "EMU MISMATCH (%s): engine status %d index %llu vs oracle status %d index %llu\n", what, e.status, (unsigned long long)e.index, o.status, (unsigned long long)o.index); return 1; }
         (*n_err)++;
         return 0;
@@ -283,12 +294,11 @@ int main(int argc, char** argv) {
             ipcfp_tipset_desc t = td;
             std::vector<uint8_t> pc(td.parent_cids, td.parent_cids + 38 * td.n_parents);
             const char* what = "intact";
-            bool loose = false;
             const Matcher* fm = nullptr;
             const ipcfp_event_spec* fs = nullptr;
             if (m > 0) {
                 switch (rnd() % 9) {
-                    case 0: what = "block mutated"; if (W.n) W.mutate(rnd() % W.n); loose = false; break;
+                    case 0: what = "block mutated"; if (W.n) W.mutate(rnd() % W.n); break;
                     case 1: what = "block missing"; if (W.n) W.drop(rnd() % W.n); break;
                     case 2: what = "two blocks mutated"; if (W.n) { W.mutate(rnd() % W.n); W.mutate(rnd() % W.n); } break;
                     case 3: {   // a forged claim
@@ -315,8 +325,7 @@ int main(int argc, char** argv) {
                     default: what = "check_event = another subnet"; fm = &m_other; fs = &spec_other; break;
                 }
             }
-            bool txfault = false;
-            Verdict e = engine_events(W, t, P, B, fm, &txfault);
+            Verdict e = engine_events(W, t, P, B, fm);
             // offsets are an artefact of the POD ABI (the reference's EventProof carries hex strings): a proof that names bytes outside
             // the data blob is ABI misuse, which the engine rejects (false) and the restated verifier — it has no blob size — cannot be
             // asked about. Expected: the intact proof's verdicts with that proof rejected.
@@ -327,10 +336,7 @@ int main(int argc, char** argv) {
             for (size_t i : outside) Pq[i] = P0[i];
             Verdict o = oracle_events(W, t, Pq, B, fs);
             if (o.status == IPCFP_OK) for (size_t i : outside) o.results[i] = 0;
-            // a mutated TxMeta block: the reference recomputes its CID before walking its AMTs, the engine reports a failed walk first —
-            // visible only in a store that was not CID-checked, which ipcfp_verify_event_proofs' contract excludes: any failure will do
-            if ((o.status == IPCFP_ERR_CID_MISMATCH || txfault) && e.status != o.status) loose = true;
-            if (compare(what, e, o, loose, &ev_ok, &ev_err)) { fprintf(stderr, "  (case %llu, mutation %llu, %llu receipts, %llu proofs)\n", (unsigned long long)c, (unsigned long long)m, (unsigned long long)sp.n_receipts, (unsigned long long)P.size()); return 1; }
+            if (compare(what, e, o, &ev_ok, &ev_err)) { fprintf(stderr, "  (case %llu, mutation %llu, %llu receipts, %llu proofs)\n", (unsigned long long)c, (unsigned long long)m, (unsigned long long)sp.n_receipts, (unsigned long long)P.size()); return 1; }
             if (m == 0 && !P.empty() && !(e.status == IPCFP_OK && std::all_of(e.results.begin(), e.results.end(), [](uint8_t x) { return x == 1; }))) { fprintf(stderr, "an intact bundle was not accepted\n"); return 1; }
             if (e.status == IPCFP_OK) for (uint8_t x : e.results) (x ? accepted : rejected)++;
         }
@@ -395,7 +401,7 @@ int main(int argc, char** argv) {
                 }
                 Verdict e = engine_storage(W, t, S);
                 Verdict o = oracle_storage(W, t, S);
-                if (compare(what, e, o, false, &st_ok, &st_err)) { fprintf(stderr, "  (storage case %llu, mutation %llu)\n", (unsigned long long)c, (unsigned long long)m); return 1; }
+                if (compare(what, e, o, &st_ok, &st_err)) { fprintf(stderr, "  (storage case %llu, mutation %llu)\n", (unsigned long long)c, (unsigned long long)m); return 1; }
                 if (m == 0 && !(e.status == IPCFP_OK && std::all_of(e.results.begin(), e.results.end(), [](uint8_t x) { return x == 1; }))) { fprintf(stderr, "intact storage proofs were not accepted\n"); return 1; }
                 if (e.status == IPCFP_OK) for (uint8_t x : e.results) (x ? accepted : rejected)++;
             }
