@@ -445,6 +445,45 @@ void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p);
 ipcfp_status ipcfp_fetch_plan_to_rpc_json(const ipcfp_fetch_plan* p, uint64_t first_id, char** out, uint64_t* out_len);
 
 /* ------------------------------------------------------------------------------------------
+ * Address resolution: Filecoin addresses to actor IDs from the state tree itself, in place of the reference's
+ * Filecoin.EthAddressToFilecoinAddress + Filecoin.StateLookupID round trip (src/proofs/common/address.rs:8-62). The path is
+ * StateRoot [version <= 5, actors, info] -> actors HAMT (width 5) -> the Init actor (ID 1) -> its state, exactly
+ * [address_map, next_id, network_name] -> address_map HAMT (width 5, key Address::to_bytes(), value the ActorID as one CBOR unsigned
+ * integer) (DESIGN.md §2 "Address resolution", §3). ipcfp_address holds Address::to_bytes(): protocol byte, then the payload.
+ * ------------------------------------------------------------------------------------------ */
+#define IPCFP_ADDRESS_MAX 65   /* 1 protocol byte + 10-byte LEB128 namespace + 54-byte subaddress */
+typedef struct ipcfp_address {
+    uint8_t len;
+    uint8_t bytes[IPCFP_ADDRESS_MAX];
+} ipcfp_address;
+typedef struct ipcfp_resolve_result {
+    uint64_t n;
+    const uint64_t* actor_ids;     /* n; 0 where status != IPCFP_OK                                                           */
+    const ipcfp_status* status;    /* n: IPCFP_OK, _ACTOR_NOT_FOUND, _MISSING_BLOCK, _DECODE, or _INVALID_ARG (bytes that are not
+                                      an Address); a non-ID address carries init_status when that is not IPCFP_OK               */
+    ipcfp_status init_status;      /* StateRoot -> actors HAMT -> Init state, walked once per call                              */
+    uint32_t _pad;
+    uint64_t n_missing;
+    const uint8_t* missing_cids;   /* n_missing*38: the blocks the walks lacked, unique, `Cid` order (ipcfp_fetch_plan's form) */
+    ipcfp_witness witness;         /* every block the walks read, the Init path's included, `Cid` order                       */
+    float ms_total, ms_lookup;     /* CUDA events on the store's stream: the call, the address_map walks                      */
+} ipcfp_resolve_result;
+/* n addresses against the state tree at state_root, one device walk per non-ID address. ID addresses (protocol 0) resolve to their
+ * own ID with no read (Lotus StateTree.LookupID). Unknown or unresolvable addresses are answers, not failures: the call fails only on
+ * null arguments, no device or CUDA errors. Missing blocks are reported in missing_cids, so a caller can fetch them (one
+ * Filecoin.ChainReadObj round: ipcfp_fetch_plan_to_rpc_json over a plan holding these CIDs) and call again.
+ * *out is released with ipcfp_resolve_result_free. */
+ipcfp_status ipcfp_resolve_addresses(ipcfp_store* s, const uint8_t state_root[IPCFP_CID_LEN], const ipcfp_address* addrs, uint64_t n,
+                                     ipcfp_resolve_result** out);
+void ipcfp_resolve_result_free(ipcfp_resolve_result* r);
+/* Host only, no device. ipcfp_address_parse: the text form ("f…" or "t…", read alike; protocols 0–4; lower-case unpadded base32 with the
+ * 4-byte Blake2b checksum of to_bytes(); protocol 4 as f4<namespace>f<base32(subaddress ‖ checksum)>) → IPCFP_ERR_INVALID_ARG when
+ * malformed. ipcfp_address_from_eth: Lotus EthAddress.ToFilecoinAddress — a masked ID (0xff, eleven zero bytes, the ID big-endian)
+ * becomes the ID address, any other address f410 (04 0a ‖ eth). */
+ipcfp_status ipcfp_address_parse(const char* text, uint64_t len, ipcfp_address* out);
+ipcfp_status ipcfp_address_from_eth(const uint8_t eth[20], ipcfp_address* out);
+
+/* ------------------------------------------------------------------------------------------
  * Wire format (src/proofs/common/bundle.rs:10-45, src/proofs/events/bundle.rs:5-30, src/proofs/storage/bundle.rs:5-14): the JSON
  * `serde_json::to_string` gives for UnifiedProofBundle / EventProofBundle — struct field order, compact, CIDs as "bafy2bzace…"
  * strings, "0x" lower-case hex, base64 block data (ProofBlock.cid as the byte array cid 0.11's Serialize emits). t supplies the

@@ -22,6 +22,8 @@
 //   verify_storage_proof(&proof, &blocks, &trusted_child)          same                                           (storage/verifier.rs:24-63)
 //   compute_mapping_slot / calculate_storage_slot / ascii_to_bytes32 / left_pad_32   same                         (storage/utils.rs:5-19, common/evm.rs:72-100)
 //   keccak256 / hash_event_signature / create_event_filter / parse_cid / parse_cids  same                         (common/evm.rs:62-88, events/verifier.rs:28-41, common/witness.rs:60-72)
+//   resolve_eth_address_to_actor_id(client, eth_addr)             resolve_eth_address_to_actor_id(store, state_root, eth_addr): the state tree
+//                                                                  instead of two RPC calls; resolve_addresses batches; parse_address  (common/address.rs:8-77)
 //   (future work "Parallel Generation", README.md:384)             ShardedComm, generate_event_proof_sharded → ShardedEventProof
 //   serde_json::to_string(&bundle) / from_str                      to_json(bundle) / bundle_from_json(text)
 //   anyhow::Error                                                  ipcfp::host::Error (status, message, index)
@@ -32,6 +34,7 @@
 #define IPCFP_HPP
 
 #include <array>
+#include <cctype>
 #include <cstdint>
 #include <cstring>
 #include <functional>
@@ -506,6 +509,56 @@ inline std::optional<std::vector<uint8_t>> read_storage_slot(GpuBlockstore& stor
     }
     ipcfp_slot_result_free(r);
     return out;
+}
+
+// ------------------------------------------------------------------------------------------ address resolution from the state tree
+// ipcfp_resolve_addresses in the reference's types. Per-address outcomes are statuses (unknown addresses are answers, not failures).
+struct ResolvedAddresses {
+    std::vector<uint64_t> actor_ids;     // 0 where status != IPCFP_OK
+    std::vector<ipcfp_status> status;
+    ipcfp_status init_status = IPCFP_OK; // StateRoot → actors HAMT → Init state
+    std::vector<Cid> missing;            // blocks the walks lacked, `Cid` order: one ChainReadObj round
+    std::vector<ProofBlock> witness;     // every block the walks read, `Cid` order
+};
+inline ResolvedAddresses resolve_addresses(GpuBlockstore& store, const Cid& state_root, const std::vector<ipcfp_address>& addrs) {
+    ipcfp_resolve_result* r = nullptr;
+    check(ipcfp_resolve_addresses(store.raw(), state_root.bytes.data(), addrs.data(), addrs.size(), &r), "resolve_addresses");
+    ResolvedAddresses out;
+    out.actor_ids.assign(r->actor_ids, r->actor_ids + r->n);
+    out.status.assign(r->status, r->status + r->n);
+    out.init_status = r->init_status;
+    for (uint64_t i = 0; i < r->n_missing; i++) out.missing.push_back(Cid::from_bytes(r->missing_cids + IPCFP_CID_LEN * i));
+    out.witness = proof_blocks(r->witness);
+    ipcfp_resolve_result_free(r);
+    return out;
+}
+// parse_address (common/address.rs:65-77): "f…" or "t…"
+inline ipcfp_address parse_address(const std::string& s) {
+    ipcfp_address a;
+    check(ipcfp_address_parse(s.data(), s.size(), &a), ("Failed to parse address '" + s + "'").c_str());
+    return a;
+}
+// the validation of resolve_eth_address_to_actor_id (common/address.rs:10-21) and EthAddressToFilecoinAddress
+inline ipcfp_address eth_to_filecoin_address(const std::string& eth_addr) {
+    size_t b = 0;
+    while (eth_addr.compare(b, 2, "0x") == 0) b += 2;   // trim_start_matches("0x")
+    const std::string h = eth_addr.substr(b);
+    if (h.size() % 2) throw Error(IPCFP_ERR_INVALID_ARG, "Invalid hex in Ethereum address: Odd number of digits");
+    for (size_t i = 0; i < h.size(); i++)
+        if (!isxdigit((unsigned char)h[i])) throw Error(IPCFP_ERR_INVALID_ARG, std::string("Invalid hex in Ethereum address: Invalid character '") + h[i] +
+                                                                            "' at position " + std::to_string(i));
+    const std::vector<uint8_t> bytes = from_hex0x(h);
+    if (bytes.size() != 20)
+        throw Error(IPCFP_ERR_INVALID_ARG, "Invalid Ethereum address length: expected 20 bytes, got " + std::to_string(bytes.size()));
+    ipcfp_address a;
+    check(ipcfp_address_from_eth(bytes.data(), &a), "eth_to_filecoin_address");
+    return a;
+}
+// resolve_eth_address_to_actor_id (common/address.rs:8-62) from the state tree at state_root (the child header's ParentStateRoot)
+inline uint64_t resolve_eth_address_to_actor_id(GpuBlockstore& store, const Cid& state_root, const std::string& eth_addr) {
+    const ResolvedAddresses r = resolve_addresses(store, state_root, {eth_to_filecoin_address(eth_addr)});
+    if (r.status[0] != IPCFP_OK) throw Error(r.status[0], "Failed to lookup ID address: ipcfp status " + std::to_string((int)r.status[0]));
+    return r.actor_ids[0];
 }
 
 // generate_proof_bundle (proofs/generator.rs:25-95): every spec against one store, blocks deduplicated as BTreeSet<(Cid, data)>

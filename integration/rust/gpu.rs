@@ -472,6 +472,28 @@ pub fn generate_storage_proof_gpu(
     res
 }
 
+/// `resolve_eth_address_to_actor_id` (`src/proofs/common/address.rs:8-62`) from the state tree at `state_root` (the child header's
+/// ParentStateRoot) instead of `Filecoin.EthAddressToFilecoinAddress` + `Filecoin.StateLookupID`: the same validation and messages,
+/// then the Init actor's address map walked on the GPU.
+pub fn resolve_eth_address_to_actor_id_gpu(store: &GpuBlockstore, state_root: &Cid, eth_addr: &str) -> Result<u64> {
+    let eth_addr = eth_addr.trim_start_matches("0x");
+    let bytes = hex::decode(eth_addr).map_err(|e| anyhow!("Invalid hex in Ethereum address: {}", e))?;
+    if bytes.len() != 20 {
+        return Err(anyhow!("Invalid Ethereum address length: expected 20 bytes, got {}", bytes.len()));
+    }
+    let mut addr = sys::ipcfp_address { len: 0, bytes: [0u8; sys::IPCFP_ADDRESS_MAX] };
+    check(unsafe { sys::ipcfp_address_from_eth(bytes.as_ptr(), &mut addr) })?;
+    let root = cid38(state_root)?;
+    let mut out = std::ptr::null_mut();
+    check(unsafe { sys::ipcfp_resolve_addresses(store.h, root.as_ptr(), &addr, 1, &mut out) })?;
+    let (st, id) = unsafe { (*(*out).status, *(*out).actor_ids) };
+    unsafe { sys::ipcfp_resolve_result_free(out) };
+    if st != sys::IPCFP_OK {
+        bail!("Failed to lookup ID address: ipcfp status {}", st);
+    }
+    Ok(id)
+}
+
 /// `generate_proof_bundle` (`src/proofs/generator.rs:25-95`): ONE store built from everything the RPC layer fetched for this tipset
 /// pair, storage specs first, then event specs, then the `BTreeSet<(Cid, Vec<u8>)>` union of the witnesses.
 pub fn generate_proof_bundle_gpu(

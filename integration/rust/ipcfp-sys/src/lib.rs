@@ -103,6 +103,13 @@ pub struct ipcfp_parsed_blocks { pub blocks: ipcfp_witness }
 pub struct ipcfp_store_json_info { pub parsed_on_device: u32, pub ms_parse: f32, pub ms_kernels: f32, pub _pad: u32 }
 #[repr(C)]
 pub struct ipcfp_fetch_plan { pub n_missing: u64, pub cids: *const u8, pub n_needed: u64, pub n_levels: u32, pub ms_total: f32 }
+pub const IPCFP_ADDRESS_MAX: usize = 65;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct ipcfp_address { pub len: u8, pub bytes: [u8; IPCFP_ADDRESS_MAX] }
+#[repr(C)]
+pub struct ipcfp_resolve_result { pub n: u64, pub actor_ids: *const u64, pub status: *const ipcfp_status, pub init_status: ipcfp_status, pub _pad: u32,
+                                  pub n_missing: u64, pub missing_cids: *const u8, pub witness: ipcfp_witness, pub ms_total: f32, pub ms_lookup: f32 }
 #[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
                           pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
@@ -168,6 +175,11 @@ extern "C" {
                             especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_fetch_plan_free(p: *mut ipcfp_fetch_plan);
     pub fn ipcfp_fetch_plan_to_rpc_json(p: *const ipcfp_fetch_plan, first_id: u64, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
+    pub fn ipcfp_resolve_addresses(s: *mut ipcfp_store, state_root: *const u8, addrs: *const ipcfp_address, n: u64,
+                                   out: *mut *mut ipcfp_resolve_result) -> ipcfp_status;
+    pub fn ipcfp_resolve_result_free(r: *mut ipcfp_resolve_result);
+    pub fn ipcfp_address_parse(text: *const c_char, len: u64, out: *mut ipcfp_address) -> ipcfp_status;
+    pub fn ipcfp_address_from_eth(eth: *const u8, out: *mut ipcfp_address) -> ipcfp_status;
 
     pub fn ipcfp_bundle_to_json(b: *const ipcfp_bundle, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_event_result_to_json(r: *const ipcfp_event_result, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;

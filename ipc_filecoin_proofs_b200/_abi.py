@@ -231,6 +231,55 @@ def fetch_plan_from_c(p):
     return FetchPlanPy(cids.reshape(-1, CID_LEN), int(p.n_needed), int(p.n_levels), float(p.ms_total))
 
 
+ADDRESS_MAX = 65
+
+
+class AddressC(C.Structure):
+    """ipcfp_address: Address::to_bytes() (protocol byte, then the payload)."""
+    _fields_ = [("len", C.c_uint8), ("bytes", C.c_uint8 * ADDRESS_MAX)]
+
+    def to_bytes(self):
+        return bytes(self.bytes[:self.len])
+
+
+def make_addresses(addresses):
+    """[bytes] (Address::to_bytes() each) → ctypes array of ipcfp_address. Inputs longer than IPCFP_ADDRESS_MAX do not fit and are
+    refused here; other malformed bytes reach the call, which reports them as IPCFP_ERR_INVALID_ARG."""
+    parts = []
+    for i, a in enumerate(addresses):
+        a = bytes(a)
+        if len(a) > ADDRESS_MAX:
+            raise ValueError(f"address {i}: {len(a)} bytes (at most {ADDRESS_MAX})")
+        parts.append(bytes([len(a)]) + a.ljust(ADDRESS_MAX, b"\0"))
+    return (AddressC * max(len(addresses), 1)).from_buffer_copy(b"".join(parts) or bytes(C.sizeof(AddressC)))
+
+
+class ResolveResultC(C.Structure):
+    """ipcfp_resolve_result (ipcfp_resolve_addresses)."""
+    _fields_ = [("n", C.c_uint64), ("actor_ids", C.c_void_p), ("status", C.c_void_p), ("init_status", C.c_int32), ("_pad", C.c_uint32),
+                ("n_missing", C.c_uint64), ("missing_cids", C.c_void_p), ("witness", Witness), ("ms_total", C.c_float), ("ms_lookup", C.c_float)]
+
+
+@dataclass
+class ResolveResultPy:
+    """Actor IDs (0 where status != OK), per-address status, the Init path's status, the CIDs the walks lacked ((m, 38), `Cid` order),
+    the blocks they read, and the device times."""
+    actor_ids: np.ndarray
+    status: np.ndarray
+    init_status: int
+    missing: np.ndarray
+    witness: "WitnessPy"
+    ms_total: float
+    ms_lookup: float
+
+
+def resolve_result_from_c(r):
+    n, m = int(r.n), int(r.n_missing)
+    return ResolveResultPy(_arr(r.actor_ids, n, np.uint64), _arr(r.status, n, np.int32), int(r.init_status),
+                           _arr(r.missing_cids, m * CID_LEN, np.uint8).reshape(m, CID_LEN), witness_from_c(r.witness), float(r.ms_total),
+                           float(r.ms_lookup))
+
+
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
 TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
 

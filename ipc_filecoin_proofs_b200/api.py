@@ -47,6 +47,7 @@ EXPORTS = [
     "ipcfp_generate_proof_bundle_resident", "ipcfp_tipset_desc_from_json", "ipcfp_parsed_tipset_free", "ipcfp_tipset_upload_json",
     "ipcfp_tipset_describe", "ipcfp_blocks_from_rpc_json", "ipcfp_parsed_blocks_free", "ipcfp_store_create_rpc_json",
     "ipcfp_plan_fetch_resident", "ipcfp_plan_fetch", "ipcfp_fetch_plan_free", "ipcfp_fetch_plan_to_rpc_json",
+    "ipcfp_resolve_addresses", "ipcfp_resolve_result_free", "ipcfp_address_parse", "ipcfp_address_from_eth",
 ]
 
 
@@ -174,6 +175,13 @@ def lib():
         L.ipcfp_fetch_plan_free.argtypes = [C.POINTER(A.FetchPlanC)]
         L.ipcfp_fetch_plan_to_rpc_json.restype = C.c_int32
         L.ipcfp_fetch_plan_to_rpc_json.argtypes = [C.POINTER(A.FetchPlanC), C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+        L.ipcfp_resolve_addresses.restype = C.c_int32
+        L.ipcfp_resolve_addresses.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.AddressC), C.c_uint64, C.POINTER(C.POINTER(A.ResolveResultC))]
+        L.ipcfp_resolve_result_free.argtypes = [C.POINTER(A.ResolveResultC)]
+        L.ipcfp_address_parse.restype = C.c_int32
+        L.ipcfp_address_parse.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(A.AddressC)]
+        L.ipcfp_address_from_eth.restype = C.c_int32
+        L.ipcfp_address_from_eth.argtypes = [C.c_void_p, C.POINTER(A.AddressC)]
         _lib = L
     return _lib
 
@@ -397,6 +405,20 @@ class BlockStore:
         finally:
             lib().ipcfp_fetch_plan_free(out)
 
+    def resolve_addresses(self, state_root, addresses):
+        """ipcfp_resolve_addresses → A.ResolveResultPy: every address (Address::to_bytes(), or text for address_parse) resolved to its
+        actor ID through the Init actor's address map of the state tree at state_root (38 bytes)."""
+        root = _u8(state_root)
+        if root.size != A.CID_LEN:
+            raise ValueError("state_root must be a 38-byte CID")
+        addrs = A.make_addresses([address_parse(a) if isinstance(a, str) else a for a in addresses])
+        out = C.POINTER(A.ResolveResultC)()
+        _check(lib().ipcfp_resolve_addresses(self._h, root.ctypes.data, addrs, len(addresses), C.byref(out)))
+        try:
+            return A.resolve_result_from_c(out.contents)
+        finally:
+            lib().ipcfp_resolve_result_free(out)
+
     def close(self):
         if self._h:
             lib().ipcfp_store_destroy(self._h)
@@ -511,6 +533,89 @@ def fetch_until_complete(fetch, upload_tipset, storage_specs, event_specs, devic
         tip = upload_tipset(store)
         rounds.append(FetchRound(plan.cids, plan.ms_total, (time.perf_counter() - t0) * 1e3))
     raise RuntimeError("fetch_until_complete: no fixed point after %d rounds" % max_rounds)
+
+
+def address_parse(text):
+    """ipcfp_address_parse (host, no device): "f…" / "t…" address text → Address::to_bytes(). Malformed text raises IpcfpError."""
+    raw = text.encode() if isinstance(text, str) else bytes(text)
+    a = A.AddressC()
+    _check(lib().ipcfp_address_parse(raw, len(raw), C.byref(a)))
+    return a.to_bytes()
+
+
+def _eth_bytes(eth_addr):
+    """The reference's validation of an Ethereum address (src/proofs/common/address.rs:10-21) → 20 bytes; ValueError with its messages."""
+    if isinstance(eth_addr, (bytes, bytearray)):
+        b = bytes(eth_addr)
+    else:
+        s = eth_addr
+        while s.startswith("0x"):          # trim_start_matches("0x")
+            s = s[2:]
+        raw = s.encode()
+        if len(raw) % 2:
+            raise ValueError("Invalid hex in Ethereum address: Odd number of digits")
+        for i, c in enumerate(raw):
+            if chr(c) not in "0123456789abcdefABCDEF":
+                raise ValueError(f"Invalid hex in Ethereum address: Invalid character {chr(c)!r} at position {i}")
+        b = bytes.fromhex(s)
+    if len(b) != 20:
+        raise ValueError(f"Invalid Ethereum address length: expected 20 bytes, got {len(b)}")
+    return b
+
+
+def address_from_eth(eth_addr):
+    """ipcfp_address_from_eth (host, no device): "0x…" hex or 20 bytes → Address::to_bytes() of the Filecoin address Lotus's
+    EthAddressToFilecoinAddress returns (a masked ID → the ID address, else f410)."""
+    b = _eth_bytes(eth_addr)
+    a = A.AddressC()
+    _check(lib().ipcfp_address_from_eth(b, C.byref(a)))
+    return a.to_bytes()
+
+
+def resolve_eth_address_to_actor_id(store, state_root, eth_addr):
+    """The reference's resolve_eth_address_to_actor_id (src/proofs/common/address.rs:8-62) from the state tree at state_root instead of
+    two RPC calls: the same validation and messages, then the Init actor's address map. Raises IpcfpError when the address does not
+    resolve (status ACTOR_NOT_FOUND, MISSING_BLOCK or DECODE)."""
+    r = store.resolve_addresses(state_root, [address_from_eth(eth_addr)])
+    st = int(r.status[0])
+    if st != A.OK:
+        raise A.IpcfpError(st, "Failed to lookup ID address", 0)
+    return int(r.actor_ids[0])
+
+
+@dataclass
+class ResolveRound:
+    """One round of resolve_until_complete: the CIDs requested and the resolver's device time before it."""
+    cids: np.ndarray
+    ms_resolve: float
+
+
+def resolve_until_complete(fetch, state_root, addresses, device=0, verify_cids=True, cids=None, texts=None, max_rounds=10000):
+    """Resolves addresses, fetching the blocks the walks lack until none is missing: fetch_until_complete's loop with the resolver's
+    missing list as the plan. fetch(cids, first_id) returns the Filecoin.ChainReadObj response texts for cids ((k, 38)) with ids
+    first_id + j. cids / texts: blocks the caller already holds (their CIDs and response texts), else an empty store.
+    Returns (store, result, rounds, cids, texts)."""
+    all_cids = np.zeros((0, A.CID_LEN), np.uint8) if cids is None else np.ascontiguousarray(cids, np.uint8).reshape(-1, A.CID_LEN)
+    texts = list(texts or [])
+    rounds = []
+
+    def make_store():
+        if len(all_cids):
+            return BlockStore.from_rpc_json(all_cids, texts, device=device, verify_cids=verify_cids)
+        return BlockStore(all_cids, np.zeros(0, np.uint64), np.zeros(0, np.uint32), np.zeros(0, np.uint8), device=device)
+
+    store = make_store()
+    for _ in range(max_rounds):
+        r = store.resolve_addresses(state_root, addresses)
+        if not len(r.missing):
+            return store, r, rounds, all_cids, texts
+        got = fetch(r.missing, len(all_cids))
+        texts += [got] if isinstance(got, (bytes, str)) else list(got)
+        all_cids = np.concatenate([all_cids, r.missing])
+        rounds.append(ResolveRound(r.missing, r.ms_total))
+        store.close()
+        store = make_store()
+    raise RuntimeError("resolve_until_complete: no fixed point after %d rounds" % max_rounds)
 
 
 def tipset_desc_from_json(parent_text, child_text, receipts_text):

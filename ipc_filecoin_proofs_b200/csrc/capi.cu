@@ -456,6 +456,45 @@ ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const 
 }
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }
 
+struct ResolveBox {
+    ipcfp_resolve_result r;   // must stay first
+    ResolveOut out;
+};
+ipcfp_status ipcfp_resolve_addresses(ipcfp_store* s, const uint8_t state_root[IPCFP_CID_LEN], const ipcfp_address* addrs, uint64_t n,
+                                     ipcfp_resolve_result** out) {
+    return guard([&] {
+        if (!s || !state_root || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        std::unique_ptr<ResolveBox> box(new ResolveBox());
+        resolve_addresses(reinterpret_cast<Store*>(s), state_root, addrs, n, box->out);
+        ipcfp_resolve_result& r = box->r;
+        memset(&r, 0, sizeof r);
+        r.n = n;
+        r.actor_ids = box->out.ids.data();
+        r.status = box->out.status.data();
+        r.init_status = box->out.init_status;
+        r.n_missing = box->out.missing.size() / 38;
+        r.missing_cids = box->out.missing.data();
+        box->out.wit.fill(r.witness);
+        r.ms_total = box->out.ms_total;
+        r.ms_lookup = box->out.ms_lookup;
+        *out = &box.release()->r;
+    });
+}
+void ipcfp_resolve_result_free(ipcfp_resolve_result* r) { delete reinterpret_cast<ResolveBox*>(r); }
+ipcfp_status ipcfp_address_parse(const char* text, uint64_t len, ipcfp_address* out) {
+    return guard([&] {
+        if (!text || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        address_parse(text, len, *out);
+    });
+}
+ipcfp_status ipcfp_address_from_eth(const uint8_t eth[20], ipcfp_address* out) {
+    return guard([&] {
+        if (!eth || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        address_from_eth(eth, *out);
+    });
+}
+
 ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
                                        uint64_t blob_size, const ipcfp_event_spec* filter, uint8_t* results) {
     return guard([&] {

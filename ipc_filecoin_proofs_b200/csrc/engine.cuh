@@ -237,6 +237,8 @@ struct FetchPlan {
 };
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
                 FetchPlan& out);
+// a list of 38-byte CIDs (n*38) into `Cid` order on the host (stable)
+void sort_cids_host(std::vector<uint8_t>& cids);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);
@@ -348,6 +350,19 @@ void materialize_witness(Store* s, const uint32_t* wbits_dev, WitnessOut& out, b
 // the union of witness lists of this store (the BTreeSet<(Cid, data)> of generate_proof_bundle): every entry's block marks its rank in a
 // fresh bitmap (block indices from WitnessOut::idx_dev), which is then materialised as one witness, in `Cid` order
 void witness_union(Store* s, const std::vector<const WitnessOut*>& lists, WitnessOut& out, bool by_ref);
+
+// resolve.cu — ipcfp_resolve_addresses (DESIGN.md §2, "Address resolution") and the host-side address codecs
+struct ResolveOut {
+    std::vector<uint64_t> ids;
+    std::vector<int32_t> status;
+    int32_t init_status = IPCFP_OK;
+    std::vector<uint8_t> missing;   // n*38, unique, `Cid` order
+    WitnessOut wit;
+    float ms_total = 0.f, ms_lookup = 0.f;
+};
+void resolve_addresses(Store* s, const uint8_t* state_root, const ipcfp_address* addrs, uint64_t n, ResolveOut& out);
+void address_parse(const char* text, uint64_t len, ipcfp_address& out);
+void address_from_eth(const uint8_t eth[20], ipcfp_address& out);
 
 // json.cu — IPCFP_RESULT_JSON: the EventProofBundle text of one call from what is on the device after k_witness_emit (all pointers device)
 struct JsonInputs {

@@ -357,7 +357,7 @@ __device__ __forceinline__ void parse_receipt(Rd& r) {
 }
 
 // ------------------------------------------------------------------ HAMT (fvm_ipld_hamt v3 layout)
-enum HamtValueKind { HV_ACTOR_STATE = 0, HV_U8VEC = 1 };
+enum HamtValueKind { HV_ACTOR_STATE = 0, HV_U8VEC = 1, HV_U64 = 2 };   // HV_U64: ActorID, the Init actor's address_map values
 // value decoders: validate and remember where the value starts
 __device__ __forceinline__ void parse_actor_state(Rd& r, uint32_t& state_cid_off) {
     rd_array_exact(r, 5);
@@ -409,6 +409,7 @@ __device__ __forceinline__ void hamt_node_lookup(Rd& r, int vkind, uint32_t idx,
                 uint32_t ko = rd_bytes(r, kl);
                 uint32_t voff = r.pos;
                 if (vkind == HV_ACTOR_STATE) { uint32_t s; parse_actor_state(r, s); }
+                else if (vkind == HV_U64) (void)rd_uint(r);
                 else { uint32_t f; (void)parse_u8vec(r, f); }
                 if (k == want && !r.err && hit.kind == 0 && kl == keylen) {
                     bool eq = true;
@@ -459,6 +460,21 @@ __device__ __forceinline__ bool skip_u8vec_fast(const uint8_t* p, uint32_t len, 
     }
     return true;
 }
+// one minimal major-0 head (rd_uint's rules); anything else goes to the strict decoder
+__device__ __forceinline__ bool skip_u64_fast(const uint8_t* p, uint32_t len, uint32_t& pos) {
+    if (pos >= len) return false;
+    const uint32_t b = p[pos];
+    if (b < 0x18) { pos += 1; return true; }
+    if (b > 0x1b) return false;
+    const uint32_t nb = 1u << (b - 0x18);
+    if (len - pos - 1 < nb) return false;
+    uint64_t v = 0;
+    for (uint32_t i = 0; i < nb; i++) v = (v << 8) | p[pos + 1 + i];
+    const uint64_t minv = b == 0x18 ? 24ull : (b == 0x19 ? 0x100ull : (b == 0x1a ? 0x10000ull : 0x100000000ull));
+    if (v < minv) return false;
+    pos += 1 + nb;
+    return true;
+}
 __device__ __forceinline__ bool hamt_node_lookup_fast(const uint8_t* p, uint32_t len, int vkind, uint32_t idx, const uint8_t* key, uint32_t keylen, HamtHit& hit) {
     hit.kind = 0; hit.val_off = 0; hit.link_off = 0;
     if (len < 3) return false;
@@ -506,6 +522,7 @@ __device__ __forceinline__ bool hamt_node_lookup_fast(const uint8_t* p, uint32_t
                 pos = ko + kl;
                 const uint32_t voff = pos;
                 if (vkind == HV_U8VEC) { if (!skip_u8vec_fast(p, len, pos)) return false; }
+                else if (vkind == HV_U64) { if (!skip_u64_fast(p, len, pos)) return false; }
                 else {
                     Rd r(p, len);
                     r.pos = pos;

@@ -259,15 +259,18 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     IPCFP_CUDA(cudaEventElapsedTime(&out.ms_total, s->ev[EV_BEGIN], s->ev[EV_END]));
     // The device order is the bytes' order, which is `Cid` order within one prefix. A CID of another prefix (one that no block of the
     // store has, so rarely more than a few) puts the list in `Cid` order on the host.
-    if (mixed != UINT64_MAX) {
-        std::vector<uint32_t> ord(m);
-        for (uint32_t k = 0; k < m; k++) ord[k] = k;
-        const uint8_t* c = out.cids.data();
-        std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return cid_less(c + 38ull * x, c + 38ull * y); });
-        std::vector<uint8_t> sorted(38 * m);
-        for (uint64_t k = 0; k < m; k++) memcpy(sorted.data() + 38 * k, c + 38ull * ord[k], 38);
-        out.cids.swap(sorted);
-    }
+    if (mixed != UINT64_MAX) sort_cids_host(out.cids);
+}
+
+void sort_cids_host(std::vector<uint8_t>& cids) {
+    const uint64_t m = cids.size() / 38;
+    std::vector<uint32_t> ord(m);
+    for (uint32_t k = 0; k < m; k++) ord[k] = k;
+    const uint8_t* c = cids.data();
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return cid_less(c + 38ull * x, c + 38ull * y); });
+    std::vector<uint8_t> sorted(38 * m);
+    for (uint64_t k = 0; k < m; k++) memcpy(sorted.data() + 38 * k, c + 38ull * ord[k], 38);
+    cids.swap(sorted);
 }
 
 }  // namespace ipcfp
