@@ -175,7 +175,7 @@ typedef struct ipcfp_event_result {
     /* shard mode only (ipcfp_generate_event_proof_shard): this shard's slice of the concatenated message list,
      * in order, as 40-byte records {digest[32], prefix[6], 0, 0} in DEVICE memory (valid until the result is
      * freed; free results before destroying the store). proofs[].message_cid is left zero and n_exec is 0:
-     * the execution order spans shards and is resolved by the caller (ipcfp_exec_* helpers). */
+     * the execution order spans shards, and only ipcfp_generate_event_proof_sharded resolves it. */
     const void* shard_exec_dev;
     uint64_t shard_exec_count;
     uint64_t shard_raw_total;         /* total length of the concatenated message list (all shards) */
@@ -573,9 +573,9 @@ ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device
 void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v);
 
 /* ------------------------------------------------------------------------------------------
- * Multi-GPU (one process per GPU; the caller owns the communicator — torch.distributed / NCCL).
- * Receipts shard by index range; each rank scans its shard, then the per-shard witness CID sets
- * are all-gathered and merged (the BTreeSet union of src/proofs/common/witness.rs:24-40).
+ * Multi-GPU (one process per GPU; the library runs the collectives itself, over NCCL).
+ * Receipts shard by index range; each rank scans its shard, and one call per rank resolves what spans
+ * shards: the execution order, the proofs' message CIDs and the union of the per-shard witness CID sets.
  * ------------------------------------------------------------------------------------------ */
 /* In-library protocol (the reference's future-work "Parallel Generation", README.md:384; SURVEY Appendix C): one communicator
  * per process/GPU over NCCL (resolved with dlopen("libnccl.so.2") at init — the library itself links only cudart). Rank 0 makes
@@ -596,38 +596,11 @@ void ipcfp_comm_destroy(ipcfp_comm* c);
 ipcfp_status ipcfp_generate_event_proof_sharded(ipcfp_comm* c, ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec,
                                                 const uint64_t* bounds /* world_size + 1 */, uint32_t flags, ipcfp_event_result** out);
 
-/* Lower-level pieces (the caller owns the collectives — e.g. torch.distributed with the gloo backend on hosts without NCCL):
- * scan receipts [lo, hi) only. events_roots/has_events_root in t cover ALL n_receipts. */
+/* One shard's scan on its own, without the cross-shard steps: receipts [lo, hi) only; events_roots/has_events_root in t cover
+ * ALL n_receipts. See ipcfp_event_result.shard_exec_dev for what the result leaves unresolved. */
 ipcfp_status ipcfp_generate_event_proof_shard(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_spec* spec,
                                               uint64_t lo, uint64_t hi, uint32_t world_size, uint32_t rank,
                                               uint32_t flags, ipcfp_event_result** out);
-/* Cross-shard execution order (events/utils.rs:56-91, "first seen wins" over ALL message AMTs): a distributed
- * hash join whose collectives the caller runs between these device helpers. All pointers *_dev are device
- * memory; an "exec entry" is 48 bytes {record[40], global position u64}.
- *   1. pos0 = sum of shard_exec_count of lower ranks (all-gather); ipcfp_exec_bucketize routes every record of
- *      the rank's slice to owner = hash(cid) % world: send_dev = world segments of `cap` entries, counts[world].
- *      Inside a segment the entries are in increasing position order.
- *   2. all-to-all of counts and segments (segment r of the received buffer comes from rank r, so the buffer is
- *      ordered by global position per CID); ipcfp_exec_dedup returns the global positions that are NOT the first
- *      occurrence of their CID (any order).
- *   3. all-gather of the duplicate lists → sorted D on every rank: exec index i ↔ raw position p with
- *      p = i + |{d ∈ D : d ≤ p}|; n_exec = shard_raw_total − |D|.
- *   4. ipcfp_exec_fetch writes the records at the requested global positions this rank holds (others untouched). */
-ipcfp_status ipcfp_exec_bucketize(int device, const void* seg_dev, uint64_t nseg, uint64_t pos0, uint32_t world, uint64_t cap,
-                                  void* send_dev, uint64_t* counts /* host, world */);
-ipcfp_status ipcfp_exec_dedup(int device, const void* recv_dev, const uint64_t* counts /* host, world */, uint32_t world, uint64_t cap,
-                              uint64_t* dup_pos_dev, uint64_t cap_out, uint64_t* n_dup);
-ipcfp_status ipcfp_exec_fetch(int device, const void* seg_dev, uint64_t nseg, uint64_t pos0, const uint64_t* req_pos_dev, uint64_t n_req,
-                              void* out_dev /* n_req*40 */);
-/* Device-resident copy of a result's sorted witness CIDs (n*38 bytes) for the collective. */
-ipcfp_status ipcfp_witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap_cids, uint64_t* n);
-/* Merge all-gathered CID lists on the device: gathered = world*cap*38 bytes, counts[world];
- * out_dev receives the sorted unique union (cap_out*38), *n_out its length.
- * Every CID must carry the first CID's 6-byte prefix (version, codec, multihash code, size): the order is the raw byte order,
- * which is `Cid` order only within one prefix. Otherwise IPCFP_ERR_UNSUPPORTED, with ipcfp_last_error_index() the first
- * position (counted over the segments' valid entries, in order) whose prefix differs, and *n_out = 0. */
-ipcfp_status ipcfp_merge_witness_cids(int device, const void* gathered_dev, const uint64_t* counts, uint32_t world,
-                                      uint64_t cap, void* out_dev, uint64_t cap_out, uint64_t* n_out);
 
 #ifdef __cplusplus
 }

@@ -199,11 +199,4 @@ extern "C" {
     pub fn ipcfp_comm_destroy(c: *mut ipcfp_comm);
     pub fn ipcfp_generate_event_proof_sharded(c: *mut ipcfp_comm, s: *mut ipcfp_store, t: *mut ipcfp_tipset, spec: *const ipcfp_event_spec,
                                               bounds: *const u64, flags: u32, out: *mut *mut ipcfp_event_result) -> ipcfp_status;
-
-    pub fn ipcfp_exec_bucketize(device: c_int, seg_dev: *const c_void, nseg: u64, pos0: u64, world: u32, cap: u64, send_dev: *mut c_void, counts: *mut u64) -> ipcfp_status;
-    pub fn ipcfp_exec_dedup(device: c_int, recv_dev: *const c_void, counts: *const u64, world: u32, cap: u64, dup_pos_dev: *mut u64, cap_out: u64, n_dup: *mut u64) -> ipcfp_status;
-    pub fn ipcfp_exec_fetch(device: c_int, seg_dev: *const c_void, nseg: u64, pos0: u64, req_pos_dev: *const u64, n_req: u64, out_dev: *mut c_void) -> ipcfp_status;
-    pub fn ipcfp_witness_cids_to_device(r: *const ipcfp_event_result, dev_ptr: *mut c_void, cap_cids: u64, n: *mut u64) -> ipcfp_status;
-    pub fn ipcfp_merge_witness_cids(device: c_int, gathered_dev: *const c_void, counts: *const u64, world: u32, cap: u64, out_dev: *mut c_void,
-                                    cap_out: u64, n_out: *mut u64) -> ipcfp_status;
 }

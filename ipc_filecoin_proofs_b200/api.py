@@ -38,9 +38,9 @@ EXPORTS = [
     "ipcfp_store_first_bad_block", "ipcfp_blake2b256_batch", "ipcfp_keccak256_batch", "ipcfp_sha256_batch",
     "ipcfp_compute_mapping_slots", "ipcfp_generate_event_proof", "ipcfp_event_result_free", "ipcfp_read_storage_slots",
     "ipcfp_slot_result_free", "ipcfp_generate_storage_proofs", "ipcfp_storage_result_free", "ipcfp_generate_proof_bundle",
-    "ipcfp_bundle_free", "ipcfp_generate_event_proof_shard", "ipcfp_witness_cids_to_device", "ipcfp_merge_witness_cids",
+    "ipcfp_bundle_free", "ipcfp_generate_event_proof_shard",
     "ipcfp_tipset_upload", "ipcfp_tipset_free", "ipcfp_generate_event_proof_resident", "ipcfp_generate_event_proof_shard_resident",
-    "ipcfp_store_stream", "ipcfp_exec_bucketize", "ipcfp_exec_dedup", "ipcfp_exec_fetch",
+    "ipcfp_store_stream",
     "ipcfp_comm_unique_id", "ipcfp_comm_init", "ipcfp_comm_destroy", "ipcfp_generate_event_proof_sharded",
     "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
     "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
@@ -115,17 +115,6 @@ def lib():
                                                                 C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.POINTER(A.EventResultC))]
         L.ipcfp_store_stream.restype = C.c_void_p
         L.ipcfp_store_stream.argtypes = [C.c_void_p]
-        L.ipcfp_exec_bucketize.restype = C.c_int32
-        L.ipcfp_exec_bucketize.argtypes = [C.c_int, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
-        L.ipcfp_exec_dedup.restype = C.c_int32
-        L.ipcfp_exec_dedup.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-        L.ipcfp_exec_fetch.restype = C.c_int32
-        L.ipcfp_exec_fetch.argtypes = [C.c_int, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
-        L.ipcfp_witness_cids_to_device.restype = C.c_int32
-        L.ipcfp_witness_cids_to_device.argtypes = [C.POINTER(A.EventResultC), C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-        L.ipcfp_merge_witness_cids.restype = C.c_int32
-        L.ipcfp_merge_witness_cids.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint64,
-                                               C.POINTER(C.c_uint64)]
         L.ipcfp_comm_unique_id.restype = C.c_int32
         L.ipcfp_comm_unique_id.argtypes = [C.c_void_p]
         L.ipcfp_comm_init.restype = C.c_int32

@@ -3,7 +3,6 @@
 #include <cstring>
 
 #include "engine.cuh"
-#include "prims.cuh"
 
 namespace ipcfp {
 
@@ -21,103 +20,6 @@ template <class F> static ipcfp_status guard(F f) {
     catch (const Error& e) { g_last_error = e.msg; g_last_index = e.index; return e.status; }
     catch (const std::bad_alloc&) { g_last_error = "out of host memory"; return IPCFP_ERR_INVALID_ARG; }
     catch (const std::exception& e) { g_last_error = e.what(); return IPCFP_ERR_INVALID_ARG; }
-}
-
-// ------------------------------------------------------------------------------------------ multi-GPU merge
-// gathered: world segments of `cap` 38-byte CIDs, counts[r] valid in segment r. Sort + unique on the device.
-// first = the first valid entry; *mixed receives the smallest position whose 6 prefix bytes differ from first's.
-struct SortCid { uint8_t b[38]; };
-__global__ void k_merge_keys(const uint8_t* __restrict__ g, const uint64_t* __restrict__ seg_off, uint32_t world, uint64_t cap, uint64_t total,
-                             const uint8_t* __restrict__ first, uint32_t* keys, uint32_t* vals, unsigned long long* mixed) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    uint32_t r = 0;
-    while (r + 1 < world && i >= seg_off[r + 1]) r++;
-    uint64_t src = (uint64_t)r * cap + (i - seg_off[r]);
-    const uint8_t* c = g + 38 * src;
-    bool same = true;
-#pragma unroll
-    for (int k = 0; k < 6; k++) same &= c[k] == first[k];
-    if (!same) atomicMin(mixed, (unsigned long long)i);
-    keys[i] = ((uint32_t)c[6] << 24) | ((uint32_t)c[7] << 16) | ((uint32_t)c[8] << 8) | c[9];
-    vals[i] = (uint32_t)src;
-}
-__device__ __forceinline__ int cid_cmp_raw(const uint8_t* a, const uint8_t* b) {
-    for (int k = 0; k < 38; k++) if (a[k] != b[k]) return a[k] < b[k] ? -1 : 1;
-    return 0;
-}
-__global__ void k_merge_tie_fix(const uint8_t* __restrict__ g, uint32_t* vals, const uint32_t* __restrict__ keys, uint64_t total) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    if (i > 0 && keys[i - 1] == keys[i]) return;
-    if (i + 1 >= total || keys[i] != keys[i + 1]) return;
-    uint64_t j = i + 1;
-    while (j + 1 < total && keys[j + 1] == keys[i]) j++;
-    for (uint64_t a = i + 1; a <= j; a++) {
-        uint32_t v = vals[a];
-        uint64_t b = a;
-        while (b > i && cid_cmp_raw(g + 38ull * vals[b - 1], g + 38ull * v) > 0) { vals[b] = vals[b - 1]; b--; }
-        vals[b] = v;
-    }
-}
-__global__ void k_merge_unique_flags(const uint8_t* __restrict__ g, const uint32_t* __restrict__ vals, uint64_t total, uint32_t* bits) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool keep = false;
-    if (i < total) keep = i == 0 || cid_cmp_raw(g + 38ull * vals[i - 1], g + 38ull * vals[i]) != 0;
-    unsigned b = __ballot_sync(0xffffffffu, keep);
-    if ((threadIdx.x & 31) == 0) bits[i >> 5] = b;
-}
-__global__ void k_merge_emit(const uint8_t* __restrict__ g, const uint32_t* __restrict__ vals, const uint32_t* __restrict__ pos, uint64_t n,
-                             uint8_t* out) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint8_t* c = g + 38ull * vals[pos[i]];
-    for (int k = 0; k < 38; k++) out[38 * i + k] = c[k];
-}
-
-void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
-                        uint64_t* n_out) {
-    // The order is the raw byte order of the 38 bytes, which is `Cid` Ord only among CIDs that share one prefix (the varint
-    // multihash code does not sort bytewise): lists with several prefixes are refused, like the sharded call refuses such stores.
-    check_device(device);
-    *n_out = 0;
-    *n_out = sort_unique_cids(nullptr, gathered, counts, world, cap, out, cap_out, nullptr);
-}
-
-uint64_t sort_unique_cids(cudaStream_t st, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
-                          uint64_t* mixed) {
-    std::vector<uint64_t> seg(world + 1, 0);
-    for (uint32_t r = 0; r < world; r++) { if (counts[r] > cap) throw Error(IPCFP_ERR_INVALID_ARG, "count exceeds segment capacity"); seg[r + 1] = seg[r] + counts[r]; }
-    uint64_t total = seg[world];
-    if (mixed) *mixed = UINT64_MAX;
-    if (!total) return 0;
-    uint32_t r0 = 0;
-    while (!counts[r0]) r0++;
-    const uint8_t* first = (const uint8_t*)gathered + 38ull * r0 * cap;
-    AsyncBuf<uint64_t> d_seg(world + 1, st);
-    IPCFP_CUDA(cudaMemcpyAsync(d_seg.p, seg.data(), (world + 1) * 8, cudaMemcpyHostToDevice, st));
-    AsyncBuf<uint32_t> keys(total, st), vals(total, st), ka(total, st), va(total, st), bits((total + 31) / 32 + 8, st), pos(total + 32, st);
-    unsigned nb = radix_blocks(total);
-    AsyncBuf<uint32_t> hist((size_t)256 * nb + 256, st);
-    AsyncBuf<uint64_t> scan_tmp((size_t)256 * nb + 256, st), scratch(scan_scratch_elems(std::max<uint64_t>((uint64_t)256 * nb, total)) + 8, st),
-        wp((total + 31) / 32 + 8, st), cnt(2, st);   // cnt[0] = unique count, cnt[1] = first mixed-prefix position
-    IPCFP_CUDA(cudaMemsetAsync(cnt.p + 1, 0xff, 8, st));
-    k_merge_keys<<<div_up(total, 256), 256, 0, st>>>((const uint8_t*)gathered, d_seg.p, world, cap, total, first, keys.p, vals.p,
-                                                     (unsigned long long*)cnt.p + 1); IPCFP_LAUNCH_CHECK();
-    radix_sort_pairs(keys.p, vals.p, ka.p, va.p, total, 32, hist.p, scan_tmp.p, scratch.p, st);
-    k_merge_tie_fix<<<div_up(total, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, keys.p, total); IPCFP_LAUNCH_CHECK();
-    k_merge_unique_flags<<<div_up((total + 31) / 32 * 32, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, total, bits.p); IPCFP_LAUNCH_CHECK();
-    bitmap_to_indices(bits.p, total, pos.p, cnt.p, wp.p, scratch.p, st);
-    uint64_t h[2] = {0, 0};
-    IPCFP_CUDA(cudaMemcpyAsync(h, cnt.p, 16, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (mixed) *mixed = h[1];
-    else if (h[1] != UINT64_MAX) throw Error(IPCFP_ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", h[1]);
-    const uint64_t n = h[0];
-    if (n > cap_out) throw Error(IPCFP_ERR_INVALID_ARG, "output buffer too small for the merged witness CID list");
-    k_merge_emit<<<div_up(n, 256), 256, 0, st>>>((const uint8_t*)gathered, vals.p, pos.p, n, (uint8_t*)out); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    return n;
 }
 
 // ------------------------------------------------------------------------------------------ bundle
@@ -545,41 +447,6 @@ ipcfp_status ipcfp_generate_event_proof_sharded(ipcfp_comm* c, ipcfp_store* s, i
         for (uint32_t k = 0; k < W; k++) if (bounds[k] > bounds[k + 1]) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must ascend");
         if (bounds[0] != 0 || bounds[W] != td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must cover [0, n_receipts)");
         *out = generate_event_proof(reinterpret_cast<Store*>(s), td, spec, flags, true, bounds[r], bounds[r + 1], cm);
-    });
-}
-
-ipcfp_status ipcfp_exec_bucketize(int device, const void* seg_dev, uint64_t nseg, uint64_t pos0, uint32_t world, uint64_t cap, void* send_dev,
-                                  uint64_t* counts) {
-    return guard([&] {
-        if ((nseg && !seg_dev) || !send_dev || !counts) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        exec_bucketize(device, seg_dev, nseg, pos0, world, cap, send_dev, counts);
-    });
-}
-ipcfp_status ipcfp_exec_dedup(int device, const void* recv_dev, const uint64_t* counts, uint32_t world, uint64_t cap, uint64_t* dup_pos_dev,
-                              uint64_t cap_out, uint64_t* n_dup) {
-    return guard([&] {
-        if (!recv_dev || !counts || !dup_pos_dev || !n_dup) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        exec_dedup(device, recv_dev, counts, world, cap, dup_pos_dev, cap_out, n_dup);
-    });
-}
-ipcfp_status ipcfp_exec_fetch(int device, const void* seg_dev, uint64_t nseg, uint64_t pos0, const uint64_t* req_pos_dev, uint64_t n_req,
-                              void* out_dev) {
-    return guard([&] {
-        if ((nseg && !seg_dev) || (n_req && (!req_pos_dev || !out_dev))) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        exec_fetch(device, seg_dev, nseg, pos0, req_pos_dev, n_req, out_dev);
-    });
-}
-ipcfp_status ipcfp_witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap_cids, uint64_t* n) {
-    return guard([&] {
-        if (!r || !dev_ptr || !n) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        witness_cids_to_device(r, dev_ptr, cap_cids, n);
-    });
-}
-ipcfp_status ipcfp_merge_witness_cids(int device, const void* gathered_dev, const uint64_t* counts, uint32_t world, uint64_t cap, void* out_dev,
-                                      uint64_t cap_out, uint64_t* n_out) {
-    return guard([&] {
-        if (!gathered_dev || !counts || !out_dev || !n_out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        merge_witness_cids(device, gathered_dev, counts, world, cap, out_dev, cap_out, n_out);
     });
 }
 

@@ -220,14 +220,6 @@ void bundle_verdict_free(ipcfp_bundle_verdict* v);
 void event_result_free(ipcfp_event_result* r);
 struct WitnessOut;
 const WitnessOut& event_result_witness(const ipcfp_event_result* r);   // the witness of a generate_event_proof result, device copies included
-void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n);
-void merge_witness_cids(int device, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
-                        uint64_t* n_out);
-// capi.cu: the body of merge_witness_cids on stream st (the raw byte order of the 38 bytes, duplicates removed, into out); returns the
-// count. mixed == nullptr: several CID prefixes are refused as merge_witness_cids refuses them; else *mixed = the first position whose
-// prefix differs from the first entry's (UINT64_MAX: none) and the list is sorted all the same.
-uint64_t sort_unique_cids(cudaStream_t st, const void* gathered, const uint64_t* counts, uint32_t world, uint64_t cap, void* out, uint64_t cap_out,
-                          uint64_t* mixed);
 // plan.cu — ipcfp_plan_fetch_resident: the CIDs of N(S) \ S for the generators of a proof bundle (DESIGN.md §2, "Fetch planning")
 struct FetchPlan {
     std::vector<uint8_t> cids;   // n*38, `Cid` order
@@ -237,8 +229,6 @@ struct FetchPlan {
 };
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
                 FetchPlan& out);
-// a list of 38-byte CIDs (n*38) into `Cid` order on the host (stable)
-void sort_cids_host(std::vector<uint8_t>& cids);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);
@@ -299,9 +289,6 @@ private:
     void union_partitioned(uint64_t cap);
     void timings(float* ms_exchange, float* ms_fetch, float* ms_union) const;   // after the call's final sync
 };
-void exec_bucketize(int device, const void* seg, uint64_t nseg, uint64_t pos0, uint32_t world, uint64_t cap, void* send, uint64_t* counts_host);
-void exec_dedup(int device, const void* recv, const uint64_t* counts, uint32_t world, uint64_t cap, uint64_t* dup_dev, uint64_t cap_out, uint64_t* n_dup);
-void exec_fetch(int device, const void* seg, uint64_t nseg, uint64_t pos0, const uint64_t* req_dev, uint64_t n, void* out_dev);
 
 // storage.cu
 ipcfp_slot_result* read_storage_slots(Store* s, const uint8_t* root, const uint8_t* slots, uint64_t k);

@@ -1067,15 +1067,4 @@ ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_ev
 void event_result_free(ipcfp_event_result* r) { delete reinterpret_cast<EventResultBox*>(r); }
 const WitnessOut& event_result_witness(const ipcfp_event_result* r) { return reinterpret_cast<const EventResultBox*>(r)->wit; }
 
-void witness_cids_to_device(const ipcfp_event_result* r, void* dev_ptr, uint64_t cap, uint64_t* n) {
-    uint64_t m = r->witness.n_blocks;
-    if (m > cap) throw Error(IPCFP_ERR_INVALID_ARG, "device buffer too small for the witness CID list");
-    const EventResultBox* box = reinterpret_cast<const EventResultBox*>(r);
-    if (m) {
-        if (box->wit.cids_dev.p) IPCFP_CUDA(cudaMemcpy(dev_ptr, box->wit.cids_dev.p, m * 38, cudaMemcpyDeviceToDevice));
-        else IPCFP_CUDA(cudaMemcpy(dev_ptr, r->witness.cids, m * 38, cudaMemcpyHostToDevice));
-    }
-    *n = m;
-}
-
 }  // namespace ipcfp

@@ -1,184 +1,4 @@
-// parallel.cu — device helpers for the cross-shard part of the path (one process per GPU; the
-// collectives themselves belong to the caller: torch.distributed / NCCL).
-//
-// The reference builds the execution order by walking every message AMT and dropping repeated CIDs
-// "first seen wins" (events/utils.rs:56-91). With the message list sharded over ranks, duplicates can
-// span shards, so the dedup is a distributed hash join:
-//   ipcfp_exec_bucketize   every rank routes (cid, global position) of its slice to owner = hash(cid) % world
-//   [all-to-all]
-//   ipcfp_exec_dedup       every owner finds, per distinct CID, the smallest position; all other positions
-//                          of that CID are duplicates → returned as a list
-//   [all-gather of the (tiny) duplicate lists]  →  exec index i ↔ raw position p(i) on the host
-//   ipcfp_exec_fetch       CIDs at requested raw positions (for EventProof.message_cid)
-#include <algorithm>
-#include <vector>
-
-#include "engine.cuh"
-#include "prims.cuh"
-#include "rawcid.cuh"
-
-namespace ipcfp {
-
-struct ExecEntry { RawCid c; uint64_t pos; };  // 48 bytes
-
-// owner of every record of the slice (key for the stable partition)
-__global__ void k_exec_owner(const RawCid* __restrict__ seg, uint64_t nseg, uint32_t world, uint32_t* keys, uint32_t* vals) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nseg) return;
-    keys[i] = (uint32_t)((rawcid_hash(seg[i]) >> 32) % world);
-    vals[i] = (uint32_t)i;
-}
-// first sorted position of every owner
-__global__ void k_exec_starts(const uint32_t* __restrict__ keys, uint64_t nseg, unsigned long long* start) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nseg) return;
-    if (j == 0 || keys[j - 1] != keys[j]) start[keys[j]] = j;
-}
-// entries leave in (owner, position) order: within a bucket the global positions are increasing
-__global__ void k_exec_scatter(const RawCid* __restrict__ seg, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint64_t nseg,
-                               uint64_t pos0, const unsigned long long* __restrict__ start, uint64_t cap, ExecEntry* send) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nseg) return;
-    uint32_t owner = keys[j], src = vals[j];
-    uint64_t slot = j - start[owner];
-    if (slot < cap) { ExecEntry e; e.c = seg[src]; e.pos = pos0 + src; send[(uint64_t)owner * cap + slot] = e; }
-}
-
-// entry k of the received buffer (world segments of `cap`, counts[r] valid in segment r)
-__device__ __forceinline__ const ExecEntry* recv_entry(const ExecEntry* recv, const uint64_t* seg_off, uint32_t world, uint64_t cap, uint64_t k) {
-    uint32_t r = 0;
-    while (r + 1 < world && k >= seg_off[r + 1]) r++;
-    return recv + (uint64_t)r * cap + (k - seg_off[r]);
-}
-// pass 1: one canonical slot per distinct CID (value = fingerprint << 32 | smallest entry ordinal + 1)
-__global__ void k_exec_claim(const ExecEntry* __restrict__ recv, const uint64_t* __restrict__ seg_off, uint32_t world, uint64_t cap, uint64_t total,
-                             unsigned long long* table, uint64_t mask) {
-    uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= total) return;
-    const ExecEntry* e = recv_entry(recv, seg_off, world, cap, k);
-    uint64_t h = rawcid_hash(e->c);
-    uint32_t fp = (uint32_t)(h >> 40) | 1u;   // bits 40..63: independent of the slot bits
-    unsigned long long mine = ((unsigned long long)fp << 32) | (unsigned long long)(k + 1);
-    uint64_t slot = h & mask;   // low bits: independent of the owner choice ((h >> 32) % world)
-    for (;;) {
-        unsigned long long v = table[slot];
-        if (v == 0) { v = atomicCAS(&table[slot], 0ull, mine); if (v == 0) return; }
-        if ((uint32_t)(v >> 32) == fp && rawcid_eq(recv_entry(recv, seg_off, world, cap, (uint32_t)v - 1)->c, e->c)) { atomicMin(&table[slot], mine); return; }
-        slot = (slot + 1) & mask;
-    }
-}
-__device__ __forceinline__ uint64_t exec_find_slot(const ExecEntry* recv, const uint64_t* seg_off, uint32_t world, uint64_t cap, const ExecEntry* e,
-                                                   const unsigned long long* table, uint64_t mask) {
-    uint64_t h = rawcid_hash(e->c);
-    uint32_t fp = (uint32_t)(h >> 40) | 1u;   // bits 40..63: independent of the slot bits
-    uint64_t slot = h & mask;   // low bits: independent of the owner choice ((h >> 32) % world)
-    for (;;) {
-        unsigned long long v = table[slot];
-        if ((uint32_t)(v >> 32) == fp && rawcid_eq(recv_entry(recv, seg_off, world, cap, (uint32_t)v - 1)->c, e->c)) return slot;
-        slot = (slot + 1) & mask;
-    }
-}
-// pass 2: the received buffer is ordered by (sender rank, position), so the smallest entry ordinal of a CID is
-// its smallest global position: every other entry of that CID is a duplicate
-__global__ void k_exec_dups(const ExecEntry* __restrict__ recv, const uint64_t* __restrict__ seg_off, uint32_t world, uint64_t cap, uint64_t total,
-                            const unsigned long long* table, uint64_t mask, uint64_t* dup, uint64_t cap_out, unsigned long long* n_dup) {
-    uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= total) return;
-    const ExecEntry* e = recv_entry(recv, seg_off, world, cap, k);
-    uint64_t slot = exec_find_slot(recv, seg_off, world, cap, e, table, mask);
-    if ((uint32_t)table[slot] - 1 != (uint32_t)k) {
-        unsigned long long j = atomicAdd(n_dup, 1ull);
-        if (j < cap_out) dup[j] = e->pos;
-    }
-}
-__global__ void k_exec_fetch(const RawCid* __restrict__ seg, uint64_t nseg, uint64_t pos0, const uint64_t* __restrict__ req, uint64_t n, RawCid* out) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    uint64_t p = req[j];
-    if (p >= pos0 && p - pos0 < nseg) out[j] = seg[p - pos0];
-}
-
-// grow-only scratch + a private non-blocking stream per device for the helpers (no allocation in steady state)
-struct HelperCtx {
-    cudaStream_t st = nullptr;
-    DevBuf<unsigned long long> table, minpos, small;
-};
-static HelperCtx& helper_ctx(int device) {
-    static HelperCtx ctx[16];
-    HelperCtx& c = ctx[device & 15];
-    if (!c.st) { IPCFP_CUDA(cudaStreamCreateWithFlags(&c.st, cudaStreamNonBlocking)); c.small.alloc(1024); }
-    return c;
-}
-
-void exec_bucketize(int device, const void* seg, uint64_t nseg, uint64_t pos0, uint32_t world, uint64_t cap, void* send, uint64_t* counts_host) {
-    check_device(device);
-    if (!world || world > 256) throw Error(IPCFP_ERR_INVALID_ARG, "bad world size");
-    if (nseg >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "slice too long");
-    HelperCtx& hc = helper_ctx(device);
-    cudaStream_t st = hc.st;
-    for (uint32_t r = 0; r < world; r++) counts_host[r] = 0;
-    if (!nseg) return;
-    unsigned nb = radix_blocks(nseg);
-    AsyncBuf<uint32_t> keys(nseg, st), vals(nseg, st), ka(nseg, st), va(nseg, st), hist((size_t)256 * nb + 256, st);
-    AsyncBuf<uint64_t> scan_tmp((size_t)256 * nb + 256, st), scratch(scan_scratch_elems((uint64_t)256 * nb) + 8, st);
-    unsigned long long* start = hc.small.p;   // [0, world]
-    std::vector<unsigned long long> h_start(world + 1, nseg);
-    IPCFP_CUDA(cudaMemcpyAsync(start, h_start.data(), (world + 1) * 8, cudaMemcpyHostToDevice, st));
-    k_exec_owner<<<div_up(nseg, 256), 256, 0, st>>>((const RawCid*)seg, nseg, world, keys.p, vals.p); IPCFP_LAUNCH_CHECK();
-    radix_sort_pairs(keys.p, vals.p, ka.p, va.p, nseg, 8, hist.p, scan_tmp.p, scratch.p, st);
-    k_exec_starts<<<div_up(nseg, 256), 256, 0, st>>>(keys.p, nseg, start); IPCFP_LAUNCH_CHECK();
-    k_exec_scatter<<<div_up(nseg, 256), 256, 0, st>>>((const RawCid*)seg, keys.p, vals.p, nseg, pos0, start, cap, (ExecEntry*)send); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaMemcpyAsync(h_start.data(), start, (world + 1) * 8, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    // owners without entries keep start == nseg; counts from consecutive starts of present owners
-    uint64_t next = nseg;
-    for (int r = (int)world - 1; r >= 0; r--) {
-        if (h_start[r] == nseg) { counts_host[r] = 0; continue; }
-        counts_host[r] = next - h_start[r];
-        next = h_start[r];
-    }
-    for (uint32_t r = 0; r < world; r++) if (counts_host[r] > cap) throw Error(IPCFP_ERR_INVALID_ARG, "bucket capacity too small", counts_host[r]);
-}
-void exec_dedup(int device, const void* recv, const uint64_t* counts, uint32_t world, uint64_t cap, uint64_t* dup_dev, uint64_t cap_out, uint64_t* n_dup) {
-    check_device(device);
-    HelperCtx& hc = helper_ctx(device);
-    cudaStream_t st = hc.st;
-    std::vector<uint64_t> seg(world + 1, 0);
-    for (uint32_t r = 0; r < world; r++) { if (counts[r] > cap) throw Error(IPCFP_ERR_INVALID_ARG, "count exceeds bucket capacity"); seg[r + 1] = seg[r] + counts[r]; }
-    uint64_t total = seg[world];
-    *n_dup = 0;
-    if (!total) return;
-    if (total >= 0xffffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^32 messages per owner");
-    uint64_t slots = 64;
-    while (slots < 2 * total) slots <<= 1;
-    if (world + 2 > 1000) throw Error(IPCFP_ERR_UNSUPPORTED, "world too large");
-    hc.table.ensure(slots);
-    uint64_t* d_seg = (uint64_t*)hc.small.p;             // [0, world]
-    unsigned long long* nd = hc.small.p + 1023;
-    IPCFP_CUDA(cudaMemsetAsync(hc.table.p, 0, slots * 8, st));
-    IPCFP_CUDA(cudaMemsetAsync(nd, 0, 8, st));
-    IPCFP_CUDA(cudaMemcpyAsync(d_seg, seg.data(), (world + 1) * 8, cudaMemcpyHostToDevice, st));
-    unsigned g = div_up(total, 256);
-    const ExecEntry* e = (const ExecEntry*)recv;
-    k_exec_claim<<<g, 256, 0, st>>>(e, d_seg, world, cap, total, hc.table.p, slots - 1); IPCFP_LAUNCH_CHECK();
-    k_exec_dups<<<g, 256, 0, st>>>(e, d_seg, world, cap, total, hc.table.p, slots - 1, dup_dev, cap_out, nd); IPCFP_LAUNCH_CHECK();
-    unsigned long long n = 0;
-    IPCFP_CUDA(cudaMemcpyAsync(&n, nd, 8, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));
-    if (n > cap_out) throw Error(IPCFP_ERR_INVALID_ARG, "duplicate list capacity too small", n);
-    *n_dup = n;
-}
-void exec_fetch(int device, const void* seg, uint64_t nseg, uint64_t pos0, const uint64_t* req_dev, uint64_t n, void* out_dev) {
-    check_device(device);
-    if (!n) return;
-    k_exec_fetch<<<div_up(n, 256), 256>>>((const RawCid*)seg, nseg, pos0, req_dev, n, (RawCid*)out_dev); IPCFP_LAUNCH_CHECK();
-    IPCFP_CUDA(cudaStreamSynchronize(nullptr));
-}
-
-}  // namespace ipcfp
-
-// =====================================================================================================================
-// In-library cross-shard protocol over NCCL (SURVEY Appendix C: ipcfp_comm_init / ipcfp_generate_event_proof_sharded).
+// parallel.cu — the in-library cross-shard protocol over NCCL (SURVEY Appendix C: ipcfp_comm_init / ipcfp_generate_event_proof_sharded).
 //
 // One process per GPU. Receipts shard by index range (events/generator.rs:209-301 is independent per receipt); what spans
 // shards is (1) the execution order — every message AMT concatenated, first occurrence of a CID wins (events/utils.rs:48-94) —
@@ -194,15 +14,23 @@ void exec_fetch(int device, const void* seg, uint64_t nseg, uint64_t pos0, const
 //        pass 2 runs with the global n_exec (so "Missing message at index" keeps its place in the error order)
 //   H2   all-gather  {first error key, matches, proofs, witness blocks}    → all ranks fail together with the SAME error
 //   F    all-gather of the wanted positions → every owner copies the CIDs it holds → all-reduce → EventProof.message_cid patched
-//   W    all-gather of the sorted per-shard witness CID lists → bucketed k-way merge + unique on every rank
+//   W    the sorted per-shard witness CID lists → bucketed k-way merge + unique: range-partitioned over the ranks (all-to-all of
+//        the pieces), or on every rank (all-gather of the lists) with IPCFP_SHARDED_UNION_FULL   [union stream, own communicator]
 // NCCL is resolved with dlopen at ipcfp_comm_init (libnccl.so.2: the copy already in the process — e.g. PyTorch's — or the
 // system one), so the library itself keeps linking only cudart and loads on machines without NCCL.
-// =====================================================================================================================
+#include <algorithm>
 #include <cstdio>
 #include <dlfcn.h>
 #include <nccl.h>
+#include <vector>
+
+#include "engine.cuh"
+#include "prims.cuh"
+#include "rawcid.cuh"
 
 namespace ipcfp {
+
+struct ExecEntry { RawCid c; uint64_t pos; };  // 48 bytes
 
 struct NcclApi {
     ncclResult_t (*GetUniqueId)(ncclUniqueId*);
@@ -529,7 +357,7 @@ __device__ __forceinline__ uint64_t bswap64_p(uint64_t x) {
     uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
     return ((uint64_t)__byte_perm(lo, 0, 0x0123) << 32) | (uint64_t)__byte_perm(hi, 0, 0x0123);
 }
-// raw byte order of (prefix, digest) — `Cid` Ord for CIDs of one prefix (the Filecoin chain case, see ipcfp_merge_witness_cids)
+// raw byte order of (prefix, digest) — `Cid` Ord for CIDs of one prefix (the Filecoin chain case; the sharded call refuses other stores)
 __device__ __forceinline__ int rec_cmp(const RawCid& a, const RawCid& b) {
     uint64_t pa = bswap64_p(a.w[4] << 16), pb = bswap64_p(b.w[4] << 16);
     if (pa != pb) return pa < pb ? -1 : 1;

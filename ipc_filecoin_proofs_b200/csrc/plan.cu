@@ -16,6 +16,7 @@
 #include "engine.cuh"
 #include "hashes.cuh"
 #include "plan_items.cuh"
+#include "prims.cuh"
 
 namespace ipcfp {
 
@@ -99,18 +100,6 @@ __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, 
     const uint32_t c = w < nwords ? (uint32_t)__popc(bits[w]) : 0u;
     const uint32_t sum = __reduce_add_sync(0xffffffffu, c);
     if ((threadIdx.x & 31) == 0 && sum) atomicAdd(out, (unsigned long long)sum);
-}
-
-// `Cid` Ord of 38-byte CIDs: (version, codec, multihash code, size) as varints, then the digest bytes
-static bool cid_less(const uint8_t* a, const uint8_t* b) {
-    uint32_t pa = 0, pb = 0;
-    for (int f = 0; f < 4; f++) {
-        uint64_t va = 0, vb = 0;
-        for (uint32_t sh = 0; pa < 38; sh += 7) { const uint8_t c = a[pa++]; if (sh < 64) va |= (uint64_t)(c & 0x7f) << sh; if (!(c & 0x80)) break; }
-        for (uint32_t sh = 0; pb < 38; sh += 7) { const uint8_t c = b[pb++]; if (sh < 64) vb |= (uint64_t)(c & 0x7f) << sh; if (!(c & 0x80)) break; }
-        if (va != vb) return va < vb;
-    }
-    return std::lexicographical_compare(a + pa, a + 38, b + pb, b + 38);
 }
 
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
@@ -250,7 +239,7 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     uint64_t m = 0, mixed = UINT64_MAX;
     if (n_miss) {
         AsyncBuf<uint8_t> sorted(38 * n_miss + 16, st);
-        m = sort_unique_cids(st, miss.p, &n_miss, 1, n_miss, sorted.p, n_miss, &mixed);
+        m = sort_unique_cids(st, miss.p, n_miss, sorted.p, &mixed);
         out.cids.resize(38 * m);
         IPCFP_CUDA(cudaMemcpyAsync(out.cids.data(), sorted.p, 38 * m, cudaMemcpyDeviceToHost, st));
     }
@@ -260,17 +249,6 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     // The device order is the bytes' order, which is `Cid` order within one prefix. A CID of another prefix (one that no block of the
     // store has, so rarely more than a few) puts the list in `Cid` order on the host.
     if (mixed != UINT64_MAX) sort_cids_host(out.cids);
-}
-
-void sort_cids_host(std::vector<uint8_t>& cids) {
-    const uint64_t m = cids.size() / 38;
-    std::vector<uint32_t> ord(m);
-    for (uint32_t k = 0; k < m; k++) ord[k] = k;
-    const uint8_t* c = cids.data();
-    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return cid_less(c + 38ull * x, c + 38ull * y); });
-    std::vector<uint8_t> sorted(38 * m);
-    for (uint64_t k = 0; k < m; k++) memcpy(sorted.data() + 38 * k, c + 38ull * ord[k], 38);
-    cids.swap(sorted);
 }
 
 }  // namespace ipcfp

@@ -1,4 +1,7 @@
-// prims.cu — scan / bitmap compaction / radix sort kernels (see prims.cuh).
+// prims.cu — scan / bitmap compaction / radix sort kernels and the CID sort built on them (see prims.cuh).
+#include <algorithm>
+#include <cstring>
+
 #include "prims.cuh"
 
 namespace ipcfp {
@@ -232,6 +235,100 @@ void radix_sort_pairs(uint32_t* keys, uint32_t* vals, uint32_t* keys_alt, uint32
         IPCFP_CUDA(cudaMemcpyAsync(keys, ki, n * 4, cudaMemcpyDeviceToDevice, st));
         IPCFP_CUDA(cudaMemcpyAsync(vals, vi, n * 4, cudaMemcpyDeviceToDevice, st));
     }
+}
+
+// ------------------------------------------------------------------------------------------ CID sort
+// radix sort on digest bytes 0-3 (bytes 6-9 of the CID), then the runs of equal keys put in order by all 38 bytes
+__global__ void k_merge_keys(const uint8_t* __restrict__ g, uint64_t n, uint32_t* keys, uint32_t* vals, unsigned long long* mixed) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t* c = g + 38 * i;
+    bool same = true;
+#pragma unroll
+    for (int k = 0; k < 6; k++) same &= c[k] == g[k];
+    if (!same) atomicMin(mixed, (unsigned long long)i);
+    keys[i] = ((uint32_t)c[6] << 24) | ((uint32_t)c[7] << 16) | ((uint32_t)c[8] << 8) | c[9];
+    vals[i] = (uint32_t)i;
+}
+__device__ __forceinline__ int cid_cmp_raw(const uint8_t* a, const uint8_t* b) {
+    for (int k = 0; k < 38; k++) if (a[k] != b[k]) return a[k] < b[k] ? -1 : 1;
+    return 0;
+}
+__global__ void k_merge_tie_fix(const uint8_t* __restrict__ g, uint32_t* vals, const uint32_t* __restrict__ keys, uint64_t total) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    if (i > 0 && keys[i - 1] == keys[i]) return;
+    if (i + 1 >= total || keys[i] != keys[i + 1]) return;
+    uint64_t j = i + 1;
+    while (j + 1 < total && keys[j + 1] == keys[i]) j++;
+    for (uint64_t a = i + 1; a <= j; a++) {
+        uint32_t v = vals[a];
+        uint64_t b = a;
+        while (b > i && cid_cmp_raw(g + 38ull * vals[b - 1], g + 38ull * v) > 0) { vals[b] = vals[b - 1]; b--; }
+        vals[b] = v;
+    }
+}
+__global__ void k_merge_unique_flags(const uint8_t* __restrict__ g, const uint32_t* __restrict__ vals, uint64_t total, uint32_t* bits) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool keep = false;
+    if (i < total) keep = i == 0 || cid_cmp_raw(g + 38ull * vals[i - 1], g + 38ull * vals[i]) != 0;
+    unsigned b = __ballot_sync(0xffffffffu, keep);
+    if ((threadIdx.x & 31) == 0) bits[i >> 5] = b;
+}
+__global__ void k_merge_emit(const uint8_t* __restrict__ g, const uint32_t* __restrict__ vals, const uint32_t* __restrict__ pos, uint64_t n,
+                             uint8_t* out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t* c = g + 38ull * vals[pos[i]];
+    for (int k = 0; k < 38; k++) out[38 * i + k] = c[k];
+}
+
+uint64_t sort_unique_cids(cudaStream_t st, const void* cids, uint64_t n, void* out, uint64_t* mixed) {
+    *mixed = UINT64_MAX;
+    if (!n) return 0;
+    const uint8_t* g = (const uint8_t*)cids;
+    AsyncBuf<uint32_t> keys(n, st), vals(n, st), ka(n, st), va(n, st), bits((n + 31) / 32 + 8, st), pos(n + 32, st);
+    unsigned nb = radix_blocks(n);
+    AsyncBuf<uint32_t> hist((size_t)256 * nb + 256, st);
+    AsyncBuf<uint64_t> scan_tmp((size_t)256 * nb + 256, st), scratch(scan_scratch_elems(std::max<uint64_t>((uint64_t)256 * nb, n)) + 8, st),
+        wp((n + 31) / 32 + 8, st), cnt(2, st);   // cnt[0] = unique count, cnt[1] = first mixed-prefix position
+    IPCFP_CUDA(cudaMemsetAsync(cnt.p + 1, 0xff, 8, st));
+    k_merge_keys<<<div_up(n, 256), 256, 0, st>>>(g, n, keys.p, vals.p, (unsigned long long*)cnt.p + 1); IPCFP_LAUNCH_CHECK();
+    radix_sort_pairs(keys.p, vals.p, ka.p, va.p, n, 32, hist.p, scan_tmp.p, scratch.p, st);
+    k_merge_tie_fix<<<div_up(n, 256), 256, 0, st>>>(g, vals.p, keys.p, n); IPCFP_LAUNCH_CHECK();
+    k_merge_unique_flags<<<div_up((n + 31) / 32 * 32, 256), 256, 0, st>>>(g, vals.p, n, bits.p); IPCFP_LAUNCH_CHECK();
+    bitmap_to_indices(bits.p, n, pos.p, cnt.p, wp.p, scratch.p, st);
+    uint64_t h[2] = {0, 0};
+    IPCFP_CUDA(cudaMemcpyAsync(h, cnt.p, 16, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    *mixed = h[1];
+    const uint64_t m = h[0];
+    k_merge_emit<<<div_up(m, 256), 256, 0, st>>>(g, vals.p, pos.p, m, (uint8_t*)out); IPCFP_LAUNCH_CHECK();
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    return m;
+}
+
+// `Cid` Ord of 38-byte CIDs: (version, codec, multihash code, size) as varints, then the digest bytes
+static bool cid_less(const uint8_t* a, const uint8_t* b) {
+    uint32_t pa = 0, pb = 0;
+    for (int f = 0; f < 4; f++) {
+        uint64_t va = 0, vb = 0;
+        for (uint32_t sh = 0; pa < 38; sh += 7) { const uint8_t c = a[pa++]; if (sh < 64) va |= (uint64_t)(c & 0x7f) << sh; if (!(c & 0x80)) break; }
+        for (uint32_t sh = 0; pb < 38; sh += 7) { const uint8_t c = b[pb++]; if (sh < 64) vb |= (uint64_t)(c & 0x7f) << sh; if (!(c & 0x80)) break; }
+        if (va != vb) return va < vb;
+    }
+    return std::lexicographical_compare(a + pa, a + 38, b + pb, b + 38);
+}
+
+void sort_cids_host(std::vector<uint8_t>& cids) {
+    const uint64_t m = cids.size() / 38;
+    std::vector<uint32_t> ord(m);
+    for (uint32_t k = 0; k < m; k++) ord[k] = k;
+    const uint8_t* c = cids.data();
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return cid_less(c + 38ull * x, c + 38ull * y); });
+    std::vector<uint8_t> sorted(38 * m);
+    for (uint64_t k = 0; k < m; k++) memcpy(sorted.data() + 38 * k, c + 38ull * ord[k], 38);
+    cids.swap(sorted);
 }
 
 }  // namespace ipcfp

@@ -1,5 +1,6 @@
 // prims.cuh — small device-wide primitives written for this engine (no CUB/Thrust):
-// exclusive scan, bitmap → ordered index list, stable LSD radix sort of (u32 key, u32 value).
+// exclusive scan, bitmap → ordered index list, stable LSD radix sort of (u32 key, u32 value), and on top of them the sort + unique
+// of a list of CIDs.
 // They implement what the reference gets from BTreeSet / Vec ordering on the CPU
 // (common/witness.rs:10,30-32; proofs/generator.rs:34,85-88; events/utils.rs:56-91).
 #pragma once
@@ -23,5 +24,13 @@ void bitmap_to_indices(const uint32_t* bits, uint64_t nbits, uint32_t* out, uint
 unsigned radix_blocks(uint64_t n);
 void radix_sort_pairs(uint32_t* keys, uint32_t* vals, uint32_t* keys_alt, uint32_t* vals_alt, uint64_t n, int nbits,
                       uint32_t* hist, uint64_t* scan_tmp, uint64_t* scratch, cudaStream_t st);
+
+// n 38-byte CIDs (device memory) ordered by digest bytes 0-3 and then all 38 bytes, duplicates removed, into out (room for n); returns
+// the count and synchronises st. Among CIDs of one 6-byte prefix that is the raw byte order, which is `Cid` order; across prefixes it
+// is not (the varint multihash code does not sort bytewise): *mixed = the first position whose prefix differs from entry 0's
+// (UINT64_MAX: none), and such a list is then put in `Cid` order on the host with sort_cids_host.
+uint64_t sort_unique_cids(cudaStream_t st, const void* cids, uint64_t n, void* out, uint64_t* mixed);
+// a list of 38-byte CIDs (n*38) into `Cid` order on the host (stable)
+void sort_cids_host(std::vector<uint8_t>& cids);
 
 }  // namespace ipcfp

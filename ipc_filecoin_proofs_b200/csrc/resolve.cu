@@ -9,6 +9,7 @@
 #include <cstring>
 
 #include "engine.cuh"
+#include "prims.cuh"
 #include "resolve_items.cuh"
 
 namespace ipcfp {
@@ -289,7 +290,7 @@ void resolve_addresses(Store* s, const uint8_t* state_root, const ipcfp_address*
     out.missing.clear();
     if (n_miss) {
         AsyncBuf<uint8_t> sorted(38 * n_miss + 16, st);
-        m = sort_unique_cids(st, miss.p, &n_miss, 1, n_miss, sorted.p, n_miss, &mixed);
+        m = sort_unique_cids(st, miss.p, n_miss, sorted.p, &mixed);
         out.missing.resize(38 * m);
         IPCFP_CUDA(cudaMemcpyAsync(out.missing.data(), sorted.p, 38 * m, cudaMemcpyDeviceToHost, st));
     }

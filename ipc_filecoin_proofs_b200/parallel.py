@@ -1,413 +1,12 @@
-"""Cross-shard plumbing of the event-proof path (one process per GPU, torch.distributed).
-
-Receipts shard by index range; pass 1 / pass 2 are local (`ipcfp_generate_event_proof_shard`).
-Two things span shards and are resolved here with a handful of small collectives:
-
-  * the execution order (reference events/utils.rs:48-94: concatenate every message AMT, first
-    occurrence of a CID wins) — a distributed hash join: bucketize → all-to-all → dedup →
-    one all-gather of the (tiny) duplicate position lists and of the exec indices each rank's proofs need →
-    exec index ↔ raw position arithmetic for everybody's requests → fetch on the owners + all-reduce;
-  * the witness CID set (reference common/witness.rs:24-40 BTreeSet union) — all-gather of the
-    per-shard sorted CID lists + merge (sort/unique) on the device.
-
-The device work goes through the engine's C ABI (`ipcfp_exec_*`, `ipcfp_merge_witness_cids`); this
-module only moves tensors. With the `nccl` backend collectives run on device tensors over NVLink;
-with `gloo` (CPU tests, or several ranks sharing one GPU) tensors are staged through the host.
-"""
-import bisect
+"""Multi-GPU event proofs: one process per GPU, receipts sharded by index range. The library resolves what spans shards (the
+execution order, the proofs' message CIDs, the union of the witness CID sets) inside one call per rank; `ShardedComm` makes it."""
 import ctypes as C
 
 import numpy as np
 
 from . import _abi as A
 
-ENTRY = 48   # exec entry: 40-byte CID record + u64 global position
-REC = 40
 
-import os
-import time
-
-PROFILE = {} if os.environ.get("IPCFP_PARALLEL_PROFILE") else None
-
-
-class _Phase:
-    """Wall-clock phase timer (only when IPCFP_PARALLEL_PROFILE is set)."""
-
-    def __init__(self, name):
-        self.name = name
-
-    def __enter__(self):
-        if PROFILE is not None:
-            self.t = time.perf_counter()
-
-    def __exit__(self, *a):
-        if PROFILE is not None:
-            PROFILE.setdefault(self.name, []).append(1e3 * (time.perf_counter() - self.t))
-
-
-class Collectives:
-    """Thin wrapper over torch.distributed that works for nccl (device tensors) and gloo (host staging)."""
-
-    def __init__(self, dist, device=None):
-        import torch
-        self.torch = torch
-        self.dist = dist
-        self.world = dist.get_world_size() if dist is not None else 1
-        self.rank = dist.get_rank() if dist is not None else 0
-        self.backend = dist.get_backend() if dist is not None else "none"
-        self.device = device if (device is not None and self.backend == "nccl") else torch.device("cpu")
-
-    def _t(self, a, dtype):
-        return self.torch.as_tensor(np.ascontiguousarray(a), dtype=dtype).to(self.device)
-
-    def all_gather_i64(self, values):
-        """values: 1-D int array of fixed length k → (world, k) numpy int64."""
-        t = self._t(np.asarray(values, dtype=np.int64).reshape(-1), self.torch.int64)
-        if self.world == 1:
-            return t.cpu().numpy().reshape(1, -1)
-        out = self.torch.empty(self.world * t.numel(), dtype=self.torch.int64, device=self.device)
-        self.dist.all_gather_into_tensor(out, t)
-        return out.cpu().numpy().reshape(self.world, -1)
-
-    def all_gather_var_u64(self, values):
-        """Variable-length u64 lists → concatenation over ranks (rank order)."""
-        values = np.asarray(values, dtype=np.uint64).reshape(-1)
-        counts = self.all_gather_i64([len(values)])[:, 0]
-        cap = int(counts.max()) if len(counts) else 0
-        if cap == 0:
-            return np.zeros(0, dtype=np.uint64), counts
-        pad = np.zeros(cap, dtype=np.int64)
-        pad[:len(values)] = values.view(np.int64)
-        allv = self.all_gather_i64(pad)
-        return np.concatenate([allv[r, :counts[r]] for r in range(self.world)]).view(np.uint64), counts
-
-    def all_to_all_bytes(self, send_t, chunk_bytes):
-        """send_t: uint8 tensor of world*chunk_bytes (CUDA or CPU) → received tensor, same shape, same device."""
-        if self.world == 1:
-            return send_t
-        src = send_t if send_t.device == self.device else send_t.to(self.device)
-        out = self.torch.empty_like(src)
-        self.dist.all_to_all_single(out, src)
-        return out if out.device == send_t.device else out.to(send_t.device)
-
-    def all_gather_bytes(self, t):
-        """t: uint8 tensor (fixed size on every rank) → concatenation, on t's device."""
-        if self.world == 1:
-            return t
-        src = t if t.device == self.device else t.to(self.device)
-        out = self.torch.empty(self.world * src.numel(), dtype=self.torch.uint8, device=self.device)
-        self.dist.all_gather_into_tensor(out, src)
-        return out if out.device == t.device else out.to(t.device)
-
-    def all_reduce_sum_i64(self, a):
-        t = self._t(np.asarray(a, dtype=np.int64), self.torch.int64)
-        if self.world > 1:
-            self.dist.all_reduce(t)
-        return t.cpu().numpy()
-
-    def all_reduce_min_i64(self, v):
-        t = self._t(np.asarray([v], dtype=np.int64), self.torch.int64)
-        if self.world > 1:
-            self.dist.all_reduce(t, op=self.dist.ReduceOp.MIN)
-        return int(t.cpu()[0])
-
-
-class CudaShardOps:
-    """Device helpers through the C ABI (torch CUDA tensors provide the buffers)."""
-
-    def __init__(self, lib, device_index):
-        import torch
-        self.torch = torch
-        self.L = lib
-        self.dev = device_index
-        self.tdev = torch.device("cuda", device_index)
-
-    def bucketize(self, seg_ptr, nseg, pos0, world, cap):
-        send = self.torch.zeros(world * cap * ENTRY, dtype=self.torch.uint8, device=self.tdev)
-        counts = np.zeros(world, dtype=np.uint64)
-        self.torch.cuda.synchronize(self.tdev)
-        st = self.L.ipcfp_exec_bucketize(self.dev, C.c_void_p(seg_ptr), nseg, pos0, world, cap, C.c_void_p(send.data_ptr()), counts.ctypes.data)
-        if st != A.OK:
-            raise A.IpcfpError(st, self.L.ipcfp_last_error().decode(), self.L.ipcfp_last_error_index())
-        return send, counts
-
-    def dedup(self, recv, counts, world, cap):
-        total = int(np.asarray(counts).sum())
-        dup = self.torch.zeros(max(total, 1), dtype=self.torch.int64, device=self.tdev)
-        n = C.c_uint64()
-        counts = np.ascontiguousarray(counts, dtype=np.uint64)
-        self.torch.cuda.synchronize(self.tdev)
-        st = self.L.ipcfp_exec_dedup(self.dev, C.c_void_p(recv.data_ptr()), counts.ctypes.data, world, cap, C.c_void_p(dup.data_ptr()), max(total, 1),
-                                     C.byref(n))
-        if st != A.OK:
-            raise A.IpcfpError(st, self.L.ipcfp_last_error().decode(), self.L.ipcfp_last_error_index())
-        return dup[:n.value].cpu().numpy().view(np.uint64)
-
-    def fetch(self, seg_ptr, nseg, pos0, req):
-        req = np.ascontiguousarray(req, dtype=np.uint64)
-        out = self.torch.zeros(max(len(req), 1) * REC, dtype=self.torch.uint8, device=self.tdev)
-        if len(req):
-            r = self.torch.as_tensor(req.view(np.int64)).to(self.tdev)
-            self.torch.cuda.synchronize(self.tdev)
-            st = self.L.ipcfp_exec_fetch(self.dev, C.c_void_p(seg_ptr), nseg, pos0, C.c_void_p(r.data_ptr()), len(req), C.c_void_p(out.data_ptr()))
-            if st != A.OK:
-                raise A.IpcfpError(st, self.L.ipcfp_last_error().decode(), self.L.ipcfp_last_error_index())
-        return out[:len(req) * REC].cpu().numpy().reshape(-1, REC)
-
-    def buffer_device(self):
-        return self.tdev
-
-    def merge_witness(self, gathered, counts, world, cap):
-        total = int(np.asarray(counts).sum())
-        out = self.torch.empty((total + 1) * 38, dtype=self.torch.uint8, device=self.tdev)
-        n = C.c_uint64()
-        counts = np.ascontiguousarray(counts, dtype=np.uint64)
-        self.torch.cuda.synchronize(self.tdev)
-        st = self.L.ipcfp_merge_witness_cids(self.dev, C.c_void_p(gathered.data_ptr()), counts.ctypes.data, world, cap, C.c_void_p(out.data_ptr()),
-                                             total + 1, C.byref(n))
-        if st != A.OK:
-            raise A.IpcfpError(st, self.L.ipcfp_last_error().decode(), self.L.ipcfp_last_error_index())
-        return out[:n.value * 38]
-
-    def upload(self, a):
-        return self.torch.as_tensor(np.ascontiguousarray(a)).to(self.tdev)
-
-    def witness_cids_device(self, res_ptr, cap):
-        """The result's sorted witness CIDs as a zero-padded device tensor of cap*38 bytes (device-to-device copy)."""
-        t = self.torch.zeros(cap * 38, dtype=self.torch.uint8, device=self.tdev)
-        n = C.c_uint64()
-        self.torch.cuda.synchronize(self.tdev)
-        st = self.L.ipcfp_witness_cids_to_device(res_ptr, C.c_void_p(t.data_ptr()), cap, C.byref(n))
-        if st != A.OK:
-            raise A.IpcfpError(st, self.L.ipcfp_last_error().decode(), self.L.ipcfp_last_error_index())
-        return t
-
-
-def raw_position_of(exec_index, dups_sorted):
-    """exec index i ↔ position p in the concatenated message list, given the sorted duplicate positions D:
-    p is the (i+1)-th position that is not in D, i.e. the fixed point of p = i + |{d ∈ D : d ≤ p}|."""
-    p = exec_index
-    while True:
-        k = bisect.bisect_right(dups_sorted, p)
-        q = exec_index + k
-        if q == p:
-            return p
-        p = q
-
-
-def raw_positions_of(exec_indices, dups_sorted):
-    """Vectorised raw_position_of for a sorted array of exec indices."""
-    i = np.asarray(exec_indices, dtype=np.uint64)
-    if len(dups_sorted) == 0 or len(i) == 0:
-        return i.copy()
-    D = np.asarray(dups_sorted, dtype=np.uint64)
-    p = i.copy()
-    while True:
-        q = i + np.searchsorted(D, p, side="right").astype(np.uint64)
-        if np.array_equal(q, p):
-            return p
-        p = q
-
-
-def resolve_execution_order(ops, coll, seg_ptr, nseg, matching, proof_exec_indices, seg_counts=None, need_counts=None, bucket_cap=None):
-    """Runs the distributed first-seen dedup and returns (n_exec, (sorted exec indices, their 40-byte records)).
-
-    seg_ptr/nseg: this rank's slice of the raw message list (device pointer for CudaShardOps);
-    matching: the rank's matching receipt indices (for the MISSING_EXEC check, events/generator.rs:244-246);
-    proof_exec_indices: exec indices whose message CID the rank's proofs need;
-    seg_counts: per-rank slice lengths if the caller already gathered them; bucket_cap: first bucket capacity to try (the same on every
-    rank; default 1.25·max/world + 1024, doubled on every rank together while some rank's split does not fit)."""
-    world, rank = coll.world, coll.rank
-    if seg_counts is None:
-        with _Phase("x.counts"):
-            seg_counts = coll.all_gather_i64([nseg])[:, 0]
-    counts = np.asarray(seg_counts, dtype=np.int64)
-    pos0 = int(counts[:rank].sum())
-    nraw = int(counts.sum())
-    # A rank-local failure of a device helper must not leave the other ranks waiting in the next collective: every helper's status
-    # rides on the collective that follows it, and all ranks continue, retry or raise TOGETHER (first failing rank's error).
-    FAIL = -1
-    cap = int(bucket_cap) if bucket_cap else int(counts.max()) // world + int(counts.max()) // (4 * world) + 1024
-    while True:
-        err = None
-        with _Phase("x.bucketize"):
-            try:
-                send, cnt = ops.bucketize(seg_ptr, nseg, pos0, world, cap)
-                row = np.asarray(cnt).view(np.int64)
-            except A.IpcfpError as e:
-                err, send, row = e, None, np.full(world, FAIL, dtype=np.int64)
-        with _Phase("x.count_matrix"):
-            cnt_matrix = coll.all_gather_i64(row)                       # [sender, owner]; a row of -1 = that sender's bucketize failed
-        failed = [r for r in range(world) if int(cnt_matrix[r, 0]) == FAIL]
-        if not failed:
-            break
-        if cap >= int(counts.max()) + 1:                                 # even one bucket holding a whole slice did not fit: not a capacity problem
-            raise err if err is not None else A.IpcfpError(A.ERR_INVALID_ARG, f"exec bucketize failed on rank {failed[0]}", failed[0])
-        cap = min(2 * cap, int(counts.max()) + 1)                        # skewed CID→owner split: every rank retries with larger buckets
-    recv_counts = cnt_matrix[:, rank].astype(np.uint64)
-    with _Phase("x.all_to_all"):
-        recv = coll.all_to_all_bytes(send, cap * ENTRY)
-    with _Phase("x.dedup"):
-        dedup_err = None
-        try:
-            dups_local = ops.dedup(recv, recv_counts, world, cap)
-        except A.IpcfpError as e:
-            dedup_err, dups_local = e, np.zeros(0, dtype=np.uint64)
-    # ONE fixed-size all-gather carries, per rank, the duplicate positions it found as an owner and the exec indices its
-    # proofs need: [n_dups, n_need, dups…(DUP_CAP), need…(capq)]. Every rank then knows D and every rank's requests, so the
-    # raw positions of ALL requests are derived locally (no second round trip). The rare overflow of the duplicate list
-    # falls back to the variable-length gather.
-    DUP_CAP = 1023
-    need = np.unique(np.asarray(proof_exec_indices, dtype=np.uint64))
-    if need_counts is None:
-        with _Phase("x.need_counts"):
-            need_counts = coll.all_gather_i64([len(need)])[:, 0]
-    req_counts = np.asarray(need_counts, dtype=np.int64)
-    capq = int(req_counts.max()) if len(req_counts) else 0
-    with _Phase("x.dups_gather"):
-        pad = np.zeros(2 + DUP_CAP + capq, dtype=np.int64)
-        pad[0] = FAIL if dedup_err is not None else len(dups_local)
-        pad[1] = len(need)
-        k = min(len(dups_local), DUP_CAP)
-        pad[2:2 + k] = dups_local[:k].view(np.int64)
-        pad[2 + DUP_CAP:2 + DUP_CAP + len(need)] = need.view(np.int64)
-        allp = coll.all_gather_i64(pad)
-        bad_ranks = [r for r in range(world) if int(allp[r, 0]) == FAIL]
-        if bad_ranks:
-            raise dedup_err if dedup_err is not None else A.IpcfpError(A.ERR_INVALID_ARG, f"exec dedup failed on rank {bad_ranks[0]}", bad_ranks[0])
-        if int(allp[:, 0].max()) > DUP_CAP:
-            dups, _ = coll.all_gather_var_u64(dups_local)
-        else:
-            dups = np.concatenate([allp[r, 2:2 + int(allp[r, 0])] for r in range(world)]).view(np.uint64)
-    D = np.sort(dups)
-    n_exec = nraw - len(D)
-    # exec.get(i) must exist for every matching receipt (checked in ascending order by the reference, events/generator.rs:244-246);
-    # each rank's verdict rides on the answer all-reduce below, so all ranks fail together
-    matching = np.asarray(matching, dtype=np.uint64)
-    bad = matching[matching >= np.uint64(n_exec)]
-    NO_BAD = np.iinfo(np.int64).max
-    my_bad = int(bad.min()) if len(bad) else NO_BAD
-    last = np.uint64(max(n_exec, 1) - 1)
-    req_all = np.concatenate([raw_positions_of(np.minimum(allp[r, 2 + DUP_CAP:2 + DUP_CAP + int(allp[r, 1])].view(np.uint64), last), D)
-                              for r in range(world)]) if capq else np.zeros(0, np.uint64)
-    with _Phase("x.fetch"):
-        fetch_err = None
-        try:
-            ans = ops.fetch(seg_ptr, nseg, pos0, req_all)            # zeros where another rank owns the position
-        except A.IpcfpError as e:
-            fetch_err, ans = e, np.zeros((len(req_all), REC), dtype=np.uint8)
-    with _Phase("x.ans_reduce"):
-        verdict = np.zeros(2 * world, dtype=np.int64)                # [first missing exec index per rank | fetch failed per rank]
-        verdict[rank] = my_bad
-        verdict[world + rank] = 1 if fetch_err is not None else 0
-        flat = np.concatenate([np.ascontiguousarray(ans).reshape(-1).view(np.int64), verdict])
-        red = coll.all_reduce_sum_i64(flat)
-        tail = red[len(red) - 2 * world:]
-        if tail[world:].any():
-            r_bad = int(np.flatnonzero(tail[world:])[0])
-            raise fetch_err if fetch_err is not None else A.IpcfpError(A.ERR_INVALID_ARG, f"exec fetch failed on rank {r_bad}", r_bad)
-        first_bad = int(tail[:world].min())
-        if first_bad != NO_BAD:
-            raise A.IpcfpError(A.ERR_MISSING_EXEC, "Missing message at index", first_bad)
-        ans = red[:len(red) - 2 * world].view(np.uint8).reshape(-1, REC)
-    start = int(req_counts[:rank].sum())
-    mine = ans[start:start + len(need)]
-    return n_exec, (need, mine)
-
-
-def record_to_cid(rec40):
-    """40-byte record {digest[32], prefix[6], 0, 0} → 38-byte CID."""
-    return bytes(rec40[32:38]) + bytes(rec40[:32])
-
-
-def _proofs_view(res_c):
-    """numpy view (n, sizeof(EventProofC)) over the result's proof records (host memory owned by the result)."""
-    n = int(res_c.n_proofs)
-    sz = C.sizeof(A.EventProofC)
-    if n == 0:
-        return np.zeros((0, sz), dtype=np.uint8)
-    addr = C.cast(res_c.proofs, C.c_void_p).value
-    return np.frombuffer((C.c_uint8 * (n * sz)).from_address(addr), dtype=np.uint8).reshape(n, sz)
-
-
-def records_to_cids(recs):
-    """(k, 40) records → (k, 38) CIDs."""
-    recs = np.asarray(recs, dtype=np.uint8).reshape(-1, REC)
-    return np.concatenate([recs[:, 32:38], recs[:, :32]], axis=1)
-
-
-def patch_message_cids(res_c, msg_of):
-    """Writes EventProof.message_cid of a shard result in place (res_c: EventResultC).
-    msg_of = (sorted exec indices, (k, 40) records)."""
-    pv = _proofs_view(res_c)
-    if not len(pv):
-        return
-    keys, recs = msg_of
-    off = A.EventProofC.message_cid.offset
-    exec_idx = pv[:, :8].copy().view(np.uint64).reshape(-1)
-    where = np.searchsorted(np.asarray(keys, dtype=np.uint64), exec_idx)
-    pv[:, off:off + 38] = records_to_cids(recs)[where]
-
-
-def gather_witness_cids(ops, coll, local_sorted_cids, counts=None, device_tensor=None):
-    """all-gather of the per-shard sorted witness CID lists + device merge → uint8 tensor (m*38) of the union.
-    device_tensor: the local list already on the device, padded to (max count + 1) * 38 bytes."""
-    if counts is None:
-        local = np.ascontiguousarray(local_sorted_cids, dtype=np.uint8).reshape(-1, 38)
-        counts = coll.all_gather_i64([len(local)])[:, 0]
-    counts = np.asarray(counts).astype(np.uint64)
-    cap = int(counts.max()) + 1
-    if device_tensor is None:
-        local = np.ascontiguousarray(local_sorted_cids, dtype=np.uint8).reshape(-1, 38)
-        buf = np.zeros((cap, 38), dtype=np.uint8)
-        buf[:len(local)] = local
-        device_tensor = ops.upload(buf.reshape(-1))
-    with _Phase("w.all_gather"):
-        gathered = coll.all_gather_bytes(device_tensor)
-    with _Phase("w.merge"):
-        merged = ops.merge_witness(gathered, counts, coll.world, cap)
-    return merged
-
-
-def generate_event_proof_distributed(lib, store_handle, tipset_handle, spec_c, lo, hi, coll, ops, flags=0):
-    """One rank's part of a sharded generate_event_proof + the cross-shard resolution.
-    Returns (POINTER(EventResultC) with message CIDs patched — caller frees it, n_exec, merged witness CIDs)."""
-    out = C.POINTER(A.EventResultC)()
-    with _Phase("local_shard_scan"):
-        st = lib.ipcfp_generate_event_proof_shard_resident(store_handle, tipset_handle, C.byref(spec_c), lo, hi, coll.world, coll.rank, flags,
-                                                           C.byref(out))
-    ok = st == A.OK
-    r = out.contents if ok else None
-    # one all-gather: status (a failing rank must not leave the others hanging), slice length, witness size
-    with _Phase("header_allgather"):
-        need = np.unique(_proofs_view(r)[:, :8].copy().view(np.uint64).reshape(-1)) if ok and r.n_proofs else np.zeros(0, np.uint64)
-        hdr = coll.all_gather_i64([st, int(r.shard_exec_count) if ok else 0, int(r.witness.n_blocks) if ok else 0, len(need)])
-    worst = int(hdr[:, 0].min())
-    if worst != A.OK:
-        if not ok:
-            raise A.IpcfpError(st, lib.ipcfp_last_error().decode(errors="replace"), lib.ipcfp_last_error_index())
-        lib.ipcfp_event_result_free(out)
-        raise A.IpcfpError(worst, "another rank failed", 0xFFFFFFFFFFFFFFFF)
-    matching = np.frombuffer((C.c_uint64 * int(r.n_matching)).from_address(r.matching_indices), dtype=np.uint64) if r.n_matching else np.zeros(0, np.uint64)
-    with _Phase("resolve_exec_total"):
-        n_exec, msg_of = resolve_execution_order(ops, coll, r.shard_exec_dev, int(r.shard_exec_count), matching, need, seg_counts=hdr[:, 1],
-                                                 need_counts=hdr[:, 3])
-    with _Phase("patch"):
-        patch_message_cids(r, msg_of)
-    with _Phase("witness_union"):
-        wcounts = hdr[:, 2]
-        dev_t = None
-        if hasattr(ops, "witness_cids_device"):
-            dev_t = ops.witness_cids_device(out, int(wcounts.max()) + 1)
-        m = int(r.witness.n_blocks)
-        local_cids = None
-        if dev_t is None:
-            local_cids = np.frombuffer((C.c_uint8 * (m * 38)).from_address(r.witness.cids), dtype=np.uint8) if m else np.zeros(0, np.uint8)
-        merged = gather_witness_cids(ops, coll, local_cids, counts=wcounts, device_tensor=dev_t)
-    return out, n_exec, merged
-
-
-# ------------------------------------------------------------------------------------------------ in-library protocol (NCCL)
 class ShardedComm:
     """Thin caller of the library's own cross-shard protocol (`ipcfp_comm_init` / `ipcfp_generate_event_proof_sharded`,
     csrc/parallel.cu): the collectives run inside the C-ABI call over NCCL, on the engine's streams. This class only moves

@@ -1,4 +1,4 @@
-"""Workers for the world_size-2 tests of the cross-shard path (spawned by torch.multiprocessing)."""
+"""Workers for the multi-process tests of the sharded call (spawned by torch.multiprocessing)."""
 import os
 import sys
 import traceback
@@ -12,195 +12,11 @@ if ROOT not in sys.path:
 PARAMS = dict(seed=123, n_receipts=3000, events_per_receipt=4, match_ppm=30000, dup_msgs=9, n_parents=3)
 
 
-class NumpyShardOps:
-    """Host restatement of the three device helpers + the witness merge (TEST ONLY: lets the gloo/CPU test
-    exercise ipc_filecoin_proofs_b200.parallel without a GPU). seg 'pointers' are numpy (n, 40) arrays."""
-
-    def bucketize(self, seg, nseg, pos0, world, cap):
-        import torch
-        send = np.zeros((world, cap, 48), dtype=np.uint8)
-        counts = np.zeros(world, dtype=np.uint64)
-        for k in range(nseg):
-            owner = int(seg[k, :8].view(np.uint64)[0] % world)
-            e = send[owner, int(counts[owner])]
-            e[:40] = seg[k]
-            e[40:] = np.frombuffer(np.uint64(pos0 + k).tobytes(), dtype=np.uint8)
-            counts[owner] += 1
-        return torch.from_numpy(send.reshape(-1)), counts
-
-    def dedup(self, recv, counts, world, cap):
-        r = recv.numpy().reshape(world, cap, 48)
-        first = {}
-        ents = []
-        for w in range(world):
-            for k in range(int(counts[w])):
-                key = r[w, k, :40].tobytes()
-                pos = int(r[w, k, 40:].view(np.uint64)[0])
-                ents.append((key, pos))
-                first[key] = min(first.get(key, pos), pos)
-        return np.array([p for key, p in ents if first[key] != p], dtype=np.uint64)
-
-    def fetch(self, seg, nseg, pos0, req):
-        out = np.zeros((len(req), 40), dtype=np.uint8)
-        for j, p in enumerate(req):
-            p = int(p)
-            if pos0 <= p < pos0 + nseg:
-                out[j] = seg[p - pos0]
-        return out
-
-    def upload(self, a):
-        import torch
-        return torch.from_numpy(np.ascontiguousarray(a))
-
-    def merge_witness(self, gathered, counts, world, cap):
-        import oracle
-        from ipc_filecoin_proofs_b200 import _abi as A
-        g = gathered.numpy().reshape(world, cap, 38)
-        allc = np.concatenate([g[w, :int(counts[w])] for w in range(world)])
-        mixed = np.flatnonzero((allc[:, :6] != allc[:1, :6]).any(axis=1)) if len(allc) else []
-        if len(mixed):   # the rule of ipcfp_merge_witness_cids
-            raise A.IpcfpError(A.ERR_UNSUPPORTED, "witness CID lists with more than one CID prefix cannot be merged on the device", int(mixed[0]))
-        return oracle.sort_unique_cids(allc).reshape(-1)
-
-
-def raw_message_list(ts):
-    """The concatenated message list (all message AMTs in order) as 40-byte records, via the Python oracle."""
-    import cbor2
-    from oracle import pyoracle as P
-    store = ts.as_dict()
-    out = []
-    for tx in ts.parent_txmeta_cids:
-        bls, secp = cbor2.loads(store[bytes(tx)])
-        for root in (bls, secp):
-            amt = P.Amt(P._link(root), P.Recorder(store), 0)
-            amt.for_each(lambda i, c: out.append(P._link(c)))
-    rec = np.zeros((len(out), 40), dtype=np.uint8)
-    for k, c in enumerate(out):
-        rec[k, :32] = np.frombuffer(c[6:], dtype=np.uint8)
-        rec[k, 32:38] = np.frombuffer(c[:6], dtype=np.uint8)
-    return rec
-
-
 def _init(rank, world, port, backend):
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group(backend, rank=rank, world_size=world)
     return dist
-
-
-def cpu_worker(rank, world, port, q):
-    """gloo / CPU: the oracle is the per-rank engine, NumpyShardOps the device helpers."""
-    try:
-        import oracle
-        import synth
-        from ipc_filecoin_proofs_b200 import _abi as A
-        from ipc_filecoin_proofs_b200 import parallel as PL
-        dist = _init(rank, world, port, "gloo")
-        N = PARAMS["n_receipts"]
-        lo, hi = N * rank // world, N * (rank + 1) // world
-        full = synth.Tipset(synth.default_params(**PARAMS))
-        spec = A.make_event_spec(full.event_signature, full.topic1, full.actor_filter)
-        ost = oracle.Store.from_tipset(full)
-        exp = ost.generate_event_proof(full, spec)
-        res = ost.generate_event_proof_shard(full, spec, lo, hi, world, rank)
-        raw = raw_message_list(full)
-        glo, ghi = len(raw) * lo // N, len(raw) * hi // N
-        seg = raw[glo:ghi]
-        coll = PL.Collectives(dist)
-        ops = NumpyShardOps()
-        n_exec, msg_of = PL.resolve_execution_order(ops, coll, seg, len(seg), res.matching, [p.exec_index for p in res.proofs])
-        assert n_exec == exp.n_exec, (n_exec, exp.n_exec)
-        keys, recs = msg_of
-        cids = PL.records_to_cids(recs)
-        for p in res.proofs:
-            k = int(np.searchsorted(keys, np.uint64(p.exec_index)))
-            assert int(keys[k]) == p.exec_index and cids[k].tobytes() == p.message_cid
-        merged = PL.gather_witness_cids(ops, coll, res.witness.cids)
-        assert np.array_equal(np.asarray(merged).reshape(-1, 38), exp.witness.cids)
-        # MISSING_EXEC agreement: pretend a receipt index beyond the execution order matched on rank 1
-        try:
-            PL.resolve_execution_order(ops, coll, seg, len(seg), list(res.matching) + ([10 ** 9] if rank == 1 else []), [])
-            raise AssertionError("expected MISSING_EXEC")
-        except A.IpcfpError as e:
-            assert e.status == A.ERR_MISSING_EXEC and e.index == 10 ** 9
-        # rank-local helper failures are agreed, not left to hang the peers (ADVICE round 1): a bucketize that reports 'bucket capacity too
-        # small' on ONE rank makes every rank retry with larger buckets; a dedup / fetch failure on one rank raises on all of them
-        class Flaky(NumpyShardOps):
-            def __init__(self, fail_rank, what):
-                self.fail_rank, self.what, self.calls = fail_rank, what, 0
-
-            def bucketize(self, seg, nseg, pos0, world, cap):
-                self.calls += 1
-                if self.what == "bucketize" and rank == self.fail_rank and self.calls == 1:
-                    raise A.IpcfpError(A.ERR_INVALID_ARG, "bucket capacity too small", 0)
-                return super().bucketize(seg, nseg, pos0, world, cap)
-
-            def dedup(self, recv, counts, world, cap):
-                if self.what == "dedup" and rank == self.fail_rank:
-                    raise A.IpcfpError(A.ERR_INVALID_ARG, "duplicate list capacity too small", 0)
-                return super().dedup(recv, counts, world, cap)
-
-            def fetch(self, seg, nseg, pos0, req):
-                if self.what == "fetch" and rank == self.fail_rank:
-                    raise A.IpcfpError(A.ERR_INVALID_ARG, "fetch failed", 0)
-                return super().fetch(seg, nseg, pos0, req)
-
-        fl = Flaky(1, "bucketize")
-        n2, _ = PL.resolve_execution_order(fl, coll, seg, len(seg), res.matching, [p.exec_index for p in res.proofs], bucket_cap=len(raw) // world)
-        assert n2 == exp.n_exec and fl.calls == 2, (n2, fl.calls)          # both ranks went round twice
-        for what, fr in (("dedup", 0), ("fetch", 1)):
-            try:
-                PL.resolve_execution_order(Flaky(fr, what), coll, seg, len(seg), res.matching, [p.exec_index for p in res.proofs])
-                raise AssertionError("expected the injected " + what + " failure on every rank")
-            except A.IpcfpError as e:
-                assert e.status == A.ERR_INVALID_ARG
-        dist.barrier()
-        dist.destroy_process_group()
-        q.put((rank, "ok"))
-    except Exception:
-        q.put((rank, traceback.format_exc()))
-
-
-def gpu_worker(rank, world, port, q):
-    """Two ranks sharing cuda:0 over gloo: the real engine on sharded stores + the CUDA helpers."""
-    try:
-        import ctypes as C
-        import oracle
-        import synth
-        from ipc_filecoin_proofs_b200 import _abi as A
-        from ipc_filecoin_proofs_b200 import api
-        from ipc_filecoin_proofs_b200 import parallel as PL
-        import torch
-        dist = _init(rank, world, port, "gloo")
-        N = PARAMS["n_receipts"]
-        lo, hi = N * rank // world, N * (rank + 1) // world
-        full = synth.Tipset(synth.default_params(**PARAMS))
-        shard = synth.Tipset(synth.default_params(shard_lo=lo, shard_hi=hi, **PARAMS))
-        spec = A.make_event_spec(full.event_signature, full.topic1, full.actor_filter)
-        exp = oracle.Store.from_tipset(full).generate_event_proof(full, spec)
-        exp_shard = oracle.Store.from_tipset(full).generate_event_proof_shard(full, spec, lo, hi, world, rank)
-        L = api.lib()
-        store = api.BlockStore.from_tipset(shard, device=0, verify_cids=True)
-        d, keep = A.make_tipset_desc(shard)
-        tip = C.c_void_p()
-        assert L.ipcfp_tipset_upload(store._h, C.byref(d), C.byref(tip)) == 0
-        coll = PL.Collectives(dist, torch.device("cuda", 0))
-        ops = PL.CudaShardOps(L, 0)
-        out, n_exec, merged = PL.generate_event_proof_distributed(L, store._h, tip, spec, lo, hi, coll, ops)
-        got = A.event_result_from_c(out.contents)
-        L.ipcfp_event_result_free(out)
-        L.ipcfp_tipset_free(tip)
-        assert n_exec == exp.n_exec
-        assert got.matching.tolist() == exp_shard.matching.tolist()
-        assert [p.key() for p in got.proofs] == [p.key() for p in exp_shard.proofs]
-        assert np.array_equal(got.witness.cids, exp_shard.witness.cids)
-        assert got.witness.blocks() == exp_shard.witness.blocks()
-        assert np.array_equal(merged.cpu().numpy().reshape(-1, 38), exp.witness.cids)
-        dist.barrier()
-        dist.destroy_process_group()
-        q.put((rank, "ok"))
-    except Exception:
-        q.put((rank, traceback.format_exc()))
 
 
 def nccl_worker(rank, world, port, q):

@@ -4,13 +4,18 @@
 //   bitmap_to_indices    nbits not a multiple of 32, empty / full / sparse / alternating bitmaps, word counts across the same limits;
 //   radix_sort_pairs     8, 16, 24 and 32 key bits (odd and even pass counts), n across 2 048 (one tile) and 131 072 (the histogram
 //                        scan leaves the single CTA); equal, two-valued, top-byte-only, sorted, reverse-sorted and random keys. The
-//                        result must be the STABLE sort by the low nbits bits, values being the original indices.
+//                        result must be the STABLE sort by the low nbits bits, values being the original indices;
+//   sort_unique_cids     one-prefix lists of 14 totals across 2 048 and 131 072, digests clustered on the radix key so that
+//                        k_merge_tie_fix orders runs of up to 512, against std::sort (the raw byte order) + unique; lists of several
+//                        prefixes: ordered by digest bytes 0-3, then the 38 bytes, the first position of another prefix is reported,
+//                        and sort_cids_host of the output is the `Cid` order.
 // Every output buffer carries a sentinel past its end that must survive.
 //
 //   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr \
 //        -o prims_check tests/gpu_prims/prims_check.cu ipc_filecoin_proofs_b200/csrc/prims.cu && ./prims_check
 // Prints one "ok: ..." line and exits 0, or names the first disagreement and exits 1.
 #include <algorithm>
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <numeric>
@@ -172,6 +177,122 @@ static bool check_sort(uint64_t n, int nbits, const char* what, const std::vecto
     return true;
 }
 
+// ------------------------------------------------------------------ sort_unique_cids
+typedef std::array<uint8_t, 38> Cid38;
+static const uint8_t FILECOIN_PREFIX[6] = {0x01, 0x71, 0xa0, 0xe4, 0x02, 0x20};   // CIDv1, dag-cbor, blake2b-256, 32 bytes
+// Eight valid CIDv1 prefixes in `Cid` order (version, codec, multihash code, size); the varint code makes their raw byte order differ
+// (0x407f = ff 80 01 sorts after 0xb220 = a0 e4 02 bytewise). Index 6 is FILECOIN_PREFIX.
+static const uint8_t MIXED_PREFIXES[8][6] = {
+    {0x01, 0x55, 0xff, 0xff, 0x01, 0x20}, {0x01, 0x55, 0xa0, 0xe4, 0x02, 0x20}, {0x01, 0x70, 0x81, 0x80, 0x02, 0x20},
+    {0x01, 0x71, 0xff, 0x80, 0x01, 0x20}, {0x01, 0x71, 0x80, 0x80, 0x02, 0x20}, {0x01, 0x71, 0x92, 0xe4, 0x02, 0x20},
+    {0x01, 0x71, 0xa0, 0xe4, 0x02, 0x20}, {0x01, 0x71, 0xff, 0xff, 0x03, 0x20}};
+
+static Cid38 make_cid(const uint8_t* prefix, const uint8_t* digest) {
+    Cid38 c;
+    std::copy(prefix, prefix + 6, c.begin());
+    std::copy(digest, digest + 32, c.begin() + 6);
+    return c;
+}
+static Cid38 random_cid(const uint8_t* prefix) {
+    uint8_t d[32];
+    for (auto& b : d) b = (uint8_t)rnd();
+    return make_cid(prefix, d);
+}
+// n digests in clusters that share their first four bytes (the radix key) and differ from byte 4 on: the first clusters hold 512 and 300
+// members, the rest 2..64, so runs of equal keys longer and shorter than a warp are put in order by k_merge_tie_fix
+static std::vector<Cid38> clustered_pool(uint64_t n) {
+    std::vector<Cid38> out;
+    for (uint64_t g = 0; out.size() < n; g++) {
+        uint8_t t[32];
+        for (auto& b : t) b = (uint8_t)rnd();
+        const uint64_t size = g == 0 ? 512 : g == 1 ? 300 : 2 + rnd() % 63;
+        const uint32_t at = 4 + (uint32_t)(rnd() % 27);   // members differ at bytes at, at + 1
+        for (uint64_t k = 0; k < size && out.size() < n; k++) {
+            uint8_t d[32];
+            std::copy(t, t + 32, d);
+            d[at] = (uint8_t)(k >> 8);
+            d[at + 1] = (uint8_t)k;
+            out.push_back(make_cid(FILECOIN_PREFIX, d));
+        }
+    }
+    return out;
+}
+
+// One call of sort_unique_cids on `cids`: ordered by digest bytes 0-3 and then the 38 bytes (within one prefix, the raw byte order) with
+// duplicates removed, the first position whose prefix differs from entry 0's (UINT64_MAX: none), nothing written past the unique
+// entries; with cid_order, sort_cids_host of the output equals cid_order.
+static bool check_cid_sort(const char* what, const std::vector<Cid38>& cids, uint64_t want_mixed, cudaStream_t st,
+                           const std::vector<Cid38>* cid_order = nullptr) {
+    const uint64_t n = cids.size();
+    std::vector<Cid38> ref(cids);
+    std::sort(ref.begin(), ref.end(), [](const Cid38& x, const Cid38& y) {
+        return std::lexicographical_compare(x.begin() + 6, x.begin() + 10, y.begin() + 6, y.begin() + 10) ||
+               (std::equal(x.begin() + 6, x.begin() + 10, y.begin() + 6) && x < y);
+    });
+    ref.erase(std::unique(ref.begin(), ref.end()), ref.end());
+    std::vector<uint8_t> in(38 * n);
+    for (uint64_t i = 0; i < n; i++) std::copy(cids[i].begin(), cids[i].end(), in.begin() + 38 * i);
+    CheckBuf<uint8_t> d_in(38 * n), d_out(38 * (n + 1));
+    if (n) up(d_in.p, in);
+    up(d_out.p, std::vector<uint8_t>(38 * (n + 1), 0xA5));
+    uint64_t mixed = 0;
+    const uint64_t m = sort_unique_cids(st, d_in.p, n, d_out.p, &mixed);
+    std::vector<uint8_t> out = down(d_out.p, 38 * (n + 1));
+    if (m != ref.size()) FAIL("cid sort n=%llu (%s): %llu unique, expected %zu", (unsigned long long)n, what, (unsigned long long)m, ref.size());
+    if (mixed != want_mixed)
+        FAIL("cid sort n=%llu (%s): first mixed position %llu, expected %llu", (unsigned long long)n, what, (unsigned long long)mixed,
+             (unsigned long long)want_mixed);
+    for (uint64_t i = 0; i < m; i++)
+        if (!std::equal(ref[i].begin(), ref[i].end(), out.begin() + 38 * i)) FAIL("cid sort n=%llu (%s): entry %llu differs", (unsigned long long)n, what, (unsigned long long)i);
+    for (uint64_t b = 38 * m; b < out.size(); b++)
+        if (out[b] != 0xA5) FAIL("cid sort n=%llu (%s): wrote past the %llu unique entries", (unsigned long long)n, what, (unsigned long long)m);
+    if (cid_order) {
+        out.resize(38 * m);
+        sort_cids_host(out);
+        if (cid_order->size() != m) FAIL("cid sort n=%llu (%s): %llu unique, the `Cid` order has %zu", (unsigned long long)n, what, (unsigned long long)m, cid_order->size());
+        for (uint64_t i = 0; i < m; i++)
+            if (!std::equal((*cid_order)[i].begin(), (*cid_order)[i].end(), out.begin() + 38 * i))
+                FAIL("cid sort n=%llu (%s): entry %llu of sort_cids_host differs from the `Cid` order", (unsigned long long)n, what, (unsigned long long)i);
+    }
+    g_cases++;
+    return true;
+}
+
+static bool cid_sorts(cudaStream_t st) {
+    // one prefix: totals on both sides of one radix tile (2 048) and of the single-CTA scan of the radix histograms (131 072), drawn with
+    // replacement from a pool of 3/4 the total, so duplicates are many
+    const uint64_t totals[] = {0, 1, 5, 128, 300, 700, 1792, 2047, 2048, 2049, 2200, 131071, 131072, 131073};
+    for (uint64_t n : totals) {
+        const std::vector<Cid38> pool = clustered_pool(std::max<uint64_t>(8, n * 3 / 4));
+        std::vector<Cid38> cids(n);
+        for (auto& c : cids) c = pool[rnd() % pool.size()];
+        if (!check_cid_sort("one prefix, clustered digests", cids, UINT64_MAX, st)) return false;
+    }
+    // several prefixes: sorted and unique all the same, the first differing position reported, `Cid` order by sort_cids_host
+    auto cid_order = [](std::vector<Cid38> v) {   // the prefixes' rank in MIXED_PREFIXES, then the digest
+        auto rank = [](const Cid38& c) { for (int k = 0; k < 8; k++) if (std::equal(c.begin(), c.begin() + 6, MIXED_PREFIXES[k])) return k; return 8; };
+        std::sort(v.begin(), v.end(), [&](const Cid38& x, const Cid38& y) { return rank(x) != rank(y) ? rank(x) < rank(y) : x < y; });
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+        return v;
+    };
+    std::vector<Cid38> a(9);
+    for (auto& c : a) c = random_cid(FILECOIN_PREFIX);
+    const Cid38 odd = random_cid(MIXED_PREFIXES[3]);   // multihash code 0x407f: `Cid` order puts it before every FILECOIN_PREFIX CID
+    std::vector<Cid38> l1(a.begin(), a.begin() + 7), l2(a.begin(), a.begin() + 3), l3(1, odd);
+    l1.push_back(odd);
+    l1.insert(l1.end(), a.begin() + 7, a.end());
+    l2.push_back(odd);
+    l3.insert(l3.end(), a.begin(), a.end());
+    std::vector<Cid38> l4(3000);
+    for (uint64_t k = 0; k < l4.size(); k++) l4[k] = random_cid(MIXED_PREFIXES[k % 8]);
+    const std::pair<const std::vector<Cid38>*, uint64_t> mixed_cases[] = {{&l1, 7}, {&l2, 3}, {&l3, 1}, {&l4, 1}};
+    for (const auto& mc : mixed_cases) {
+        const std::vector<Cid38> want = cid_order(*mc.first);
+        if (!check_cid_sort("several prefixes", *mc.first, mc.second, st, &want)) return false;
+    }
+    return true;
+}
+
 static bool sorts(cudaStream_t st) {
     const uint64_t sizes[] = {0, 1, 2, 33, 2047, 2048, 2049, 131071, 131072, 131073, 300001, (1u << 20) + 3};
     const int widths[] = {8, 16, 24, 32};
@@ -209,10 +330,10 @@ int main() {
         }
         cudaStream_t st;
         IPCFP_CUDA(cudaStreamCreate(&st));
-        bool ok = scans(st) && bitmaps(st) && sorts(st);
+        bool ok = scans(st) && bitmaps(st) && sorts(st) && cid_sorts(st);
         IPCFP_CUDA(cudaStreamDestroy(st));
         if (!ok) return 1;
-        printf("ok: exclusive_scan_u32, bitmap_to_indices and radix_sort_pairs equal the CPU references in %llu cases\n", (unsigned long long)g_cases);
+        printf("ok: exclusive_scan_u32, bitmap_to_indices, radix_sort_pairs and sort_unique_cids equal the CPU references in %llu cases\n", (unsigned long long)g_cases);
         return 0;
     } catch (const Error& e) {
         fprintf(stderr, "FAIL: %s\n", e.msg.c_str());

@@ -311,67 +311,3 @@ def test_store_refuses_an_unparseable_prefix(api, at):
     with pytest.raises(A.IpcfpError) as ei:
         _store(api, cids, [rng.bytes(8) for _ in cids])
     assert ei.value.status == A.ERR_UNSUPPORTED
-
-
-# ------------------------------------------------------------------ ipcfp_merge_witness_cids
-def _merge(api, lists, cap, pad_prefix=U.MIXED_PREFIXES[0]):
-    """lists → world segments of `cap` entries (the unused tail filled with CIDs of another prefix, which must be ignored) → the
-    device merge through parallel.CudaShardOps."""
-    import torch
-    from ipc_filecoin_proofs_b200.parallel import CudaShardOps
-    rng = np.random.default_rng(len(lists))
-    world = len(lists)
-    g = np.zeros((world, cap, 38), dtype=np.uint8)
-    for r, lst in enumerate(lists):
-        if lst:
-            g[r, :len(lst)] = np.frombuffer(b"".join(lst), dtype=np.uint8).reshape(-1, 38)
-        for k in range(len(lst), min(cap, len(lst) + 64)):
-            g[r, k] = np.frombuffer(pad_prefix + rng.bytes(32), dtype=np.uint8)
-    counts = np.array([len(lst) for lst in lists], dtype=np.uint64)
-    out = CudaShardOps(api.lib(), 0).merge_witness(torch.from_numpy(g.reshape(-1)).to("cuda:0"), counts, world, cap)
-    return out.cpu().numpy().reshape(-1, 38)
-
-
-def _lists(pool, sizes, rng):
-    """lists drawn with replacement from pool: duplicates inside and between lists."""
-    return [[pool[int(i)] for i in rng.integers(0, len(pool), s)] for s in sizes]
-
-
-@pytest.mark.parametrize("sizes,cap", [
-    ([0], 8), ([1], 1), ([700], 700),
-    ([300, 0], 300), ([2047, 0], 2047), ([1000, 1048], 1048), ([1024, 1025], 1025),
-    ([0, 0, 5], 5), ([682, 683, 683], 683), ([700, 0, 1500], 1500),
-    ([16] * 8, 16), ([0, 256, 256, 0, 256, 256, 256, 512], 512),
-    ([65536, 65535], 65536), ([65536, 65536], 65536), ([43691, 43691, 43691], 43691),
-])
-def test_merge_single_prefix(api, oracle_mod, sizes, cap):
-    """Totals on both sides of one radix tile (2 048) and of the single-CTA scan of the radix histograms (131 072); counts == cap,
-    empty lists, world 1, 2, 3 and 8."""
-    rng = np.random.default_rng(sum(sizes) + len(sizes))
-    pool = [U.FILECOIN_PREFIX + d for d in U.clustered_digests(max(8, (sum(sizes) * 3) // 4), rng)]
-    lists = _lists(pool, sizes, rng)
-    got = _merge(api, lists, cap)
-    allc = [c for lst in lists for c in lst]
-    exp = oracle_mod.sort_unique_cids(np.frombuffer(b"".join(allc), dtype=np.uint8)) if allc else np.zeros((0, 38), dtype=np.uint8)
-    assert got.shape == exp.shape and np.array_equal(got, exp)
-    if len(allc) >= 16:
-        assert len(exp) < len(allc)
-
-
-def test_merge_refuses_mixed_prefixes(api):
-    """Raw byte order is not `Cid` order across prefixes (0x407f = ff 80 01 sorts after 0xb220 = a0 e4 02), so the device merge refuses
-    lists with more than one prefix, like the sharded call, naming the first position whose prefix differs from the first entry's."""
-    from ipc_filecoin_proofs_b200.parallel import CudaShardOps   # noqa: F401  (the binding under test)
-    rng = np.random.default_rng(9)
-    a = [U.FILECOIN_PREFIX + rng.bytes(32) for _ in range(9)]
-    odd = bytes.fromhex("0171ff800120") + rng.bytes(32)            # multihash code 0x407f
-    for lists, index in (([[], a[:5], a[5:7] + [odd] + a[7:]], 7), ([a[:3] + [odd]], 3), ([[odd], a], 1)):
-        with pytest.raises(A.IpcfpError) as ei:
-            _merge(api, lists, 16, pad_prefix=U.FILECOIN_PREFIX)
-        assert ei.value.status == A.ERR_UNSUPPORTED and ei.value.index == index
-    b = [U.MIXED_PREFIXES[k % 8] + rng.bytes(32) for k in range(3000)]
-    with pytest.raises(A.IpcfpError) as ei:
-        _merge(api, [b[:1500], b[1500:]], 1500)
-    assert ei.value.status == A.ERR_UNSUPPORTED and ei.value.index == 1
-    got = _merge(api, [a[:4], a[4:]], 8)   # the next call still merges
-    assert np.array_equal(got, np.frombuffer(b"".join(sorted(a)), dtype=np.uint8).reshape(-1, 38))

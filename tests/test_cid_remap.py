@@ -6,7 +6,6 @@ import re
 import numpy as np
 import pytest
 
-from ipc_filecoin_proofs_b200 import _abi as A
 from tests import util as U
 from tests.util import spec_of
 
@@ -104,24 +103,6 @@ def test_oracle_storage_on_rewritten_tipset_equals_image(oracle_mod, ts3_small, 
     assert [vars(p) for p in got.proofs] == cm.storage_proofs(exp.proofs)
     assert ([bytes(c) for c in got.witness.cids], got.witness.blocks()) == cm.witness(exp.witness)
     assert got.spec_witness == cm.spec_witness(exp)
-
-
-def test_numpy_merge_refuses_mixed_prefixes():
-    """The CPU restatement of ipcfp_merge_witness_cids refuses what the device merge refuses, at the same position."""
-    from tests.dist_worker import NumpyShardOps
-    import torch
-    rng = np.random.default_rng(3)
-    cids = [U.FILECOIN_PREFIX + rng.bytes(32) for _ in range(10)]
-    g = np.zeros((2, 8, 38), dtype=np.uint8)
-    g[0, :5] = np.frombuffer(b"".join(cids[:5]), dtype=np.uint8).reshape(5, 38)
-    g[1, :5] = np.frombuffer(b"".join(cids[5:]), dtype=np.uint8).reshape(5, 38)
-    counts = np.array([5, 5], dtype=np.uint64)
-    ok = NumpyShardOps().merge_witness(torch.from_numpy(g.reshape(-1).copy()), counts, 2, 8)
-    assert len(ok) == 10 * 38
-    g[1, 2, :6] = np.frombuffer(U.MIXED_PREFIXES[3], dtype=np.uint8)
-    with pytest.raises(A.IpcfpError) as ei:
-        NumpyShardOps().merge_witness(torch.from_numpy(g.reshape(-1).copy()), counts, 2, 8)
-    assert ei.value.status == A.ERR_UNSUPPORTED and ei.value.index == 7
 
 
 def test_python_hash_copy_matches_the_device_source():

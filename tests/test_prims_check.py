@@ -1,4 +1,4 @@
-"""The device-wide primitives of csrc/prims.cu (exclusive scan, bitmap → indices, stable radix sort), called directly by
+"""The device-wide primitives of csrc/prims.cu (exclusive scan, bitmap → indices, stable radix sort, CID sort), called directly by
 tests/gpu_prims/prims_check.cu and compared there with plain CPU references at the sizes where their launch shapes change. The
 program is compiled with the library's own nvcc flags (the Makefile's NVFLAGS); the compile needs no GPU, running it does."""
 import os
@@ -44,4 +44,4 @@ def test_prims_match_cpu_references(prims_check_exe):
     assert out.returncode == 0, (out.stdout[-2000:], out.stderr[-3000:])
     ok = [line for line in out.stdout.splitlines() if line.startswith("ok:")]
     assert len(ok) == 1, out.stdout
-    assert int(ok[0].split(" in ")[1].split()[0]) == 407, ok[0]   # 30 scans, 41 bitmaps, 336 sorts: no case may go missing
+    assert int(ok[0].split(" in ")[1].split()[0]) == 425, ok[0]   # 30 scans, 41 bitmaps, 336 sorts, 18 CID sorts: no case may go missing
