@@ -126,6 +126,32 @@ typedef struct ipcfp_event_spec {
     uint64_t actor_id_filter;
 } ipcfp_event_spec;
 
+/* An eth_getLogs-style log filter: one predicate over the events extract_evm_log (common/evm.rs:13-59) accepts, with the topics and
+ * the emitter the EventProof carries. Topic k of a log is its t(k+1) value (Case B) or bytes 32k..32k+32 of its `topics` blob (Case A,
+ * which may hold zero or more than four topics). An event matches when all of these hold:
+ *   - extract_evm_log returns Some for it;
+ *   - n_emitters == 0, or EventData.emitter is one of emitters[];
+ *   - the log has at least n_positions topics;
+ *   - for every k < n_positions with n_values[k] > 0, topic k equals one of the 32-byte values[k][..], byte for byte.
+ * Duplicates in a set are allowed. A position with n_values[k] == 0 is a wildcard; positions past 3 are never constrained.
+ * Trailing wildcards count: n_positions plays the length of go-ethereum's `topics` list, whose filterLogs refuses logs with fewer
+ * topics than the list has entries. {n_positions = 3, values = [{A}, {}, {}]} is `[A, null, null]` and needs three topics; a caller
+ * who wants only the constrained positions to count sets n_positions to 1 + the highest constrained position ([A] needs one topic).
+ * The spec {sig, t1, actor?} is the filter {emitters = [actor] or none, n_positions = 2, values = [{keccak256(sig)}, {ascii_to_bytes32(t1)}]}.
+ * IPCFP_ERR_INVALID_ARG: n_positions > 4, n_values[k] > 0 for k >= n_positions, a NULL array with a nonzero count, more than
+ * IPCFP_LOG_FILTER_MAX_VALUES values at a position or more than IPCFP_LOG_FILTER_MAX_EMITTERS emitters. Emitters are actor IDs:
+ * resolve Ethereum addresses first (ipcfp_resolve_addresses). */
+#define IPCFP_LOG_FILTER_MAX_VALUES 65536u
+#define IPCFP_LOG_FILTER_MAX_EMITTERS 65536u
+typedef struct ipcfp_log_filter {
+    uint64_t n_emitters;          /* 0: any emitter; else EventData.emitter must be one of emitters[]        */
+    const uint64_t* emitters;     /* actor IDs                                                                */
+    uint32_t n_positions;         /* 0..4: an event needs at least this many topics                           */
+    uint32_t _pad;
+    uint64_t n_values[4];         /* per position; 0 = wildcard                                               */
+    const uint8_t* values[4];     /* n_values[k] * 32 bytes; topic k must equal one of them, byte for byte     */
+} ipcfp_log_filter;
+
 /* StorageProofSpec (src/proofs/generator.rs:12-15) */
 typedef struct ipcfp_storage_spec {
     uint64_t actor_id;
@@ -286,6 +312,15 @@ ipcfp_status ipcfp_generate_event_proof_resident(ipcfp_store* s, ipcfp_tipset* t
 ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, uint64_t lo,
                                                        uint64_t hi, uint32_t world_size, uint32_t rank, uint32_t flags,
                                                        ipcfp_event_result** out);
+/* generate_event_proof with a log filter (ipcfp_log_filter above) in place of the spec's EventMatcher: the same call, flags
+ * (IPCFP_WITNESS_BY_REFERENCE, IPCFP_RESULT_JSON, IPCFP_SCAN_SKIP_TX_AMTS) and result, one EventProofBundle. matching_indices are the
+ * receipts with at least one matching event; proofs are in (exec_index, event_index) order; a failure is the one the reference's
+ * generator with this predicate meets first. The proofs verify with ipcfp_verify_event_proofs (filter NULL or any spec they satisfy)
+ * and with ipcfp_verify_event_proofs_log. ipcfp_generate_log_proof = ipcfp_tipset_upload, then the resident call. */
+ipcfp_status ipcfp_generate_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
+                                               ipcfp_event_result** out);
+ipcfp_status ipcfp_generate_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_log_filter* filter, uint32_t flags,
+                                      ipcfp_event_result** out);
 /* The CUDA stream (cudaStream_t) all work of this store is issued on — for callers that time with
  * CUDA events or order their own device work after the engine's. */
 void* ipcfp_store_stream(ipcfp_store* s);
@@ -438,6 +473,10 @@ ipcfp_status ipcfp_plan_fetch_resident(ipcfp_store* s, ipcfp_tipset* t, const ip
 ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                               const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out);
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p);
+/* One fetch round for ipcfp_generate_log_proof_resident: the rules of ipcfp_plan_fetch_resident for event specs, with the filter as
+ * rule 3's predicate (the receipts with a matching event add their receipts-AMT paths). Any flag bit is IPCFP_ERR_INVALID_ARG. */
+ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
+                                           ipcfp_fetch_plan** out);
 /* The round as one Filecoin.ChainReadObj batch: request k asks for plan->cids[k] with "id": first_id + k, compact JSON
  *   [{"jsonrpc":"2.0","method":"Filecoin.ChainReadObj","params":[{"/":"b…"}],"id":<first_id + k>},…]
  * With first_id = the number of blocks already held, the responses go straight to ipcfp_store_create_rpc_json with
@@ -528,6 +567,11 @@ ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* witness_store, const ipcfp_t
                                        const uint8_t* data_blob, uint64_t data_blob_size, const ipcfp_event_spec* filter, uint8_t* results);
 ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n_proofs,
                                          uint8_t* results);
+/* ipcfp_verify_event_proofs with a log filter as check_event (never NULL): a proof that verifies is true only when its event matches
+ * `filter` (emitter set included). Invalid filters are refused as by ipcfp_generate_log_proof. */
+ipcfp_status ipcfp_verify_event_proofs_log(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs,
+                                           uint64_t n_proofs, const uint8_t* data_blob, uint64_t data_blob_size, const ipcfp_log_filter* filter,
+                                           uint8_t* results);
 
 /* ------------------------------------------------------------------------------------------
  * verify_proof_bundle (src/proofs/verifier.rs:12-60) from the JSON text: parse, witness store and verification on the GPU.

@@ -259,6 +259,27 @@ struct EventProofSpec {
     std::string topic_1;           // ASCII, right-padded to 32 bytes by the matcher
     std::optional<uint64_t> actor_id_filter;
 };
+// An eth_getLogs-style log filter (ipcfp_log_filter): emitters empty = any; topics[k] empty = any value at position k; topics.size()
+// is n_positions (an event needs at least that many topics).
+struct LogFilter {
+    std::vector<uint64_t> emitters;
+    std::vector<std::vector<H256>> topics;
+};
+inline ipcfp_log_filter log_filter_c(const LogFilter& f, std::vector<std::vector<uint8_t>>& keep) {
+    ipcfp_log_filter c;
+    memset(&c, 0, sizeof c);
+    c.n_emitters = f.emitters.size();
+    c.emitters = f.emitters.empty() ? nullptr : f.emitters.data();   // borrowed: f must outlive the call
+    c.n_positions = (uint32_t)f.topics.size();
+    for (size_t k = 0; k < f.topics.size() && k < 4; k++) {
+        if (f.topics[k].empty()) continue;
+        keep.emplace_back();
+        for (const H256& v : f.topics[k]) keep.back().insert(keep.back().end(), v.begin(), v.end());
+        c.n_values[k] = f.topics[k].size();
+        c.values[k] = keep.back().data();
+    }
+    return c;
+}
 inline ipcfp_event_spec spec_c(const std::string& sig, const std::string& topic_1, const std::optional<uint64_t>& filter) {
     ipcfp_event_spec s;
     memset(&s, 0, sizeof s);
@@ -469,6 +490,25 @@ inline EventProofBundle generate_event_proof(GpuBlockstore& store, const ApiTips
     ipcfp_event_spec spec = spec_c(event_signature, topic_1, actor_id_filter);
     ipcfp_event_result* r = nullptr;
     check(ipcfp_generate_event_proof(store.raw(), t.c(), &spec, 0, &r), "generate_event_proof");
+    EventProofBundle b;
+    try {
+        b.proofs = event_proofs(*r, t);
+        b.blocks = proof_blocks(r->witness);
+    } catch (...) { ipcfp_event_result_free(r); throw; }
+    ipcfp_event_result_free(r);
+    return b;
+}
+
+// generate_event_proof with a log filter as the predicate: one EventProofBundle (ipcfp_generate_log_proof). More than four topic
+// positions is refused like any other invalid filter.
+inline EventProofBundle generate_log_proof(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                           const LogFilter& filter) {
+    if (filter.topics.size() > 4) throw Error(IPCFP_ERR_INVALID_ARG, "generate_log_proof: more than four topic positions");
+    TipsetDesc t(parent, child, receipts);
+    std::vector<std::vector<uint8_t>> keep;
+    const ipcfp_log_filter f = log_filter_c(filter, keep);
+    ipcfp_event_result* r = nullptr;
+    check(ipcfp_generate_log_proof(store.raw(), t.c(), &f, 0, &r), "generate_log_proof");
     EventProofBundle b;
     try {
         b.proofs = event_proofs(*r, t);

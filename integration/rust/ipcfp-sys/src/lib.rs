@@ -46,6 +46,11 @@ pub struct ipcfp_tipset_desc {
 }
 #[repr(C)]
 pub struct ipcfp_event_spec { pub event_signature: *const c_char, pub topic_1: *const c_char, pub has_actor_id_filter: u8, pub actor_id_filter: u64 }
+pub const IPCFP_LOG_FILTER_MAX_VALUES: u32 = 65536;
+pub const IPCFP_LOG_FILTER_MAX_EMITTERS: u32 = 65536;
+#[repr(C)]
+pub struct ipcfp_log_filter { pub n_emitters: u64, pub emitters: *const u64, pub n_positions: u32, pub _pad: u32, pub n_values: [u64; 4],
+                              pub values: [*const u8; 4] }
 #[repr(C)]
 pub struct ipcfp_storage_spec { pub actor_id: u64, pub slot: [u8; 32] }
 #[repr(C)]
@@ -154,6 +159,10 @@ extern "C" {
                                        device: c_int, flags: u32, out: *mut *mut ipcfp_store, info: *mut ipcfp_store_json_info) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, spec: *const ipcfp_event_spec, flags: u32,
                                                out: *mut *mut ipcfp_event_result) -> ipcfp_status;
+    pub fn ipcfp_generate_log_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, filter: *const ipcfp_log_filter, flags: u32,
+                                             out: *mut *mut ipcfp_event_result) -> ipcfp_status;
+    pub fn ipcfp_generate_log_proof(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, filter: *const ipcfp_log_filter, flags: u32,
+                                    out: *mut *mut ipcfp_event_result) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_shard(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, spec: *const ipcfp_event_spec, lo: u64, hi: u64,
                                             world_size: u32, rank: u32, flags: u32, out: *mut *mut ipcfp_event_result) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_shard_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, spec: *const ipcfp_event_spec, lo: u64, hi: u64,
@@ -173,6 +182,8 @@ extern "C" {
                                      especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_plan_fetch(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                             especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_plan_fetch_log_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, filter: *const ipcfp_log_filter, flags: u32,
+                                         out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_fetch_plan_free(p: *mut ipcfp_fetch_plan);
     pub fn ipcfp_fetch_plan_to_rpc_json(p: *const ipcfp_fetch_plan, first_id: u64, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_resolve_addresses(s: *mut ipcfp_store, state_root: *const u8, addrs: *const ipcfp_address, n: u64,
@@ -188,6 +199,8 @@ extern "C" {
     pub fn ipcfp_parsed_bundle_free(b: *mut ipcfp_parsed_bundle);
     pub fn ipcfp_verify_event_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_event_proof, n_proofs: u64,
                                      data_blob: *const u8, data_blob_size: u64, filter: *const ipcfp_event_spec, results: *mut u8) -> ipcfp_status;
+    pub fn ipcfp_verify_event_proofs_log(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_event_proof, n_proofs: u64,
+                                         data_blob: *const u8, data_blob_size: u64, filter: *const ipcfp_log_filter, results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_storage_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_storage_proof, n_proofs: u64,
                                        results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_bundle_json(json: *const c_char, len: u64, device: c_int, trusted_parent: ipcfp_trusted_parent_ts_fn,

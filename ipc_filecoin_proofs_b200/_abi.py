@@ -57,6 +57,22 @@ class EventSpec(C.Structure):
     ]
 
 
+LOG_FILTER_MAX_VALUES = 65536
+LOG_FILTER_MAX_EMITTERS = 65536
+
+
+class LogFilterC(C.Structure):
+    """ipcfp_log_filter"""
+    _fields_ = [
+        ("n_emitters", C.c_uint64),
+        ("emitters", C.c_void_p),
+        ("n_positions", C.c_uint32),
+        ("_pad", C.c_uint32),
+        ("n_values", C.c_uint64 * 4),
+        ("values", C.c_void_p * 4),
+    ]
+
+
 class StorageSpec(C.Structure):
     _fields_ = [("actor_id", C.c_uint64), ("slot", C.c_uint8 * 32)]
 

@@ -48,6 +48,7 @@ EXPORTS = [
     "ipcfp_tipset_describe", "ipcfp_blocks_from_rpc_json", "ipcfp_parsed_blocks_free", "ipcfp_store_create_rpc_json",
     "ipcfp_plan_fetch_resident", "ipcfp_plan_fetch", "ipcfp_fetch_plan_free", "ipcfp_fetch_plan_to_rpc_json",
     "ipcfp_resolve_addresses", "ipcfp_resolve_result_free", "ipcfp_address_parse", "ipcfp_address_from_eth",
+    "ipcfp_generate_log_proof", "ipcfp_generate_log_proof_resident", "ipcfp_plan_fetch_log_resident", "ipcfp_verify_event_proofs_log",
 ]
 
 
@@ -125,6 +126,17 @@ def lib():
                                                          C.POINTER(C.POINTER(A.EventResultC))]
         L.ipcfp_verify_event_proofs.restype = C.c_int32
         L.ipcfp_verify_event_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+        L.ipcfp_generate_log_proof.restype = C.c_int32
+        L.ipcfp_generate_log_proof.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(A.LogFilterC), C.c_uint32,
+                                               C.POINTER(C.POINTER(A.EventResultC))]
+        L.ipcfp_generate_log_proof_resident.restype = C.c_int32
+        L.ipcfp_generate_log_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32,
+                                                        C.POINTER(C.POINTER(A.EventResultC))]
+        L.ipcfp_plan_fetch_log_resident.restype = C.c_int32
+        L.ipcfp_plan_fetch_log_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32, C.POINTER(C.POINTER(A.FetchPlanC))]
+        L.ipcfp_verify_event_proofs_log.restype = C.c_int32
+        L.ipcfp_verify_event_proofs_log.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                                    C.POINTER(A.LogFilterC), C.c_void_p]
         L.ipcfp_verify_storage_proofs.restype = C.c_int32
         L.ipcfp_verify_storage_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p]
         for name in ("ipcfp_bundle_to_json", "ipcfp_event_result_to_json"):
@@ -199,6 +211,70 @@ class EventProofSpec:  # reference src/proofs/generator.rs:18-22
 
     def as_c(self):
         return A.make_event_spec(self.event_signature, self.topic_1, self.actor_id_filter)
+
+
+def _topic32(v):
+    if isinstance(v, str):
+        v = bytes.fromhex(v[2:] if v[:2] in ("0x", "0X") else v)
+    v = bytes(v)
+    if len(v) != 32:
+        raise ValueError(f"a topic value is 32 bytes, got {len(v)}")
+    return v
+
+
+class LogFilter:
+    """An eth_getLogs-style log filter (ipcfp_log_filter): `emitters` — None / [] for any emitter, else actor IDs (resolve Ethereum
+    addresses first with resolve_eth_address_to_actor_id); `topics` — one entry per position, each None (any value), a 32-byte value
+    (bytes or hex) or a list of them (an empty list is a wildcard, as None). An event matches when extract_evm_log accepts it, its emitter is in the set, it has at least
+    len(topics) topics and topic k is in topics[k] wherever that is not None. Trailing None entries count towards the topic minimum,
+    as in go-ethereum's filterLogs."""
+
+    def __init__(self, emitters=None, topics=()):
+        topics = list(topics)
+        if len(topics) > 4:
+            raise ValueError("a log filter has at most 4 topic positions")
+        self.emitters = [int(e) for e in (emitters or [])]
+        self.topics = []
+        for t in topics:
+            if t is None or (isinstance(t, (list, tuple)) and not t):   # None or an empty list: any value (go-ethereum's rule)
+                self.topics.append(None)
+            elif isinstance(t, (bytes, bytearray, str)):
+                self.topics.append([_topic32(t)])
+            else:
+                self.topics.append([_topic32(v) for v in t])
+
+    @classmethod
+    def from_spec(cls, spec, device=0):
+        """The filter an EventProofSpec stands for: topic 0 = keccak256(signature) (hashed on `device`), topic 1 =
+        ascii_to_bytes32(topic_1), at least two topics, the actor (if any) as the only emitter."""
+        t1 = spec.topic_1.encode()[:32]
+        t0 = bytes(keccak256_batch([spec.event_signature.encode()], device)[0])
+        return cls(None if spec.actor_id_filter is None else [spec.actor_id_filter], [t0, t1 + bytes(32 - len(t1))])
+
+    def as_c(self):
+        """(ipcfp_log_filter, keepalive)"""
+        f = A.LogFilterC()
+        keep = []
+        em = np.ascontiguousarray(self.emitters, dtype=np.uint64)
+        keep.append(em)
+        f.n_emitters = len(em)
+        f.emitters = em.ctypes.data if em.size else None
+        f.n_positions = len(self.topics)
+        for k, vals in enumerate(self.topics):
+            if vals:
+                a = np.frombuffer(b"".join(vals), dtype=np.uint8).copy()
+                keep.append(a)
+                f.n_values[k] = len(vals)
+                f.values[k] = a.ctypes.data
+        return f, keep
+
+    def matches(self, emitter, topics):
+        """The predicate on one extracted log (emitter, list of 32-byte topics)."""
+        if self.emitters and emitter not in self.emitters:
+            return False
+        if len(topics) < len(self.topics):
+            return False
+        return all(vals is None or bytes(topics[k]) in vals for k, vals in enumerate(self.topics))
 
 
 @dataclass
@@ -310,6 +386,28 @@ class BlockStore:
         finally:
             lib().ipcfp_event_result_free(out)
 
+    def generate_log_proof(self, ts, log_filter, flags=0):
+        """ipcfp_generate_log_proof: generate_event_proof with a LogFilter as the predicate → A.EventResultPy."""
+        d, keep = A.make_tipset_desc(ts)
+        f, fkeep = log_filter.as_c()
+        out = C.POINTER(A.EventResultC)()
+        _check(lib().ipcfp_generate_log_proof(self._h, C.byref(d), C.byref(f), flags, C.byref(out)))
+        try:
+            return A.event_result_from_c(out.contents)
+        finally:
+            lib().ipcfp_event_result_free(out)
+
+    def generate_log_proof_resident(self, tip, log_filter, flags=0):
+        """ipcfp_generate_log_proof_resident against a ResidentTipset of this store. flags: WITNESS_BY_REFERENCE, RESULT_JSON,
+        SCAN_SKIP_TX_AMTS."""
+        f, fkeep = log_filter.as_c()
+        out = C.POINTER(A.EventResultC)()
+        _check(lib().ipcfp_generate_log_proof_resident(self._h, tip._h, C.byref(f), flags, C.byref(out)))
+        try:
+            return A.event_result_from_c(out.contents)
+        finally:
+            lib().ipcfp_event_result_free(out)
+
     def generate_event_proof_shard(self, ts, spec, lo, hi, world, rank, flags=0):
         d, keep = A.make_tipset_desc(ts)
         cs = spec.as_c() if isinstance(spec, EventProofSpec) else spec
@@ -389,6 +487,16 @@ class BlockStore:
         sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
         out = C.POINTER(A.FetchPlanC)()
         _check(lib().ipcfp_plan_fetch_resident(self._h, tip._h, sarr, ns, earr, ne, flags, C.byref(out)))
+        try:
+            return A.fetch_plan_from_c(out.contents)
+        finally:
+            lib().ipcfp_fetch_plan_free(out)
+
+    def plan_fetch_logs(self, tip, log_filter, flags=0):
+        """ipcfp_plan_fetch_log_resident → A.FetchPlanPy: one fetch round for generate_log_proof_resident(tip, log_filter)."""
+        f, fkeep = log_filter.as_c()
+        out = C.POINTER(A.FetchPlanC)()
+        _check(lib().ipcfp_plan_fetch_log_resident(self._h, tip._h, C.byref(f), flags, C.byref(out)))
         try:
             return A.fetch_plan_from_c(out.contents)
         finally:
@@ -728,7 +836,8 @@ def verify_bundle_json(text, trusted_parent=None, trusted_child=None, filter_spe
 
 def verify_event_proofs(witness, ts, result, filter_spec=None, device=0):
     """verify_event_proof (events/verifier.rs:51-74) batched on the GPU: the witness (WitnessPy) becomes a store with every block
-    Blake2b-checked against its CID, then every proof of `result` (EventResultPy) is replayed. → list of bools."""
+    Blake2b-checked against its CID, then every proof of `result` (EventResultPy) is replayed. filter_spec (check_event): None, an
+    EventProofSpec or a LogFilter (ipcfp_verify_event_proofs_log). → list of bools."""
     store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
     try:
         d, keep = A.make_tipset_desc(ts)
@@ -736,6 +845,11 @@ def verify_event_proofs(witness, ts, result, filter_spec=None, device=0):
         res = np.zeros(max(n, 1), dtype=np.uint8)
         raw = np.ascontiguousarray(result.raw_proofs)
         blob = np.ascontiguousarray(result.data_blob)
+        if isinstance(filter_spec, LogFilter):
+            f, fkeep = filter_spec.as_c()
+            _check(lib().ipcfp_verify_event_proofs_log(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None,
+                                                       blob.size, C.byref(f), res.ctypes.data))
+            return [bool(x) for x in res[:n]]
         fs = filter_spec.as_c() if isinstance(filter_spec, EventProofSpec) else filter_spec
         _check(lib().ipcfp_verify_event_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None, blob.size,
                                                C.addressof(fs) if fs is not None else None, res.ctypes.data))

@@ -285,6 +285,25 @@ ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tip
         *out = generate_event_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), spec, flags, true, lo, hi);
     });
 }
+ipcfp_status ipcfp_generate_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
+                                               ipcfp_event_result** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = generate_log_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), filter, flags);
+    });
+}
+ipcfp_status ipcfp_generate_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_log_filter* filter, uint32_t flags,
+                                      ipcfp_event_result** out) {
+    return guard([&] {
+        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        Store* st = reinterpret_cast<Store*>(s);
+        TipsetDev td;
+        tipset_upload(st, t, td);
+        *out = generate_log_proof(st, td, filter, flags);
+    });
+}
 void* ipcfp_store_stream(ipcfp_store* s) { return s ? (void*)reinterpret_cast<Store*>(s)->stream : nullptr; }
 
 ipcfp_status ipcfp_read_storage_slots(ipcfp_store* s, const uint8_t root[IPCFP_CID_LEN], const uint8_t* slots, uint64_t k, ipcfp_slot_result** out) {
@@ -356,6 +375,17 @@ ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const 
         *out = &box.release()->r;
     });
 }
+ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags, ipcfp_fetch_plan** out) {
+    return guard([&] {
+        if (!s || !t || !out || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+        plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), nullptr, 0, nullptr, 0, box->plan, filter);
+        box->fill();
+        *out = &box.release()->r;
+    });
+}
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }
 
 struct ResolveBox {
@@ -402,6 +432,13 @@ ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* 
     return guard([&] {
         if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, filter, results);
+    });
+}
+ipcfp_status ipcfp_verify_event_proofs_log(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
+                                           uint64_t blob_size, const ipcfp_log_filter* filter, uint8_t* results) {
+    return guard([&] {
+        if (!s || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filter);
     });
 }
 ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results) {

@@ -205,13 +205,15 @@ struct ExecOrderOut {
 };
 ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
                                          Comm* comm = nullptr, ExecOrderOut* exo = nullptr);
-// verify.cu — batched verifiers over a witness store
+// ipcfp_generate_log_proof_resident: the same call with a log filter as the predicate
+ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags);
+// verify.cu — batched verifiers over a witness store; log_filter (if not null) is check_event in place of `filter`
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
-                         const ipcfp_event_spec* filter, uint8_t* results);
+                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter = nullptr);
 void verify_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results);
 // … the same with the proofs (and the data blob, padded by 16 bytes) already in device memory
 void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
-                             const ipcfp_event_spec* filter, uint8_t* results);
+                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter = nullptr);
 void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* d_proofs, uint64_t n, uint8_t* results);
 // json_parse.cu — ipcfp_verify_bundle_json
 ipcfp_bundle_verdict* verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
@@ -227,8 +229,9 @@ struct FetchPlan {
     uint32_t n_levels = 0;
     float ms_total = 0.f;
 };
+// log_filter (if not null, with no specs): rule 3's predicate in place of the event specs'
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out);
+                FetchPlan& out, const ipcfp_log_filter* log_filter = nullptr);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);

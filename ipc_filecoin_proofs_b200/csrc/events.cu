@@ -19,6 +19,7 @@
 #include <chrono>
 #include <cstddef>
 #include <optional>
+#include <type_traits>
 #include <cooperative_groups.h>
 #include "engine.cuh"
 #include "hashes.cuh"
@@ -40,7 +41,8 @@ namespace cg = cooperative_groups;
 // chain serialised by divergence: ≈ 1 000 matches in 8 CTAs keep 8 of the GPU's 132 SMs busy. One warp per match is the shape
 // k_read_slots uses for the same reason (storage.cu); above 16 384 matches the grid fills the machine either way and one match per
 // thread is kept. Same per-item code, so results are identical by construction.
-__global__ void __launch_bounds__(128) k_pass2(Pass2Args a) {
+template <class P>
+__global__ void __launch_bounds__(128) k_pass2(Pass2ArgsT<P> a) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a.per_warp) { if (threadIdx.x & 31) return; t >>= 5; }
     if (t >= a.n_match) return;
@@ -79,7 +81,7 @@ struct SetupArgs {
     unsigned long long* f_count;
     const uint8_t* sig;     // event signature bytes (zero padded to a multiple of 8) and the Matcher whose t0 this kernel fills
     uint32_t sig_len;
-    Matcher* matcher;
+    Matcher* matcher;       // null for a log filter: nothing to hash
     // plan_dense: also plan the dense walk (unsharded calls) into pro->plan, against these limits
     uint32_t plan_dense;
     uint64_t frontier_cap, max_raw;
@@ -125,7 +127,7 @@ __global__ void __launch_bounds__(256) k_setup(SetupArgs a) {
             if (b < 0) a.pro->misc[1] = 1; else witness_mark(s, a.wbits, (uint32_t)b);
         }
     }
-    if (t == 96) {
+    if (t == 96 && a.matcher) {   // a log filter's values arrive raw
         Digest d;
         keccak256(a.sig, a.sig_len, d);
         for (int k = 0; k < 4; k++) a.matcher->t0[k] = a.pro->t0[k] = d.w[k];
@@ -469,11 +471,15 @@ static constexpr size_t STAGE_TABLES = 32768;   // second half of the store's st
 //   execution-order only: walk, snapshot_and_sync, then dedup reads n_exec back and the call ends
 //   sharded over NCCL: besides, every H0 / H2 gather, ShardExchange::agree_results and finish, a late H0 that fails, and fill's copy of
 //                     the union partition (IPCFP_SHARDED_UNION_TO_HOST)
+// P: the predicate. Matcher: `spec` is the call's EventProofSpec (t0 = keccak256(signature) is computed by k_setup). LogFilter: `filter`
+// is a log filter (unsharded calls only), its values raw, its large sets uploaded beside it.
+template <class P>
 struct EventCall {
     Store* s;
     cudaStream_t st;
     TipsetDev& td;
     const ipcfp_event_spec* spec;
+    const ipcfp_log_filter* filter = nullptr;
     uint32_t flags;
     bool sharded;
     uint64_t lo, hi;
@@ -487,11 +493,13 @@ struct EventCall {
     unsigned long long* dw;
     uint64_t* hw;
     // stage
-    Matcher mh;
+    P mh;
     size_t siglen = 0, tables_off = 0;
     AsyncBuf<uint8_t> small;
     uint8_t *d_sig = nullptr, *d_cids = nullptr;
-    Matcher* d_matcher = nullptr;
+    P* d_matcher = nullptr;
+    AsyncBuf<uint64_t> d_sets;   // LogFilter: the large sets and their bitmaps, and their pinned host copy
+    PinnedArray sets_h;
     // setup
     AsyncBuf<uint32_t> wbits;
     uint32_t namt = 0;
@@ -559,7 +567,7 @@ struct EventCall {
     void publish_prologue() { publish_words(s, HW_PROLOGUE, PRO_HEAD_WORDS, pro.p); }
     void read_prologue() {   // the fault words as the prologue left them, and its head
         early_fault = hw[DW_ERR] != IPCFP_NO_ERROR || hw[DW_TX_ERR] != IPCFP_NO_ERROR;
-        memcpy(mh.t0, ph->t0, 32);
+        if constexpr (std::is_same_v<P, Matcher>) memcpy(mh.t0, ph->t0, 32);
         receipts_root_blk = ph->misc[0];
         missing_base = ph->misc[1] != 0;
         last_round = 0;
@@ -574,7 +582,12 @@ struct EventCall {
     void stage() {
         s->use();
         t_enter = std::chrono::steady_clock::now();
-        if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+        LogFilterHost lfh;
+        if constexpr (std::is_same_v<P, Matcher>) {
+            if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+        } else {
+            log_filter_build(filter, lfh);
+        }
         // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
         if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
         if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !s->caller_blob)
@@ -596,7 +609,7 @@ struct EventCall {
         IPCFP_CUDA(cudaMemsetAsync(dw + DW_TX_ERR, 0xff, 8, st));
 
         memset(&mh, 0, sizeof mh);
-        {
+        if constexpr (std::is_same_v<P, Matcher>) {
             size_t n1 = strlen(spec->topic_1);
             uint8_t t1[32];
             memset(t1, 0, 32);
@@ -604,23 +617,32 @@ struct EventCall {
             memcpy(mh.t1, t1, 32);
             mh.actor = spec->actor_id_filter;
             mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
+            siglen = strlen(spec->event_signature);
+        } else {
+            if (!lfh.dev.empty()) {   // through pinned memory that lives as long as the call: no host synchronisation
+                sets_h = PinnedArray(s->pool, lfh.dev.size() * 8);
+                memcpy(sets_h.p, lfh.dev.data(), lfh.dev.size() * 8);
+                d_sets.alloc(lfh.dev.size(), st);
+                IPCFP_CUDA(cudaMemcpyAsync(d_sets.p, sets_h.p, lfh.dev.size() * 8, cudaMemcpyHostToDevice, st));
+            }
+            lfh.place(d_sets.p);
+            mh = lfh.f;
         }
-        //   [0,1024) Matcher (t0 is filled in on the device) | signature, zero padded | parent, TxMeta, child, receipts-root CIDs
-        siglen = strlen(spec->event_signature);
+        //   [0,1024) Matcher (t0 is filled in on the device) or LogFilter | signature, zero padded | parent, TxMeta, child, receipts-root CIDs
         const size_t sig_cap = (siglen + 64) & ~(size_t)63;
         const size_t cids_bytes = 38ull * (2 * td.n_parents + 2);
         const size_t small_bytes = 1024 + sig_cap + cids_bytes + 64;
-        static_assert(sizeof(Matcher) <= 1024, "Matcher must fit its staging slot");
+        static_assert(sizeof(P) <= 1024, "the predicate must fit its staging slot");
         tables_off = std::max<size_t>(STAGE_TABLES, (small_bytes + 63) & ~(size_t)63);
         if (!s->stage.p || s->stage.cap < tables_off + STAGE_TABLES) s->stage = PinnedArray(s->pool, tables_off + STAGE_TABLES);
         small.alloc(small_bytes, st);
         d_sig = small.p + 1024;                       // 8-byte aligned
         d_cids = small.p + 1024 + sig_cap;
-        d_matcher = (Matcher*)small.p;
+        d_matcher = (P*)small.p;
         uint8_t* hs = s->stage.as<uint8_t>();
         memset(hs, 0, small_bytes);
-        memcpy(hs, &mh, sizeof(Matcher));
-        memcpy(hs + 1024, spec->event_signature, siglen);
+        memcpy(hs, &mh, sizeof(P));
+        if (siglen) memcpy(hs + 1024, spec->event_signature, siglen);
         uint8_t* hc = hs + 1024 + sig_cap;
         memcpy(hc, td.parent_cids.data(), td.parent_cids.size()); hc += td.parent_cids.size();
         memcpy(hc, td.txmeta_cids.data(), td.txmeta_cids.size()); hc += td.txmeta_cids.size();
@@ -655,7 +677,8 @@ struct EventCall {
         sa.skip_tx = skip_tx; sa.skip_receipts = exo ? 1 : 0; sa.wbits = wbits.p; sa.err = dw + DW_ERR; sa.txerr = dw + DW_TX_ERR;
         sa.pro = pro.p;
         sa.f_blk = fA_blk.p; sa.f_meta = fA_meta.p; sa.f_base = fA_base.p; sa.f_count = dw + DW_FRONTIER_A;
-        sa.sig = d_sig; sa.sig_len = (uint32_t)siglen; sa.matcher = d_matcher;
+        sa.sig = d_sig; sa.sig_len = (uint32_t)siglen;
+        if constexpr (std::is_same_v<P, Matcher>) sa.matcher = d_matcher; else sa.matcher = nullptr;
         sa.plan_dense = plan_on_device ? 1 : 0; sa.frontier_cap = frontier_cap; sa.max_raw = max_raw_dev;
         k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_SETUP], st));
@@ -902,14 +925,14 @@ struct EventCall {
     void pass1() {
         match_bits.alloc((N + 31) / 32 + 8, st); cnt.alloc(N + 8, st); nby.alloc(N + 8, st);
         pbase.alloc(N + 8, st); bbase.alloc(N + 8, st);
-        Pass1Args p1;
+        Pass1ArgsT<P> p1;
         p1.store = s->view; p1.store_dev = s->view_dev.p; p1.m_dev = d_matcher; p1.m = mh; p1.events_roots = td.events_roots.p; p1.has_root = td.has_root.p; p1.lo = lo; p1.hi = hi;
         p1.match_bits = match_bits.p; p1.cnt = cnt.p; p1.nbytes = nby.p; p1.err = dw + DW_ERR; p1.stats = dw + DW_STATS;
         if (N) {
             // 4 warps per CTA, 3 CTAs per SM; every lane has a ring of 4 chunks of 128 bytes, one chunk filled per pass (pass1_stage.cuh)
             const int smem = 4 * StageGeom<128, 4, 1>::WARP_BYTES;
-            IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            k_pass1_stage<128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
+            IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<P, 128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            k_pass1_stage<P, 128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
         }
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS1], st));
         match_rel.alloc(N + 32, st);
@@ -933,7 +956,7 @@ struct EventCall {
         d_proofs.alloc(n_proofs + 1, st);
         d_blob.alloc(n_bytes + 16, st);
         if (M) {
-            Pass2Args p2;
+            Pass2ArgsT<P> p2;
             p2.store = s->view; p2.store_dev = s->view_dev.p; p2.m_dev = d_matcher; p2.m = mh; p2.events_roots = td.events_roots.p; p2.lo = lo; p2.match_rel = match_rel.p; p2.n_match = M;
             p2.receipts_root_blk = receipts_root_blk; p2.exec_cids = exec_raw.p; p2.exec_idx = exec_idx.p; p2.n_exec = n_exec_dev;
             p2.wbits = wbits.p; p2.err = dw + DW_ERR; p2.cnt = cnt.p; p2.proof_base = pbase.p; p2.byte_base = bbase.p;
@@ -1052,12 +1075,27 @@ struct EventCall {
 
 ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
                                          Comm* comm, ExecOrderOut* exo) {
-    EventCall c(s, td, spec, flags, sharded, lo, hi, comm, exo);
+    EventCall<Matcher> c(s, td, spec, flags, sharded, lo, hi, comm, exo);
     c.stage();
     c.setup();
     c.walk();
     c.settle_walk();
     if (!c.dedup()) return nullptr;
+    c.pass1();
+    c.pass2();
+    c.read_back();
+    return c.fill();
+}
+
+// the same call with a log filter as the predicate (unsharded)
+ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags) {
+    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr, nullptr);
+    c.filter = filter;
+    c.stage();
+    c.setup();
+    c.walk();
+    c.settle_walk();
+    c.dedup();
     c.pass1();
     c.pass2();
     c.read_back();

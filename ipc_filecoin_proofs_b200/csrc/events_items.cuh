@@ -3,6 +3,7 @@
 // events.cu; they live in a header so that tests/host_fuzz can run the very same code on the CPU against the oracle.
 #pragma once
 #include "ipld.cuh"
+#include "log_filter.cuh"
 #include "rawcid.cuh"
 
 namespace ipcfp {
@@ -47,8 +48,9 @@ __device__ __forceinline__ void emit_proof(const uint8_t* p, const EvLog& ev, ui
 
 // Decodes the values of one events-AMT node. Returns false on a decode error (r.err set).
 // PREFETCH: an L2 prefetch 2 lines ahead of the dependent walk before every event (off in the staged pass 1's arena fallback).
-template <int MODE, bool PREFETCH = true>
-__device__ __forceinline__ void node_events(Rd& r, const uint8_t* p, const AmtNodeHdr& h, uint32_t nv, uint64_t base, const Matcher& m,
+// P: the predicate (Matcher for a spec, LogFilter for a log filter; event_matches of either).
+template <int MODE, bool PREFETCH = true, class P>
+__device__ __forceinline__ void node_events(Rd& r, const uint8_t* p, const AmtNodeHdr& h, uint32_t nv, uint64_t base, const P& m,
                                             WalkOut& wo, EmitCtx* ec) {
     for (uint32_t v = 0; v < nv && !r.err; v++) {
         if (PREFETCH && r.pos + 256 < r.n) prefetch_l2(r.p + r.pos + 256);
@@ -69,12 +71,15 @@ __device__ __forceinline__ void node_events(Rd& r, const uint8_t* p, const AmtNo
 
 // Full in-order walk of Amt<StampedEvent> (v3) rooted at block root_blk — `for_each` of
 // fvm_ipld_amt [UPSTREAM]: every reachable node is loaded through the store (and recorded when
-// wbits != nullptr). Returns 0 ok, else DevCode; detail in *detail.
-template <int MODE>
-static __device__ __noinline__ uint32_t walk_events(const StoreView* sp, uint32_t root_blk, const Matcher* mp, uint32_t* wbits, WalkOut& wo, EmitCtx* ec,
+// wbits != nullptr). Returns 0 ok, else DevCode; detail in *detail. A Matcher is copied into registers; a LogFilter, whose inline
+// sets are indexed per value, is read where it lies.
+template <class P> struct PredLocal { using T = const P&; };
+template <> struct PredLocal<Matcher> { using T = const Matcher; };
+template <int MODE, class P>
+static __device__ __noinline__ uint32_t walk_events(const StoreView* sp, uint32_t root_blk, const P* mp, uint32_t* wbits, WalkOut& wo, EmitCtx* ec,
                                 uint32_t* detail) {
     const StoreView& s = *sp;
-    const Matcher m = *mp;
+    typename PredLocal<P>::T m = *mp;
     struct Frame { uint32_t blk; uint32_t k; uint64_t base; };
     Frame stk[66];
     int depth = 0;
@@ -109,11 +114,11 @@ static __device__ __noinline__ uint32_t walk_events(const StoreView* sp, uint32_
 }
 
 // ------------------------------------------------------------------------------------------ pass 1
-struct Pass1Args {
+template <class P> struct Pass1ArgsT {
     StoreView store;
     const StoreView* store_dev;    // same view in device memory (for the out-of-line walker)
-    const Matcher* m_dev;
-    Matcher m;
+    const P* m_dev;
+    P m;
     const uint8_t* events_roots;
     const uint8_t* has_root;
     uint64_t lo, hi;
@@ -123,6 +128,7 @@ struct Pass1Args {
     unsigned long long* err;
     unsigned long long* stats;     // [0] nodes scanned, [1] bytes scanned
 };
+using Pass1Args = Pass1ArgsT<Matcher>;
 
 // ------------------------------------------------------------------------------------------ receipts AMT
 // Amtv0<Receipt>::get(i) with recording (events/generator.rs:249). 1 = Some, 0 = None, <0 = -DevCode. missing (may be null): on
@@ -162,11 +168,11 @@ static __device__ int receipts_get(const StoreView& s, uint32_t root_blk, uint64
 }
 
 // ------------------------------------------------------------------------------------------ pass 2
-struct Pass2Args {
+template <class P> struct Pass2ArgsT {
     StoreView store;
     const StoreView* store_dev;
-    const Matcher* m_dev;
-    Matcher m;
+    const P* m_dev;
+    P m;
     const uint8_t* events_roots;
     uint64_t lo;
     const uint32_t* match_rel;     // positions relative to lo, ascending
@@ -187,11 +193,13 @@ struct Pass2Args {
     uint32_t resolve_msg;          // 1: exec.get(i) check + message CID from exec_cids; 0: neither (shard: the execution order spans shards and
                                    // is resolved afterwards — by the caller, or by the in-library protocol with k_check_exec)
 };
+using Pass2Args = Pass2ArgsT<Matcher>;
 
 // One thread per matching receipt (events/generator.rs:242-301): exec.get(i), r_amt.get(i) with path
 // recording, full in-order walk of its events AMT with recording, EventProof emission at the
 // offsets pass 1 already counted.
-__device__ __forceinline__ void pass2_item(const Pass2Args& a, uint64_t t) {
+template <class P>
+__device__ __forceinline__ void pass2_item(const Pass2ArgsT<P>& a, uint64_t t) {
     uint32_t rel = a.match_rel[t];
     uint64_t i = a.lo + rel;
     // exec.get(i) comes first (:244-246)

@@ -17,6 +17,7 @@
 // events_items.cuh, so results are identical by construction; tests/host_fuzz/emu_stage.cu runs this very code on the CPU (with the
 // asynchronous copies modelled adversarially) against the arena path.
 #pragma once
+#include <type_traits>
 #include "events_items.cuh"
 
 namespace ipcfp {
@@ -71,6 +72,31 @@ template <class GEO> struct StageWin {
         return a == w[2] && b == w[3];
     }
 };
+
+// event_matches for a log filter on an event the fast path decoded from the ring: hit, or have = false when the topic of a constrained
+// position is not resident yet (the residency check of the spec's topics 0 and 1, StageLane::step, over every constrained position)
+template <class GEO> __device__ __forceinline__ void stage_match(StageWin<GEO>& win, uint32_t skew, const EvLog& ev, const LogFilter& f, bool& have, bool& hit) {
+    if (!lf_candidate(f, ev)) return;
+    uint32_t hi_off = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        const uint32_t o = topic_offset(ev, k) + 32 + 8;
+        if (k < f.npos && f.nv[k] && o > hi_off) hi_off = o;
+    }
+    if (skew + hi_off > win.resident_end) { have = false; return; }
+    bool ok = true;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        if (ok && k < f.npos && f.nv[k]) {
+            const uint32_t o = topic_offset(ev, k);
+            uint64_t w[4];
+            win.load(o, w[0], w[1]);
+            win.load(o + 16, w[2], w[3]);
+            ok = lf_value_ok(f, k, w);
+        }
+    }
+    hit = ok;
+}
 
 // per-lane state of the staged scan (registers on the device)
 template <class GEO> struct StageLane {
@@ -130,7 +156,7 @@ template <class GEO> struct StageLane {
         taken = !((nv && height != 0) || pc != nv || cur != len);
     }
     // one parse step: at most one event
-    __device__ __forceinline__ void step(const Matcher& m) {
+    template <class P> __device__ __forceinline__ void step(const P& m) {
         if (state == 1) {
             const uint32_t need = skew + (len < 64 ? len : 64);   // every byte begin() may look at
             if (landed * GEO::CH < need && landed < nchunks) return;   // header bytes not there yet
@@ -145,11 +171,15 @@ template <class GEO> struct StageLane {
         bool hit = false, have = false;
         if (!win.shortfall && nx != FAST_FAIL) {
             have = true;
-            if ((!m.has_actor || ev.emitter == m.actor) && ev.some && ev.ntopics >= 2) {   // event_matches, topic bytes from the ring
-                const uint32_t o0 = ev.toff[0], o1 = ev.case_a ? ev.toff[0] + 32 : ev.toff[1];
-                const uint32_t hi_off = (o0 > o1 ? o0 : o1) + 32 + 8;                      // + the window's over-read
-                if (skew + hi_off > win.resident_end) have = false;
-                else hit = win.eq32(o0, m.t0) && win.eq32(o1, m.t1);
+            if constexpr (std::is_same_v<P, Matcher>) {
+                if ((!m.has_actor || ev.emitter == m.actor) && ev.some && ev.ntopics >= 2) {   // event_matches, topic bytes from the ring
+                    const uint32_t o0 = ev.toff[0], o1 = ev.case_a ? ev.toff[0] + 32 : ev.toff[1];
+                    const uint32_t hi_off = (o0 > o1 ? o0 : o1) + 32 + 8;                      // + the window's over-read
+                    if (skew + hi_off > win.resident_end) have = false;
+                    else hit = win.eq32(o0, m.t0) && win.eq32(o1, m.t1);
+                }
+            } else {
+                stage_match(win, skew, ev, m, have, hit);
             }
         }
         if (!have) {
@@ -201,8 +231,8 @@ __device__ __forceinline__ void cp_async16(uint8_t* dst_smem, const uint8_t* src
 #endif
 
 // W warps per CTA, each with its own rings; no CTA-wide synchronisation anywhere.
-template <int CH, int NSLOT, int CPP, int W, int MINB>
-__global__ void __launch_bounds__(32 * W, MINB) k_pass1_stage(Pass1Args a) {
+template <class P, int CH, int NSLOT, int CPP, int W, int MINB>
+__global__ void __launch_bounds__(32 * W, MINB) k_pass1_stage(Pass1ArgsT<P> a) {
 #ifdef __CUDA_ARCH__
     using GEO = StageGeom<CH, NSLOT, CPP>;
     extern __shared__ __align__(16) uint8_t stage_smem[];

@@ -77,8 +77,9 @@ __global__ void k_plan_matchers(const uint8_t* sig, const uint64_t* sig_off, con
     }
 }
 
+template <class P>
 __global__ void __launch_bounds__(128) k_plan_match(StoreView s, const StoreView* s_dev, const uint8_t* __restrict__ roots, const uint8_t* __restrict__ has,
-                                                    uint64_t n, const Matcher* m, uint64_t n_specs, const uint8_t* receipts_root, uint32_t* needed,
+                                                    uint64_t n, const P* m, uint64_t n_specs, const uint8_t* receipts_root, uint32_t* needed,
                                                     uint8_t* miss, unsigned long long* ctr) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || !has[i]) return;
@@ -103,8 +104,11 @@ __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, 
 }
 
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out) {
+                FetchPlan& out, const ipcfp_log_filter* log_filter) {
     if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
+    LogFilterHost lfh;
+    if (log_filter) log_filter_build(log_filter, lfh);
+    const bool events = n_especs || log_filter;   // the event path's rules (1–3) apply
     if (n_sspecs && !td.has_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
     for (uint64_t k = 0; k < n_especs; k++)
         if (!especs[k].event_signature || !especs[k].topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
@@ -113,14 +117,14 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
     const StoreView& v = s->view;
     const uint64_t nwords = (s->n + 31) / 32 + 1;
-    const uint64_t n_rcpt = n_especs ? td.n_receipts : 0;
+    const uint64_t n_rcpt = events ? td.n_receipts : 0;
 
     // the base roots (collect_base_witness, events/generator.rs:112-145; generate_storage_proof's child header and StateRoot), then every
     // spec's inputs, in one upload
     std::vector<uint8_t> roots;
     std::vector<uint32_t> kinds;
     auto root = [&](const uint8_t* c, uint32_t kind) { roots.insert(roots.end(), c, c + 38); kinds.push_back(kind); };
-    if (n_especs) {
+    if (events) {
         for (uint32_t k = 0; k < td.n_parents; k++) root(td.parent_cids.data() + 38 * k, PK_BLOCK);
         root(td.child_cid, PK_BLOCK);
         root(td.receipts_root, PK_BLOCK);
@@ -157,6 +161,18 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     if (n_sspecs) memcpy(h.data() + o_ss, sspecs, n_sspecs * sizeof(ipcfp_storage_spec));
     AsyncBuf<uint8_t> d(size, st);
     IPCFP_CUDA(cudaMemcpyAsync(d.p, h.data(), size, cudaMemcpyHostToDevice, st));
+    // the log filter and its large sets, in one upload
+    const uint64_t lf_words = (sizeof(LogFilter) + 7) / 8;
+    AsyncBuf<uint64_t> d_lf;
+    std::vector<uint64_t> h_lf;
+    if (log_filter) {
+        d_lf.alloc(lf_words + lfh.dev.size(), st);
+        lfh.place(d_lf.p + lf_words);
+        h_lf.assign(lf_words + lfh.dev.size(), 0);
+        memcpy(h_lf.data(), &lfh.f, sizeof(LogFilter));
+        std::copy(lfh.dev.begin(), lfh.dev.end(), h_lf.begin() + lf_words);
+        IPCFP_CUDA(cudaMemcpyAsync(d_lf.p, h_lf.data(), h_lf.size() * 8, cudaMemcpyHostToDevice, st));
+    }
 
     AsyncBuf<uint32_t> needed(nwords, st), visited(PLAN_CLASSES * nwords, st);
     needed.zero();
@@ -212,11 +228,16 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
 
     // ---- rule 3: the receipts-AMT paths of the matching receipts, once every events-AMT block of N(S) is in the store
     if (n_rcpt && events_complete) {
-        k_plan_matchers<<<1, 32, 0, st>>>(d.p + o_sig, (const uint64_t*)(d.p + o_so), (const uint32_t*)(d.p + o_sl), n_especs, (Matcher*)(d.p + o_m));
-        IPCFP_LAUNCH_CHECK();
         const uint8_t* rr = d.p + o_roots + 38ull * (td.n_parents + 1);
-        k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const Matcher*)(d.p + o_m),
-                                                          n_especs, rr, needed.p, miss.p, ctr.p);
+        if (log_filter) {
+            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const LogFilter*)d_lf.p, 1,
+                                                              rr, needed.p, miss.p, ctr.p);
+        } else {
+            k_plan_matchers<<<1, 32, 0, st>>>(d.p + o_sig, (const uint64_t*)(d.p + o_so), (const uint32_t*)(d.p + o_sl), n_especs, (Matcher*)(d.p + o_m));
+            IPCFP_LAUNCH_CHECK();
+            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const Matcher*)(d.p + o_m),
+                                                              n_especs, rr, needed.p, miss.p, ctr.p);
+        }
         IPCFP_LAUNCH_CHECK();
     }
     // ---- rule 4: the storage paths

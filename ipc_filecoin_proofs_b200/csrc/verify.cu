@@ -30,7 +30,8 @@ __global__ void k_verify_txmeta(StoreView s, const uint8_t* txmeta_cids, uint32_
     verify_txmeta_item(s, txmeta_cids, k, err);
 }
 // one warp per proof, lane 0 walks (see storage.cu for why)
-__global__ void __launch_bounds__(128) k_verify_events(VerifyEventArgs a) {
+template <class F>
+__global__ void __launch_bounds__(128) k_verify_events(VerifyEventArgsT<F> a) {
     const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= a.n || (threadIdx.x & 31)) return;
     verify_event_item(a, t);
@@ -48,25 +49,31 @@ static void throw_verify_error(uint64_t key) {
 }
 
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
-                         const ipcfp_event_spec* filter, uint8_t* results) {
+                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter) {
     s->use();
     if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
     if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
     if (n && (!proofs || !results)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-    if (n == 0) return;
+    if (n == 0) {   // a refused log filter fails whatever the proofs are
+        LogFilterHost lfh;
+        if (log_filter) log_filter_build(log_filter, lfh);
+        return;
+    }
     cudaStream_t st = s->stream;
     AsyncBuf<uint8_t> d_blob(blob_size + 16, st);
     AsyncBuf<ipcfp_event_proof> d_proofs(n, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_event_proof), cudaMemcpyHostToDevice, st));
     if (blob_size) IPCFP_CUDA(cudaMemcpyAsync(d_blob.p, data_blob, blob_size, cudaMemcpyHostToDevice, st));
-    verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results);
+    verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results, log_filter);
 }
 
 // the proofs and their data blob (blob_size bytes + 16 of padding) already on the device, on the store's device
 void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
-                             const ipcfp_event_spec* filter, uint8_t* results) {
+                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter) {
     if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
     if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
+    LogFilterHost lfh;
+    if (log_filter) log_filter_build(log_filter, lfh);
     if (n == 0) return;
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
@@ -150,12 +157,31 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         IPCFP_CUDA(cudaMemcpyAsync(d_filter.p, &m, sizeof m, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));   // m is a stack object
     }
-    VerifyEventArgs va;
-    va.store = s->view; va.proofs = d_proofs; va.n = n; va.blob = d_blob; va.blob_size = blob_size;
-    va.consistent = d_flags.p; va.receipts_root_blk = d_flags.p + 1;
-    va.exec_raw = exo.exec_raw.p; va.exec_idx = exo.exec_idx.p; va.n_exec = exo.n_exec;
-    va.filter = filter ? d_filter.p : nullptr; va.results = d_res.p; va.err = dw;
-    k_verify_events<<<div_up(n * 32, 128), 128, 0, st>>>(va); IPCFP_LAUNCH_CHECK();
+    auto launch = [&](auto& va) {
+        va.store = s->view; va.proofs = d_proofs; va.n = n; va.blob = d_blob; va.blob_size = blob_size;
+        va.consistent = d_flags.p; va.receipts_root_blk = d_flags.p + 1;
+        va.exec_raw = exo.exec_raw.p; va.exec_idx = exo.exec_idx.p; va.n_exec = exo.n_exec;
+        va.results = d_res.p; va.err = dw;
+        k_verify_events<<<div_up(n * 32, 128), 128, 0, st>>>(va); IPCFP_LAUNCH_CHECK();
+    };
+    AsyncBuf<uint64_t> d_sets;
+    if (log_filter) {   // the filter and its large sets in one upload
+        const uint64_t fw = (sizeof(LogFilter) + 7) / 8;
+        d_sets.alloc(lfh.dev.size() + fw, st);
+        lfh.place(d_sets.p + fw);
+        std::vector<uint64_t> h(fw + lfh.dev.size(), 0);
+        memcpy(h.data(), &lfh.f, sizeof(LogFilter));
+        std::copy(lfh.dev.begin(), lfh.dev.end(), h.begin() + fw);
+        IPCFP_CUDA(cudaMemcpyAsync(d_sets.p, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
+        IPCFP_CUDA(cudaStreamSynchronize(st));   // h is a stack object
+        VerifyEventArgsT<LogFilter> va;
+        va.filter = (const LogFilter*)d_sets.p;
+        launch(va);
+    } else {
+        VerifyEventArgs va;
+        va.filter = filter ? d_filter.p : nullptr;
+        launch(va);
+    }
     IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));

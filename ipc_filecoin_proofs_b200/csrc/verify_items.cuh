@@ -198,7 +198,19 @@ static __device__ int events_get_value(const StoreView& s, uint32_t root_blk, ui
     }
 }
 
-struct VerifyEventArgs {
+// check_event: matches_log of a spec (events/generator.rs:38-40), without its actor filter; nullptr: no predicate
+__device__ __forceinline__ bool verify_check(const Matcher* f, const uint8_t* eblk, const EvLog& ev) {
+    if (f) {
+        if (ev.ntopics < 2) return false;
+        const uint32_t o0 = ev.toff[0], o1 = ev.case_a ? ev.toff[0] + 32 : ev.toff[1];
+        if (!(eq32(eblk + o0, f->t0) && eq32(eblk + o1, f->t1))) return false;
+    }
+    return true;
+}
+// check_event: the whole log filter, emitter set included
+__device__ __forceinline__ bool verify_check(const LogFilter* f, const uint8_t* eblk, const EvLog& ev) { return event_matches(eblk, ev, *f); }
+
+template <class F> struct VerifyEventArgsT {
     StoreView store;
     const ipcfp_event_proof* proofs;
     uint64_t n;
@@ -209,11 +221,13 @@ struct VerifyEventArgs {
     const RawCid* exec_raw;
     const uint32_t* exec_idx;
     uint64_t n_exec;
-    const Matcher* filter;        // nullptr: no predicate
+    const F* filter;              // nullptr: no predicate (Matcher only)
     uint8_t* results;
     unsigned long long* err;
 };
-__device__ __forceinline__ void verify_event_item(const VerifyEventArgs& a, uint64_t t) {
+using VerifyEventArgs = VerifyEventArgsT<Matcher>;
+template <class F>
+__device__ __forceinline__ void verify_event_item(const VerifyEventArgsT<F>& a, uint64_t t) {
     const StoreView& s = a.store;
     const ipcfp_event_proof& p = a.proofs[t];
     a.results[t] = 0;
@@ -251,11 +265,7 @@ __device__ __forceinline__ void verify_event_item(const VerifyEventArgs& a, uint
     }
     if (ev.data_len != p.data_len) return;
     for (uint32_t q = 0; q < ev.data_len; q++) if (eblk[ev.data_off + q] != a.blob[p.data_off + q]) return;
-    if (a.filter) {   // the optional semantic check: matches_log of the spec (events/generator.rs:38-40)
-        if (ev.ntopics < 2) return;
-        const uint32_t o0 = ev.toff[0], o1 = ev.case_a ? ev.toff[0] + 32 : ev.toff[1];
-        if (!(eq32(eblk + o0, a.filter->t0) && eq32(eblk + o1, a.filter->t1))) return;
-    }
+    if (!verify_check(a.filter, eblk, ev)) return;   // the optional semantic check (check_event)
     a.results[t] = 1;
 }
 
