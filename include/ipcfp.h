@@ -448,6 +448,19 @@ ipcfp_status ipcfp_generate_proof_bundle(ipcfp_store* s, const ipcfp_tipset_desc
  * Storage specs need a tipset uploaded with child_parent_state_root (else IPCFP_ERR_INVALID_ARG). */
 ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                                   const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_bundle** out);
+/* generate_proof_bundle with log filters in place of event specs: the storage specs in one batch, then filters[0..n_filters) in order
+ * (events[k] is filter k's EventProofBundle, what ipcfp_generate_log_proof_resident gives for it with the same IPCFP_WITNESS_BY_REFERENCE
+ * bit), then the union of every proof's blocks. Flags, the storage specs' tipset rule and the JSON text are those of
+ * ipcfp_generate_proof_bundle_resident; the text is the UnifiedProofBundle ipcfp_bundle_to_json renders for the flagless bundle.
+ * An event spec is the filter {emitters = [actor] or none, n_positions = 2, values = [{keccak256(sig)}, {ascii_to_bytes32(t1)}]}, and
+ * a bundle of those filters is byte for byte the bundle of the specs. Every filter is checked before any device work: a refused filter
+ * gives IPCFP_ERR_INVALID_ARG with its position as the index. Otherwise the status and index of a failure are those of the first
+ * generator that fails, in the order storage, filter 0, filter 1, … (the order of the spec bundle). ipcfp_generate_log_bundle =
+ * ipcfp_tipset_upload, then the resident call. */
+ipcfp_status ipcfp_generate_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out);
+ipcfp_status ipcfp_generate_log_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                       const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out);
 void ipcfp_bundle_free(ipcfp_bundle* b);
 
 /* ------------------------------------------------------------------------------------------
@@ -477,6 +490,11 @@ void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p);
  * rule 3's predicate (the receipts with a matching event add their receipts-AMT paths). Any flag bit is IPCFP_ERR_INVALID_ARG. */
 ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
                                            ipcfp_fetch_plan** out);
+/* One fetch round for ipcfp_generate_log_bundle_resident: rules 1–4 of ipcfp_plan_fetch_resident, with rule 3's predicate "matches at
+ * least one of filters[]". ipcfp_plan_fetch_log_resident is the case of one filter and no storage spec. Refused filters, flags and
+ * storage specs fail as in ipcfp_generate_log_bundle_resident / ipcfp_plan_fetch_resident. */
+ipcfp_status ipcfp_plan_fetch_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                  const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_fetch_plan** out);
 /* The round as one Filecoin.ChainReadObj batch: request k asks for plan->cids[k] with "id": first_id + k, compact JSON
  *   [{"jsonrpc":"2.0","method":"Filecoin.ChainReadObj","params":[{"/":"b…"}],"id":<first_id + k>},…]
  * With first_id = the number of blocks already held, the responses go straight to ipcfp_store_create_rpc_json with
@@ -572,6 +590,14 @@ ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* witness_store, const ipcfp
 ipcfp_status ipcfp_verify_event_proofs_log(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs,
                                            uint64_t n_proofs, const uint8_t* data_blob, uint64_t data_blob_size, const ipcfp_log_filter* filter,
                                            uint8_t* results);
+/* ipcfp_verify_event_proofs with a set of log filters as check_event: results[i] = OR over k of what ipcfp_verify_event_proofs_log gives
+ * with filters[k] for proof i. n_filters == 0: no check_event (ipcfp_verify_event_proofs with filter NULL). The check is the last step
+ * of a proof's verification, so the status and index of a failing call never depend on the filters: they are those of the unfiltered
+ * call. A refused filter gives IPCFP_ERR_INVALID_ARG with its position as the index. This verifies a bundle of
+ * ipcfp_generate_log_bundle against the filters it was made from. */
+ipcfp_status ipcfp_verify_event_proofs_any(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs,
+                                           uint64_t n_proofs, const uint8_t* data_blob, uint64_t data_blob_size, const ipcfp_log_filter* filters,
+                                           uint64_t n_filters, uint8_t* results);
 
 /* ------------------------------------------------------------------------------------------
  * verify_proof_bundle (src/proofs/verifier.rs:12-60) from the JSON text: parse, witness store and verification on the GPU.
@@ -614,6 +640,12 @@ typedef struct ipcfp_bundle_verdict {
 ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
                                       ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
                                       ipcfp_bundle_verdict** out);
+/* ipcfp_verify_bundle_json with "matches at least one of filters[]" as check_event: steps 1–4 above, step 4 calling
+ * ipcfp_verify_event_proofs_any (n_filters == 0: no check_event). Every filter is checked first: a refused filter gives
+ * IPCFP_ERR_INVALID_ARG with its position as the index. */
+ipcfp_status ipcfp_verify_bundle_json_any(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
+                                          ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_log_filter* filters,
+                                          uint64_t n_filters, ipcfp_bundle_verdict** out);
 void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v);
 
 /* ------------------------------------------------------------------------------------------

@@ -264,6 +264,8 @@ struct EventProofSpec {
 struct LogFilter {
     std::vector<uint64_t> emitters;
     std::vector<std::vector<H256>> topics;
+    // the filter a spec stands for: {[actor] or any, 2 positions, [{keccak256(sig)}, {ascii_to_bytes32(topic_1)}]} (keccak on `device`)
+    static LogFilter from_spec(const EventProofSpec& spec, int device = 0);
 };
 inline ipcfp_log_filter log_filter_c(const LogFilter& f, std::vector<std::vector<uint8_t>>& keep) {
     ipcfp_log_filter c;
@@ -601,22 +603,8 @@ inline uint64_t resolve_eth_address_to_actor_id(GpuBlockstore& store, const Cid&
     return r.actor_ids[0];
 }
 
-// generate_proof_bundle (proofs/generator.rs:25-95): every spec against one store, blocks deduplicated as BTreeSet<(Cid, data)>
-inline UnifiedProofBundle generate_proof_bundle(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
-                                                const std::vector<StorageProofSpec>& storage_specs, const std::vector<EventProofSpec>& event_specs) {
-    TipsetDesc t(parent, child, receipts);
-    std::vector<ipcfp_storage_spec> ss(storage_specs.size());
-    for (size_t i = 0; i < ss.size(); i++) {
-        memset(&ss[i], 0, sizeof ss[i]);
-        ss[i].actor_id = storage_specs[i].actor_id;
-        memcpy(ss[i].slot, storage_specs[i].slot.data(), 32);
-    }
-    std::vector<ipcfp_event_spec> es;
-    es.reserve(event_specs.size());
-    for (const auto& e : event_specs) es.push_back(spec_c(e.event_signature, e.topic_1, e.actor_id_filter));
-    ipcfp_bundle* b = nullptr;
-    check(ipcfp_generate_proof_bundle(store.raw(), t.c(), ss.empty() ? nullptr : ss.data(), ss.size(), es.empty() ? nullptr : es.data(), es.size(), &b),
-          "generate_proof_bundle");
+// the UnifiedProofBundle of an ipcfp_bundle, which it frees
+inline UnifiedProofBundle unified_bundle(ipcfp_bundle* b, const TipsetDesc& t) {
     UnifiedProofBundle u;
     try {
         if (b->storage)
@@ -630,6 +618,45 @@ inline UnifiedProofBundle generate_proof_bundle(GpuBlockstore& store, const ApiT
     ipcfp_bundle_free(b);
     return u;
 }
+inline std::vector<ipcfp_storage_spec> storage_specs_c(const std::vector<StorageProofSpec>& storage_specs) {
+    std::vector<ipcfp_storage_spec> ss(storage_specs.size());
+    for (size_t i = 0; i < ss.size(); i++) {
+        memset(&ss[i], 0, sizeof ss[i]);
+        ss[i].actor_id = storage_specs[i].actor_id;
+        memcpy(ss[i].slot, storage_specs[i].slot.data(), 32);
+    }
+    return ss;
+}
+
+// generate_proof_bundle (proofs/generator.rs:25-95): every spec against one store, blocks deduplicated as BTreeSet<(Cid, data)>
+inline UnifiedProofBundle generate_proof_bundle(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                                const std::vector<StorageProofSpec>& storage_specs, const std::vector<EventProofSpec>& event_specs) {
+    TipsetDesc t(parent, child, receipts);
+    const std::vector<ipcfp_storage_spec> ss = storage_specs_c(storage_specs);
+    std::vector<ipcfp_event_spec> es;
+    es.reserve(event_specs.size());
+    for (const auto& e : event_specs) es.push_back(spec_c(e.event_signature, e.topic_1, e.actor_id_filter));
+    ipcfp_bundle* b = nullptr;
+    check(ipcfp_generate_proof_bundle(store.raw(), t.c(), ss.empty() ? nullptr : ss.data(), ss.size(), es.empty() ? nullptr : es.data(), es.size(), &b),
+          "generate_proof_bundle");
+    return unified_bundle(b, t);
+}
+// the same bundle with log filters in place of event specs (ipcfp_generate_log_bundle): the storage proofs, then every filter's event
+// proofs in order. The filters of LogFilter::from_spec give the spec bundle, byte for byte.
+inline UnifiedProofBundle generate_proof_bundle(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                                const std::vector<StorageProofSpec>& storage_specs, const std::vector<LogFilter>& log_filters) {
+    for (const auto& f : log_filters)
+        if (f.topics.size() > 4) throw Error(IPCFP_ERR_INVALID_ARG, "generate_proof_bundle: more than four topic positions");
+    TipsetDesc t(parent, child, receipts);
+    const std::vector<ipcfp_storage_spec> ss = storage_specs_c(storage_specs);
+    std::vector<std::vector<uint8_t>> keep;
+    std::vector<ipcfp_log_filter> fs;
+    for (const auto& f : log_filters) fs.push_back(log_filter_c(f, keep));
+    ipcfp_bundle* b = nullptr;
+    check(ipcfp_generate_log_bundle(store.raw(), t.c(), ss.empty() ? nullptr : ss.data(), ss.size(), fs.empty() ? nullptr : fs.data(), fs.size(), 0, &b),
+          "generate_proof_bundle");
+    return unified_bundle(b, t);
+}
 
 // keccak256 / hash_event_signature (common/evm.rs:62-69, :81-88), on the GPU
 inline H256 keccak256(const std::vector<uint8_t>& bytes, int device = 0) {
@@ -641,6 +668,12 @@ inline H256 keccak256(const std::vector<uint8_t>& bytes, int device = 0) {
     return out;
 }
 inline H256 hash_event_signature(const std::string& s, int device = 0) { return keccak256(std::vector<uint8_t>(s.begin(), s.end()), device); }
+inline LogFilter LogFilter::from_spec(const EventProofSpec& spec, int device) {
+    LogFilter f;
+    if (spec.actor_id_filter) f.emitters.push_back(*spec.actor_id_filter);
+    f.topics = {{hash_event_signature(spec.event_signature, device)}, {ascii_to_bytes32(spec.topic_1)}};
+    return f;
+}
 // create_event_filter(event_sig, subnet_id) (events/verifier.rs:28-41): the predicate verify_event_proof takes as check_event
 inline EventProofSpec create_event_filter(const std::string& event_sig, const std::string& subnet_id) { return EventProofSpec{event_sig, subnet_id, std::nullopt}; }
 // parse_cid / parse_cids (common/witness.rs:60-72): the error names what was being parsed
@@ -828,12 +861,10 @@ inline UnifiedVerificationResult verify_proof_bundle(const UnifiedProofBundle& b
     return r;
 }
 
-// verify_proof_bundle from the bundle's JSON text (EventProofBundle or UnifiedProofBundle), through ipcfp_verify_bundle_json: parse, witness
-// store and verification on the GPU (text not in serde_json's canonical form is read by the host parser, with the same results). Each
-// closure is called at most once, on this thread.
-inline UnifiedVerificationResult verify_proof_bundle_json(const std::string& text, const TrustedParentTs& is_trusted_parent_ts,
-                                                          const TrustedChildHeader& is_trusted_child_header, const EventProofSpec* check_event = nullptr,
-                                                          int device = 0) {
+namespace detail {
+// ipcfp_verify_bundle_json or its _any form: call(tp, tc, ctx, &verdict) with the closures turned into C callbacks
+template <class Call>
+inline UnifiedVerificationResult verify_json_with(const TrustedParentTs& is_trusted_parent_ts, const TrustedChildHeader& is_trusted_child_header, Call call) {
     struct Ctx { const TrustedParentTs* parent; const TrustedChildHeader* child; } ctx{&is_trusted_parent_ts, &is_trusted_child_header};
     auto tp = [](void* c, int64_t epoch, const uint8_t* cids, uint32_t n) -> int {
         std::vector<Cid> parents;
@@ -841,15 +872,41 @@ inline UnifiedVerificationResult verify_proof_bundle_json(const std::string& tex
         return (*static_cast<Ctx*>(c)->parent)(epoch, parents) ? 1 : 0;
     };
     auto tc = [](void* c, int64_t epoch, const uint8_t* cid) -> int { return (*static_cast<Ctx*>(c)->child)(epoch, Cid::from_bytes(cid)) ? 1 : 0; };
-    ipcfp_event_spec filter;
-    if (check_event) filter = spec_c(check_event->event_signature, check_event->topic_1, check_event->actor_id_filter);
     ipcfp_bundle_verdict* v = nullptr;
-    check(ipcfp_verify_bundle_json(text.data(), text.size(), device, tp, tc, &ctx, check_event ? &filter : nullptr, &v), "verify_proof_bundle_json");
+    check(call(+tp, +tc, (void*)&ctx, &v), "verify_proof_bundle_json");
     UnifiedVerificationResult r;
     for (uint64_t i = 0; i < v->n_storage_proofs; i++) r.storage_results.push_back(v->storage_results[i] != 0);
     for (uint64_t i = 0; i < v->n_event_proofs; i++) r.event_results.push_back(v->event_results[i] != 0);
     ipcfp_bundle_verdict_free(v);
     return r;
+}
+}  // namespace detail
+
+// verify_proof_bundle from the bundle's JSON text (EventProofBundle or UnifiedProofBundle), through ipcfp_verify_bundle_json: parse, witness
+// store and verification on the GPU (text not in serde_json's canonical form is read by the host parser, with the same results). Each
+// closure is called at most once, on this thread.
+inline UnifiedVerificationResult verify_proof_bundle_json(const std::string& text, const TrustedParentTs& is_trusted_parent_ts,
+                                                          const TrustedChildHeader& is_trusted_child_header, const EventProofSpec* check_event = nullptr,
+                                                          int device = 0) {
+    ipcfp_event_spec filter;
+    if (check_event) filter = spec_c(check_event->event_signature, check_event->topic_1, check_event->actor_id_filter);
+    return detail::verify_json_with(is_trusted_parent_ts, is_trusted_child_header, [&](auto tp, auto tc, void* ctx, ipcfp_bundle_verdict** v) {
+        return ipcfp_verify_bundle_json(text.data(), text.size(), device, tp, tc, ctx, check_event ? &filter : nullptr, v);
+    });
+}
+// the same with a set of log filters as check_event (ipcfp_verify_bundle_json_any): an event proof is true only when its event matches
+// at least one of check_any; an empty set is no check_event
+inline UnifiedVerificationResult verify_proof_bundle_json(const std::string& text, const TrustedParentTs& is_trusted_parent_ts,
+                                                          const TrustedChildHeader& is_trusted_child_header, const std::vector<LogFilter>& check_any,
+                                                          int device = 0) {
+    for (const auto& f : check_any)
+        if (f.topics.size() > 4) throw Error(IPCFP_ERR_INVALID_ARG, "verify_proof_bundle_json: more than four topic positions");
+    std::vector<std::vector<uint8_t>> keep;
+    std::vector<ipcfp_log_filter> fs;
+    for (const auto& f : check_any) fs.push_back(log_filter_c(f, keep));
+    return detail::verify_json_with(is_trusted_parent_ts, is_trusted_child_header, [&](auto tp, auto tc, void* ctx, ipcfp_bundle_verdict** v) {
+        return ipcfp_verify_bundle_json_any(text.data(), text.size(), device, tp, tc, ctx, fs.empty() ? nullptr : fs.data(), fs.size(), v);
+    });
 }
 
 // ------------------------------------------------------------------------------------------ wire format (serde_json of the bundle structs)

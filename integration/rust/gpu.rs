@@ -8,6 +8,7 @@
 //! * `generate_event_proof_gpu` replaces the body of `generate_event_proof` (`src/proofs/events/generator.rs:60-107`);
 //! * `generate_storage_proof_gpu` replaces `generate_storage_proof` (`src/proofs/storage/generator.rs:29-67`), batched;
 //! * `generate_proof_bundle_gpu` replaces the two loops of `generate_proof_bundle` (`src/proofs/generator.rs:25-95`);
+//!   `generate_proof_bundle_logs_gpu` is the same bundle with eth_getLogs-style log filters in place of event specs;
 //! * `verify_event_proof_gpu` / `verify_storage_proof_gpu` replace `verify_event_proof` / `verify_storage_proof`
 //!   (`src/proofs/events/verifier.rs:51-74`, `src/proofs/storage/verifier.rs:24-63`) with every witness block CID-checked.
 //!
@@ -523,13 +524,68 @@ pub fn generate_proof_bundle_gpu(
     check(unsafe {
         sys::ipcfp_generate_proof_bundle(store.h, &desc.raw(), ss.as_ptr(), ss.len() as u64, es_raw.as_ptr(), es_raw.len() as u64, &mut out)
     })?;
+    unified_bundle_of(out, parent, child, &desc)
+}
+
+/// An eth_getLogs-style log filter (`ipcfp_log_filter`): `emitters` empty for any emitter, else actor IDs; `topics[k]` `None` for any
+/// value at position k, else the 32-byte values topic k may take. A log needs at least `topics.len()` topics. The spec
+/// `{sig, t1, actor}` is `LogFilter { emitters: actor.into_iter().collect(), topics: vec![Some(vec![keccak(sig)]), Some(vec![ascii_to_bytes32(t1)])] }`.
+pub struct LogFilter {
+    pub emitters: Vec<u64>,
+    pub topics: Vec<Option<Vec<[u8; 32]>>>,
+}
+
+fn log_filter_c(f: &LogFilter) -> Result<sys::ipcfp_log_filter> {
+    if f.topics.len() > 4 {
+        bail!("a log filter has at most 4 topic positions");
+    }
+    let mut c = sys::ipcfp_log_filter {
+        n_emitters: f.emitters.len() as u64,
+        emitters: f.emitters.as_ptr(),
+        n_positions: f.topics.len() as u32,
+        _pad: 0,
+        n_values: [0; 4],
+        values: [std::ptr::null(); 4],
+    };
+    for (k, t) in f.topics.iter().enumerate() {
+        if let Some(v) = t {
+            c.n_values[k] = v.len() as u64;
+            c.values[k] = v.as_ptr() as *const u8;
+        }
+    }
+    Ok(c)
+}
+
+/// `generate_proof_bundle` with log filters in place of event specs (`ipcfp_generate_log_bundle`): the storage specs, then one
+/// EventProofBundle per filter in order, then the union of the witnesses. A bundle of the filters the specs stand for is the spec
+/// bundle, byte for byte.
+pub fn generate_proof_bundle_logs_gpu(
+    store: &GpuBlockstore,
+    parent: &ApiTipset,
+    child: &ApiTipset,
+    receipts: &[ApiReceipt],
+    storage_specs: Vec<StorageProofSpec>,
+    log_filters: &[LogFilter],
+) -> Result<UnifiedProofBundle> {
+    let desc = TipsetDesc::new(parent, child, receipts)?;
+    let ss: Vec<sys::ipcfp_storage_spec> = storage_specs.iter().map(|s| sys::ipcfp_storage_spec { actor_id: s.actor_id, slot: s.slot.0 }).collect();
+    let fs: Vec<sys::ipcfp_log_filter> = log_filters.iter().map(log_filter_c).collect::<Result<_>>()?;
+    let mut out = std::ptr::null_mut();
+    check(unsafe {
+        sys::ipcfp_generate_log_bundle(store.h, &desc.raw(), ss.as_ptr(), ss.len() as u64, fs.as_ptr(), fs.len() as u64, 0, &mut out)
+    })?;
+    unified_bundle_of(out, parent, child, &desc)
+}
+
+/// The UnifiedProofBundle of an `ipcfp_bundle`, which it frees.
+fn unified_bundle_of(out: *mut sys::ipcfp_bundle, parent: &ApiTipset, child: &ApiTipset, desc: &TipsetDesc) -> Result<UnifiedProofBundle> {
     let b = unsafe { &*out };
     let res = (|| -> Result<UnifiedProofBundle> {
         let mut storage_proofs = Vec::new();
         if !b.storage.is_null() {
             let s = unsafe { &*b.storage };
             for i in 0..s.n_proofs as usize {
-                storage_proofs.push(storage_proof_of(unsafe { &*s.proofs.add(i) }, child, &desc)?);
+                storage_proofs.push(storage_proof_of(unsafe { &*s.proofs.add(i) }, child, desc)?);
             }
         }
         let mut event_proofs = Vec::new();

@@ -177,6 +177,10 @@ extern "C" {
                                        especs: *const ipcfp_event_spec, n_especs: u64, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
     pub fn ipcfp_generate_proof_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                                                 especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
+    pub fn ipcfp_generate_log_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                                              filters: *const ipcfp_log_filter, n_filters: u64, flags: u32, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
+    pub fn ipcfp_generate_log_bundle(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                                     filters: *const ipcfp_log_filter, n_filters: u64, flags: u32, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
     pub fn ipcfp_bundle_free(b: *mut ipcfp_bundle);
     pub fn ipcfp_plan_fetch_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                                      especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
@@ -184,6 +188,8 @@ extern "C" {
                             especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_plan_fetch_log_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, filter: *const ipcfp_log_filter, flags: u32,
                                          out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_plan_fetch_log_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
+                                                filters: *const ipcfp_log_filter, n_filters: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_fetch_plan_free(p: *mut ipcfp_fetch_plan);
     pub fn ipcfp_fetch_plan_to_rpc_json(p: *const ipcfp_fetch_plan, first_id: u64, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_resolve_addresses(s: *mut ipcfp_store, state_root: *const u8, addrs: *const ipcfp_address, n: u64,
@@ -201,11 +207,17 @@ extern "C" {
                                      data_blob: *const u8, data_blob_size: u64, filter: *const ipcfp_event_spec, results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_event_proofs_log(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_event_proof, n_proofs: u64,
                                          data_blob: *const u8, data_blob_size: u64, filter: *const ipcfp_log_filter, results: *mut u8) -> ipcfp_status;
+    pub fn ipcfp_verify_event_proofs_any(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_event_proof, n_proofs: u64,
+                                         data_blob: *const u8, data_blob_size: u64, filters: *const ipcfp_log_filter, n_filters: u64,
+                                         results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_storage_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_storage_proof, n_proofs: u64,
                                        results: *mut u8) -> ipcfp_status;
     pub fn ipcfp_verify_bundle_json(json: *const c_char, len: u64, device: c_int, trusted_parent: ipcfp_trusted_parent_ts_fn,
                                     trusted_child: ipcfp_trusted_child_header_fn, trust_ctx: *mut c_void, filter: *const ipcfp_event_spec,
                                     out: *mut *mut ipcfp_bundle_verdict) -> ipcfp_status;
+    pub fn ipcfp_verify_bundle_json_any(json: *const c_char, len: u64, device: c_int, trusted_parent: ipcfp_trusted_parent_ts_fn,
+                                        trusted_child: ipcfp_trusted_child_header_fn, trust_ctx: *mut c_void, filters: *const ipcfp_log_filter,
+                                        n_filters: u64, out: *mut *mut ipcfp_bundle_verdict) -> ipcfp_status;
     pub fn ipcfp_bundle_verdict_free(v: *mut ipcfp_bundle_verdict);
     pub fn ipcfp_comm_unique_id(id: *mut u8) -> ipcfp_status;
     pub fn ipcfp_comm_init(id: *const u8, world_size: u32, rank: u32, device: c_int, out: *mut *mut ipcfp_comm) -> ipcfp_status;

@@ -49,6 +49,8 @@ EXPORTS = [
     "ipcfp_plan_fetch_resident", "ipcfp_plan_fetch", "ipcfp_fetch_plan_free", "ipcfp_fetch_plan_to_rpc_json",
     "ipcfp_resolve_addresses", "ipcfp_resolve_result_free", "ipcfp_address_parse", "ipcfp_address_from_eth",
     "ipcfp_generate_log_proof", "ipcfp_generate_log_proof_resident", "ipcfp_plan_fetch_log_resident", "ipcfp_verify_event_proofs_log",
+    "ipcfp_generate_log_bundle", "ipcfp_generate_log_bundle_resident", "ipcfp_plan_fetch_log_bundle_resident", "ipcfp_verify_event_proofs_any",
+    "ipcfp_verify_bundle_json_any",
 ]
 
 
@@ -137,6 +139,21 @@ def lib():
         L.ipcfp_verify_event_proofs_log.restype = C.c_int32
         L.ipcfp_verify_event_proofs_log.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                                     C.POINTER(A.LogFilterC), C.c_void_p]
+        L.ipcfp_generate_log_bundle.restype = C.c_int32
+        L.ipcfp_generate_log_bundle.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
+                                                C.c_uint32, C.POINTER(C.POINTER(A.BundleC))]
+        L.ipcfp_generate_log_bundle_resident.restype = C.c_int32
+        L.ipcfp_generate_log_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
+                                                         C.c_uint32, C.POINTER(C.POINTER(A.BundleC))]
+        L.ipcfp_plan_fetch_log_bundle_resident.restype = C.c_int32
+        L.ipcfp_plan_fetch_log_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
+                                                           C.c_uint32, C.POINTER(C.POINTER(A.FetchPlanC))]
+        L.ipcfp_verify_event_proofs_any.restype = C.c_int32
+        L.ipcfp_verify_event_proofs_any.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                                    C.POINTER(A.LogFilterC), C.c_uint64, C.c_void_p]
+        L.ipcfp_verify_bundle_json_any.restype = C.c_int32
+        L.ipcfp_verify_bundle_json_any.argtypes = [C.c_char_p, C.c_uint64, C.c_int, A.TrustedParentFn, A.TrustedChildFn, C.c_void_p,
+                                                   C.POINTER(A.LogFilterC), C.c_uint64, C.POINTER(C.POINTER(A.BundleVerdictC))]
         L.ipcfp_verify_storage_proofs.restype = C.c_int32
         L.ipcfp_verify_storage_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p]
         for name in ("ipcfp_bundle_to_json", "ipcfp_event_result_to_json"):
@@ -275,6 +292,16 @@ class LogFilter:
         if len(topics) < len(self.topics):
             return False
         return all(vals is None or bytes(topics[k]) in vals for k, vals in enumerate(self.topics))
+
+
+def _log_filters_c(log_filters):
+    """(ipcfp_log_filter array, count, keepalive) of a sequence of LogFilters"""
+    cs, keep = [], []
+    for f in log_filters:
+        c, k = f.as_c()
+        cs.append(c)
+        keep.append(k)
+    return (A.LogFilterC * max(len(cs), 1))(*cs), len(cs), keep
 
 
 @dataclass
@@ -492,6 +519,42 @@ class BlockStore:
         finally:
             lib().ipcfp_fetch_plan_free(out)
 
+    def generate_log_bundle(self, ts, storage_specs, log_filters, flags=0):
+        """ipcfp_generate_log_bundle: generate_proof_bundle with LogFilters in place of event specs (events[k] is filter k's result)
+        → A.BundlePy. flags: WITNESS_BY_REFERENCE, RESULT_JSON."""
+        sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
+        farr, nf, fkeep = _log_filters_c(log_filters)
+        d, keep = A.make_tipset_desc(ts)
+        out = C.POINTER(A.BundleC)()
+        _check(lib().ipcfp_generate_log_bundle(self._h, C.byref(d), sarr, ns, farr, nf, flags, C.byref(out)))
+        try:
+            return A.bundle_from_c(out.contents)
+        finally:
+            lib().ipcfp_bundle_free(out)
+
+    def generate_log_bundle_resident(self, tip, storage_specs, log_filters, flags=0):
+        """ipcfp_generate_log_bundle_resident against a ResidentTipset of this store → A.BundlePy."""
+        sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
+        farr, nf, fkeep = _log_filters_c(log_filters)
+        out = C.POINTER(A.BundleC)()
+        _check(lib().ipcfp_generate_log_bundle_resident(self._h, tip._h, sarr, ns, farr, nf, flags, C.byref(out)))
+        try:
+            return A.bundle_from_c(out.contents)
+        finally:
+            lib().ipcfp_bundle_free(out)
+
+    def plan_fetch_log_bundle(self, tip, storage_specs, log_filters, flags=0):
+        """ipcfp_plan_fetch_log_bundle_resident → A.FetchPlanPy: one fetch round for generate_log_bundle_resident(tip, storage_specs,
+        log_filters)."""
+        sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
+        farr, nf, fkeep = _log_filters_c(log_filters)
+        out = C.POINTER(A.FetchPlanC)()
+        _check(lib().ipcfp_plan_fetch_log_bundle_resident(self._h, tip._h, sarr, ns, farr, nf, flags, C.byref(out)))
+        try:
+            return A.fetch_plan_from_c(out.contents)
+        finally:
+            lib().ipcfp_fetch_plan_free(out)
+
     def plan_fetch_logs(self, tip, log_filter, flags=0):
         """ipcfp_plan_fetch_log_resident → A.FetchPlanPy: one fetch round for generate_log_proof_resident(tip, log_filter)."""
         f, fkeep = log_filter.as_c()
@@ -612,12 +675,25 @@ def fetch_until_complete(fetch, upload_tipset, storage_specs, event_specs, devic
     upload_tipset_json). Starts from an empty store; each round rebuilds it with BlockStore.from_rpc_json over every response so far.
     Returns (store, tipset, rounds, cids, texts): the complete store, its tipset, the FetchRounds, and the CIDs and texts it was built
     from."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch(tip, storage_specs, event_specs), fetch, upload_tipset, device, verify_cids,
+                       max_rounds)
+
+
+def fetch_log_bundle_until_complete(fetch, upload_tipset, storage_specs, log_filters, device=0, verify_cids=True, max_rounds=10000):
+    """fetch_until_complete for generate_log_bundle_resident(tip, storage_specs, log_filters): the same loop, planned with
+    plan_fetch_log_bundle."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch_log_bundle(tip, storage_specs, log_filters), fetch, upload_tipset, device,
+                       verify_cids, max_rounds)
+
+
+def _fetch_loop(plan_round, fetch, upload_tipset, device, verify_cids, max_rounds):
+    """fetch_until_complete's loop; plan_round(store, tip) → the round's A.FetchPlanPy"""
     import time
     all_cids, texts, rounds = np.zeros((0, A.CID_LEN), np.uint8), [], []
     store = BlockStore(all_cids, np.zeros(0, np.uint64), np.zeros(0, np.uint32), np.zeros(0, np.uint8), device=device)
     tip = upload_tipset(store)
     for _ in range(max_rounds):
-        plan = store.plan_fetch(tip, storage_specs, event_specs)
+        plan = plan_round(store, tip)
         if not len(plan.cids):
             return store, tip, rounds, all_cids, texts
         got = fetch(plan.cids, len(all_cids))
@@ -817,17 +893,37 @@ class BundleVerdict:
         self.ms = dict(total=c.ms_total, parse=c.ms_parse, store=c.ms_store, verify=c.ms_verify)
 
 
+def _trust_callbacks(trusted_parent, trusted_child):
+    cb_p = A.TrustedParentFn(lambda ctx, e, p, n: int(bool(trusted_parent(int(e), C.string_at(p, 38 * n) if n else b""))))\
+        if trusted_parent else A.TrustedParentFn()
+    cb_c = A.TrustedChildFn(lambda ctx, e, c: int(bool(trusted_child(int(e), C.string_at(c, 38))))) if trusted_child else A.TrustedChildFn()
+    return cb_p, cb_c
+
+
 def verify_bundle_json(text, trusted_parent=None, trusted_child=None, filter_spec=None, device=0):
     """ipcfp_verify_bundle_json. trusted_parent(epoch, parent_cids: bytes) / trusted_child(epoch, child_cid: bytes) → bool, None = accept
     all. filter_spec: an A.EventSpec (check_event) or None. → BundleVerdict; failures raise IpcfpError (status, index)."""
     raw = text.encode() if isinstance(text, str) else bytes(text)
-    cb_p = A.TrustedParentFn(lambda ctx, e, p, n: int(bool(trusted_parent(int(e), C.string_at(p, 38 * n) if n else b""))))\
-        if trusted_parent else A.TrustedParentFn()
-    cb_c = A.TrustedChildFn(lambda ctx, e, c: int(bool(trusted_child(int(e), C.string_at(c, 38))))) if trusted_child else A.TrustedChildFn()
+    cb_p, cb_c = _trust_callbacks(trusted_parent, trusted_child)
     out = C.POINTER(A.BundleVerdictC)()
     L = lib()
     _check(L.ipcfp_verify_bundle_json(raw, len(raw), device, cb_p, cb_c, None, C.addressof(filter_spec) if filter_spec is not None else None,
                                       C.byref(out)))
+    try:
+        return BundleVerdict(out.contents)
+    finally:
+        L.ipcfp_bundle_verdict_free(out)
+
+
+def verify_bundle_json_any(text, trusted_parent=None, trusted_child=None, log_filters=(), device=0):
+    """ipcfp_verify_bundle_json_any: verify_bundle_json with check_event = "matches at least one of log_filters" (LogFilters; empty: no
+    check_event). → BundleVerdict; failures raise IpcfpError (status, index)."""
+    raw = text.encode() if isinstance(text, str) else bytes(text)
+    cb_p, cb_c = _trust_callbacks(trusted_parent, trusted_child)
+    farr, nf, fkeep = _log_filters_c(log_filters)
+    out = C.POINTER(A.BundleVerdictC)()
+    L = lib()
+    _check(L.ipcfp_verify_bundle_json_any(raw, len(raw), device, cb_p, cb_c, None, farr, nf, C.byref(out)))
     try:
         return BundleVerdict(out.contents)
     finally:
@@ -853,6 +949,24 @@ def verify_event_proofs(witness, ts, result, filter_spec=None, device=0):
         fs = filter_spec.as_c() if isinstance(filter_spec, EventProofSpec) else filter_spec
         _check(lib().ipcfp_verify_event_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None, blob.size,
                                                C.addressof(fs) if fs is not None else None, res.ctypes.data))
+        return [bool(x) for x in res[:n]]
+    finally:
+        store.close()
+
+
+def verify_event_proofs_any(witness, ts, result, log_filters, device=0):
+    """verify_event_proofs with check_event = "matches at least one of log_filters" (ipcfp_verify_event_proofs_any; an empty sequence:
+    no check_event). result: anything with raw_proofs, data_blob and proofs (A.EventResultPy). → list of bools."""
+    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
+    try:
+        d, keep = A.make_tipset_desc(ts)
+        n = len(result.proofs)
+        res = np.zeros(max(n, 1), dtype=np.uint8)
+        raw = np.ascontiguousarray(result.raw_proofs)
+        blob = np.ascontiguousarray(result.data_blob)
+        farr, nf, fkeep = _log_filters_c(log_filters)
+        _check(lib().ipcfp_verify_event_proofs_any(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None,
+                                                   blob.size, farr, nf, res.ctypes.data))
         return [bool(x) for x in res[:n]]
     finally:
         store.close()

@@ -3,6 +3,7 @@
 #include <cstring>
 
 #include "engine.cuh"
+#include "log_filter.cuh"
 
 namespace ipcfp {
 
@@ -53,13 +54,16 @@ struct FetchPlanBox {
 
 #define IPCFP_BUNDLE_FLAGS (IPCFP_WITNESS_BY_REFERENCE | IPCFP_RESULT_JSON)
 
-// generate_proof_bundle (proofs/generator.rs:25-95) against a device-resident tipset: the storage specs in one batch, then every event
-// spec in order, then the BTreeSet<(Cid, data)> union of every proof's blocks on the device (witness_union: OR of the lists' rank bits,
-// one compaction) and, with IPCFP_RESULT_JSON, the UnifiedProofBundle text rendered from device memory.
-static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
-                                           const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags) {
+// generate_proof_bundle (proofs/generator.rs:25-95) against a device-resident tipset: the storage specs in one batch, then event item
+// 0 .. n_events - 1 in order (gen(k) makes item k's EventProofBundle: an event spec's or a log filter's), then the BTreeSet<(Cid, data)>
+// union of every proof's blocks on the device (witness_union: OR of the lists' rank bits, one compaction) and, with IPCFP_RESULT_JSON,
+// the UnifiedProofBundle text rendered from device memory. check() runs before any device work.
+template <class Check, class Gen>
+static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, uint64_t n_events,
+                                           uint32_t flags, Check check, Gen gen) {
     if (flags & ~(uint32_t)IPCFP_BUNDLE_FLAGS) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a proof bundle");
-    if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
+    if (n_sspecs && !sspecs) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
+    check();
     if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !st->caller_blob)
         throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_WITNESS_BY_REFERENCE needs a store made from a caller's blob (ipcfp_store_create)");
     st->use();
@@ -75,8 +79,8 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
         box->r.storage = generate_storage_proofs(st, td.child_cid, td.child_state_root, sspecs, n_sspecs, by_ref);
         lists.push_back(&storage_result_witness(box->r.storage));
     }
-    for (uint64_t i = 0; i < n_especs; i++) {
-        box->ev.push_back(generate_event_proof(st, td, &especs[i], flags & IPCFP_WITNESS_BY_REFERENCE, false, 0, 0));
+    for (uint64_t i = 0; i < n_events; i++) {
+        box->ev.push_back(gen(i));
         lists.push_back(&event_result_witness(box->ev.back()));
     }
     witness_union(st, lists, box->wit, by_ref);
@@ -128,6 +132,22 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
         IPCFP_CUDA(cudaEventElapsedTime(&ms, j0.e, j1.e)); box->r.ms_json = ms;
     }
     return &box.release()->r;
+}
+
+// the bundle of event specs
+static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                           const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags) {
+    return generate_proof_bundle(
+        st, td, sspecs, n_sspecs, n_especs, flags,
+        [&] { if (n_especs && !especs) throw Error(IPCFP_ERR_INVALID_ARG, "null specs"); },
+        [&](uint64_t i) { return generate_event_proof(st, td, &especs[i], flags & IPCFP_WITNESS_BY_REFERENCE, false, 0, 0); });
+}
+// the bundle of log filters: every filter is checked before any device work
+static ipcfp_bundle* generate_log_bundle(Store* st, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                         const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags) {
+    return generate_proof_bundle(
+        st, td, sspecs, n_sspecs, n_filters, flags, [&] { LogFilterSet::check(filters, n_filters); },
+        [&](uint64_t k) { return generate_log_proof(st, td, &filters[k], flags & IPCFP_WITNESS_BY_REFERENCE); });
 }
 
 }  // namespace ipcfp
@@ -346,8 +366,34 @@ ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* 
         *out = generate_proof_bundle(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, especs, n_especs, flags);
     });
 }
+ipcfp_status ipcfp_generate_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = generate_log_bundle(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, filters, n_filters, flags);
+    });
+}
+ipcfp_status ipcfp_generate_log_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                       const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out) {
+    return guard([&] {
+        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        Store* st = reinterpret_cast<Store*>(s);
+        TipsetDev td;
+        tipset_upload(st, t, td);
+        *out = generate_log_bundle(st, td, sspecs, n_sspecs, filters, n_filters, flags);
+    });
+}
 void ipcfp_bundle_free(ipcfp_bundle* b) { delete reinterpret_cast<BundleBox*>(b); }
 
+static void plan_fetch_log_bundle(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_log_filter* filters,
+                                  uint64_t n_filters, ipcfp_fetch_plan** out) {
+    std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+    plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, nullptr, 0, box->plan, filters, n_filters);
+    box->fill();
+    *out = &box.release()->r;
+}
 ipcfp_status ipcfp_plan_fetch_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                        const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out) {
     return guard([&] {
@@ -375,15 +421,23 @@ ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const 
         *out = &box.release()->r;
     });
 }
+ipcfp_status ipcfp_plan_fetch_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
+                                                  const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_fetch_plan** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+        plan_fetch_log_bundle(s, t, sspecs, n_sspecs, filters, n_filters, out);
+    });
+}
+// the bundle plan of one filter and no storage spec; a refused filter has no index
 ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags, ipcfp_fetch_plan** out) {
     return guard([&] {
         if (!s || !t || !out || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
         if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
-        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
-        plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), nullptr, 0, nullptr, 0, box->plan, filter);
-        box->fill();
-        *out = &box.release()->r;
+        log_filter_check(filter);
+        plan_fetch_log_bundle(s, t, nullptr, 0, filter, 1, out);
     });
 }
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }
@@ -434,11 +488,23 @@ ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* 
         verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, filter, results);
     });
 }
+// check_event = the set of one filter; a refused filter has no index
 ipcfp_status ipcfp_verify_event_proofs_log(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
                                            uint64_t blob_size, const ipcfp_log_filter* filter, uint8_t* results) {
     return guard([&] {
         if (!s || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filter);
+        try { verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filter, 1); }
+        catch (Error& e) {
+            if (e.status == IPCFP_ERR_INVALID_ARG && e.index == 0) e.index = UINT64_MAX;
+            throw;
+        }
+    });
+}
+ipcfp_status ipcfp_verify_event_proofs_any(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* blob,
+                                           uint64_t blob_size, const ipcfp_log_filter* filters, uint64_t n_filters, uint8_t* results) {
+    return guard([&] {
+        if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filters, n_filters);
     });
 }
 ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results) {
@@ -455,6 +521,16 @@ ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device
         if (!json || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         *out = nullptr;
         *out = verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, filter);
+    });
+}
+ipcfp_status ipcfp_verify_bundle_json_any(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
+                                          ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_log_filter* filters,
+                                          uint64_t n_filters, ipcfp_bundle_verdict** out) {
+    return guard([&] {
+        if (!json || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        LogFilterSet::check(filters, n_filters);
+        *out = verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, nullptr, filters, n_filters);
     });
 }
 void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v) { if (v) bundle_verdict_free(v); }

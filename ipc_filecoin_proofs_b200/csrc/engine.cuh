@@ -207,17 +207,20 @@ ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_ev
                                          Comm* comm = nullptr, ExecOrderOut* exo = nullptr);
 // ipcfp_generate_log_proof_resident: the same call with a log filter as the predicate
 ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags);
-// verify.cu — batched verifiers over a witness store; log_filter (if not null) is check_event in place of `filter`
+// verify.cu — batched verifiers over a witness store; n_log_filters > 0: check_event is "matches at least one of log_filters[]", in place
+// of `filter`
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
-                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter = nullptr);
+                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0);
 void verify_storage_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results);
 // … the same with the proofs (and the data blob, padded by 16 bytes) already in device memory
 void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
-                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter = nullptr);
+                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0);
 void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* d_proofs, uint64_t n, uint8_t* results);
 // json_parse.cu — ipcfp_verify_bundle_json
+// (log_filters, n_log_filters): check_event of the event verifier, as verify_event_proofs takes it
 ipcfp_bundle_verdict* verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
-                                         ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter);
+                                         ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
+                                         const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0);
 void bundle_verdict_free(ipcfp_bundle_verdict* v);
 void event_result_free(ipcfp_event_result* r);
 struct WitnessOut;
@@ -229,9 +232,9 @@ struct FetchPlan {
     uint32_t n_levels = 0;
     float ms_total = 0.f;
 };
-// log_filter (if not null, with no specs): rule 3's predicate in place of the event specs'
+// n_log_filters > 0 (with no event specs): rule 3's predicate is "matches at least one of log_filters[]", in place of the event specs'
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out, const ipcfp_log_filter* log_filter = nullptr);
+                FetchPlan& out, const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);

@@ -160,7 +160,8 @@ template <class VS, class VE> static void run_verifiers(const Trust& tr, uint64_
 
 // the composition itself, on the host parser's arrays
 static void verify_host_path(VerdictBox& B, const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn tp, ipcfp_trusted_child_header_fn tc,
-                             void* ctx, const ipcfp_event_spec* filter, Clock::time_point t0) {
+                             void* ctx, const ipcfp_event_spec* filter, const ipcfp_log_filter* lf, uint64_t n_lf,
+                             Clock::time_point t0) {
     ipcfp_bundle_verdict& v = B.v;
     const ipcfp_status st = ipcfp_bundle_from_json(json, len, &B.pb);
     if (st != IPCFP_OK) throw Error(st, "ipcfp_bundle_from_json refused the text");
@@ -185,13 +186,14 @@ static void verify_host_path(VerdictBox& B, const char* json, uint64_t len, int 
     const Clock::time_point t2 = Clock::now();
     run_verifiers(tr, pb.n_storage_proofs, pb.n_event_proofs,
                   [&] { verify_storage_proofs(s.get(), &pb.tipset, pb.storage_proofs, pb.n_storage_proofs, B.sres.data()); },
-                  [&] { verify_event_proofs(s.get(), &pb.tipset, pb.event_proofs, pb.n_event_proofs, pb.data_blob, pb.data_blob_size, filter, B.eres.data()); });
+                  [&] { verify_event_proofs(s.get(), &pb.tipset, pb.event_proofs, pb.n_event_proofs, pb.data_blob, pb.data_blob_size, filter, B.eres.data(), lf, n_lf); });
     v.ms_verify = ms_since(t2);
 }
 
 // the device path; false: the text is not canonical (nothing of B has been set)
 static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn tp, ipcfp_trusted_child_header_fn tc,
-                               void* ctx, const ipcfp_event_spec* filter, Clock::time_point t0) {
+                               void* ctx, const ipcfp_event_spec* filter, const ipcfp_log_filter* lf, uint64_t n_lf,
+                               Clock::time_point t0) {
     if (len < 2 || len > 0xffffff00ull) return false;   // record starts are u32
     try { check_device(device); }
     catch (const Error&) { return false; }   // the host path meets the same failure where the composition does
@@ -278,20 +280,21 @@ static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, in
     v.ms_store = ms_since(t1);
     const Clock::time_point t2 = Clock::now();
     run_verifiers(tr, nS, nE, [&] { verify_storage_proofs_dev(s.get(), &v.tipset, d_sp.p, nS, B.sres.data()); },
-                  [&] { verify_event_proofs_dev(s.get(), &v.tipset, d_ep.p, nE, d_blob.p, m.e_total, filter, B.eres.data()); });
+                  [&] { verify_event_proofs_dev(s.get(), &v.tipset, d_ep.p, nE, d_blob.p, m.e_total, filter, B.eres.data(), lf, n_lf); });
     v.ms_verify = ms_since(t2);
     return true;
 }
 
 ipcfp_bundle_verdict* verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
-                                         ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter) {
+                                         ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
+                                         const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
     const Clock::time_point t0 = Clock::now();
     std::unique_ptr<VerdictBox> B(new VerdictBox());
     memset(&B->v, 0, sizeof B->v);
-    if (!verify_device_path(*B, json, len, device, trusted_parent, trusted_child, trust_ctx, filter, t0)) {
+    if (!verify_device_path(*B, json, len, device, trusted_parent, trusted_child, trust_ctx, filter, log_filters, n_log_filters, t0)) {
         B.reset(new VerdictBox());
         memset(&B->v, 0, sizeof B->v);
-        verify_host_path(*B, json, len, device, trusted_parent, trusted_child, trust_ctx, filter, t0);
+        verify_host_path(*B, json, len, device, trusted_parent, trusted_child, trust_ctx, filter, log_filters, n_log_filters, t0);
     }
     B->v.ms_total = ms_since(t0);
     return &B.release()->v;

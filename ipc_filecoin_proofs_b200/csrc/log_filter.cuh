@@ -102,6 +102,18 @@ __device__ __forceinline__ bool event_matches(const uint8_t* p, const EvLog& ev,
     return ok;
 }
 
+// A set of filters (ipcfp_verify_event_proofs_any's check_event): an event matches when it matches at least one of f[0..n). The
+// structs live in device memory, each pointing at its own large sets.
+struct LogFilterAny {
+    const LogFilter* f;
+    uint32_t n;
+};
+__device__ __forceinline__ bool event_matches(const uint8_t* p, const EvLog& ev, const LogFilterAny& a) {
+    for (uint32_t k = 0; k < a.n; k++)
+        if (event_matches(p, ev, a.f[k])) return true;
+    return false;
+}
+
 // ------------------------------------------------------------------------------------------ host side
 // The filter as the kernels take it. The large sets and their bitmaps go into `dev` (one upload); place() points the struct at the
 // device copy.
@@ -124,8 +136,8 @@ inline uint32_t lf_bitmap_lb(uint64_t n) {   // 64 bits per value, at least 4096
     return lb;
 }
 
-// Checks the filter (ipcfp.h's rules) and builds it; throws Error(IPCFP_ERR_INVALID_ARG) on a refused filter.
-inline void log_filter_build(const ipcfp_log_filter* in, LogFilterHost& out) {
+// ipcfp.h's rules; throws Error(IPCFP_ERR_INVALID_ARG) on a refused filter
+inline void log_filter_check(const ipcfp_log_filter* in) {
     if (!in) throw Error(IPCFP_ERR_INVALID_ARG, "null log filter");
     if (in->n_positions > 4) throw Error(IPCFP_ERR_INVALID_ARG, "log filter: n_positions > 4");
     if (in->n_emitters > IPCFP_LOG_FILTER_MAX_EMITTERS) throw Error(IPCFP_ERR_INVALID_ARG, "log filter: more emitters than IPCFP_LOG_FILTER_MAX_EMITTERS");
@@ -135,6 +147,11 @@ inline void log_filter_build(const ipcfp_log_filter* in, LogFilterHost& out) {
         if (in->n_values[k] > IPCFP_LOG_FILTER_MAX_VALUES) throw Error(IPCFP_ERR_INVALID_ARG, "log filter: more values than IPCFP_LOG_FILTER_MAX_VALUES");
         if (in->n_values[k] && !in->values[k]) throw Error(IPCFP_ERR_INVALID_ARG, "log filter: null values with a nonzero count");
     }
+}
+
+// Checks the filter (log_filter_check) and builds it.
+inline void log_filter_build(const ipcfp_log_filter* in, LogFilterHost& out) {
+    log_filter_check(in);
     LogFilter& f = out.f;
     memset(&f, 0, sizeof f);
     out.dev.clear();
@@ -177,5 +194,38 @@ inline void log_filter_build(const ipcfp_log_filter* in, LogFilterHost& out) {
         for (uint64_t x : e) set_bit(4, lf_hash64(x, f.lb[4]));
     }
 }
+
+// filters[0..n) as the kernels take them, in one upload: n LogFilter structs, then every filter's large sets and bitmaps.
+// check() / build() check every filter before any is built (a refused filter's Error carries its position); place(d) writes `words`
+// for the device copy at d.
+struct LogFilterSet {
+    std::vector<LogFilterHost> h;
+    std::vector<uint64_t> words;
+    static constexpr uint64_t FW = (sizeof(LogFilter) + 7) / 8;   // words per struct
+
+    static void check(const ipcfp_log_filter* in, uint64_t n) {
+        if (n && !in) throw Error(IPCFP_ERR_INVALID_ARG, "null log filters");
+        for (uint64_t k = 0; k < n; k++) {
+            try { log_filter_check(&in[k]); }
+            catch (Error& e) { e.index = k; throw; }
+        }
+    }
+    void build(const ipcfp_log_filter* in, uint64_t n) {
+        check(in, n);
+        h.resize(n);
+        uint64_t total = FW * n;
+        for (uint64_t k = 0; k < n; k++) { log_filter_build(&in[k], h[k]); total += h[k].dev.size(); }
+        words.assign(total, 0);
+    }
+    void place(const uint64_t* d) {
+        uint64_t off = FW * h.size();
+        for (size_t k = 0; k < h.size(); k++) {
+            h[k].place(d + off);
+            memcpy(words.data() + FW * k, &h[k].f, sizeof(LogFilter));
+            std::copy(h[k].dev.begin(), h[k].dev.end(), words.begin() + off);
+            off += h[k].dev.size();
+        }
+    }
+};
 
 }  // namespace ipcfp

@@ -104,11 +104,11 @@ __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, 
 }
 
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out, const ipcfp_log_filter* log_filter) {
+                FetchPlan& out, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
     if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
-    LogFilterHost lfh;
-    if (log_filter) log_filter_build(log_filter, lfh);
-    const bool events = n_especs || log_filter;   // the event path's rules (1–3) apply
+    LogFilterSet fs;
+    fs.build(log_filters, n_log_filters);
+    const bool events = n_especs || n_log_filters;   // the event path's rules (1–3) apply
     if (n_sspecs && !td.has_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
     for (uint64_t k = 0; k < n_especs; k++)
         if (!especs[k].event_signature || !especs[k].topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
@@ -161,17 +161,12 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     if (n_sspecs) memcpy(h.data() + o_ss, sspecs, n_sspecs * sizeof(ipcfp_storage_spec));
     AsyncBuf<uint8_t> d(size, st);
     IPCFP_CUDA(cudaMemcpyAsync(d.p, h.data(), size, cudaMemcpyHostToDevice, st));
-    // the log filter and its large sets, in one upload
-    const uint64_t lf_words = (sizeof(LogFilter) + 7) / 8;
+    // the log filters and their large sets, in one upload (fs.words outlives the copy: the stream is synchronised before return)
     AsyncBuf<uint64_t> d_lf;
-    std::vector<uint64_t> h_lf;
-    if (log_filter) {
-        d_lf.alloc(lf_words + lfh.dev.size(), st);
-        lfh.place(d_lf.p + lf_words);
-        h_lf.assign(lf_words + lfh.dev.size(), 0);
-        memcpy(h_lf.data(), &lfh.f, sizeof(LogFilter));
-        std::copy(lfh.dev.begin(), lfh.dev.end(), h_lf.begin() + lf_words);
-        IPCFP_CUDA(cudaMemcpyAsync(d_lf.p, h_lf.data(), h_lf.size() * 8, cudaMemcpyHostToDevice, st));
+    if (n_log_filters) {
+        d_lf.alloc(fs.words.size(), st);
+        fs.place(d_lf.p);
+        IPCFP_CUDA(cudaMemcpyAsync(d_lf.p, fs.words.data(), fs.words.size() * 8, cudaMemcpyHostToDevice, st));
     }
 
     AsyncBuf<uint32_t> needed(nwords, st), visited(PLAN_CLASSES * nwords, st);
@@ -229,9 +224,9 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     // ---- rule 3: the receipts-AMT paths of the matching receipts, once every events-AMT block of N(S) is in the store
     if (n_rcpt && events_complete) {
         const uint8_t* rr = d.p + o_roots + 38ull * (td.n_parents + 1);
-        if (log_filter) {
-            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const LogFilter*)d_lf.p, 1,
-                                                              rr, needed.p, miss.p, ctr.p);
+        if (n_log_filters) {
+            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const LogFilter*)d_lf.p,
+                                                              n_log_filters, rr, needed.p, miss.p, ctr.p);
         } else {
             k_plan_matchers<<<1, 32, 0, st>>>(d.p + o_sig, (const uint64_t*)(d.p + o_so), (const uint32_t*)(d.p + o_sl), n_especs, (Matcher*)(d.p + o_m));
             IPCFP_LAUNCH_CHECK();

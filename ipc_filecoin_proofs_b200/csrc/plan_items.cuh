@@ -65,7 +65,7 @@ __device__ __forceinline__ uint32_t plan_children(const uint8_t* p, uint32_t len
 
 // ---- rule 3: does receipt i match one of the specs (pass 1's rule: walk_events over the whole events AMT, actor filter included)?
 // A receipt whose events AMT fails to decode (or, which the gate rules out, lacks a block) does not match.
-// P: Matcher (n_specs specs) or LogFilter (one filter).
+// P: Matcher (n_specs specs) or LogFilter (n_specs filters: a receipt matches when one of them does).
 template <class P>
 __device__ __forceinline__ bool plan_receipt_matches(const StoreView* s_dev, uint32_t root_blk, const P* m, uint64_t n_specs) {
     for (uint64_t k = 0; k < n_specs; k++) {

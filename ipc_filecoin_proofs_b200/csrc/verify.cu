@@ -49,14 +49,14 @@ static void throw_verify_error(uint64_t key) {
 }
 
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
-                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter) {
+                         const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
     s->use();
     if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
     if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
     if (n && (!proofs || !results)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
     if (n == 0) {   // a refused log filter fails whatever the proofs are
-        LogFilterHost lfh;
-        if (log_filter) log_filter_build(log_filter, lfh);
+        LogFilterSet fs;
+        fs.build(log_filters, n_log_filters);
         return;
     }
     cudaStream_t st = s->stream;
@@ -64,16 +64,16 @@ void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event
     AsyncBuf<ipcfp_event_proof> d_proofs(n, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_event_proof), cudaMemcpyHostToDevice, st));
     if (blob_size) IPCFP_CUDA(cudaMemcpyAsync(d_blob.p, data_blob, blob_size, cudaMemcpyHostToDevice, st));
-    verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results, log_filter);
+    verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results, log_filters, n_log_filters);
 }
 
 // the proofs and their data blob (blob_size bytes + 16 of padding) already on the device, on the store's device
 void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
-                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filter) {
+                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
     if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
     if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
-    LogFilterHost lfh;
-    if (log_filter) log_filter_build(log_filter, lfh);
+    LogFilterSet fs;
+    fs.build(log_filters, n_log_filters);
     if (n == 0) return;
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
@@ -165,17 +165,18 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         k_verify_events<<<div_up(n * 32, 128), 128, 0, st>>>(va); IPCFP_LAUNCH_CHECK();
     };
     AsyncBuf<uint64_t> d_sets;
-    if (log_filter) {   // the filter and its large sets in one upload
-        const uint64_t fw = (sizeof(LogFilter) + 7) / 8;
-        d_sets.alloc(lfh.dev.size() + fw, st);
-        lfh.place(d_sets.p + fw);
-        std::vector<uint64_t> h(fw + lfh.dev.size(), 0);
-        memcpy(h.data(), &lfh.f, sizeof(LogFilter));
-        std::copy(lfh.dev.begin(), lfh.dev.end(), h.begin() + fw);
+    if (n_log_filters) {   // the filters, their large sets and the LogFilterAny in one upload
+        const uint64_t aw = (sizeof(LogFilterAny) + 7) / 8;
+        d_sets.alloc(fs.words.size() + aw, st);
+        fs.place(d_sets.p + aw);
+        std::vector<uint64_t> h(aw, 0);
+        const LogFilterAny any{(const LogFilter*)(d_sets.p + aw), (uint32_t)n_log_filters};
+        memcpy(h.data(), &any, sizeof any);
+        h.insert(h.end(), fs.words.begin(), fs.words.end());
         IPCFP_CUDA(cudaMemcpyAsync(d_sets.p, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));   // h is a stack object
-        VerifyEventArgsT<LogFilter> va;
-        va.filter = (const LogFilter*)d_sets.p;
+        VerifyEventArgsT<LogFilterAny> va;
+        va.filter = (const LogFilterAny*)d_sets.p;
         launch(va);
     } else {
         VerifyEventArgs va;

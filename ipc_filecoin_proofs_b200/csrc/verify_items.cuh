@@ -207,8 +207,8 @@ __device__ __forceinline__ bool verify_check(const Matcher* f, const uint8_t* eb
     }
     return true;
 }
-// check_event: the whole log filter, emitter set included
-__device__ __forceinline__ bool verify_check(const LogFilter* f, const uint8_t* eblk, const EvLog& ev) { return event_matches(eblk, ev, *f); }
+// check_event: a set of log filters, emitter sets included; one filter is the set of one
+__device__ __forceinline__ bool verify_check(const LogFilterAny* f, const uint8_t* eblk, const EvLog& ev) { return event_matches(eblk, ev, *f); }
 
 template <class F> struct VerifyEventArgsT {
     StoreView store;
