@@ -167,7 +167,7 @@ typedef struct ipcfp_witness {
     const uint8_t* cids;      /* n_blocks*38, sorted by (version, codec, multihash) */
     const uint64_t* offsets;  /* n_blocks: block i = blob[offsets[i] .. offsets[i]+lengths[i])   */
     const uint32_t* lengths;  /* n_blocks                                                        */
-    const uint8_t* blob;      /* block bytes; blocks may sit in any order / with padding in here. NULL with IPCFP_WITNESS_BY_REFERENCE: offsets then index the blob given to ipcfp_store_create */
+    const uint8_t* blob;      /* block bytes; blocks may sit in any order / with padding in here (pad bytes unspecified). NULL with IPCFP_WITNESS_BY_REFERENCE: offsets then index the blob given to ipcfp_store_create */
     uint64_t blob_size;
 } ipcfp_witness;
 

@@ -28,6 +28,7 @@ __global__ void __launch_bounds__(128) k_storage_proofs(StorageArgs a) {
     Recorder rec{a.rec_list + t * REC_CAP, 0, a.wbits, false};
     rec.rank_of = a.store.rank_of;
     ipcfp_storage_proof q;
+    memset(&q, 0, sizeof q);   // the 4 bytes of tail padding too: the proofs reach the caller byte for byte (raw_proofs, the verifiers)
     Fail f{0, 0};
     if (!storage_proof_one(a, t, rec, q, f)) { report_error(a.err, ST_STORAGE, t, f.code, f.detail); a.rec_n[t] = 0; return; }
     if (rec.overflow) { report_error(a.err, ST_STORAGE, t, DC_UNSUPPORTED, 2); a.rec_n[t] = 0; return; }
