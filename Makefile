@@ -51,6 +51,6 @@ clean:
 
 # The host-compiled device headers (tests/host_fuzz) and the JSON parser under AddressSanitizer + UBSan (DESIGN.md §7.12)
 sanitize:
-	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_tail_bytes_host.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py tests/test_rpc_json_host.py tests/test_rpc_blocks_host.py tests/test_plan_fetch_host.py tests/test_resolve_host.py tests/test_log_filter_host.py tests/test_log_bundle_host.py -q
+	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_tail_bytes_host.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py tests/test_rpc_json_host.py tests/test_rpc_blocks_host.py tests/test_plan_fetch_host.py tests/test_resolve_host.py tests/test_log_filter_host.py tests/test_log_bundle_host.py tests/test_message_proof_host.py -q
 
 .PHONY: all clean sanitize

@@ -321,6 +321,34 @@ ipcfp_status ipcfp_generate_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, 
                                                ipcfp_event_result** out);
 ipcfp_status ipcfp_generate_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_log_filter* filter, uint32_t flags,
                                       ipcfp_event_result** out);
+/* The logs of given messages: eth_getTransactionReceipt(tx).logs with a proof, for the messages a caller names by CID.
+ * message_cids (n*38) are message CIDs as the parent blocks' message AMTs hold them: the CIDs reconstruct_execution_order yields (the
+ * `Cid` fields of Filecoin.ChainGetParentMessages). filter may be NULL: every log extract_evm_log accepts.
+ *   Selection  receipt i is selected when i < n_exec, i < n_receipts and exec[i] is one of message_cids.
+ *   Result     what ipcfp_generate_log_proof_resident gives with the same filter (NULL: the all-wildcard filter) and flags
+ *              (IPCFP_WITNESS_BY_REFERENCE, IPCFP_RESULT_JSON, IPCFP_SCAN_SKIP_TX_AMTS), with its receipt loop restricted to the selected
+ *              receipts: matching_indices are the selected receipts with at least one matching event, proofs are in (exec_index,
+ *              event_index) order, the witness is the base witness, the message AMTs and the receipts-AMT paths and events AMTs of the
+ *              matching selected receipts. It is an ordinary EventProofBundle: ipcfp_verify_event_proofs* and ipcfp_verify_bundle_json
+ *              accept it.
+ *   Reads      the events-AMT blocks of unselected receipts are never read: a store that lacks them, or holds other bytes under their
+ *              CIDs, gives the same result.
+ *   Failures   a fault in the header, TxMeta or message AMTs as ipcfp_generate_log_proof_resident reports it; after that the first fault
+ *              of the restricted loop over the selected receipts in ascending order (pass 1's events-AMT decode, then pass 2's reads),
+ *              status and index as for the log-filter call.
+ *   exec_indices (caller-allocated, n entries): exec_indices[j] is message j's position in the execution order, UINT64_MAX when the
+ *              tipset did not execute it. Duplicates are allowed and reported per position; a CID the tipset did not execute is not an
+ *              error. Written only when the call succeeds.
+ *   Refusals   IPCFP_ERR_INVALID_ARG before any device work: message_cids or exec_indices NULL with n > 0, n > IPCFP_MESSAGE_MAX, an
+ *              invalid filter (the rules of ipcfp_log_filter).
+ * ipcfp_generate_message_log_proof = ipcfp_tipset_upload, then the resident call. */
+#define IPCFP_MESSAGE_MAX 65536u
+ipcfp_status ipcfp_generate_message_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids /* n*38 */, uint64_t n,
+                                                       const ipcfp_log_filter* filter /* may be NULL */, uint32_t flags, uint64_t* exec_indices,
+                                                       ipcfp_event_result** out);
+ipcfp_status ipcfp_generate_message_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const uint8_t* message_cids /* n*38 */, uint64_t n,
+                                              const ipcfp_log_filter* filter /* may be NULL */, uint32_t flags, uint64_t* exec_indices,
+                                              ipcfp_event_result** out);
 /* The CUDA stream (cudaStream_t) all work of this store is issued on — for callers that time with
  * CUDA events or order their own device work after the engine's. */
 void* ipcfp_store_stream(ipcfp_store* s);
@@ -490,6 +518,13 @@ void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p);
  * rule 3's predicate (the receipts with a matching event add their receipts-AMT paths). Any flag bit is IPCFP_ERR_INVALID_ARG. */
 ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
                                            ipcfp_fetch_plan** out);
+/* One fetch round for ipcfp_generate_message_log_proof_resident: the rules of ipcfp_plan_fetch_log_resident, with two changes. While any
+ * TxMeta or message-AMT block is missing (the execution order, and so the selection, needs all of them), the round plans the base roots,
+ * the TxMeta blocks and the message AMTs only. Once they are all present, the planner builds the execution order on the device and plans
+ * the events AMTs of the selected receipts only, and the receipts-AMT paths of the selected receipts that match. exec_indices is not
+ * reported. Refusals are those of the generate call; any flag bit is IPCFP_ERR_INVALID_ARG. */
+ipcfp_status ipcfp_plan_fetch_message_log_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids /* n*38 */, uint64_t n,
+                                                   const ipcfp_log_filter* filter /* may be NULL */, uint32_t flags, ipcfp_fetch_plan** out);
 /* One fetch round for ipcfp_generate_log_bundle_resident: rules 1–4 of ipcfp_plan_fetch_resident, with rule 3's predicate "matches at
  * least one of filters[]". ipcfp_plan_fetch_log_resident is the case of one filter and no storage spec. Refused filters, flags and
  * storage specs fail as in ipcfp_generate_log_bundle_resident / ipcfp_plan_fetch_resident. */

@@ -520,6 +520,37 @@ inline EventProofBundle generate_log_proof(GpuBlockstore& store, const ApiTipset
     return b;
 }
 
+// The logs of given messages (ipcfp_generate_message_log_proof): the EventProofBundle of `filter` (none: every log) restricted to the
+// receipts of `message_cids`, and every message's position in the execution order (std::nullopt: the tipset did not execute it). Only
+// the selected receipts' events AMTs are read. More than IPCFP_MESSAGE_MAX messages or four topic positions is refused.
+struct MessageLogProof {
+    EventProofBundle bundle;
+    std::vector<std::optional<uint64_t>> exec_indices;
+};
+inline MessageLogProof generate_event_proof(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                            const std::vector<Cid>& message_cids, const std::optional<LogFilter>& filter = std::nullopt) {
+    if (filter && filter->topics.size() > 4) throw Error(IPCFP_ERR_INVALID_ARG, "generate_event_proof: more than four topic positions");
+    TipsetDesc t(parent, child, receipts);
+    std::vector<std::vector<uint8_t>> keep;
+    ipcfp_log_filter f;
+    if (filter) f = log_filter_c(*filter, keep);
+    std::vector<uint8_t> cids(IPCFP_CID_LEN * message_cids.size());
+    for (size_t k = 0; k < message_cids.size(); k++) memcpy(cids.data() + IPCFP_CID_LEN * k, message_cids[k].bytes.data(), IPCFP_CID_LEN);
+    std::vector<uint64_t> idx(message_cids.size());
+    ipcfp_event_result* r = nullptr;
+    check(ipcfp_generate_message_log_proof(store.raw(), t.c(), cids.empty() ? nullptr : cids.data(), message_cids.size(), filter ? &f : nullptr, 0,
+                                           idx.empty() ? nullptr : idx.data(), &r),
+          "generate_event_proof");
+    MessageLogProof m;
+    try {
+        m.bundle.proofs = event_proofs(*r, t);
+        m.bundle.blocks = proof_blocks(r->witness);
+    } catch (...) { ipcfp_event_result_free(r); throw; }
+    ipcfp_event_result_free(r);
+    for (uint64_t i : idx) m.exec_indices.push_back(i == UINT64_MAX ? std::nullopt : std::optional<uint64_t>(i));
+    return m;
+}
+
 // generate_storage_proof (storage/generator.rs:29-67) → (StorageProof, Vec<ProofBlock>)
 inline std::pair<StorageProof, std::vector<ProofBlock>> generate_storage_proof(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child,
                                                                                uint64_t actor_id, const H256& slot) {

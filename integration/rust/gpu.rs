@@ -577,6 +577,37 @@ pub fn generate_proof_bundle_logs_gpu(
     unified_bundle_of(out, parent, child, &desc)
 }
 
+/// The logs of given messages with their proofs (`ipcfp_generate_message_log_proof`): the EventProofBundle of `log_filter` (`None`:
+/// every log) restricted to the receipts of `message_cids`, and every message's position in the execution order (`None`: the tipset
+/// did not execute it). Only the selected receipts' events AMTs are read.
+pub fn generate_message_log_proof_gpu(
+    store: &GpuBlockstore,
+    parent: &ApiTipset,
+    child: &ApiTipset,
+    receipts: &[ApiReceipt],
+    message_cids: &[Cid],
+    log_filter: Option<&LogFilter>,
+) -> Result<(EventProofBundle, Vec<Option<u64>>)> {
+    let desc = TipsetDesc::new(parent, child, receipts)?;
+    let mut cids = Vec::with_capacity(message_cids.len() * CID_LEN);
+    for c in message_cids {
+        cids.extend_from_slice(&cid38(c)?);
+    }
+    let f = log_filter.map(log_filter_c).transpose()?;
+    let fp = f.as_ref().map_or(std::ptr::null(), |f| f as *const sys::ipcfp_log_filter);
+    let mut idx = vec![0u64; message_cids.len()];
+    let mut out = std::ptr::null_mut();
+    check(unsafe {
+        sys::ipcfp_generate_message_log_proof(store.h, &desc.raw(), cids.as_ptr(), message_cids.len() as u64, fp, 0, idx.as_mut_ptr(), &mut out)
+    })?;
+    let r = unsafe { &*out };
+    let res = (|| -> Result<EventProofBundle> {
+        Ok(EventProofBundle { proofs: event_proofs_of(r, parent, child)?, blocks: witness_blocks(&r.witness)? })
+    })();
+    unsafe { sys::ipcfp_event_result_free(out) };
+    Ok((res?, idx.into_iter().map(|i| if i == u64::MAX { None } else { Some(i) }).collect()))
+}
+
 /// The UnifiedProofBundle of an `ipcfp_bundle`, which it frees.
 fn unified_bundle_of(out: *mut sys::ipcfp_bundle, parent: &ApiTipset, child: &ApiTipset, desc: &TipsetDesc) -> Result<UnifiedProofBundle> {
     let b = unsafe { &*out };

@@ -186,6 +186,14 @@ extern "C" {
                                      especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_plan_fetch(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                             especs: *const ipcfp_event_spec, n_especs: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_generate_message_log_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, message_cids: *const u8, n: u64,
+                                                     filter: *const ipcfp_log_filter, flags: u32, exec_indices: *mut u64,
+                                                     out: *mut *mut ipcfp_event_result) -> ipcfp_status;
+    pub fn ipcfp_generate_message_log_proof(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, message_cids: *const u8, n: u64,
+                                            filter: *const ipcfp_log_filter, flags: u32, exec_indices: *mut u64,
+                                            out: *mut *mut ipcfp_event_result) -> ipcfp_status;
+    pub fn ipcfp_plan_fetch_message_log_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, message_cids: *const u8, n: u64,
+                                                 filter: *const ipcfp_log_filter, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_plan_fetch_log_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, filter: *const ipcfp_log_filter, flags: u32,
                                          out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_plan_fetch_log_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,

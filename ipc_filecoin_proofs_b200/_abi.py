@@ -58,6 +58,7 @@ class EventSpec(C.Structure):
 
 
 LOG_FILTER_MAX_VALUES = 65536
+MESSAGE_MAX = 65536   # IPCFP_MESSAGE_MAX: message CIDs of one ipcfp_generate_message_log_proof call
 LOG_FILTER_MAX_EMITTERS = 65536
 
 

@@ -50,7 +50,8 @@ EXPORTS = [
     "ipcfp_resolve_addresses", "ipcfp_resolve_result_free", "ipcfp_address_parse", "ipcfp_address_from_eth",
     "ipcfp_generate_log_proof", "ipcfp_generate_log_proof_resident", "ipcfp_plan_fetch_log_resident", "ipcfp_verify_event_proofs_log",
     "ipcfp_generate_log_bundle", "ipcfp_generate_log_bundle_resident", "ipcfp_plan_fetch_log_bundle_resident", "ipcfp_verify_event_proofs_any",
-    "ipcfp_verify_bundle_json_any",
+    "ipcfp_verify_bundle_json_any", "ipcfp_generate_message_log_proof", "ipcfp_generate_message_log_proof_resident",
+    "ipcfp_plan_fetch_message_log_resident",
 ]
 
 
@@ -134,6 +135,15 @@ def lib():
         L.ipcfp_generate_log_proof_resident.restype = C.c_int32
         L.ipcfp_generate_log_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32,
                                                         C.POINTER(C.POINTER(A.EventResultC))]
+        L.ipcfp_generate_message_log_proof.restype = C.c_int32
+        L.ipcfp_generate_message_log_proof.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC),
+                                                       C.c_uint32, C.c_void_p, C.POINTER(C.POINTER(A.EventResultC))]
+        L.ipcfp_generate_message_log_proof_resident.restype = C.c_int32
+        L.ipcfp_generate_message_log_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC),
+                                                                C.c_uint32, C.c_void_p, C.POINTER(C.POINTER(A.EventResultC))]
+        L.ipcfp_plan_fetch_message_log_resident.restype = C.c_int32
+        L.ipcfp_plan_fetch_message_log_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint32,
+                                                            C.POINTER(C.POINTER(A.FetchPlanC))]
         L.ipcfp_plan_fetch_log_resident.restype = C.c_int32
         L.ipcfp_plan_fetch_log_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32, C.POINTER(C.POINTER(A.FetchPlanC))]
         L.ipcfp_verify_event_proofs_log.restype = C.c_int32
@@ -435,6 +445,51 @@ class BlockStore:
         finally:
             lib().ipcfp_event_result_free(out)
 
+    @staticmethod
+    def _message_args(message_cids, log_filter):
+        cids = np.ascontiguousarray(message_cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+        f, fkeep = log_filter.as_c() if log_filter is not None else (None, None)
+        idx = np.zeros(len(cids), np.uint64)
+        return cids, (C.byref(f) if f is not None else None), fkeep, idx
+
+    def generate_message_log_proof(self, ts, message_cids, log_filter=None, flags=0):
+        """ipcfp_generate_message_log_proof: the logs of the given messages (message_cids: (n, 38) message CIDs as the message AMTs hold
+        them) that match log_filter (None: every log) → (A.EventResultPy, exec_indices): exec_indices[j] is message j's position in the
+        execution order, 2**64 - 1 when the tipset did not execute it."""
+        d, keep = A.make_tipset_desc(ts)
+        cids, fp, fkeep, idx = self._message_args(message_cids, log_filter)
+        out = C.POINTER(A.EventResultC)()
+        _check(lib().ipcfp_generate_message_log_proof(self._h, C.byref(d), cids.ctypes.data if cids.size else None, len(cids), fp, flags,
+                                                      idx.ctypes.data if idx.size else None, C.byref(out)))
+        try:
+            return A.event_result_from_c(out.contents), idx
+        finally:
+            lib().ipcfp_event_result_free(out)
+
+    def generate_message_log_proof_resident(self, tip, message_cids, log_filter=None, flags=0):
+        """ipcfp_generate_message_log_proof_resident against a ResidentTipset of this store → (A.EventResultPy, exec_indices). flags:
+        WITNESS_BY_REFERENCE, RESULT_JSON, SCAN_SKIP_TX_AMTS."""
+        cids, fp, fkeep, idx = self._message_args(message_cids, log_filter)
+        out = C.POINTER(A.EventResultC)()
+        _check(lib().ipcfp_generate_message_log_proof_resident(self._h, tip._h, cids.ctypes.data if cids.size else None, len(cids), fp, flags,
+                                                               idx.ctypes.data if idx.size else None, C.byref(out)))
+        try:
+            return A.event_result_from_c(out.contents), idx
+        finally:
+            lib().ipcfp_event_result_free(out)
+
+    def plan_fetch_messages(self, tip, message_cids, log_filter=None, flags=0):
+        """ipcfp_plan_fetch_message_log_resident → A.FetchPlanPy: one fetch round for generate_message_log_proof_resident(tip, message_cids,
+        log_filter)."""
+        cids, fp, fkeep, _ = self._message_args(message_cids, log_filter)
+        out = C.POINTER(A.FetchPlanC)()
+        _check(lib().ipcfp_plan_fetch_message_log_resident(self._h, tip._h, cids.ctypes.data if cids.size else None, len(cids), fp, flags,
+                                                           C.byref(out)))
+        try:
+            return A.fetch_plan_from_c(out.contents)
+        finally:
+            lib().ipcfp_fetch_plan_free(out)
+
     def generate_event_proof_shard(self, ts, spec, lo, hi, world, rank, flags=0):
         d, keep = A.make_tipset_desc(ts)
         cs = spec.as_c() if isinstance(spec, EventProofSpec) else spec
@@ -684,6 +739,13 @@ def fetch_log_bundle_until_complete(fetch, upload_tipset, storage_specs, log_fil
     plan_fetch_log_bundle."""
     return _fetch_loop(lambda store, tip: store.plan_fetch_log_bundle(tip, storage_specs, log_filters), fetch, upload_tipset, device,
                        verify_cids, max_rounds)
+
+
+def fetch_messages_until_complete(fetch, upload_tipset, message_cids, log_filter=None, device=0, verify_cids=True, max_rounds=10000):
+    """fetch_until_complete for generate_message_log_proof_resident(tip, message_cids, log_filter): the same loop, planned with
+    plan_fetch_messages."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch_messages(tip, message_cids, log_filter), fetch, upload_tipset, device, verify_cids,
+                       max_rounds)
 
 
 def _fetch_loop(plan_round, fetch, upload_tipset, device, verify_cids, max_rounds):

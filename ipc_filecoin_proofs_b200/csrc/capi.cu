@@ -324,6 +324,29 @@ ipcfp_status ipcfp_generate_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t
         *out = generate_log_proof(st, td, filter, flags);
     });
 }
+ipcfp_status ipcfp_generate_message_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n,
+                                                       const ipcfp_log_filter* filter, uint32_t flags, uint64_t* exec_indices, ipcfp_event_result** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = generate_message_log_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), message_cids, n, filter, flags, exec_indices);
+    });
+}
+ipcfp_status ipcfp_generate_message_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const uint8_t* message_cids, uint64_t n,
+                                              const ipcfp_log_filter* filter, uint32_t flags, uint64_t* exec_indices, ipcfp_event_result** out) {
+    return guard([&] {
+        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        // the resident call's refusals come before the upload: no device work for a refused request
+        if (n && (!message_cids || !exec_indices)) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs or exec indices with a nonzero count");
+        if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+        if (filter) log_filter_check(filter);
+        Store* st = reinterpret_cast<Store*>(s);
+        TipsetDev td;
+        tipset_upload(st, t, td);
+        *out = generate_message_log_proof(st, td, message_cids, n, filter, flags, exec_indices);
+    });
+}
 void* ipcfp_store_stream(ipcfp_store* s) { return s ? (void*)reinterpret_cast<Store*>(s)->stream : nullptr; }
 
 ipcfp_status ipcfp_read_storage_slots(ipcfp_store* s, const uint8_t root[IPCFP_CID_LEN], const uint8_t* slots, uint64_t k, ipcfp_slot_result** out) {
@@ -438,6 +461,18 @@ ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, cons
         if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
         log_filter_check(filter);
         plan_fetch_log_bundle(s, t, nullptr, 0, filter, 1, out);
+    });
+}
+ipcfp_status ipcfp_plan_fetch_message_log_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n,
+                                                   const ipcfp_log_filter* filter, uint32_t flags, ipcfp_fetch_plan** out) {
+    return guard([&] {
+        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+        plan_fetch_messages(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), message_cids, n, filter, box->plan);
+        box->fill();
+        *out = &box.release()->r;
     });
 }
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }

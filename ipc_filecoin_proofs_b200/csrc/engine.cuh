@@ -207,6 +207,13 @@ ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_ev
                                          Comm* comm = nullptr, ExecOrderOut* exo = nullptr);
 // ipcfp_generate_log_proof_resident: the same call with a log filter as the predicate
 ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags);
+// ipcfp_generate_message_log_proof_resident: that call with its receipt loop restricted to the receipts of message_cids (n*38, host);
+// filter null: every log extract_evm_log accepts. exec_indices[j] (host): request j's execution position, UINT64_MAX when not executed.
+ipcfp_event_result* generate_message_log_proof(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter,
+                                               uint32_t flags, uint64_t* exec_indices);
+// plan.cu's selection: has_sel[i] (device, n_receipts) = the receipt has an events root and is selected by message_cids (n*38, host)
+// against the execution order exo (the tipset's, built on this store); left as it is when nothing is selected
+void message_selection_mask(Store* s, TipsetDev& td, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint8_t* has_sel);
 // verify.cu — batched verifiers over a witness store; n_log_filters > 0: check_event is "matches at least one of log_filters[]", in place
 // of `filter`
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
@@ -233,8 +240,11 @@ struct FetchPlan {
     float ms_total = 0.f;
 };
 // n_log_filters > 0 (with no event specs): rule 3's predicate is "matches at least one of log_filters[]", in place of the event specs'
+// has_dev (device, n_receipts; null: the tipset's has-events-root flags): the receipts rules 1 and 3 take, those with a nonzero entry
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out, const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0);
+                FetchPlan& out, const ipcfp_log_filter* log_filters = nullptr, uint64_t n_log_filters = 0, const uint8_t* has_dev = nullptr);
+// ipcfp_plan_fetch_message_log_resident: one round for generate_message_log_proof (filter null: the all-wildcard filter)
+void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, FetchPlan& out);
 
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);

@@ -27,6 +27,7 @@
 #include "prims.cuh"
 #include "walk.cuh"
 #include "events_items.cuh"
+#include "msg_select_items.cuh"
 #include "pass1_stage.cuh"
 #include "rawcid.cuh"
 
@@ -47,6 +48,50 @@ __global__ void __launch_bounds__(128) k_pass2(Pass2ArgsT<P> a) {
     if (a.per_warp) { if (threadIdx.x & 31) return; t >>= 5; }
     if (t >= a.n_match) return;
     pass2_item(a, t);
+}
+
+// ------------------------------------------------------------------------------------------ message selection (per-item code: msg_select_items.cuh)
+// The requests sorted once (msg_sort_key): keys of one slice in the current order, and the final gather
+__global__ void k_msg_iota(uint32_t* perm, uint32_t n) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) perm[t] = t;
+}
+__global__ void k_msg_keys(const RawCid* __restrict__ req, const uint32_t* __restrict__ perm, uint32_t n, uint32_t q, uint32_t* keys) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) keys[t] = msg_sort_key(req[perm[t]], q);
+}
+__global__ void k_msg_gather(const RawCid* __restrict__ req, const uint32_t* __restrict__ perm, uint32_t n, RawCid* sorted, uint32_t* sorted_pos) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) { sorted[t] = req[perm[t]]; sorted_pos[t] = perm[t]; }
+}
+// sorted[0..n) = the requests in (CID words, input position) order, sorted_pos their input positions; enqueued on st
+static void sort_requests(const RawCid* req, uint32_t n, RawCid* sorted, uint32_t* sorted_pos, cudaStream_t st) {
+    if (!n) return;
+    const unsigned nb = radix_blocks(n);
+    AsyncBuf<uint32_t> keys(n, st), perm(n, st), ka(n, st), pa(n, st), hist((size_t)256 * nb + 256, st);
+    AsyncBuf<uint64_t> scan_tmp((size_t)256 * nb + 256, st), scratch(scan_scratch_elems(std::max<uint64_t>((uint64_t)256 * nb, n)) + 8, st);
+    k_msg_iota<<<div_up(n, 256), 256, 0, st>>>(perm.p, n); IPCFP_LAUNCH_CHECK();
+    for (uint32_t q = MSG_SORT_SLICES; q-- > 0;) {
+        k_msg_keys<<<div_up(n, 256), 256, 0, st>>>(req, perm.p, n, q, keys.p); IPCFP_LAUNCH_CHECK();
+        radix_sort_pairs(keys.p, perm.p, ka.p, pa.p, n, 32, hist.p, scan_tmp.p, scratch.p, st);
+    }
+    k_msg_gather<<<div_up(n, 256), 256, 0, st>>>(req, perm.p, n, sorted, sorted_pos); IPCFP_LAUNCH_CHECK();
+}
+// one thread per execution position: the requests that name it, and the selected-receipt bitmap
+__global__ void __launch_bounds__(256) k_msg_select(const RawCid* __restrict__ exec_raw, const uint32_t* __restrict__ exec_idx, const unsigned long long* n_exec,
+                                                    const RawCid* __restrict__ sorted, const uint32_t* __restrict__ sorted_pos, uint32_t n, uint64_t n_receipts,
+                                                    uint64_t* exec_indices, uint32_t* sel_bits) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= *n_exec) return;
+    if (msg_select_item(exec_raw, exec_idx, i, sorted, sorted_pos, n, n_receipts, exec_indices)) atomicOr(sel_bits + (i >> 5), 1u << (i & 31));
+}
+// one selected receipt per warp (lane 0 walks), as k_pass2 takes its matches; above 16 384 one per thread
+template <class P>
+__global__ void __launch_bounds__(128) k_msg_match(MsgMatchArgsT<P> a) {
+    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (a.per_warp) { if (threadIdx.x & 31) return; t >>= 5; }
+    if (t >= a.n_sel_max || t >= *a.n_sel) return;
+    msg_match_item(a, t);
 }
 
 // ------------------------------------------------------------------------------------------ setup + message AMT walk
@@ -553,6 +598,14 @@ struct EventCall {
     bool any_skip = false;
     PinnedArray rel;
     uint64_t json_len = 0;
+    // message selection (generate_message_log_proof): the requested CIDs (host), sorted once on the device, and what they select
+    const uint8_t* msg_cids = nullptr;
+    uint64_t n_msg = 0;
+    PinnedArray msg_h, exec_indices_h;
+    AsyncBuf<RawCid> msg_raw, msg_sorted;
+    AsyncBuf<uint32_t> msg_pos, sel_bits, sel;
+    AsyncBuf<uint64_t> d_exec_indices, wp_sel;
+    AsyncBuf<unsigned long long> n_sel;
 
     EventCall(Store* s_, TipsetDev& td_, const ipcfp_event_spec* spec_, uint32_t flags_, bool sharded_, uint64_t lo_, uint64_t hi_, Comm* comm_,
               ExecOrderOut* exo_)
@@ -934,6 +987,10 @@ struct EventCall {
             IPCFP_CUDA(cudaFuncSetAttribute(k_pass1_stage<P, 128, 4, 1, 4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
             k_pass1_stage<P, 128, 4, 1, 4, 3><<<div_up(N, 128), 128, smem, st>>>(p1); IPCFP_LAUNCH_CHECK();
         }
+        finish_pass1();
+    }
+    // pass 1's tail: the matching list, the proof and byte offsets, and their counts on the host
+    void finish_pass1() {
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS1], st));
         match_rel.alloc(N + 32, st);
         wp3.alloc((N + 31) / 32 + 8, st);
@@ -947,6 +1004,50 @@ struct EventCall {
         M = hw[DW_N_MATCH];
         pass1_nodes = hw[DW_STATS]; pass1_bytes = hw[DW_STATS + 1];
         n_proofs = hw[DW_N_PROOFS]; n_bytes = hw[DW_BLOB_BYTES];
+    }
+
+    // ---- message selection, in place of pass 1 (generate_message_log_proof). The requests go up as RawCid and are sorted on the
+    // engine stream ahead of k_setup (the same stream: nothing overlaps); the selection needs the execution order, so it runs behind the
+    // dedup.
+    void stage_messages() {
+        if (!n_msg) return;
+        msg_h = PinnedArray(s->pool, n_msg * sizeof(RawCid));
+        RawCid* h = msg_h.as<RawCid>();
+        for (uint64_t j = 0; j < n_msg; j++) h[j] = rawcid_from_bytes(msg_cids + 38 * j);
+        msg_raw.alloc(n_msg, st); msg_sorted.alloc(n_msg, st); msg_pos.alloc(n_msg, st);
+        IPCFP_CUDA(cudaMemcpyAsync(msg_raw.p, h, n_msg * sizeof(RawCid), cudaMemcpyHostToDevice, st));
+        sort_requests(msg_raw.p, (uint32_t)n_msg, msg_sorted.p, msg_pos.p, st);
+    }
+    // k_msg_select over the execution order → the selected receipts (ascending) and every request's execution index; then the match of
+    // the selected receipts only (k_msg_match: pass 1's per-receipt result) → match bits, counts and bytes of those receipts, zero
+    // elsewhere; then pass 1's tail. No events AMT of an unselected receipt is read.
+    void select_and_match() {
+        const uint64_t nw = (N + 31) / 32 + 8, n_sel_max = std::min<uint64_t>(n_msg, N);
+        d_exec_indices.alloc(n_msg + 1, st);
+        IPCFP_CUDA(cudaMemsetAsync(d_exec_indices.p, 0xff, (n_msg + 1) * 8, st));
+        sel_bits.alloc(nw, st); sel_bits.zero();
+        match_bits.alloc(nw, st); match_bits.zero();
+        cnt.alloc(N + 8, st); cnt.zero(); nby.alloc(N + 8, st); nby.zero();
+        pbase.alloc(N + 8, st); bbase.alloc(N + 8, st);
+        n_sel.alloc(1, st); n_sel.zero();
+        if (n_msg && nraw) {
+            k_msg_select<<<div_up(nraw, 256), 256, 0, st>>>(exec_raw.p, exec_idx.p, n_exec_dev, msg_sorted.p, msg_pos.p, (uint32_t)n_msg, N, d_exec_indices.p,
+                                                             sel_bits.p);
+            IPCFP_LAUNCH_CHECK();
+        }
+        if (n_sel_max) {
+            sel.alloc(n_sel_max + 32, st); wp_sel.alloc(nw, st);
+            bitmap_to_indices(sel_bits.p, (N + 31) / 32 * 32, sel.p, (uint64_t*)n_sel.p, wp_sel.p, scratch.p, st);
+            MsgMatchArgsT<P> a;
+            a.store = s->view; a.store_dev = s->view_dev.p; a.m_dev = d_matcher; a.events_roots = td.events_roots.p; a.has_root = td.has_root.p;
+            a.sel = sel.p; a.n_sel = n_sel.p; a.n_sel_max = n_sel_max;
+            a.match_bits = match_bits.p; a.cnt = cnt.p; a.nbytes = nby.p; a.err = dw + DW_ERR; a.stats = dw + DW_STATS;
+            a.per_warp = n_sel_max <= 16384 ? 1 : 0;
+            k_msg_match<<<div_up(a.per_warp ? n_sel_max * 32 : n_sel_max, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK();
+        }
+        exec_indices_h = PinnedArray(s->pool, (n_msg + 1) * 8);
+        if (n_msg) IPCFP_CUDA(cudaMemcpyAsync(exec_indices_h.p, d_exec_indices.p, n_msg * 8, cudaMemcpyDeviceToHost, st));
+        finish_pass1();
     }
 
     // ---- pass 2: receipts-AMT paths, events walks, EventProofs; the late witness blocks
@@ -1100,6 +1201,58 @@ ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_
     c.pass2();
     c.read_back();
     return c.fill();
+}
+
+// the same call with its receipt loop restricted to the receipts of the given messages (filter null: every log extract_evm_log accepts)
+ipcfp_event_result* generate_message_log_proof(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter,
+                                               uint32_t flags, uint64_t* exec_indices) {
+    if (n && (!message_cids || !exec_indices)) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs or exec indices with a nonzero count");
+    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+    ipcfp_log_filter any;
+    memset(&any, 0, sizeof any);
+    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr, nullptr);
+    c.filter = filter ? filter : &any;
+    c.msg_cids = message_cids;
+    c.n_msg = n;
+    c.stage();
+    c.stage_messages();
+    c.setup();
+    c.walk();
+    c.settle_walk();
+    c.dedup();
+    c.select_and_match();
+    c.pass2();
+    c.read_back();
+    ipcfp_event_result* r = c.fill();
+    if (n) memcpy(exec_indices, c.exec_indices_h.p, n * 8);
+    return r;
+}
+
+__global__ void k_msg_mask(const uint8_t* __restrict__ has_root, const uint32_t* __restrict__ sel_bits, uint64_t n, uint8_t* has_sel) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) has_sel[i] = has_root[i] && ((sel_bits[i >> 5] >> (i & 31)) & 1u) ? 1 : 0;
+}
+void message_selection_mask(Store* s, TipsetDev& td, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint8_t* has_sel) {
+    cudaStream_t st = s->stream;
+    const uint64_t N = td.n_receipts;
+    AsyncBuf<uint32_t> bits((N + 31) / 32 + 8, st);
+    bits.zero();
+    if (n && exo.n_exec) {
+        std::vector<RawCid> h(n);
+        for (uint64_t j = 0; j < n; j++) h[j] = rawcid_from_bytes(message_cids + 38 * j);
+        AsyncBuf<RawCid> raw(n, st), sorted(n, st);
+        AsyncBuf<uint32_t> pos(n, st);
+        AsyncBuf<uint64_t> idx(n, st);
+        AsyncBuf<unsigned long long> n_exec(1, st);
+        const unsigned long long ne = exo.n_exec;
+        IPCFP_CUDA(cudaMemcpyAsync(raw.p, h.data(), n * sizeof(RawCid), cudaMemcpyHostToDevice, st));
+        IPCFP_CUDA(cudaMemcpyAsync(n_exec.p, &ne, 8, cudaMemcpyHostToDevice, st));
+        sort_requests(raw.p, (uint32_t)n, sorted.p, pos.p, st);
+        k_msg_select<<<div_up(exo.n_exec, 256), 256, 0, st>>>(exo.exec_raw.p, exo.exec_idx.p, n_exec.p, sorted.p, pos.p, (uint32_t)n, N, idx.p, bits.p);
+        IPCFP_LAUNCH_CHECK();
+        if (N) { k_msg_mask<<<div_up(N, 256), 256, 0, st>>>(td.has_root.p, bits.p, N, has_sel); IPCFP_LAUNCH_CHECK(); }
+        IPCFP_CUDA(cudaStreamSynchronize(st));   // the host copies above are read until here
+    }
 }
 
 void event_result_free(ipcfp_event_result* r) { delete reinterpret_cast<EventResultBox*>(r); }

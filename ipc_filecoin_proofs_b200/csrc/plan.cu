@@ -104,7 +104,7 @@ __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, 
 }
 
 void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_event_spec* especs, uint64_t n_especs,
-                FetchPlan& out, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
+                FetchPlan& out, const ipcfp_log_filter* log_filters, uint64_t n_log_filters, const uint8_t* has_dev) {
     if ((n_sspecs && !sspecs) || (n_especs && !especs)) throw Error(IPCFP_ERR_INVALID_ARG, "null specs");
     LogFilterSet fs;
     fs.build(log_filters, n_log_filters);
@@ -118,6 +118,7 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     const StoreView& v = s->view;
     const uint64_t nwords = (s->n + 31) / 32 + 1;
     const uint64_t n_rcpt = events ? td.n_receipts : 0;
+    const uint8_t* has = has_dev ? has_dev : td.has_root.p;
 
     // the base roots (collect_base_witness, events/generator.rs:112-145; generate_storage_proof's child header and StateRoot), then every
     // spec's inputs, in one upload
@@ -201,7 +202,7 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
         for (uint64_t k = 0; k < nh; k++) seeds[k] = PlanItem{d.p + o_roots + 38 * k, kinds[k], kinds[k] == PK_TXMETA ? 3u : 0u};
         IPCFP_CUDA(cudaMemcpyAsync(cur.p, seeds.data(), nh * sizeof(PlanItem), cudaMemcpyHostToDevice, st));
     }
-    if (n_rcpt) { k_plan_seed_events<<<div_up(n_rcpt, 256), 256, 0, st>>>(td.events_roots.p, td.has_root.p, n_rcpt, cur.p + nh); IPCFP_LAUNCH_CHECK(); }
+    if (n_rcpt) { k_plan_seed_events<<<div_up(n_rcpt, 256), 256, 0, st>>>(td.events_roots.p, has, n_rcpt, cur.p + nh); IPCFP_LAUNCH_CHECK(); }
     uint32_t levels = 0;
     while (n) {
         ensure_miss(n);
@@ -225,12 +226,12 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     if (n_rcpt && events_complete) {
         const uint8_t* rr = d.p + o_roots + 38ull * (td.n_parents + 1);
         if (n_log_filters) {
-            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const LogFilter*)d_lf.p,
+            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, has, n_rcpt, (const LogFilter*)d_lf.p,
                                                               n_log_filters, rr, needed.p, miss.p, ctr.p);
         } else {
             k_plan_matchers<<<1, 32, 0, st>>>(d.p + o_sig, (const uint64_t*)(d.p + o_so), (const uint32_t*)(d.p + o_sl), n_especs, (Matcher*)(d.p + o_m));
             IPCFP_LAUNCH_CHECK();
-            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, td.has_root.p, n_rcpt, (const Matcher*)(d.p + o_m),
+            k_plan_match<<<div_up(n_rcpt, 128), 128, 0, st>>>(v, s->view_dev.p, td.events_roots.p, has, n_rcpt, (const Matcher*)(d.p + o_m),
                                                               n_especs, rr, needed.p, miss.p, ctr.p);
         }
         IPCFP_LAUNCH_CHECK();
@@ -265,6 +266,36 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     // The device order is the bytes' order, which is `Cid` order within one prefix. A CID of another prefix (one that no block of the
     // store has, so rarely more than a few) puts the list in `Cid` order on the host.
     if (mixed != UINT64_MAX) sort_cids_host(out.cids);
+}
+
+// The message call's round (include/ipcfp.h): the execution order first (the engine's own walk and dedup). While it cannot be built — a
+// TxMeta or message-AMT block is missing, or one does not decode, which the generator then reports — no receipt is taken, and the round
+// is the base roots, the TxMeta blocks and the message AMTs. Once it is built, the receipts rules 1 and 3 take are the selected ones.
+void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, FetchPlan& out) {
+    if (n && !message_cids) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs with a nonzero count");
+    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+    ipcfp_log_filter any;
+    memset(&any, 0, sizeof any);
+    if (filter) log_filter_check(filter);
+    s->use();
+    AsyncBuf<uint8_t> has(td.n_receipts + 64, s->stream);
+    has.zero();
+    ExecOrderOut exo;
+    bool have_order = true;
+    try {
+        ipcfp_event_spec dummy;
+        memset(&dummy, 0, sizeof dummy);
+        dummy.event_signature = "";
+        dummy.topic_1 = "";
+        (void)generate_event_proof(s, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, nullptr, &exo);
+    } catch (Error& e) {
+        // a block the walk lacks, or one that does not decode (the generator reports it): no receipt is taken this round. Anything
+        // else (device, allocation, unsupported input) is the planner's own failure.
+        if (e.status != IPCFP_ERR_MISSING_BLOCK && e.status != IPCFP_ERR_DECODE) throw;
+        have_order = false;
+    }
+    if (have_order) message_selection_mask(s, td, exo, message_cids, n, has.p);
+    plan_fetch(s, td, nullptr, 0, nullptr, 0, out, filter ? filter : &any, 1, has.p);
 }
 
 }  // namespace ipcfp
