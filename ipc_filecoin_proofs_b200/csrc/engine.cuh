@@ -167,7 +167,6 @@ struct ScopedStatus;  // capi.cu
 struct Comm;          // parallel.cu: NCCL communicator pair + exchange scratch of one rank
 
 void set_last_error(const std::string& msg, uint64_t index);
-ipcfp_status status_from_devcode(uint32_t code);
 
 // store.cu
 Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size,
@@ -199,12 +198,15 @@ void tipset_upload_json(Store* s, const char* parent, uint64_t parent_len, const
 void tipset_describe(TipsetDev& td, bool with_roots, ipcfp_tipset_info* out);
 // the reconstructed execution order of a tipset on the device (reconstruct_execution_order, events/utils.rs:16-30): exec[i] = exec_raw[exec_idx[i]]
 struct ExecOrderOut {
-    uint64_t n_exec = 0, nraw = 0;
+    uint64_t n_exec = 0;
     AsyncBuf<RawCid> exec_raw;
     AsyncBuf<uint32_t> exec_idx;
 };
+// the execution order of a tipset of n_parents parent blocks, from their TxMeta CIDs (n_parents*38, host): the message-AMT walk and the
+// dedup that generate_event_proof runs, with no witness and no receipts root (the batched verifier, the message fetch round)
+void build_execution_order(Store* s, uint32_t n_parents, const uint8_t* txmeta_cids, ExecOrderOut& out);
 ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
-                                         Comm* comm = nullptr, ExecOrderOut* exo = nullptr);
+                                         Comm* comm = nullptr);
 // ipcfp_generate_log_proof_resident: the same call with a log filter as the predicate
 ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags);
 // ipcfp_generate_message_log_proof_resident: that call with its receipt loop restricted to the receipts of message_cids (n*38, host);

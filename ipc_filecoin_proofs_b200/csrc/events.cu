@@ -504,47 +504,33 @@ void tipset_upload(Store* s, const ipcfp_tipset_desc* t, TipsetDev& td) {
 namespace {
 static constexpr size_t STAGE_TABLES = 32768;   // second half of the store's staging block: dense-walk tables
 
-// One generate_event_proof call: its arguments, its state and buffers, and its phases, which generate_event_proof runs in order.
-// comm != nullptr: this call is one shard of a multi-GPU call and runs the cross-shard protocol itself (parallel.cu). Failures are then
-// not thrown where they are seen: every rank keeps taking part in the collectives and all ranks fail together, with the error the
-// reference's sequential order meets first across ALL shards.
-// Host synchronisations, per mode:
-//   unsharded         snapshot_and_sync after the walk (again after a dense walk that gave up; once more for k_amt_first_fault),
-//                     pass1, pass2, read_back's witness join (IPCFP_RESULT_JSON: render_event_json's one before it), fill
-//   IPCFP_BFS_GENERAL, sharded, execution-order only: walk reads the prologue back first; run_general synchronises after its range
-//                     upload, after the fused rounds and once per level below them
-//   execution-order only: walk, snapshot_and_sync, then dedup reads n_exec back and the call ends
-//   sharded over NCCL: besides, every H0 / H2 gather, ShardExchange::agree_results and finish, a late H0 that fails, and fill's copy of
-//                     the union partition (IPCFP_SHARDED_UNION_TO_HOST)
-// P: the predicate. Matcher: `spec` is the call's EventProofSpec (t0 = keccak256(signature) is computed by k_setup). LogFilter: `filter`
-// is a log filter (unsharded calls only), its values raw, its large sets uploaded beside it.
-template <class P>
-struct EventCall {
+// The execution order of a tipset (events/generator.rs:122-196: collect_base_witness, record_transaction_amts, build_execution_order):
+// k_setup, the message-AMT walk and the first-seen dedup, with the host synchronisations and fault handling around them. Two modes,
+// fixed at construction:
+//   with witness  (generate_event_proof) base and message-AMT blocks are recorded (unless IPCFP_SCAN_SKIP_TX_AMTS), the receipts root
+//                 is loaded, and the witness snapshot and its copy start behind the walk
+//   order only    (build_execution_order) no witness and no receipts root: the verifier and the message fetch round
+// xch != nullptr: this call is one shard of a multi-GPU call (see EventCall); a failure is then kept in pend_tx / pend_err.
+struct ExecOrderBuild {
     Store* s;
     cudaStream_t st;
-    TipsetDev& td;
-    const ipcfp_event_spec* spec;
-    const ipcfp_log_filter* filter = nullptr;
-    uint32_t flags;
+    const TipsetDev* td;   // with witness: the call's tipset; null: order only
+    const bool with_witness;
+    uint32_t n_parents;
+    const uint8_t* txmeta_cids_h;
+    uint64_t n_receipts;
     bool sharded;
     uint64_t lo, hi;
-    Comm* comm;
-    ExecOrderOut* exo;
-    std::chrono::steady_clock::time_point t_enter;
-    uint64_t N = 0, nblk = 0;
-    bool skip_tx = false;
-    std::unique_ptr<ShardExchange> xch;
+    ShardExchange* xch;
+    bool skip_tx, by_ref;
+    uint64_t nblk;
     uint64_t pend_tx = IPCFP_NO_ERROR, pend_err = IPCFP_NO_ERROR;   // first failure seen so far (xch mode)
     unsigned long long* dw;
     uint64_t* hw;
     // stage
-    P mh;
-    size_t siglen = 0, tables_off = 0;
+    size_t tables_off = 0;
     AsyncBuf<uint8_t> small;
-    uint8_t *d_sig = nullptr, *d_cids = nullptr;
-    P* d_matcher = nullptr;
-    AsyncBuf<uint64_t> d_sets;   // LogFilter: the large sets and their bitmaps, and their pinned host copy
-    PinnedArray sets_h;
+    uint8_t* d_cids = nullptr;
     // setup
     AsyncBuf<uint32_t> wbits;
     uint32_t namt = 0;
@@ -556,7 +542,7 @@ struct EventCall {
     uint32_t frontier_cap = 0;
     uint64_t max_raw_dev = 0;
     bool force_general = false, plan_on_device = false;
-    SetupArgs sa;
+    SetupArgs sa{};   // order only: no parent, child or receipts-root CID (k_setup reads them to record the witness and load the root)
     // walk
     const Prologue* ph;   // the prologue's head as the host reads it, once publish_prologue and a synchronisation have run
     bool early_fault = false, missing_base = false;
@@ -584,33 +570,16 @@ struct EventCall {
     // dedup
     AsyncBuf<uint32_t> exec_idx, keep_bits;
     unsigned long long* n_exec_dev = nullptr;
-    // pass 1
-    AsyncBuf<uint32_t> match_bits, cnt, nby;
-    AsyncBuf<uint64_t> pbase, bbase;
-    AsyncBuf<uint32_t> match_rel;
-    AsyncBuf<uint64_t> wp3;
-    uint64_t n_exec = 0, M = 0, pass1_nodes = 0, pass1_bytes = 0, n_proofs = 0, n_bytes = 0;
-    // pass 2 and the result
-    std::unique_ptr<EventResultBox> box;
-    AsyncBuf<ipcfp_event_proof> d_proofs;
-    AsyncBuf<uint8_t> d_blob;
-    uint64_t mB = 0;
-    bool any_skip = false;
-    PinnedArray rel;
-    uint64_t json_len = 0;
-    // message selection (generate_message_log_proof): the requested CIDs (host), sorted once on the device, and what they select
-    const uint8_t* msg_cids = nullptr;
-    uint64_t n_msg = 0;
-    PinnedArray msg_h, exec_indices_h;
-    AsyncBuf<RawCid> msg_raw, msg_sorted;
-    AsyncBuf<uint32_t> msg_pos, sel_bits, sel;
-    AsyncBuf<uint64_t> d_exec_indices, wp_sel;
-    AsyncBuf<unsigned long long> n_sel;
 
-    EventCall(Store* s_, TipsetDev& td_, const ipcfp_event_spec* spec_, uint32_t flags_, bool sharded_, uint64_t lo_, uint64_t hi_, Comm* comm_,
-              ExecOrderOut* exo_)
-        : s(s_), st(s_->stream), td(td_), spec(spec_), flags(flags_), sharded(sharded_), lo(lo_), hi(hi_), comm(comm_), exo(exo_),
-          dw(s_->dev_words.p), hw(s_->host_words.p), ph((const Prologue*)(s_->host_words.p + HW_PROLOGUE)) {}
+    // order only: the tipset of n_parents parent blocks with these TxMeta CIDs (host)
+    ExecOrderBuild(Store* s_, uint32_t n_parents_, const uint8_t* txmeta_cids) : ExecOrderBuild(s_, nullptr, n_parents_, txmeta_cids, IPCFP_SCAN_SKIP_TX_AMTS) {}
+    // with witness: the tipset td_, the call's flags, its receipt range [lo, hi) and, sharded over NCCL, its exchange
+    ExecOrderBuild(Store* s_, const TipsetDev* td_, uint32_t n_parents_, const uint8_t* txmeta_cids, uint32_t flags, bool sharded_ = false,
+                   uint64_t lo_ = 0, uint64_t hi_ = 0, ShardExchange* xch_ = nullptr)
+        : s(s_), st(s_->stream), td(td_), with_witness(td_ != nullptr), n_parents(n_parents_), txmeta_cids_h(txmeta_cids),
+          n_receipts(td_ ? td_->n_receipts : 0), sharded(sharded_), lo(lo_), hi(hi_), xch(xch_), skip_tx((flags & IPCFP_SCAN_SKIP_TX_AMTS) != 0),
+          by_ref((flags & IPCFP_WITNESS_BY_REFERENCE) != 0), nblk(s_->n), dw(s_->dev_words.p), hw(s_->host_words.p),
+          ph((const Prologue*)(s_->host_words.p + HW_PROLOGUE)) {}
 
     void note_errors() {   // the fault words as the last publish left them
         if (!xch) { throw_first(hw[DW_TX_ERR], hw[DW_ERR]); return; }
@@ -620,95 +589,60 @@ struct EventCall {
     void publish_prologue() { publish_words(s, HW_PROLOGUE, PRO_HEAD_WORDS, pro.p); }
     void read_prologue() {   // the fault words as the prologue left them, and its head
         early_fault = hw[DW_ERR] != IPCFP_NO_ERROR || hw[DW_TX_ERR] != IPCFP_NO_ERROR;
-        if constexpr (std::is_same_v<P, Matcher>) memcpy(mh.t0, ph->t0, 32);
         receipts_root_blk = ph->misc[0];
         missing_base = ph->misc[1] != 0;
         last_round = 0;
         for (uint32_t k = 0; k < namt; k++) last_round = std::max(last_round, ph->misc[64 + k]);
-        nraw_total = shard_amt_ranges(namt, ph->amt_count, sharded, lo, hi, td.n_receipts, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS);
+        nraw_total = shard_amt_ranges(namt, ph->amt_count, sharded, lo, hi, n_receipts, h_rng.data(), h_rng.data() + 2 * IPCFP_MAX_PARENTS);
     }
     void ensure_scratch(uint64_t n) {   // scan scratch for n items
         if (scratch.n < scan_scratch_elems(n + 64) + 64) scratch.alloc(scan_scratch_elems(n + 64) + 64, st);
     }
 
-    // ---- checks, and the spec + tipset CIDs up in ONE copy from the store's pinned staging block (no host sync)
-    void stage() {
-        s->use();
-        t_enter = std::chrono::steady_clock::now();
-        LogFilterHost lfh;
-        if constexpr (std::is_same_v<P, Matcher>) {
-            if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
-        } else {
-            log_filter_build(filter, lfh);
-        }
-        // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
-        if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
-        if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !s->caller_blob)
-            throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_WITNESS_BY_REFERENCE needs a store made from a caller's blob (ipcfp_store_create)");
-        if (!sharded) { lo = 0; hi = td.n_receipts; }
-        if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
-        N = hi - lo;
-        nblk = s->n;
-        skip_tx = (flags & IPCFP_SCAN_SKIP_TX_AMTS) != 0;
-        if (comm) {
-            if (!sharded) throw Error(IPCFP_ERR_INVALID_ARG, "communicator given for an unsharded call");
-            if (s->class_prefix.size() > 1) throw Error(IPCFP_ERR_UNSUPPORTED, "sharded calls need a store with one CID prefix");
-            xch.reset(new ShardExchange(comm, s, lo, hi));
-        }
-
+    // ---- the call's device words reset; then a head of `head` bytes, which fill_head writes at its host address (zeroed), and the
+    // tipset CIDs go up in ONE copy from the store's pinned staging block (no host sync). Returns the head's device address.
+    template <class F>
+    uint8_t* stage(size_t head, F&& fill_head) {
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
         IPCFP_CUDA(cudaMemsetAsync(dw + DW_ERR, 0xff, 8, st));
         IPCFP_CUDA(cudaMemsetAsync(dw + DW_FRONTIER_A, 0, 40 * 8, st));   // the 40 counters behind the error word
         IPCFP_CUDA(cudaMemsetAsync(dw + DW_TX_ERR, 0xff, 8, st));
 
-        memset(&mh, 0, sizeof mh);
-        if constexpr (std::is_same_v<P, Matcher>) {
-            size_t n1 = strlen(spec->topic_1);
-            uint8_t t1[32];
-            memset(t1, 0, 32);
-            memcpy(t1, spec->topic_1, n1 < 32 ? n1 : 32);  // ascii_to_bytes32 (evm.rs:72-78)
-            memcpy(mh.t1, t1, 32);
-            mh.actor = spec->actor_id_filter;
-            mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
-            siglen = strlen(spec->event_signature);
-        } else {
-            if (!lfh.dev.empty()) {   // through pinned memory that lives as long as the call: no host synchronisation
-                sets_h = PinnedArray(s->pool, lfh.dev.size() * 8);
-                memcpy(sets_h.p, lfh.dev.data(), lfh.dev.size() * 8);
-                d_sets.alloc(lfh.dev.size(), st);
-                IPCFP_CUDA(cudaMemcpyAsync(d_sets.p, sets_h.p, lfh.dev.size() * 8, cudaMemcpyHostToDevice, st));
-            }
-            lfh.place(d_sets.p);
-            mh = lfh.f;
-        }
-        //   [0,1024) Matcher (t0 is filled in on the device) or LogFilter | signature, zero padded | parent, TxMeta, child, receipts-root CIDs
-        const size_t sig_cap = (siglen + 64) & ~(size_t)63;
-        const size_t cids_bytes = 38ull * (2 * td.n_parents + 2);
-        const size_t small_bytes = 1024 + sig_cap + cids_bytes + 64;
-        static_assert(sizeof(P) <= 1024, "the predicate must fit its staging slot");
+        //   head | TxMeta, parent, child, receipts-root CIDs (order only: the TxMeta CIDs)
+        const size_t cids_bytes = with_witness ? 38ull * (2 * n_parents + 2) : 38ull * n_parents;
+        const size_t small_bytes = head + cids_bytes + 64;
         tables_off = std::max<size_t>(STAGE_TABLES, (small_bytes + 63) & ~(size_t)63);
         if (!s->stage.p || s->stage.cap < tables_off + STAGE_TABLES) s->stage = PinnedArray(s->pool, tables_off + STAGE_TABLES);
-        small.alloc(small_bytes, st);
-        d_sig = small.p + 1024;                       // 8-byte aligned
-        d_cids = small.p + 1024 + sig_cap;
-        d_matcher = (P*)small.p;
         uint8_t* hs = s->stage.as<uint8_t>();
         memset(hs, 0, small_bytes);
-        memcpy(hs, &mh, sizeof(P));
-        if (siglen) memcpy(hs + 1024, spec->event_signature, siglen);
-        uint8_t* hc = hs + 1024 + sig_cap;
-        memcpy(hc, td.parent_cids.data(), td.parent_cids.size()); hc += td.parent_cids.size();
-        memcpy(hc, td.txmeta_cids.data(), td.txmeta_cids.size()); hc += td.txmeta_cids.size();
-        memcpy(hc, td.child_cid, 38); hc += 38;
-        memcpy(hc, td.receipts_root, 38);
+        fill_head(hs);
+        small.alloc(small_bytes, st);
+        d_cids = small.p + head;
+        uint8_t* hc = hs + head;
+        memcpy(hc, txmeta_cids_h, 38ull * n_parents); hc += 38ull * n_parents;
+        if (with_witness) {
+            memcpy(hc, td->parent_cids.data(), td->parent_cids.size()); hc += td->parent_cids.size();
+            memcpy(hc, td->child_cid, 38); hc += 38;
+            memcpy(hc, td->receipts_root, 38);
+        }
         IPCFP_CUDA(cudaMemcpyAsync(small.p, hs, small_bytes, cudaMemcpyHostToDevice, st));
+        return small.p;
+    }
+
+    // ---- the execution order: k_setup (sig / matcher: the event signature whose keccak256 it writes into the Matcher's t0; null for
+    // none), the walk and its settlement, the dedup
+    void build(const uint8_t* sig, uint32_t sig_len, Matcher* matcher) {
+        setup(sig, sig_len, matcher);
+        walk();
+        settle_walk();
+        dedup();
     }
 
     // ---- witness bitmap + k_setup
-    void setup() {
+    void setup(const uint8_t* sig, uint32_t sig_len, Matcher* matcher) {
         wbits.alloc((nblk + 31) / 32 + 8, st);
         wbits.zero();
-        namt = 2 * td.n_parents;   // k_setup seeds one frontier item per message AMT
+        namt = 2 * n_parents;   // k_setup seeds one frontier item per message AMT
         cap = 4 * nblk + 1024;
         fA_blk.alloc(cap, st); fA_meta.alloc(cap, st); fB_blk.alloc(cap, st); fB_meta.alloc(cap, st);
         fA_base.alloc(cap, st); fB_base.alloc(cap, st);
@@ -718,20 +652,20 @@ struct EventCall {
         frontier_cap = (uint32_t)std::min<uint64_t>(cap, 0xffffffffull);
         // Every message of a parent block is executed, so no message AMT counts more values than there are receipts: a dense walk of an
         // unsharded call writes at most n_parents × n_receipts entries (a plan above that goes to the general walk).
-        max_raw_dev = std::min<uint64_t>(8ull * cap, (uint64_t)td.n_parents * td.n_receipts + 1024);
+        max_raw_dev = std::min<uint64_t>(8ull * cap, (uint64_t)n_parents * n_receipts + 1024);
         force_general = getenv("IPCFP_BFS_GENERAL") != nullptr;   // read per call: tests toggle it
         // Unsharded calls plan the dense walk on the device (k_setup) and read the prologue back only together with the witness
         // snapshot's counts. A sharded call needs its share's length on the host before its walk (early H0, below), and the
-        // execution-order-only mode keeps its own sequence: both read the prologue back first (host synchronisation 1).
-        plan_on_device = !sharded && !exo && !force_general;
-        sa.store = s->view; sa.n_parents = td.n_parents;
-        sa.parent_cids = d_cids; sa.txmeta_cids = d_cids + 38ull * td.n_parents;
-        sa.child_cid = d_cids + 76ull * td.n_parents; sa.receipts_root = sa.child_cid + 38;
-        sa.skip_tx = skip_tx; sa.skip_receipts = exo ? 1 : 0; sa.wbits = wbits.p; sa.err = dw + DW_ERR; sa.txerr = dw + DW_TX_ERR;
+        // order-only mode has no receipt count for the device plan's bound: both read the prologue back first (host synchronisation 1).
+        plan_on_device = with_witness && !sharded && !force_general;
+        sa.store = s->view; sa.n_parents = n_parents;
+        sa.txmeta_cids = d_cids;
+        if (with_witness) { sa.parent_cids = d_cids + 38ull * n_parents; sa.child_cid = d_cids + 76ull * n_parents; sa.receipts_root = sa.child_cid + 38; }
+        sa.skip_tx = skip_tx; sa.skip_receipts = with_witness ? 0 : 1; sa.wbits = wbits.p; sa.err = dw + DW_ERR; sa.txerr = dw + DW_TX_ERR;
         sa.pro = pro.p;
         sa.f_blk = fA_blk.p; sa.f_meta = fA_meta.p; sa.f_base = fA_base.p; sa.f_count = dw + DW_FRONTIER_A;
-        sa.sig = d_sig; sa.sig_len = (uint32_t)siglen;
-        if constexpr (std::is_same_v<P, Matcher>) sa.matcher = d_matcher; else sa.matcher = nullptr;
+        sa.sig = sig; sa.sig_len = sig_len;
+        sa.matcher = matcher;
         sa.plan_dense = plan_on_device ? 1 : 0; sa.frontier_cap = frontier_cap; sa.max_raw = max_raw_dev;
         k_setup<<<1, 256, 0, st>>>(sa); IPCFP_LAUNCH_CHECK();
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_SETUP], st));
@@ -740,7 +674,7 @@ struct EventCall {
     // ---- message AMT walk (recording + raw execution list): dense if the plan holds, else general
     void walk() {
         counts.alloc(cap + 1024, st);
-        out_off.alloc(cap + 1024, st); scratch.alloc(scan_scratch_elems(std::max<uint64_t>(cap, N) + 64) + 64, st);
+        out_off.alloc(cap + 1024, st); scratch.alloc(scan_scratch_elems(std::max<uint64_t>(cap, hi - lo) + 64) + 64, st);
         ccount = dw + DW_FRONTIER_A; ncount = dw + DW_FRONTIER_B; total_dev = dw + DW_LEVEL_TOTAL;
         if (!plan_on_device) {   // the dense walk planned here
             publish_words(s, 0, DW_TX_ERR + 1);
@@ -879,7 +813,7 @@ struct EventCall {
     // Witness snapshot: base witness + every message-AMT block are final at this point — start moving them to the host while pass 1 /
     // pass 2 run (witness.cu). Publishes the error word, frontier counters, witness counts, dense-walk flag and gather split.
     void snapshot_and_sync(bool with_prologue) {
-        if (!exo) wbuild->snapshot(wbits.p);
+        if (with_witness) wbuild->snapshot(wbits.p);
         publish_words(s, 0, DW_SPLIT_BYTES + 1);
         if (with_prologue) publish_prologue();
         IPCFP_CUDA(cudaStreamSynchronize(st));
@@ -898,8 +832,10 @@ struct EventCall {
             xch_early = xch->all_early;
             if (xch_early) xch->start_exchange(exec_raw.p);
         }
-        wbuild.emplace(s);
-        wbuild->by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
+        if (with_witness) {
+            wbuild.emplace(s);
+            wbuild->by_ref = by_ref;
+        }
         snapshot_and_sync(plan_on_device);
         if (dense_used && hw[DW_DENSE_FAIL] != 0) {   // the AMTs are not what the dense walk assumes (or its plan was not ok): redo the walk with the general kernels
             dense_used = false;
@@ -935,7 +871,7 @@ struct EventCall {
             xch->agree_slices(pend_tx, pend_err, 0);
             throw_first(xch->g_tx, xch->g_err);
         }
-        if (!exo) wbuild->start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_SPLIT_IDX], hw[DW_SPLIT_BYTES]);
+        if (with_witness) wbuild->start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_SPLIT_IDX], hw[DW_SPLIT_BYTES]);
         if (xch && !xch_early) {
             // LATE H0 (some shard could not promise its slice before its walk was over): agree on the slices now and start the exchange
             xch->agree_slices(IPCFP_NO_ERROR, IPCFP_NO_ERROR, nraw);
@@ -944,8 +880,8 @@ struct EventCall {
         }
     }
 
-    // ---- first-seen dedup of the raw list: the execution order. False: execution-order-only mode, which ends here
-    bool dedup() {
+    // ---- first-seen dedup of the raw list: the execution order
+    void dedup() {
         exec_idx.alloc(nraw + 32, st); keep_bits.alloc((nraw + 31) / 32 + 8, st);
         n_exec_dev = dw + DW_N_EXEC;
         if (sharded) IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));   // execution order is resolved across ranks by the caller
@@ -963,15 +899,164 @@ struct EventCall {
             bitmap_to_indices(keep_bits.p, nraw, exec_idx.p, (uint64_t*)n_exec_dev, wp2.p, scratch.p, st);
         } else IPCFP_CUDA(cudaMemsetAsync(n_exec_dev, 0, 8, st));
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_EXEC_ORDER], st));
-        if (!exo) return true;
-        // execution-order-only mode (the batched verifier, verify.cu): hand the order over and stop before the scan
-        publish_words(s, DW_N_EXEC, 1);
-        IPCFP_CUDA(cudaStreamSynchronize(st));
-        exo->n_exec = hw[DW_N_EXEC];
-        exo->nraw = nraw;
-        exo->exec_raw = std::move(exec_raw);
-        exo->exec_idx = std::move(exec_idx);
-        return false;
+    }
+};
+
+// Requested message CIDs (n*38, host): up as RawCid through pinned memory and sorted once on the device (msg_sort_key), and what
+// they select in an execution order (k_msg_select)
+struct MsgRequests {
+    uint64_t n = 0;
+    PinnedArray h;
+    AsyncBuf<RawCid> raw, sorted;
+    AsyncBuf<uint32_t> pos;
+    void stage(Store* s, const uint8_t* cids, uint64_t n_) {
+        n = n_;
+        if (!n) return;
+        cudaStream_t st = s->stream;
+        h = PinnedArray(s->pool, n * sizeof(RawCid));
+        RawCid* hr = h.as<RawCid>();
+        for (uint64_t j = 0; j < n; j++) hr[j] = rawcid_from_bytes(cids + 38 * j);
+        raw.alloc(n, st); sorted.alloc(n, st); pos.alloc(n, st);
+        IPCFP_CUDA(cudaMemcpyAsync(raw.p, hr, n * sizeof(RawCid), cudaMemcpyHostToDevice, st));
+        sort_requests(raw.p, (uint32_t)n, sorted.p, pos.p, st);
+    }
+    // over the execution order exec_raw[exec_idx[i]], i < *n_exec ≤ n_max: the selected receipts below n_receipts → sel_bits, request
+    // j's execution position → exec_indices[j] (left as it is when the message is not executed)
+    void select(cudaStream_t st, const RawCid* exec_raw, const uint32_t* exec_idx, const unsigned long long* n_exec, uint64_t n_max, uint64_t n_receipts,
+                uint64_t* exec_indices, uint32_t* sel_bits) const {
+        if (!n || !n_max) return;
+        k_msg_select<<<div_up(n_max, 256), 256, 0, st>>>(exec_raw, exec_idx, n_exec, sorted.p, pos.p, (uint32_t)n, n_receipts, exec_indices, sel_bits);
+        IPCFP_LAUNCH_CHECK();
+    }
+};
+
+// One generate_event_proof call: its arguments, the predicate's and the scan's state and buffers, and its phases, which
+// generate_event_proof runs in order; the execution order is the ExecOrderBuild's.
+// comm != nullptr: this call is one shard of a multi-GPU call and runs the cross-shard protocol itself (parallel.cu). Failures are then
+// not thrown where they are seen: every rank keeps taking part in the collectives and all ranks fail together, with the error the
+// reference's sequential order meets first across ALL shards.
+// Host synchronisations, per mode:
+//   unsharded         snapshot_and_sync after the walk (again after a dense walk that gave up; once more for k_amt_first_fault),
+//                     pass1, pass2, read_back's witness join (IPCFP_RESULT_JSON: render_event_json's one before it), fill
+//   IPCFP_BFS_GENERAL, sharded, order only (build_execution_order): walk reads the prologue back first; run_general synchronises after
+//                     its range upload, after the fused rounds and once per level below them
+//   order only:       walk, snapshot_and_sync, then build_execution_order reads n_exec back
+//   sharded over NCCL: besides, every H0 / H2 gather, ShardExchange::agree_results and finish, a late H0 that fails, and fill's copy of
+//                     the union partition (IPCFP_SHARDED_UNION_TO_HOST)
+// P: the predicate. Matcher: `spec` is the call's EventProofSpec (t0 = keccak256(signature) is computed by k_setup). LogFilter: `filter`
+// is a log filter (unsharded calls only), its values raw, its large sets uploaded beside it.
+template <class P>
+struct EventCall {
+    Store* s;
+    cudaStream_t st;
+    TipsetDev& td;
+    const ipcfp_event_spec* spec;
+    const ipcfp_log_filter* filter = nullptr;
+    uint32_t flags;
+    bool sharded;
+    uint64_t lo, hi;
+    Comm* comm;
+    std::chrono::steady_clock::time_point t_enter;
+    uint64_t N = 0;
+    std::unique_ptr<ShardExchange> xch;
+    std::optional<ExecOrderBuild> ob;
+    unsigned long long* dw;
+    uint64_t* hw;
+    // stage
+    P mh;
+    size_t siglen = 0;
+    uint8_t* d_sig = nullptr;
+    P* d_matcher = nullptr;
+    AsyncBuf<uint64_t> d_sets;   // LogFilter: the large sets and their bitmaps, and their pinned host copy
+    PinnedArray sets_h;
+    // pass 1
+    AsyncBuf<uint32_t> match_bits, cnt, nby;
+    AsyncBuf<uint64_t> pbase, bbase;
+    AsyncBuf<uint32_t> match_rel;
+    AsyncBuf<uint64_t> wp3;
+    uint64_t n_exec = 0, M = 0, pass1_nodes = 0, pass1_bytes = 0, n_proofs = 0, n_bytes = 0;
+    // pass 2 and the result
+    std::unique_ptr<EventResultBox> box;
+    AsyncBuf<ipcfp_event_proof> d_proofs;
+    AsyncBuf<uint8_t> d_blob;
+    uint64_t mB = 0;
+    bool any_skip = false;
+    PinnedArray rel;
+    uint64_t json_len = 0;
+    // message selection (generate_message_log_proof): the requested CIDs, sorted once on the device, and what they select
+    MsgRequests msg;
+    PinnedArray exec_indices_h;
+    AsyncBuf<uint32_t> sel_bits, sel;
+    AsyncBuf<uint64_t> d_exec_indices, wp_sel;
+    AsyncBuf<unsigned long long> n_sel;
+
+    EventCall(Store* s_, TipsetDev& td_, const ipcfp_event_spec* spec_, uint32_t flags_, bool sharded_, uint64_t lo_, uint64_t hi_, Comm* comm_)
+        : s(s_), st(s_->stream), td(td_), spec(spec_), flags(flags_), sharded(sharded_), lo(lo_), hi(hi_), comm(comm_), dw(s_->dev_words.p),
+          hw(s_->host_words.p) {}
+
+    // ---- checks, and the spec + tipset CIDs up in ONE copy from the store's pinned staging block (no host sync)
+    void stage() {
+        s->use();
+        t_enter = std::chrono::steady_clock::now();
+        LogFilterHost lfh;
+        if constexpr (std::is_same_v<P, Matcher>) {
+            if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+            siglen = strlen(spec->event_signature);
+        } else {
+            log_filter_build(filter, lfh);
+        }
+        // a shard's result is not an EventProofBundle: its witness is distributed and its message CIDs are resolved later
+        if (sharded && (flags & IPCFP_RESULT_JSON)) throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_RESULT_JSON is not available for sharded calls");
+        if ((flags & IPCFP_WITNESS_BY_REFERENCE) && !s->caller_blob)
+            throw Error(IPCFP_ERR_UNSUPPORTED, "IPCFP_WITNESS_BY_REFERENCE needs a store made from a caller's blob (ipcfp_store_create)");
+        if (!sharded) { lo = 0; hi = td.n_receipts; }
+        if (lo > hi || hi > td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "receipt range out of bounds");
+        N = hi - lo;
+        if (comm) {
+            if (!sharded) throw Error(IPCFP_ERR_INVALID_ARG, "communicator given for an unsharded call");
+            if (s->class_prefix.size() > 1) throw Error(IPCFP_ERR_UNSUPPORTED, "sharded calls need a store with one CID prefix");
+            xch.reset(new ShardExchange(comm, s, lo, hi));
+        }
+        ob.emplace(s, &td, td.n_parents, td.txmeta_cids.data(), flags, sharded, lo, hi, xch.get());
+
+        //   [0,1024) Matcher (t0 is filled in on the device) or LogFilter | signature, zero padded | the tipset CIDs (ExecOrderBuild::stage)
+        const size_t sig_cap = (siglen + 64) & ~(size_t)63;
+        static_assert(sizeof(P) <= 1024, "the predicate must fit its staging slot");
+        uint8_t* d_head = ob->stage(1024 + sig_cap, [&](uint8_t* hs) {
+            memset(&mh, 0, sizeof mh);
+            if constexpr (std::is_same_v<P, Matcher>) {
+                size_t n1 = strlen(spec->topic_1);
+                uint8_t t1[32];
+                memset(t1, 0, 32);
+                memcpy(t1, spec->topic_1, n1 < 32 ? n1 : 32);  // ascii_to_bytes32 (evm.rs:72-78)
+                memcpy(mh.t1, t1, 32);
+                mh.actor = spec->actor_id_filter;
+                mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
+            } else {
+                if (!lfh.dev.empty()) {   // through pinned memory that lives as long as the call: no host synchronisation
+                    sets_h = PinnedArray(s->pool, lfh.dev.size() * 8);
+                    memcpy(sets_h.p, lfh.dev.data(), lfh.dev.size() * 8);
+                    d_sets.alloc(lfh.dev.size(), st);
+                    IPCFP_CUDA(cudaMemcpyAsync(d_sets.p, sets_h.p, lfh.dev.size() * 8, cudaMemcpyHostToDevice, st));
+                }
+                lfh.place(d_sets.p);
+                mh = lfh.f;
+            }
+            memcpy(hs, &mh, sizeof(P));
+            if (siglen) memcpy(hs + 1024, spec->event_signature, siglen);
+        });
+        d_sig = d_head + 1024;                       // 8-byte aligned
+        d_matcher = (P*)d_head;
+    }
+
+    // ---- the execution order. The Matcher's t0 is computed by k_setup: it comes from the prologue's head as the builder read it back.
+    void exec_order() {
+        if constexpr (std::is_same_v<P, Matcher>) {
+            ob->build(d_sig, (uint32_t)siglen, d_matcher);
+            memcpy(mh.t0, ob->ph->t0, 32);
+        } else {
+            ob->build(d_sig, (uint32_t)siglen, nullptr);   // a log filter's values arrive raw: nothing to hash
+        }
     }
 
     // ---- pass 1: matching receipts, per-receipt proof counts and bytes
@@ -994,12 +1079,12 @@ struct EventCall {
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS1], st));
         match_rel.alloc(N + 32, st);
         wp3.alloc((N + 31) / 32 + 8, st);
-        bitmap_to_indices(match_bits.p, (N + 31) / 32 * 32, match_rel.p, (uint64_t*)(dw + DW_N_MATCH), wp3.p, scratch.p, st);
-        exclusive_scan_u32(cnt.p, pbase.p, N, (uint64_t*)(dw + DW_N_PROOFS), scratch.p, st);
-        exclusive_scan_u32(nby.p, bbase.p, N, (uint64_t*)(dw + DW_BLOB_BYTES), scratch.p, st);
+        bitmap_to_indices(match_bits.p, (N + 31) / 32 * 32, match_rel.p, (uint64_t*)(dw + DW_N_MATCH), wp3.p, ob->scratch.p, st);
+        exclusive_scan_u32(cnt.p, pbase.p, N, (uint64_t*)(dw + DW_N_PROOFS), ob->scratch.p, st);
+        exclusive_scan_u32(nby.p, bbase.p, N, (uint64_t*)(dw + DW_BLOB_BYTES), ob->scratch.p, st);
         publish_words(s, 0, DW_TX_ERR + 1);
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        note_errors();
+        ob->note_errors();
         n_exec = hw[DW_N_EXEC];
         M = hw[DW_N_MATCH];
         pass1_nodes = hw[DW_STATS]; pass1_bytes = hw[DW_STATS + 1];
@@ -1007,22 +1092,13 @@ struct EventCall {
     }
 
     // ---- message selection, in place of pass 1 (generate_message_log_proof). The requests go up as RawCid and are sorted on the
-    // engine stream ahead of k_setup (the same stream: nothing overlaps); the selection needs the execution order, so it runs behind the
-    // dedup.
-    void stage_messages() {
-        if (!n_msg) return;
-        msg_h = PinnedArray(s->pool, n_msg * sizeof(RawCid));
-        RawCid* h = msg_h.as<RawCid>();
-        for (uint64_t j = 0; j < n_msg; j++) h[j] = rawcid_from_bytes(msg_cids + 38 * j);
-        msg_raw.alloc(n_msg, st); msg_sorted.alloc(n_msg, st); msg_pos.alloc(n_msg, st);
-        IPCFP_CUDA(cudaMemcpyAsync(msg_raw.p, h, n_msg * sizeof(RawCid), cudaMemcpyHostToDevice, st));
-        sort_requests(msg_raw.p, (uint32_t)n_msg, msg_sorted.p, msg_pos.p, st);
-    }
+    // engine stream ahead of k_setup (msg.stage; the same stream: nothing overlaps); the selection needs the execution order, so it runs
+    // behind the dedup.
     // k_msg_select over the execution order → the selected receipts (ascending) and every request's execution index; then the match of
     // the selected receipts only (k_msg_match: pass 1's per-receipt result) → match bits, counts and bytes of those receipts, zero
     // elsewhere; then pass 1's tail. No events AMT of an unselected receipt is read.
     void select_and_match() {
-        const uint64_t nw = (N + 31) / 32 + 8, n_sel_max = std::min<uint64_t>(n_msg, N);
+        const uint64_t n_msg = msg.n, nw = (N + 31) / 32 + 8, n_sel_max = std::min<uint64_t>(n_msg, N);
         d_exec_indices.alloc(n_msg + 1, st);
         IPCFP_CUDA(cudaMemsetAsync(d_exec_indices.p, 0xff, (n_msg + 1) * 8, st));
         sel_bits.alloc(nw, st); sel_bits.zero();
@@ -1030,14 +1106,10 @@ struct EventCall {
         cnt.alloc(N + 8, st); cnt.zero(); nby.alloc(N + 8, st); nby.zero();
         pbase.alloc(N + 8, st); bbase.alloc(N + 8, st);
         n_sel.alloc(1, st); n_sel.zero();
-        if (n_msg && nraw) {
-            k_msg_select<<<div_up(nraw, 256), 256, 0, st>>>(exec_raw.p, exec_idx.p, n_exec_dev, msg_sorted.p, msg_pos.p, (uint32_t)n_msg, N, d_exec_indices.p,
-                                                             sel_bits.p);
-            IPCFP_LAUNCH_CHECK();
-        }
+        msg.select(st, ob->exec_raw.p, ob->exec_idx.p, ob->n_exec_dev, ob->nraw, N, d_exec_indices.p, sel_bits.p);
         if (n_sel_max) {
             sel.alloc(n_sel_max + 32, st); wp_sel.alloc(nw, st);
-            bitmap_to_indices(sel_bits.p, (N + 31) / 32 * 32, sel.p, (uint64_t*)n_sel.p, wp_sel.p, scratch.p, st);
+            bitmap_to_indices(sel_bits.p, (N + 31) / 32 * 32, sel.p, (uint64_t*)n_sel.p, wp_sel.p, ob->scratch.p, st);
             MsgMatchArgsT<P> a;
             a.store = s->view; a.store_dev = s->view_dev.p; a.m_dev = d_matcher; a.events_roots = td.events_roots.p; a.has_root = td.has_root.p;
             a.sel = sel.p; a.n_sel = n_sel.p; a.n_sel_max = n_sel_max;
@@ -1059,23 +1131,23 @@ struct EventCall {
         if (M) {
             Pass2ArgsT<P> p2;
             p2.store = s->view; p2.store_dev = s->view_dev.p; p2.m_dev = d_matcher; p2.m = mh; p2.events_roots = td.events_roots.p; p2.lo = lo; p2.match_rel = match_rel.p; p2.n_match = M;
-            p2.receipts_root_blk = receipts_root_blk; p2.exec_cids = exec_raw.p; p2.exec_idx = exec_idx.p; p2.n_exec = n_exec_dev;
-            p2.wbits = wbits.p; p2.err = dw + DW_ERR; p2.cnt = cnt.p; p2.proof_base = pbase.p; p2.byte_base = bbase.p;
-            p2.proofs = d_proofs.p; p2.blob = d_blob.p; p2.any_skip = misc + 2; p2.resolve_msg = sharded ? 0 : 1;
+            p2.receipts_root_blk = ob->receipts_root_blk; p2.exec_cids = ob->exec_raw.p; p2.exec_idx = ob->exec_idx.p; p2.n_exec = ob->n_exec_dev;
+            p2.wbits = ob->wbits.p; p2.err = dw + DW_ERR; p2.cnt = cnt.p; p2.proof_base = pbase.p; p2.byte_base = bbase.p;
+            p2.proofs = d_proofs.p; p2.blob = d_blob.p; p2.any_skip = ob->misc + 2; p2.resolve_msg = sharded ? 0 : 1;
             p2.per_warp = (M <= 16384 && !getenv("IPCFP_PASS2_PER_THREAD")) ? 1 : 0;
             k_pass2<<<div_up(p2.per_warp ? M * 32 : M, 128), 128, 0, st>>>(p2); IPCFP_LAUNCH_CHECK();
         }
         // pass 2 did not wait for the cross-shard exchange; now that both are done: P (parallel.cu)
-        if (xch) xch->positions_for(match_rel.p, M, n_exec_dev);
+        if (xch) xch->positions_for(match_rel.p, M, ob->n_exec_dev);
         // blocks recorded by pass 2 (receipt paths + events AMTs of the matches): the late part of the witness
-        wbuild->finish_enqueue(wbits.p);
+        ob->wbuild->finish_enqueue(ob->wbits.p);
         publish_words(s, 0, DW_EXEC_CHECK + 1);
-        publish_words(s, HW_ANY_SKIP, HW_ANY_SKIP_WORDS, misc);
+        publish_words(s, HW_ANY_SKIP, HW_ANY_SKIP_WORDS, ob->misc);
         IPCFP_CUDA(cudaStreamSynchronize(st));
-        note_errors();
+        ob->note_errors();
         // base-witness CIDs (parent headers, child header, TxMeta) are only dereferenced by WitnessCollector::materialize
         // (common/witness.rs:43-56, events/generator.rs:104), i.e. AFTER every receipts-root / pass-1 / pass-2 failure
-        if (!xch && missing_base && !skip_tx) throw_first(IPCFP_NO_ERROR, IPCFP_NO_ERROR, true);
+        if (!xch && ob->missing_base && !ob->skip_tx) throw_first(IPCFP_NO_ERROR, IPCFP_NO_ERROR, true);
         mB = hw[DW_WIT_B];
         any_skip = ((const uint32_t*)(hw + HW_ANY_SKIP))[2] != 0;
         IPCFP_CUDA(cudaEventRecord(s->ev[EV_PASS2], st));
@@ -1090,10 +1162,12 @@ struct EventCall {
         if (M) IPCFP_CUDA(cudaMemcpyAsync(rel.p, match_rel.p, M * 4, cudaMemcpyDeviceToHost, st));
         if (n_proofs && !xch) IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_proofs.p, n_proofs * sizeof(ipcfp_event_proof), cudaMemcpyDeviceToHost, st));
         if (n_bytes) IPCFP_CUDA(cudaMemcpyAsync(box->blob.p, d_blob.p, n_bytes, cudaMemcpyDeviceToHost, st));
-        wbuild->finish_start(mB, hw[DW_WIT_B_BYTES], box->wit);
+        WitnessBuilder& wbuild = *ob->wbuild;
+        wbuild.finish_start(mB, hw[DW_WIT_B_BYTES], box->wit);
         if (xch) {
-            if (!xch->agree_results(pend_tx, pend_err, missing_base && !skip_tx, n_proofs, hw[DW_WIT_A] + mB, xch_stale, exec_raw.p, nraw)) {
-                wbuild->finish_join(box->wit);   // nothing of this call may be in flight when its buffers go
+            if (!xch->agree_results(ob->pend_tx, ob->pend_err, ob->missing_base && !ob->skip_tx, n_proofs, hw[DW_WIT_A] + mB, ob->xch_stale, ob->exec_raw.p,
+                                    ob->nraw)) {
+                wbuild.finish_join(box->wit);   // nothing of this call may be in flight when its buffers go
                 throw_first(xch->g_tx, xch->g_err, xch->g_missing_base);
                 throw Error(IPCFP_ERR_UNSUPPORTED, "execution-order exchange: bucket overflow (skewed CID hash distribution)");
             }
@@ -1104,11 +1178,11 @@ struct EventCall {
         if (flags & IPCFP_RESULT_JSON) {
             IPCFP_CUDA(cudaEventRecord(s->ev[EV_JSON_BEGIN], st));
             JsonInputs ji{d_proofs.p, n_proofs, d_blob.p, box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n,
-                          td.parent_epoch, td.child_epoch, td.n_parents, sa.parent_cids, sa.child_cid};
+                          td.parent_epoch, td.child_epoch, td.n_parents, ob->sa.parent_cids, ob->sa.child_cid};
             json_len = render_event_json(s, ji, box->json);
             IPCFP_CUDA(cudaEventRecord(s->ev[EV_JSON_END], st));
         }
-        wbuild->finish_join(box->wit);
+        wbuild.finish_join(box->wit);
         if (xch) xch->finish();
     }
 
@@ -1145,8 +1219,8 @@ struct EventCall {
             r.json = box->json.as<char>(); r.json_len = json_len;
             IPCFP_CUDA(cudaEventElapsedTime(&ms, s->ev[EV_JSON_BEGIN], s->ev[EV_JSON_END])); r.ms_json = ms;
         }
-        r.shard_raw_total = nraw_total;
-        if (sharded) { r.n_exec = 0; r.shard_exec_count = nraw; box->shard_exec = std::move(exec_raw); r.shard_exec_dev = box->shard_exec.p; }
+        r.shard_raw_total = ob->nraw_total;
+        if (sharded) { r.n_exec = 0; r.shard_exec_count = ob->nraw; box->shard_exec = std::move(ob->exec_raw); r.shard_exec_dev = box->shard_exec.p; }
         if (xch) {
             xch->fill_result(r);
             if (getenv("IPCFP_XCH_TRACE")) {
@@ -1175,13 +1249,10 @@ struct EventCall {
 }  // namespace
 
 ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_event_spec* spec, uint32_t flags, bool sharded, uint64_t lo, uint64_t hi,
-                                         Comm* comm, ExecOrderOut* exo) {
-    EventCall<Matcher> c(s, td, spec, flags, sharded, lo, hi, comm, exo);
+                                         Comm* comm) {
+    EventCall<Matcher> c(s, td, spec, flags, sharded, lo, hi, comm);
     c.stage();
-    c.setup();
-    c.walk();
-    c.settle_walk();
-    if (!c.dedup()) return nullptr;
+    c.exec_order();
     c.pass1();
     c.pass2();
     c.read_back();
@@ -1190,13 +1261,10 @@ ipcfp_event_result* generate_event_proof(Store* s, TipsetDev& td, const ipcfp_ev
 
 // the same call with a log filter as the predicate (unsharded)
 ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_filter* filter, uint32_t flags) {
-    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr, nullptr);
+    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr);
     c.filter = filter;
     c.stage();
-    c.setup();
-    c.walk();
-    c.settle_walk();
-    c.dedup();
+    c.exec_order();
     c.pass1();
     c.pass2();
     c.read_back();
@@ -1210,22 +1278,29 @@ ipcfp_event_result* generate_message_log_proof(Store* s, TipsetDev& td, const ui
     if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
     ipcfp_log_filter any;
     memset(&any, 0, sizeof any);
-    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr, nullptr);
+    EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr);
     c.filter = filter ? filter : &any;
-    c.msg_cids = message_cids;
-    c.n_msg = n;
     c.stage();
-    c.stage_messages();
-    c.setup();
-    c.walk();
-    c.settle_walk();
-    c.dedup();
+    c.msg.stage(s, message_cids, n);
+    c.exec_order();
     c.select_and_match();
     c.pass2();
     c.read_back();
     ipcfp_event_result* r = c.fill();
     if (n) memcpy(exec_indices, c.exec_indices_h.p, n * 8);
     return r;
+}
+
+void build_execution_order(Store* s, uint32_t n_parents, const uint8_t* txmeta_cids, ExecOrderOut& out) {
+    s->use();
+    ExecOrderBuild b(s, n_parents, txmeta_cids);
+    b.stage(0, [](uint8_t*) {});
+    b.build(nullptr, 0, nullptr);
+    publish_words(s, DW_N_EXEC, 1);
+    IPCFP_CUDA(cudaStreamSynchronize(b.st));
+    out.n_exec = b.hw[DW_N_EXEC];
+    out.exec_raw = std::move(b.exec_raw);
+    out.exec_idx = std::move(b.exec_idx);
 }
 
 __global__ void k_msg_mask(const uint8_t* __restrict__ has_root, const uint32_t* __restrict__ sel_bits, uint64_t n, uint8_t* has_sel) {
@@ -1238,18 +1313,13 @@ void message_selection_mask(Store* s, TipsetDev& td, const ExecOrderOut& exo, co
     AsyncBuf<uint32_t> bits((N + 31) / 32 + 8, st);
     bits.zero();
     if (n && exo.n_exec) {
-        std::vector<RawCid> h(n);
-        for (uint64_t j = 0; j < n; j++) h[j] = rawcid_from_bytes(message_cids + 38 * j);
-        AsyncBuf<RawCid> raw(n, st), sorted(n, st);
-        AsyncBuf<uint32_t> pos(n, st);
+        MsgRequests req;
+        req.stage(s, message_cids, n);
         AsyncBuf<uint64_t> idx(n, st);
         AsyncBuf<unsigned long long> n_exec(1, st);
         const unsigned long long ne = exo.n_exec;
-        IPCFP_CUDA(cudaMemcpyAsync(raw.p, h.data(), n * sizeof(RawCid), cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaMemcpyAsync(n_exec.p, &ne, 8, cudaMemcpyHostToDevice, st));
-        sort_requests(raw.p, (uint32_t)n, sorted.p, pos.p, st);
-        k_msg_select<<<div_up(exo.n_exec, 256), 256, 0, st>>>(exo.exec_raw.p, exo.exec_idx.p, n_exec.p, sorted.p, pos.p, (uint32_t)n, N, idx.p, bits.p);
-        IPCFP_LAUNCH_CHECK();
+        req.select(st, exo.exec_raw.p, exo.exec_idx.p, n_exec.p, exo.n_exec, N, idx.p, bits.p);
         if (N) { k_msg_mask<<<div_up(N, 256), 256, 0, st>>>(td.has_root.p, bits.p, N, has_sel); IPCFP_LAUNCH_CHECK(); }
         IPCFP_CUDA(cudaStreamSynchronize(st));   // the host copies above are read until here
     }

@@ -283,11 +283,7 @@ void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, u
     ExecOrderOut exo;
     bool have_order = true;
     try {
-        ipcfp_event_spec dummy;
-        memset(&dummy, 0, sizeof dummy);
-        dummy.event_signature = "";
-        dummy.topic_1 = "";
-        (void)generate_event_proof(s, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, nullptr, &exo);
+        build_execution_order(s, td.n_parents, td.txmeta_cids.data(), exo);
     } catch (Error& e) {
         // a block the walk lacks, or one that does not decode (the generator reports it): no receipt is taken this round. Anything
         // else (device, allocation, unsupported input) is the planner's own failure.

@@ -102,24 +102,11 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         // collect_exec_list(verify_txmeta = true) once for the whole batch: TxMeta recompute, then the engine's own message-AMT walk
         // + first-seen dedup (the same kernels generate_event_proof uses), on the TxMeta links taken from the parent HEADERS
         k_verify_txmeta<<<div_up(P, 64), 64, 0, st>>>(s->view, d_tx, P, dw); IPCFP_LAUNCH_CHECK();
-        TipsetDev td;
-        td.parent_epoch = t->parent_epoch; td.child_epoch = t->child_epoch; td.n_parents = P;
-        td.parent_cids.assign(t->parent_cids, t->parent_cids + 38ull * P);
-        td.txmeta_cids.assign(h_tx.begin(), h_tx.begin() + 38ull * P);
-        memcpy(td.child_cid, t->child_cid, 38);
-        memcpy(td.receipts_root, t->child_cid, 38);   // unused in execution-order-only mode (any CID of the store)
-        td.n_receipts = 0;
-        td.events_roots.alloc(64);
-        td.has_root.alloc(64);
-        ipcfp_event_spec dummy;
-        memset(&dummy, 0, sizeof dummy);
-        dummy.event_signature = "";
-        dummy.topic_1 = "";
         IPCFP_CUDA(cudaMemcpyAsync(hw + HW_PARKED_KEY, dw, 8, cudaMemcpyDeviceToHost, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));
         const uint64_t tx_key = hw[HW_PARKED_KEY];
         try {
-            (void)generate_event_proof(s, td, &dummy, IPCFP_SCAN_SKIP_TX_AMTS, false, 0, 0, nullptr, &exo);
+            build_execution_order(s, P, h_tx.data(), exo);
         } catch (Error& e) {
             // collect_exec_list takes the parents in order and checks parent k's TxMeta CID before it walks parent k's two message AMTs.
             // The walk's fault key names the parent it met (eidx / 3: its TxMeta, BLS or SECP AMT); a mismatching TxMeta of an earlier
