@@ -112,6 +112,14 @@ def test_python_hash_copy_matches_the_device_source():
     mix = re.search(r"uint64_t mix64\(uint64_t x\) \{\s*(.*?)\s*return x;", src, re.S).group(1)
     assert mix.replace(" ", "") == "x^=x>>33;x*=0xff51afd7ed558ccdULL;x^=x>>33;x*=0xc4ceb9fe1a85ec53ULL;x^=x>>33;"
     assert "digest_hash(const Digest& d, uint32_t cls) { return mix64(d.w[0] ^ (d.w[2] * 0x9E3779B97F4A7C15ULL) ^ cls); }" in src
+    # tests/gpu_prims/shard_check.cu builds message CIDs to chosen owners and claim-table slots with its own copy of this hash (and
+    # checks that copy against the device on every input)
+    raw = open(os.path.join(ROOT, "ipc_filecoin_proofs_b200", "csrc", "rawcid.cuh")).read()
+    assert "uint64_t rawcid_hash(const RawCid& c) { return mix64(c.w[0] ^ (c.w[2] * 0x9E3779B97F4A7C15ULL) ^ c.w[4]); }" in raw
+    check = open(os.path.join(ROOT, "tests", "gpu_prims", "shard_check.cu")).read()
+    assert "static uint64_t rawcid_hash_h(const RawCid& c) { return mix64_h(c.w[0] ^ (c.w[2] * GOLD) ^ c.w[4]); }" in check
+    assert "x ^= x >> 33; x *= M1; x ^= x >> 33; x *= M2; x ^= x >> 33;" in check
+    assert "M1 = 0xff51afd7ed558ccdULL, M2 = 0xc4ceb9fe1a85ec53ULL" in check and "GOLD = 0x9E3779B97F4A7C15ULL" in check
     store = open(os.path.join(ROOT, "ipc_filecoin_proofs_b200", "csrc", "store.cu")).read()
     assert re.search(r"uint64_t slots = 64;\s*while \(slots < 2 \* n\) slots <<= 1;", store)
     assert [U.table_slots(n) for n in (0, 1, 31, 32, 33, 63, 64, 65, 1023, 1024, 1025)] == [64, 64, 64, 64, 128, 128, 128, 256, 2048, 2048, 4096]

@@ -1,8 +1,10 @@
-"""Index arithmetic the partitioned witness union relies on (csrc/parallel.cu: `part_lo`, `k_part_pack`, `k_part_bounds`), restated in
-numpy and checked exhaustively: for every world size the library accepts (1..256) the owner the pack kernel computes for a bucket,
-`(bucket * world) >> 16`, is the rank whose range `[part_lo(r), part_lo(r+1))` holds it, the ranges tile the 65 536 buckets in rank
-order (so concatenating the partitions in rank order is the sorted set), and the default piece capacity never exceeds the
-cannot-overflow capacity. A restatement — the kernels themselves are exercised by tests/test_parallel.py::test_sharded_call_over_nccl."""
+"""Index arithmetic the partitioned witness union relies on (csrc/shard_kernels.cuh: `part_lo`, `k_part_pack`, `k_part_bounds`),
+restated in numpy and checked exhaustively: for every world size the library accepts (1..256) the owner the pack kernel computes for a
+bucket, `(bucket * world) >> 16`, is the rank whose range `[part_lo(r), part_lo(r+1))` holds it, the ranges tile the 65 536 buckets in
+rank order (so concatenating the partitions in rank order is the sorted set), and the default piece capacity never exceeds the
+cannot-overflow capacity. A restatement — the kernels themselves run in tests/gpu_prims/shard_check.cu (tests/test_shard_check.py),
+W simulated ranks on one GPU at world sizes 1 to 255 against CPU references, and in tests/test_parallel.py::test_sharded_call_over_nccl
+where the GPUs for several ranks exist."""
 import numpy as np
 
 BUCKETS = 65536
