@@ -32,27 +32,94 @@ def build_lib(force=False, jobs=8):
 
 _lib = None
 
-EXPORTS = [
-    "ipcfp_last_error", "ipcfp_last_error_index", "ipcfp_version", "ipcfp_kernel_launch_count", "ipcfp_host_alloc", "ipcfp_host_free",
-    "ipcfp_store_create", "ipcfp_store_destroy", "ipcfp_store_n_blocks", "ipcfp_store_get", "ipcfp_store_has",
-    "ipcfp_store_first_bad_block", "ipcfp_blake2b256_batch", "ipcfp_keccak256_batch", "ipcfp_sha256_batch",
-    "ipcfp_compute_mapping_slots", "ipcfp_generate_event_proof", "ipcfp_event_result_free", "ipcfp_read_storage_slots",
-    "ipcfp_slot_result_free", "ipcfp_generate_storage_proofs", "ipcfp_storage_result_free", "ipcfp_generate_proof_bundle",
-    "ipcfp_bundle_free", "ipcfp_generate_event_proof_shard",
-    "ipcfp_tipset_upload", "ipcfp_tipset_free", "ipcfp_generate_event_proof_resident", "ipcfp_generate_event_proof_shard_resident",
-    "ipcfp_store_stream",
-    "ipcfp_comm_unique_id", "ipcfp_comm_init", "ipcfp_comm_destroy", "ipcfp_generate_event_proof_sharded",
-    "ipcfp_verify_event_proofs", "ipcfp_verify_storage_proofs", "ipcfp_bundle_to_json", "ipcfp_event_result_to_json", "ipcfp_json_free",
-    "ipcfp_bundle_from_json", "ipcfp_parsed_bundle_free", "ipcfp_verify_bundle_json", "ipcfp_bundle_verdict_free",
-    "ipcfp_generate_proof_bundle_resident", "ipcfp_tipset_desc_from_json", "ipcfp_parsed_tipset_free", "ipcfp_tipset_upload_json",
-    "ipcfp_tipset_describe", "ipcfp_blocks_from_rpc_json", "ipcfp_parsed_blocks_free", "ipcfp_store_create_rpc_json",
-    "ipcfp_plan_fetch_resident", "ipcfp_plan_fetch", "ipcfp_fetch_plan_free", "ipcfp_fetch_plan_to_rpc_json",
-    "ipcfp_resolve_addresses", "ipcfp_resolve_result_free", "ipcfp_address_parse", "ipcfp_address_from_eth",
-    "ipcfp_generate_log_proof", "ipcfp_generate_log_proof_resident", "ipcfp_plan_fetch_log_resident", "ipcfp_verify_event_proofs_log",
-    "ipcfp_generate_log_bundle", "ipcfp_generate_log_bundle_resident", "ipcfp_plan_fetch_log_bundle_resident", "ipcfp_verify_event_proofs_any",
-    "ipcfp_verify_bundle_json_any", "ipcfp_generate_message_log_proof", "ipcfp_generate_message_log_proof_resident",
-    "ipcfp_plan_fetch_message_log_resident",
-]
+_vp, _u64, _u32, _int, _st = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_int32
+_P = C.POINTER
+
+
+def _PP(t):
+    return C.POINTER(C.POINTER(t))
+
+
+_HASH_BATCH = [_vp, _u64, _vp, _vp, _u64, _int, _vp]
+_TO_JSON = [_vp, _P(A.TipsetDesc), _P(_vp), _P(_u64)]
+
+# Every function of include/ipcfp.h, in its order: name -> (restype, argtypes). None leaves ctypes' default: the int result of a void
+# function, the unchecked argument list of a (void) one. tests/test_abi_bindings.py checks the table against the header.
+SIGNATURES = {
+    "ipcfp_last_error": (C.c_char_p, None),
+    "ipcfp_last_error_index": (_u64, None),
+    "ipcfp_version": (C.c_char_p, None),
+    "ipcfp_kernel_launch_count": (_u64, None),
+    "ipcfp_host_alloc": (_st, [C.c_size_t, _P(_vp)]),
+    "ipcfp_host_free": (None, [_vp]),
+    "ipcfp_store_create": (_st, [_vp, _vp, _vp, _vp, _u64, _u64, _int, _u32, _P(_vp)]),
+    "ipcfp_store_destroy": (None, [_vp]),
+    "ipcfp_store_n_blocks": (_u64, [_vp]),
+    "ipcfp_store_get": (_st, [_vp, _vp, _vp, _u32, _P(_u32), _P(_int)]),
+    "ipcfp_store_has": (_st, [_vp, _vp, _P(_int)]),
+    "ipcfp_store_first_bad_block": (_u64, [_vp]),
+    "ipcfp_blake2b256_batch": (_st, _HASH_BATCH),
+    "ipcfp_keccak256_batch": (_st, _HASH_BATCH),
+    "ipcfp_sha256_batch": (_st, _HASH_BATCH),
+    "ipcfp_compute_mapping_slots": (_st, [_vp, _vp, _u64, _int, _vp]),
+    "ipcfp_generate_event_proof": (_st, [_vp, _P(A.TipsetDesc), _P(A.EventSpec), _u32, _PP(A.EventResultC)]),
+    "ipcfp_event_result_free": (None, [_P(A.EventResultC)]),
+    "ipcfp_tipset_upload": (_st, [_vp, _P(A.TipsetDesc), _P(_vp)]),
+    "ipcfp_tipset_free": (None, [_vp]),
+    "ipcfp_generate_event_proof_resident": (_st, [_vp, _vp, _P(A.EventSpec), _u32, _PP(A.EventResultC)]),
+    "ipcfp_generate_event_proof_shard_resident": (_st, [_vp, _vp, _P(A.EventSpec), _u64, _u64, _u32, _u32, _u32, _PP(A.EventResultC)]),
+    "ipcfp_generate_log_proof_resident": (_st, [_vp, _vp, _P(A.LogFilterC), _u32, _PP(A.EventResultC)]),
+    "ipcfp_generate_log_proof": (_st, [_vp, _P(A.TipsetDesc), _P(A.LogFilterC), _u32, _PP(A.EventResultC)]),
+    "ipcfp_generate_message_log_proof_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u32, _vp, _PP(A.EventResultC)]),
+    "ipcfp_generate_message_log_proof": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _P(A.LogFilterC), _u32, _vp, _PP(A.EventResultC)]),
+    "ipcfp_store_stream": (_vp, [_vp]),
+    "ipcfp_tipset_desc_from_json": (_st, [C.c_char_p, _u64, C.c_char_p, _u64, C.c_char_p, _u64, _PP(A.ParsedTipsetC)]),
+    "ipcfp_parsed_tipset_free": (None, [_P(A.ParsedTipsetC)]),
+    "ipcfp_tipset_upload_json": (_st, [_vp, C.c_char_p, _u64, C.c_char_p, _u64, C.c_char_p, _u64, _P(_vp)]),
+    "ipcfp_tipset_describe": (_st, [_vp, _int, _P(A.TipsetInfoC)]),
+    "ipcfp_blocks_from_rpc_json": (_st, [_vp, _u64, _P(C.c_char_p), _P(_u64), _u64, _PP(A.ParsedBlocksC)]),
+    "ipcfp_parsed_blocks_free": (None, [_P(A.ParsedBlocksC)]),
+    "ipcfp_store_create_rpc_json": (_st, [_vp, _u64, _P(C.c_char_p), _P(_u64), _u64, _int, _u32, _P(_vp), _P(A.StoreJsonInfoC)]),
+    "ipcfp_read_storage_slots": (_st, [_vp, _vp, _vp, _u64, _PP(A.SlotResultC)]),
+    "ipcfp_slot_result_free": (None, [_P(A.SlotResultC)]),
+    "ipcfp_generate_storage_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _PP(A.StorageResultC)]),
+    "ipcfp_storage_result_free": (None, [_P(A.StorageResultC)]),
+    "ipcfp_generate_proof_bundle": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _PP(A.BundleC)]),
+    "ipcfp_generate_proof_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _vp, _u64, _u32, _PP(A.BundleC)]),
+    "ipcfp_generate_log_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u64, _u32, _PP(A.BundleC)]),
+    "ipcfp_generate_log_bundle": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _P(A.LogFilterC), _u64, _u32, _PP(A.BundleC)]),
+    "ipcfp_bundle_free": (None, [_P(A.BundleC)]),
+    "ipcfp_plan_fetch_resident": (_st, [_vp, _vp, _vp, _u64, _vp, _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_plan_fetch": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_fetch_plan_free": (None, [_P(A.FetchPlanC)]),
+    "ipcfp_plan_fetch_log_resident": (_st, [_vp, _vp, _P(A.LogFilterC), _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_plan_fetch_message_log_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_plan_fetch_log_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_fetch_plan_to_rpc_json": (_st, [_P(A.FetchPlanC), _u64, _P(_vp), _P(_u64)]),
+    "ipcfp_resolve_addresses": (_st, [_vp, _vp, _P(A.AddressC), _u64, _PP(A.ResolveResultC)]),
+    "ipcfp_resolve_result_free": (None, [_P(A.ResolveResultC)]),
+    "ipcfp_address_parse": (_st, [C.c_char_p, _u64, _P(A.AddressC)]),
+    "ipcfp_address_from_eth": (_st, [_vp, _P(A.AddressC)]),
+    "ipcfp_bundle_to_json": (_st, _TO_JSON),
+    "ipcfp_event_result_to_json": (_st, _TO_JSON),
+    "ipcfp_json_free": (None, [_vp]),
+    "ipcfp_bundle_from_json": (_st, [C.c_char_p, _u64, _PP(A.ParsedBundleC)]),
+    "ipcfp_parsed_bundle_free": (None, [_P(A.ParsedBundleC)]),
+    "ipcfp_verify_event_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _vp, _vp]),
+    "ipcfp_verify_storage_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp]),
+    "ipcfp_verify_event_proofs_log": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _P(A.LogFilterC), _vp]),
+    "ipcfp_verify_event_proofs_any": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _P(A.LogFilterC), _u64, _vp]),
+    "ipcfp_verify_bundle_json": (_st, [C.c_char_p, _u64, _int, A.TrustedParentFn, A.TrustedChildFn, _vp, _vp, _PP(A.BundleVerdictC)]),
+    "ipcfp_verify_bundle_json_any": (_st, [C.c_char_p, _u64, _int, A.TrustedParentFn, A.TrustedChildFn, _vp, _P(A.LogFilterC), _u64,
+                                          _PP(A.BundleVerdictC)]),
+    "ipcfp_bundle_verdict_free": (None, [_P(A.BundleVerdictC)]),
+    "ipcfp_comm_unique_id": (_st, [_vp]),
+    "ipcfp_comm_init": (_st, [_vp, _u32, _u32, _int, _P(_vp)]),
+    "ipcfp_comm_destroy": (None, [_vp]),
+    "ipcfp_generate_event_proof_sharded": (_st, [_vp, _vp, _vp, _P(A.EventSpec), _vp, _u32, _PP(A.EventResultC)]),
+    "ipcfp_generate_event_proof_shard": (_st, [_vp, _P(A.TipsetDesc), _P(A.EventSpec), _u64, _u64, _u32, _u32, _u32, _PP(A.EventResultC)]),
+}
+EXPORTS = list(SIGNATURES)
 
 
 def lib():
@@ -62,154 +129,12 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(f"{LIB_PATH} is missing: run `make` (or __graft_entry__.build()). There is no CPU fallback.")
         L = C.CDLL(LIB_PATH)
-        L.ipcfp_last_error.restype = C.c_char_p
-        L.ipcfp_last_error_index.restype = C.c_uint64
-        L.ipcfp_version.restype = C.c_char_p
-        L.ipcfp_kernel_launch_count.restype = C.c_uint64
-        L.ipcfp_host_alloc.restype = C.c_int32
-        L.ipcfp_host_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p)]
-        L.ipcfp_host_free.argtypes = [C.c_void_p]
-        L.ipcfp_store_create.restype = C.c_int32
-        L.ipcfp_store_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_uint32,
-                                         C.POINTER(C.c_void_p)]
-        L.ipcfp_store_destroy.argtypes = [C.c_void_p]
-        L.ipcfp_store_n_blocks.restype = C.c_uint64
-        L.ipcfp_store_n_blocks.argtypes = [C.c_void_p]
-        L.ipcfp_store_first_bad_block.restype = C.c_uint64
-        L.ipcfp_store_first_bad_block.argtypes = [C.c_void_p]
-        L.ipcfp_store_get.restype = C.c_int32
-        L.ipcfp_store_get.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
-        L.ipcfp_store_has.restype = C.c_int32
-        L.ipcfp_store_has.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-        for name in ("ipcfp_blake2b256_batch", "ipcfp_keccak256_batch", "ipcfp_sha256_batch"):
+        for name, (restype, argtypes) in SIGNATURES.items():
             f = getattr(L, name)
-            f.restype = C.c_int32
-            f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]
-        L.ipcfp_compute_mapping_slots.restype = C.c_int32
-        L.ipcfp_compute_mapping_slots.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]
-        L.ipcfp_generate_event_proof.restype = C.c_int32
-        L.ipcfp_generate_event_proof.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(A.EventSpec), C.c_uint32,
-                                                 C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_generate_event_proof_shard.restype = C.c_int32
-        L.ipcfp_generate_event_proof_shard.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(A.EventSpec), C.c_uint64, C.c_uint64,
-                                                       C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_event_result_free.argtypes = [C.POINTER(A.EventResultC)]
-        L.ipcfp_read_storage_slots.restype = C.c_int32
-        L.ipcfp_read_storage_slots.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.POINTER(A.SlotResultC))]
-        L.ipcfp_slot_result_free.argtypes = [C.POINTER(A.SlotResultC)]
-        L.ipcfp_generate_storage_proofs.restype = C.c_int32
-        L.ipcfp_generate_storage_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64,
-                                                    C.POINTER(C.POINTER(A.StorageResultC))]
-        L.ipcfp_storage_result_free.argtypes = [C.POINTER(A.StorageResultC)]
-        L.ipcfp_generate_proof_bundle.restype = C.c_int32
-        L.ipcfp_generate_proof_bundle.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
-                                                  C.POINTER(C.POINTER(A.BundleC))]
-        L.ipcfp_generate_proof_bundle_resident.restype = C.c_int32
-        L.ipcfp_generate_proof_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
-                                                           C.POINTER(C.POINTER(A.BundleC))]
-        L.ipcfp_bundle_free.argtypes = [C.POINTER(A.BundleC)]
-        L.ipcfp_tipset_upload.restype = C.c_int32
-        L.ipcfp_tipset_upload.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(C.c_void_p)]
-        L.ipcfp_tipset_free.argtypes = [C.c_void_p]
-        L.ipcfp_generate_event_proof_resident.restype = C.c_int32
-        L.ipcfp_generate_event_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.EventSpec), C.c_uint32,
-                                                          C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_generate_event_proof_shard_resident.restype = C.c_int32
-        L.ipcfp_generate_event_proof_shard_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.EventSpec), C.c_uint64, C.c_uint64,
-                                                                C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_store_stream.restype = C.c_void_p
-        L.ipcfp_store_stream.argtypes = [C.c_void_p]
-        L.ipcfp_comm_unique_id.restype = C.c_int32
-        L.ipcfp_comm_unique_id.argtypes = [C.c_void_p]
-        L.ipcfp_comm_init.restype = C.c_int32
-        L.ipcfp_comm_init.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(C.c_void_p)]
-        L.ipcfp_comm_destroy.argtypes = [C.c_void_p]
-        L.ipcfp_generate_event_proof_sharded.restype = C.c_int32
-        L.ipcfp_generate_event_proof_sharded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(A.EventSpec), C.c_void_p, C.c_uint32,
-                                                         C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_verify_event_proofs.restype = C.c_int32
-        L.ipcfp_verify_event_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
-        L.ipcfp_generate_log_proof.restype = C.c_int32
-        L.ipcfp_generate_log_proof.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(A.LogFilterC), C.c_uint32,
-                                               C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_generate_log_proof_resident.restype = C.c_int32
-        L.ipcfp_generate_log_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32,
-                                                        C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_generate_message_log_proof.restype = C.c_int32
-        L.ipcfp_generate_message_log_proof.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC),
-                                                       C.c_uint32, C.c_void_p, C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_generate_message_log_proof_resident.restype = C.c_int32
-        L.ipcfp_generate_message_log_proof_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC),
-                                                                C.c_uint32, C.c_void_p, C.POINTER(C.POINTER(A.EventResultC))]
-        L.ipcfp_plan_fetch_message_log_resident.restype = C.c_int32
-        L.ipcfp_plan_fetch_message_log_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint32,
-                                                            C.POINTER(C.POINTER(A.FetchPlanC))]
-        L.ipcfp_plan_fetch_log_resident.restype = C.c_int32
-        L.ipcfp_plan_fetch_log_resident.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.LogFilterC), C.c_uint32, C.POINTER(C.POINTER(A.FetchPlanC))]
-        L.ipcfp_verify_event_proofs_log.restype = C.c_int32
-        L.ipcfp_verify_event_proofs_log.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
-                                                    C.POINTER(A.LogFilterC), C.c_void_p]
-        L.ipcfp_generate_log_bundle.restype = C.c_int32
-        L.ipcfp_generate_log_bundle.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
-                                                C.c_uint32, C.POINTER(C.POINTER(A.BundleC))]
-        L.ipcfp_generate_log_bundle_resident.restype = C.c_int32
-        L.ipcfp_generate_log_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
-                                                         C.c_uint32, C.POINTER(C.POINTER(A.BundleC))]
-        L.ipcfp_plan_fetch_log_bundle_resident.restype = C.c_int32
-        L.ipcfp_plan_fetch_log_bundle_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(A.LogFilterC), C.c_uint64,
-                                                           C.c_uint32, C.POINTER(C.POINTER(A.FetchPlanC))]
-        L.ipcfp_verify_event_proofs_any.restype = C.c_int32
-        L.ipcfp_verify_event_proofs_any.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
-                                                    C.POINTER(A.LogFilterC), C.c_uint64, C.c_void_p]
-        L.ipcfp_verify_bundle_json_any.restype = C.c_int32
-        L.ipcfp_verify_bundle_json_any.argtypes = [C.c_char_p, C.c_uint64, C.c_int, A.TrustedParentFn, A.TrustedChildFn, C.c_void_p,
-                                                   C.POINTER(A.LogFilterC), C.c_uint64, C.POINTER(C.POINTER(A.BundleVerdictC))]
-        L.ipcfp_verify_storage_proofs.restype = C.c_int32
-        L.ipcfp_verify_storage_proofs.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p]
-        for name in ("ipcfp_bundle_to_json", "ipcfp_event_result_to_json"):
-            f = getattr(L, name)
-            f.restype = C.c_int32
-            f.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        L.ipcfp_json_free.argtypes = [C.c_void_p]
-        L.ipcfp_bundle_from_json.restype = C.c_int32
-        L.ipcfp_bundle_from_json.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.POINTER(A.ParsedBundleC))]
-        L.ipcfp_parsed_bundle_free.argtypes = [C.POINTER(A.ParsedBundleC)]
-        L.ipcfp_verify_bundle_json.restype = C.c_int32
-        L.ipcfp_verify_bundle_json.argtypes = [C.c_char_p, C.c_uint64, C.c_int, A.TrustedParentFn, A.TrustedChildFn, C.c_void_p, C.c_void_p,
-                                               C.POINTER(C.POINTER(A.BundleVerdictC))]
-        L.ipcfp_bundle_verdict_free.argtypes = [C.POINTER(A.BundleVerdictC)]
-        L.ipcfp_tipset_desc_from_json.restype = C.c_int32
-        L.ipcfp_tipset_desc_from_json.argtypes = [C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64,
-                                                  C.POINTER(C.POINTER(A.ParsedTipsetC))]
-        L.ipcfp_parsed_tipset_free.argtypes = [C.POINTER(A.ParsedTipsetC)]
-        L.ipcfp_tipset_upload_json.restype = C.c_int32
-        L.ipcfp_tipset_upload_json.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64,
-                                               C.POINTER(C.c_void_p)]
-        L.ipcfp_tipset_describe.restype = C.c_int32
-        L.ipcfp_tipset_describe.argtypes = [C.c_void_p, C.c_int, C.POINTER(A.TipsetInfoC)]
-        L.ipcfp_blocks_from_rpc_json.restype = C.c_int32
-        L.ipcfp_blocks_from_rpc_json.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_uint64,
-                                                 C.POINTER(C.POINTER(A.ParsedBlocksC))]
-        L.ipcfp_parsed_blocks_free.argtypes = [C.POINTER(A.ParsedBlocksC)]
-        L.ipcfp_store_create_rpc_json.restype = C.c_int32
-        L.ipcfp_store_create_rpc_json.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.c_uint64, C.c_int,
-                                                  C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(A.StoreJsonInfoC)]
-        L.ipcfp_plan_fetch_resident.restype = C.c_int32
-        L.ipcfp_plan_fetch_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
-                                                C.POINTER(C.POINTER(A.FetchPlanC))]
-        L.ipcfp_plan_fetch.restype = C.c_int32
-        L.ipcfp_plan_fetch.argtypes = [C.c_void_p, C.POINTER(A.TipsetDesc), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32,
-                                       C.POINTER(C.POINTER(A.FetchPlanC))]
-        L.ipcfp_fetch_plan_free.argtypes = [C.POINTER(A.FetchPlanC)]
-        L.ipcfp_fetch_plan_to_rpc_json.restype = C.c_int32
-        L.ipcfp_fetch_plan_to_rpc_json.argtypes = [C.POINTER(A.FetchPlanC), C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        L.ipcfp_resolve_addresses.restype = C.c_int32
-        L.ipcfp_resolve_addresses.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(A.AddressC), C.c_uint64, C.POINTER(C.POINTER(A.ResolveResultC))]
-        L.ipcfp_resolve_result_free.argtypes = [C.POINTER(A.ResolveResultC)]
-        L.ipcfp_address_parse.restype = C.c_int32
-        L.ipcfp_address_parse.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(A.AddressC)]
-        L.ipcfp_address_from_eth.restype = C.c_int32
-        L.ipcfp_address_from_eth.argtypes = [C.c_void_p, C.POINTER(A.AddressC)]
+            if restype is not None:
+                f.restype = restype
+            if argtypes is not None:
+                f.argtypes = argtypes
         _lib = L
     return _lib
 
@@ -224,6 +149,23 @@ def _check(st):
     if st != A.OK:
         L = lib()
         raise A.IpcfpError(st, L.ipcfp_last_error().decode(errors="replace"), L.ipcfp_last_error_index())
+
+
+def _result(fn, out_type, convert, free, *args):
+    """Calls lib().<fn>(*args, &out) for an out_type object → convert(out.contents), then releases the object with lib().<free>."""
+    L = lib()
+    out = C.POINTER(out_type)()
+    _check(getattr(L, fn)(*args, C.byref(out)))
+    try:
+        return convert(out.contents)
+    finally:
+        getattr(L, free)(out)
+
+
+# (out_type, convert, free) of _result for the result kinds several calls return
+_EVENT_RESULT = (A.EventResultC, A.event_result_from_c, "ipcfp_event_result_free")
+_BUNDLE = (A.BundleC, A.bundle_from_c, "ipcfp_bundle_free")
+_FETCH_PLAN = (A.FetchPlanC, A.fetch_plan_from_c, "ipcfp_fetch_plan_free")
 
 
 def kernel_launch_count():
@@ -356,13 +298,16 @@ class BlockStore:
         st = lib().ipcfp_store_create(cids.ctypes.data if cids.size else None, offsets.ctypes.data if offsets.size else None,
                                       lengths.ctypes.data if lengths.size else None, blob.ctypes.data if blob.size else None, blob.size,
                                       self.n_blocks, device, A.STORE_VERIFY_CIDS if verify_cids else 0, C.byref(h))
+        self._adopt(st, h)
+
+    def _adopt(self, st, h):
+        """Takes the handle a store-creating call returned with status st. On failure the store is released and IpcfpError raised, with
+        .first_bad_block (None when no store was made)."""
         self._h = h
         if st != A.OK:
             bad = lib().ipcfp_store_first_bad_block(h) if h else None
             msg, idx = lib().ipcfp_last_error().decode(errors="replace"), lib().ipcfp_last_error_index()
-            if h:
-                lib().ipcfp_store_destroy(h)
-                self._h = None
+            self.close()
             e = A.IpcfpError(st, msg, idx)
             e.first_bad_block = bad
             raise e
@@ -384,15 +329,8 @@ class BlockStore:
         h, info = C.c_void_p(), A.StoreJsonInfoC()
         st = lib().ipcfp_store_create_rpc_json(cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep), device,
                                                A.STORE_VERIFY_CIDS if verify_cids else 0, C.byref(h), C.byref(info))
-        self._h = h
         self.json_info = A.StoreJsonInfoPy(bool(info.parsed_on_device), float(info.ms_parse), float(info.ms_kernels))
-        if st != A.OK:
-            bad = lib().ipcfp_store_first_bad_block(h) if h else None
-            msg, idx = lib().ipcfp_last_error().decode(errors="replace"), lib().ipcfp_last_error_index()
-            self.close()
-            e = A.IpcfpError(st, msg, idx)
-            e.first_bad_block = bad
-            raise e
+        self._adopt(st, h)
         return self
 
     def get(self, cid):
@@ -416,112 +354,72 @@ class BlockStore:
     def generate_event_proof(self, ts, spec, flags=0):
         d, keep = A.make_tipset_desc(ts)
         cs = spec.as_c() if isinstance(spec, EventProofSpec) else spec
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_event_proof(self._h, C.byref(d), C.byref(cs), flags, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return _result("ipcfp_generate_event_proof", *_EVENT_RESULT, self._h, C.byref(d), C.byref(cs), flags)
 
     def generate_log_proof(self, ts, log_filter, flags=0):
         """ipcfp_generate_log_proof: generate_event_proof with a LogFilter as the predicate → A.EventResultPy."""
         d, keep = A.make_tipset_desc(ts)
-        f, fkeep = log_filter.as_c()
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_log_proof(self._h, C.byref(d), C.byref(f), flags, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return self._log_proof("ipcfp_generate_log_proof", C.byref(d), log_filter, flags)
 
     def generate_log_proof_resident(self, tip, log_filter, flags=0):
         """ipcfp_generate_log_proof_resident against a ResidentTipset of this store. flags: WITNESS_BY_REFERENCE, RESULT_JSON,
         SCAN_SKIP_TX_AMTS."""
-        f, fkeep = log_filter.as_c()
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_log_proof_resident(self._h, tip._h, C.byref(f), flags, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return self._log_proof("ipcfp_generate_log_proof_resident", tip._h, log_filter, flags)
 
-    @staticmethod
-    def _message_args(message_cids, log_filter):
-        cids = np.ascontiguousarray(message_cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
-        f, fkeep = log_filter.as_c() if log_filter is not None else (None, None)
-        idx = np.zeros(len(cids), np.uint64)
-        return cids, (C.byref(f) if f is not None else None), fkeep, idx
+    def _log_proof(self, fn, tipset, log_filter, flags):
+        f, fkeep = log_filter.as_c()
+        return _result(fn, *_EVENT_RESULT, self._h, tipset, C.byref(f), flags)
 
     def generate_message_log_proof(self, ts, message_cids, log_filter=None, flags=0):
         """ipcfp_generate_message_log_proof: the logs of the given messages (message_cids: (n, 38) message CIDs as the message AMTs hold
         them) that match log_filter (None: every log) → (A.EventResultPy, exec_indices): exec_indices[j] is message j's position in the
         execution order, 2**64 - 1 when the tipset did not execute it."""
         d, keep = A.make_tipset_desc(ts)
-        cids, fp, fkeep, idx = self._message_args(message_cids, log_filter)
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_message_log_proof(self._h, C.byref(d), cids.ctypes.data if cids.size else None, len(cids), fp, flags,
-                                                      idx.ctypes.data if idx.size else None, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents), idx
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return self._message_log_proof("ipcfp_generate_message_log_proof", C.byref(d), message_cids, log_filter, flags)
 
     def generate_message_log_proof_resident(self, tip, message_cids, log_filter=None, flags=0):
         """ipcfp_generate_message_log_proof_resident against a ResidentTipset of this store → (A.EventResultPy, exec_indices). flags:
         WITNESS_BY_REFERENCE, RESULT_JSON, SCAN_SKIP_TX_AMTS."""
-        cids, fp, fkeep, idx = self._message_args(message_cids, log_filter)
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_message_log_proof_resident(self._h, tip._h, cids.ctypes.data if cids.size else None, len(cids), fp, flags,
-                                                               idx.ctypes.data if idx.size else None, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents), idx
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return self._message_log_proof("ipcfp_generate_message_log_proof_resident", tip._h, message_cids, log_filter, flags)
+
+    @staticmethod
+    def _message_args(message_cids, log_filter):
+        cids = np.ascontiguousarray(message_cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+        f, fkeep = log_filter.as_c() if log_filter is not None else (None, None)
+        return cids, (C.byref(f) if f is not None else None), fkeep
+
+    def _message_log_proof(self, fn, tipset, message_cids, log_filter, flags):
+        cids, fp, fkeep = self._message_args(message_cids, log_filter)
+        idx = np.zeros(len(cids), np.uint64)
+        return _result(fn, *_EVENT_RESULT, self._h, tipset, cids.ctypes.data if cids.size else None, len(cids), fp, flags,
+                       idx.ctypes.data if idx.size else None), idx
 
     def plan_fetch_messages(self, tip, message_cids, log_filter=None, flags=0):
         """ipcfp_plan_fetch_message_log_resident → A.FetchPlanPy: one fetch round for generate_message_log_proof_resident(tip, message_cids,
         log_filter)."""
-        cids, fp, fkeep, _ = self._message_args(message_cids, log_filter)
-        out = C.POINTER(A.FetchPlanC)()
-        _check(lib().ipcfp_plan_fetch_message_log_resident(self._h, tip._h, cids.ctypes.data if cids.size else None, len(cids), fp, flags,
-                                                           C.byref(out)))
-        try:
-            return A.fetch_plan_from_c(out.contents)
-        finally:
-            lib().ipcfp_fetch_plan_free(out)
+        cids, fp, fkeep = self._message_args(message_cids, log_filter)
+        return _result("ipcfp_plan_fetch_message_log_resident", *_FETCH_PLAN, self._h, tip._h, cids.ctypes.data if cids.size else None,
+                       len(cids), fp, flags)
 
     def generate_event_proof_shard(self, ts, spec, lo, hi, world, rank, flags=0):
         d, keep = A.make_tipset_desc(ts)
         cs = spec.as_c() if isinstance(spec, EventProofSpec) else spec
-        out = C.POINTER(A.EventResultC)()
-        _check(lib().ipcfp_generate_event_proof_shard(self._h, C.byref(d), C.byref(cs), lo, hi, world, rank, flags, C.byref(out)))
-        try:
-            return A.event_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_event_result_free(out)
+        return _result("ipcfp_generate_event_proof_shard", *_EVENT_RESULT, self._h, C.byref(d), C.byref(cs), lo, hi, world, rank, flags)
 
     # --- read_storage_slot (storage/decode.rs:36-97), batched
     def read_storage_slots(self, root, slots):
         root = _u8(root)
         slots = _u8(slots).reshape(-1, 32)
-        out = C.POINTER(A.SlotResultC)()
-        _check(lib().ipcfp_read_storage_slots(self._h, root.ctypes.data, slots.ctypes.data if slots.size else None, len(slots), C.byref(out)))
-        try:
-            return A.slot_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_slot_result_free(out)
+        return _result("ipcfp_read_storage_slots", A.SlotResultC, A.slot_result_from_c, "ipcfp_slot_result_free", self._h, root.ctypes.data,
+                       slots.ctypes.data if slots.size else None, len(slots))
 
     # --- generate_storage_proof (storage/generator.rs:29-67), batched
     def generate_storage_proofs(self, ts, specs):
         specs = [(s.actor_id, s.slot) if isinstance(s, StorageProofSpec) else s for s in specs]
         d, keep = A.make_tipset_desc(ts)
         arr = A.make_storage_specs(specs)
-        out = C.POINTER(A.StorageResultC)()
-        _check(lib().ipcfp_generate_storage_proofs(self._h, C.byref(d), arr, len(specs), C.byref(out)))
-        try:
-            return A.storage_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_storage_result_free(out)
+        return _result("ipcfp_generate_storage_proofs", A.StorageResultC, A.storage_result_from_c, "ipcfp_storage_result_free", self._h,
+                       C.byref(d), arr, len(specs))
 
     # --- generate_proof_bundle (proofs/generator.rs:25-95)
     @staticmethod
@@ -531,14 +429,8 @@ class BlockStore:
         return A.make_storage_specs(sspecs), len(sspecs), (A.EventSpec * len(especs))(*especs), len(especs)
 
     def generate_proof_bundle(self, ts, storage_specs, event_specs):
-        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
         d, keep = A.make_tipset_desc(ts)
-        out = C.POINTER(A.BundleC)()
-        _check(lib().ipcfp_generate_proof_bundle(self._h, C.byref(d), sarr, ns, earr, ne, C.byref(out)))
-        try:
-            return A.bundle_from_c(out.contents)
-        finally:
-            lib().ipcfp_bundle_free(out)
+        return _result("ipcfp_generate_proof_bundle", *_BUNDLE, self._h, C.byref(d), *self._bundle_specs(storage_specs, event_specs))
 
     def upload_tipset(self, ts):
         """ipcfp_tipset_upload: the tipset's descriptor on the device, for any number of _resident calls. close() releases it."""
@@ -555,70 +447,38 @@ class BlockStore:
 
     def generate_proof_bundle_resident(self, tip, storage_specs, event_specs, flags=0):
         """ipcfp_generate_proof_bundle_resident against a ResidentTipset of this store. flags: WITNESS_BY_REFERENCE, RESULT_JSON."""
-        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
-        out = C.POINTER(A.BundleC)()
-        _check(lib().ipcfp_generate_proof_bundle_resident(self._h, tip._h, sarr, ns, earr, ne, flags, C.byref(out)))
-        try:
-            return A.bundle_from_c(out.contents)
-        finally:
-            lib().ipcfp_bundle_free(out)
+        return _result("ipcfp_generate_proof_bundle_resident", *_BUNDLE, self._h, tip._h, *self._bundle_specs(storage_specs, event_specs),
+                       flags)
 
     def plan_fetch(self, tip, storage_specs, event_specs, flags=0):
         """ipcfp_plan_fetch_resident → A.FetchPlanPy: the CIDs this store lacks of the blocks generate_proof_bundle_resident(tip,
         storage_specs, event_specs) would read, as far as the blocks it holds tell (one round; see fetch_until_complete)."""
-        sarr, ns, earr, ne = self._bundle_specs(storage_specs, event_specs)
-        out = C.POINTER(A.FetchPlanC)()
-        _check(lib().ipcfp_plan_fetch_resident(self._h, tip._h, sarr, ns, earr, ne, flags, C.byref(out)))
-        try:
-            return A.fetch_plan_from_c(out.contents)
-        finally:
-            lib().ipcfp_fetch_plan_free(out)
+        return _result("ipcfp_plan_fetch_resident", *_FETCH_PLAN, self._h, tip._h, *self._bundle_specs(storage_specs, event_specs), flags)
 
     def generate_log_bundle(self, ts, storage_specs, log_filters, flags=0):
         """ipcfp_generate_log_bundle: generate_proof_bundle with LogFilters in place of event specs (events[k] is filter k's result)
         → A.BundlePy. flags: WITNESS_BY_REFERENCE, RESULT_JSON."""
-        sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
-        farr, nf, fkeep = _log_filters_c(log_filters)
         d, keep = A.make_tipset_desc(ts)
-        out = C.POINTER(A.BundleC)()
-        _check(lib().ipcfp_generate_log_bundle(self._h, C.byref(d), sarr, ns, farr, nf, flags, C.byref(out)))
-        try:
-            return A.bundle_from_c(out.contents)
-        finally:
-            lib().ipcfp_bundle_free(out)
+        return self._log_bundle("ipcfp_generate_log_bundle", _BUNDLE, C.byref(d), storage_specs, log_filters, flags)
 
     def generate_log_bundle_resident(self, tip, storage_specs, log_filters, flags=0):
         """ipcfp_generate_log_bundle_resident against a ResidentTipset of this store → A.BundlePy."""
-        sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
-        farr, nf, fkeep = _log_filters_c(log_filters)
-        out = C.POINTER(A.BundleC)()
-        _check(lib().ipcfp_generate_log_bundle_resident(self._h, tip._h, sarr, ns, farr, nf, flags, C.byref(out)))
-        try:
-            return A.bundle_from_c(out.contents)
-        finally:
-            lib().ipcfp_bundle_free(out)
+        return self._log_bundle("ipcfp_generate_log_bundle_resident", _BUNDLE, tip._h, storage_specs, log_filters, flags)
 
     def plan_fetch_log_bundle(self, tip, storage_specs, log_filters, flags=0):
         """ipcfp_plan_fetch_log_bundle_resident → A.FetchPlanPy: one fetch round for generate_log_bundle_resident(tip, storage_specs,
         log_filters)."""
+        return self._log_bundle("ipcfp_plan_fetch_log_bundle_resident", _FETCH_PLAN, tip._h, storage_specs, log_filters, flags)
+
+    def _log_bundle(self, fn, result, tipset, storage_specs, log_filters, flags):
         sarr, ns, _, _ = self._bundle_specs(storage_specs, [])
         farr, nf, fkeep = _log_filters_c(log_filters)
-        out = C.POINTER(A.FetchPlanC)()
-        _check(lib().ipcfp_plan_fetch_log_bundle_resident(self._h, tip._h, sarr, ns, farr, nf, flags, C.byref(out)))
-        try:
-            return A.fetch_plan_from_c(out.contents)
-        finally:
-            lib().ipcfp_fetch_plan_free(out)
+        return _result(fn, *result, self._h, tipset, sarr, ns, farr, nf, flags)
 
     def plan_fetch_logs(self, tip, log_filter, flags=0):
         """ipcfp_plan_fetch_log_resident → A.FetchPlanPy: one fetch round for generate_log_proof_resident(tip, log_filter)."""
         f, fkeep = log_filter.as_c()
-        out = C.POINTER(A.FetchPlanC)()
-        _check(lib().ipcfp_plan_fetch_log_resident(self._h, tip._h, C.byref(f), flags, C.byref(out)))
-        try:
-            return A.fetch_plan_from_c(out.contents)
-        finally:
-            lib().ipcfp_fetch_plan_free(out)
+        return _result("ipcfp_plan_fetch_log_resident", *_FETCH_PLAN, self._h, tip._h, C.byref(f), flags)
 
     def resolve_addresses(self, state_root, addresses):
         """ipcfp_resolve_addresses → A.ResolveResultPy: every address (Address::to_bytes(), or text for address_parse) resolved to its
@@ -627,12 +487,8 @@ class BlockStore:
         if root.size != A.CID_LEN:
             raise ValueError("state_root must be a 38-byte CID")
         addrs = A.make_addresses([address_parse(a) if isinstance(a, str) else a for a in addresses])
-        out = C.POINTER(A.ResolveResultC)()
-        _check(lib().ipcfp_resolve_addresses(self._h, root.ctypes.data, addrs, len(addresses), C.byref(out)))
-        try:
-            return A.resolve_result_from_c(out.contents)
-        finally:
-            lib().ipcfp_resolve_result_free(out)
+        return _result("ipcfp_resolve_addresses", A.ResolveResultC, A.resolve_result_from_c, "ipcfp_resolve_result_free", self._h,
+                       root.ctypes.data, addrs, len(addresses))
 
     def close(self):
         if self._h:
@@ -693,13 +549,8 @@ def blocks_from_rpc_json(cids, texts):
     A.WitnessPy (cids, 16-aligned offsets, lengths, blob). Failures raise IpcfpError with the status and the index include/ipcfp.h gives."""
     cids = np.ascontiguousarray(cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
     arr, lens, keep = _text_array(texts)
-    out = C.POINTER(A.ParsedBlocksC)()
-    L = lib()
-    _check(L.ipcfp_blocks_from_rpc_json(cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep), C.byref(out)))
-    try:
-        return A.witness_from_c(out.contents.blocks)
-    finally:
-        L.ipcfp_parsed_blocks_free(out)
+    return _result("ipcfp_blocks_from_rpc_json", A.ParsedBlocksC, lambda c: A.witness_from_c(c.blocks), "ipcfp_parsed_blocks_free",
+                   cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep))
 
 
 def fetch_plan_to_rpc_json(cids, first_id=0):
@@ -857,13 +708,8 @@ def tipset_desc_from_json(parent_text, child_text, receipts_text):
     """ipcfp_tipset_desc_from_json (host parser, no device): the descriptor of the Lotus JSON-RPC texts as an A.TipsetInfoPy. Failures raise
     IpcfpError with the status and the receipt index (UINT64_MAX outside the receipt list's elements)."""
     p, c, r = (_text(x) for x in (parent_text, child_text, receipts_text))
-    out = C.POINTER(A.ParsedTipsetC)()
-    L = lib()
-    _check(L.ipcfp_tipset_desc_from_json(p, len(p), c, len(c), r, len(r), C.byref(out)))
-    try:
-        return A.tipset_info_from_c(out.contents.desc)
-    finally:
-        L.ipcfp_parsed_tipset_free(out)
+    return _result("ipcfp_tipset_desc_from_json", A.ParsedTipsetC, lambda t: A.tipset_info_from_c(t.desc), "ipcfp_parsed_tipset_free",
+                   p, len(p), c, len(c), r, len(r))
 
 
 def _to_json(fn, obj_ptr, ts):
@@ -955,6 +801,9 @@ class BundleVerdict:
         self.ms = dict(total=c.ms_total, parse=c.ms_parse, store=c.ms_store, verify=c.ms_verify)
 
 
+_VERDICT = (A.BundleVerdictC, BundleVerdict, "ipcfp_bundle_verdict_free")
+
+
 def _trust_callbacks(trusted_parent, trusted_child):
     cb_p = A.TrustedParentFn(lambda ctx, e, p, n: int(bool(trusted_parent(int(e), C.string_at(p, 38 * n) if n else b""))))\
         if trusted_parent else A.TrustedParentFn()
@@ -967,14 +816,8 @@ def verify_bundle_json(text, trusted_parent=None, trusted_child=None, filter_spe
     all. filter_spec: an A.EventSpec (check_event) or None. → BundleVerdict; failures raise IpcfpError (status, index)."""
     raw = text.encode() if isinstance(text, str) else bytes(text)
     cb_p, cb_c = _trust_callbacks(trusted_parent, trusted_child)
-    out = C.POINTER(A.BundleVerdictC)()
-    L = lib()
-    _check(L.ipcfp_verify_bundle_json(raw, len(raw), device, cb_p, cb_c, None, C.addressof(filter_spec) if filter_spec is not None else None,
-                                      C.byref(out)))
-    try:
-        return BundleVerdict(out.contents)
-    finally:
-        L.ipcfp_bundle_verdict_free(out)
+    return _result("ipcfp_verify_bundle_json", *_VERDICT, raw, len(raw), device, cb_p, cb_c, None,
+                   C.addressof(filter_spec) if filter_spec is not None else None)
 
 
 def verify_bundle_json_any(text, trusted_parent=None, trusted_child=None, log_filters=(), device=0):
@@ -983,69 +826,48 @@ def verify_bundle_json_any(text, trusted_parent=None, trusted_child=None, log_fi
     raw = text.encode() if isinstance(text, str) else bytes(text)
     cb_p, cb_c = _trust_callbacks(trusted_parent, trusted_child)
     farr, nf, fkeep = _log_filters_c(log_filters)
-    out = C.POINTER(A.BundleVerdictC)()
-    L = lib()
-    _check(L.ipcfp_verify_bundle_json_any(raw, len(raw), device, cb_p, cb_c, None, farr, nf, C.byref(out)))
+    return _result("ipcfp_verify_bundle_json_any", *_VERDICT, raw, len(raw), device, cb_p, cb_c, None, farr, nf)
+
+
+def _verify(witness, ts, result, device, fn, *args, blob=True):
+    """lib().<fn>(store, descriptor, proofs, n, [data blob, blob size,] *args, results) over the witness (WitnessPy) as a store with every
+    block Blake2b-checked against its CID → list of bools, one per proof of `result`. blob: pass result.data_blob."""
+    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
     try:
-        return BundleVerdict(out.contents)
+        d, keep = A.make_tipset_desc(ts)
+        n = len(result.proofs)
+        res = np.zeros(max(n, 1), dtype=np.uint8)
+        raw = np.ascontiguousarray(result.raw_proofs)
+        if blob:
+            data = np.ascontiguousarray(result.data_blob)
+            args = (data.ctypes.data if data.size else None, data.size) + args
+        _check(getattr(lib(), fn)(store._h, C.byref(d), raw.ctypes.data if n else None, n, *args, res.ctypes.data))
+        return [bool(x) for x in res[:n]]
     finally:
-        L.ipcfp_bundle_verdict_free(out)
+        store.close()
 
 
 def verify_event_proofs(witness, ts, result, filter_spec=None, device=0):
     """verify_event_proof (events/verifier.rs:51-74) batched on the GPU: the witness (WitnessPy) becomes a store with every block
     Blake2b-checked against its CID, then every proof of `result` (EventResultPy) is replayed. filter_spec (check_event): None, an
     EventProofSpec or a LogFilter (ipcfp_verify_event_proofs_log). → list of bools."""
-    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
-    try:
-        d, keep = A.make_tipset_desc(ts)
-        n = len(result.proofs)
-        res = np.zeros(max(n, 1), dtype=np.uint8)
-        raw = np.ascontiguousarray(result.raw_proofs)
-        blob = np.ascontiguousarray(result.data_blob)
-        if isinstance(filter_spec, LogFilter):
-            f, fkeep = filter_spec.as_c()
-            _check(lib().ipcfp_verify_event_proofs_log(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None,
-                                                       blob.size, C.byref(f), res.ctypes.data))
-            return [bool(x) for x in res[:n]]
-        fs = filter_spec.as_c() if isinstance(filter_spec, EventProofSpec) else filter_spec
-        _check(lib().ipcfp_verify_event_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None, blob.size,
-                                               C.addressof(fs) if fs is not None else None, res.ctypes.data))
-        return [bool(x) for x in res[:n]]
-    finally:
-        store.close()
+    if isinstance(filter_spec, LogFilter):
+        f, fkeep = filter_spec.as_c()
+        return _verify(witness, ts, result, device, "ipcfp_verify_event_proofs_log", C.byref(f))
+    fs = filter_spec.as_c() if isinstance(filter_spec, EventProofSpec) else filter_spec
+    return _verify(witness, ts, result, device, "ipcfp_verify_event_proofs", C.addressof(fs) if fs is not None else None)
 
 
 def verify_event_proofs_any(witness, ts, result, log_filters, device=0):
     """verify_event_proofs with check_event = "matches at least one of log_filters" (ipcfp_verify_event_proofs_any; an empty sequence:
     no check_event). result: anything with raw_proofs, data_blob and proofs (A.EventResultPy). → list of bools."""
-    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
-    try:
-        d, keep = A.make_tipset_desc(ts)
-        n = len(result.proofs)
-        res = np.zeros(max(n, 1), dtype=np.uint8)
-        raw = np.ascontiguousarray(result.raw_proofs)
-        blob = np.ascontiguousarray(result.data_blob)
-        farr, nf, fkeep = _log_filters_c(log_filters)
-        _check(lib().ipcfp_verify_event_proofs_any(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None,
-                                                   blob.size, farr, nf, res.ctypes.data))
-        return [bool(x) for x in res[:n]]
-    finally:
-        store.close()
+    farr, nf, fkeep = _log_filters_c(log_filters)
+    return _verify(witness, ts, result, device, "ipcfp_verify_event_proofs_any", farr, nf)
 
 
 def verify_storage_proofs(witness, ts, result, device=0):
     """verify_storage_proof (storage/verifier.rs:24-63) batched on the GPU over a CID-checked witness store."""
-    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
-    try:
-        d, keep = A.make_tipset_desc(ts)
-        n = len(result.proofs)
-        res = np.zeros(max(n, 1), dtype=np.uint8)
-        raw = np.ascontiguousarray(result.raw_proofs)
-        _check(lib().ipcfp_verify_storage_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, res.ctypes.data))
-        return [bool(x) for x in res[:n]]
-    finally:
-        store.close()
+    return _verify(witness, ts, result, device, "ipcfp_verify_storage_proofs", blob=False)
 
 
 def _hash_batch(fn, messages, device=0):

@@ -23,6 +23,56 @@ template <class F> static ipcfp_status guard(F f) {
     catch (const std::exception& e) { g_last_error = e.what(); return IPCFP_ERR_INVALID_ARG; }
 }
 
+// guard() with the prologue of every entry point that makes an object: "null argument" unless `ok` (its pointer arguments are set) and
+// `out` is set, *out cleared, then *out = f()
+template <class R, class F> static ipcfp_status produce(bool ok, R** out, F f) {
+    return guard([&] {
+        if (!ok || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        *out = nullptr;
+        *out = f();
+    });
+}
+
+static Store* store_of(ipcfp_store* s) { return reinterpret_cast<Store*>(s); }
+static TipsetDev& tipset_of(ipcfp_tipset* t) { return *reinterpret_cast<TipsetDev*>(t); }
+
+// f(store, tipset) with the descriptor uploaded into a call-local TipsetDev, asynchronously on the store's stream (ipcfp_tipset_upload
+// would add a host synchronisation)
+template <class F> static auto with_uploaded_tipset(Store* st, const ipcfp_tipset_desc* t, F f) {
+    TipsetDev td;
+    tipset_upload(st, t, td);
+    return f(st, td);
+}
+
+// produce() of a call on a tipset, *out = f(store, tipset): a resident tipset as it is, a descriptor through with_uploaded_tipset
+template <class R, class F> static ipcfp_status on_tipset(ipcfp_store* s, ipcfp_tipset* t, R** out, F f) {
+    return produce(s && t, out, [&] { return f(store_of(s), tipset_of(t)); });
+}
+template <class R, class F> static ipcfp_status on_tipset(ipcfp_store* s, const ipcfp_tipset_desc* t, R** out, F f) {
+    return produce(s != nullptr, out, [&] { return with_uploaded_tipset(store_of(s), t, f); });
+}
+
+// *out = the store make() creates; a block that fails its CID check is reported with the store in *out
+template <class F> static ipcfp_status make_store(ipcfp_store** out, F make) {
+    return guard([&] {
+        if (!out) throw Error(IPCFP_ERR_INVALID_ARG, "null out");
+        *out = nullptr;
+        Store* s = make();
+        *out = reinterpret_cast<ipcfp_store*>(s);
+        if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
+    });
+}
+// *out = a resident tipset that upload(store, tipset) fills, complete on the device when the call returns
+template <class F> static ipcfp_status make_resident(ipcfp_store* s, ipcfp_tipset** out, F upload) {
+    return produce(s != nullptr, out, [&] {
+        Store* st = store_of(s);
+        std::unique_ptr<TipsetDev> td(new TipsetDev());
+        upload(st, *td);
+        IPCFP_CUDA(cudaStreamSynchronize(st->stream));
+        return reinterpret_cast<ipcfp_tipset*>(td.release());
+    });
+}
+
 // ------------------------------------------------------------------------------------------ bundle
 struct BundleBox {
     ipcfp_bundle r;   // must stay first
@@ -43,14 +93,23 @@ struct TimingEvent {
 struct FetchPlanBox {
     ipcfp_fetch_plan r;   // must stay first
     FetchPlan plan;
-    void fill() {
-        r.n_missing = plan.cids.size() / 38;
-        r.cids = plan.cids.data();
-        r.n_needed = plan.n_needed;
-        r.n_levels = plan.n_levels;
-        r.ms_total = plan.ms_total;
-    }
 };
+
+static void plan_flags_check(uint32_t flags) {
+    if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+}
+// the fetch plan that plan(FetchPlan&) makes, in the box ipcfp_fetch_plan_free releases
+template <class F> static ipcfp_fetch_plan* make_plan(F plan) {
+    std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
+    FetchPlan& p = box->plan;
+    plan(p);
+    box->r.n_missing = p.cids.size() / 38;
+    box->r.cids = p.cids.data();
+    box->r.n_needed = p.n_needed;
+    box->r.n_levels = p.n_levels;
+    box->r.ms_total = p.ms_total;
+    return &box.release()->r;
+}
 
 #define IPCFP_BUNDLE_FLAGS (IPCFP_WITNESS_BY_REFERENCE | IPCFP_RESULT_JSON)
 
@@ -182,24 +241,15 @@ void ipcfp_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 ipcfp_status ipcfp_store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size,
                                 uint64_t n_blocks, int device, uint32_t flags, ipcfp_store** out) {
-    return guard([&] {
-        if (!out) throw Error(IPCFP_ERR_INVALID_ARG, "null out");
-        *out = nullptr;
-        Store* s = store_create(cids, offsets, lengths, blob, blob_size, n_blocks, device, flags);
-        *out = reinterpret_cast<ipcfp_store*>(s);
-        if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
-    });
+    return make_store(out, [&] { return store_create(cids, offsets, lengths, blob, blob_size, n_blocks, device, flags); });
 }
 ipcfp_status ipcfp_store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts,
                                          int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info) {
-    return guard([&] {
-        if (!out) throw Error(IPCFP_ERR_INVALID_ARG, "null out");
-        *out = nullptr;
+    return make_store(out, [&] {
         ipcfp_store_json_info si;
         Store* s = store_create_rpc_json(cids, n_blocks, texts, text_lens, n_texts, device, flags, si);
-        *out = reinterpret_cast<ipcfp_store*>(s);
         if (info) *info = si;
-        if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
+        return s;
     });
 }
 void ipcfp_store_destroy(ipcfp_store* s) { delete reinterpret_cast<Store*>(s); }
@@ -208,14 +258,14 @@ uint64_t ipcfp_store_first_bad_block(const ipcfp_store* s) { return s ? reinterp
 ipcfp_status ipcfp_store_get(ipcfp_store* s, const uint8_t cid[IPCFP_CID_LEN], uint8_t* buf, uint32_t cap, uint32_t* len, int* found) {
     return guard([&] {
         if (!s || !cid || !found) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        store_get(reinterpret_cast<Store*>(s), cid, buf, cap, len, found);
+        store_get(store_of(s), cid, buf, cap, len, found);
     });
 }
 ipcfp_status ipcfp_store_has(ipcfp_store* s, const uint8_t cid[IPCFP_CID_LEN], int* found) {
     return guard([&] {
         if (!s || !cid || !found) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
         uint32_t len;
-        store_get(reinterpret_cast<Store*>(s), cid, nullptr, 0, &len, found);
+        store_get(store_of(s), cid, nullptr, 0, &len, found);
     });
 }
 
@@ -237,134 +287,73 @@ ipcfp_status ipcfp_compute_mapping_slots(const uint8_t* keys32, const uint64_t* 
 
 ipcfp_status ipcfp_generate_event_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_spec* spec, uint32_t flags,
                                         ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_event_proof(st, td, spec, flags, false, 0, 0);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_event_proof(st, td, spec, flags, false, 0, 0); });
 }
 ipcfp_status ipcfp_generate_event_proof_shard(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_event_spec* spec, uint64_t lo, uint64_t hi,
                                               uint32_t world_size, uint32_t rank, uint32_t flags, ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_event_proof(st, td, spec, flags, true, lo, hi);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_event_proof(st, td, spec, flags, true, lo, hi); });
 }
 void ipcfp_event_result_free(ipcfp_event_result* r) { if (r) event_result_free(r); }
 
 ipcfp_status ipcfp_tipset_upload(ipcfp_store* s, const ipcfp_tipset_desc* t, ipcfp_tipset** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        std::unique_ptr<TipsetDev> td(new TipsetDev());
-        tipset_upload(st, t, *td);
-        IPCFP_CUDA(cudaStreamSynchronize(st->stream));
-        *out = reinterpret_cast<ipcfp_tipset*>(td.release());
-    });
+    return make_resident(s, out, [&](Store* st, TipsetDev& td) { tipset_upload(st, t, td); });
 }
 void ipcfp_tipset_free(ipcfp_tipset* t) { delete reinterpret_cast<TipsetDev*>(t); }
 ipcfp_status ipcfp_tipset_upload_json(ipcfp_store* s, const char* parent, uint64_t parent_len, const char* child, uint64_t child_len,
                                       const char* receipts, uint64_t receipts_len, ipcfp_tipset** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        std::unique_ptr<TipsetDev> td(new TipsetDev());
-        tipset_upload_json(st, parent, parent_len, child, child_len, receipts, receipts_len, *td);
-        IPCFP_CUDA(cudaStreamSynchronize(st->stream));
-        *out = reinterpret_cast<ipcfp_tipset*>(td.release());
+    return make_resident(s, out, [&](Store* st, TipsetDev& td) {
+        tipset_upload_json(st, parent, parent_len, child, child_len, receipts, receipts_len, td);
     });
 }
 ipcfp_status ipcfp_tipset_describe(ipcfp_tipset* t, int with_events_roots, ipcfp_tipset_info* out) {
     return guard([&] {
         if (!t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        tipset_describe(*reinterpret_cast<TipsetDev*>(t), with_events_roots != 0, out);
+        tipset_describe(tipset_of(t), with_events_roots != 0, out);
     });
 }
 ipcfp_status ipcfp_generate_event_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, uint32_t flags,
                                                  ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), spec, flags, false, 0, 0);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_event_proof(st, td, spec, flags, false, 0, 0); });
 }
 ipcfp_status ipcfp_generate_event_proof_shard_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, uint64_t lo, uint64_t hi,
                                                        uint32_t world_size, uint32_t rank, uint32_t flags, ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), spec, flags, true, lo, hi);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_event_proof(st, td, spec, flags, true, lo, hi); });
 }
 ipcfp_status ipcfp_generate_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags,
                                                ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_log_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), filter, flags);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_log_proof(st, td, filter, flags); });
 }
 ipcfp_status ipcfp_generate_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_log_filter* filter, uint32_t flags,
                                       ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_log_proof(st, td, filter, flags);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_log_proof(st, td, filter, flags); });
 }
 ipcfp_status ipcfp_generate_message_log_proof_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n,
                                                        const ipcfp_log_filter* filter, uint32_t flags, uint64_t* exec_indices, ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_message_log_proof(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), message_cids, n, filter, flags, exec_indices);
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        return generate_message_log_proof(st, td, message_cids, n, filter, flags, exec_indices);
     });
 }
 ipcfp_status ipcfp_generate_message_log_proof(ipcfp_store* s, const ipcfp_tipset_desc* t, const uint8_t* message_cids, uint64_t n,
                                               const ipcfp_log_filter* filter, uint32_t flags, uint64_t* exec_indices, ipcfp_event_result** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        // the resident call's refusals come before the upload: no device work for a refused request
-        if (n && (!message_cids || !exec_indices)) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs or exec indices with a nonzero count");
-        if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
-        if (filter) log_filter_check(filter);
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_message_log_proof(st, td, message_cids, n, filter, flags, exec_indices);
+    return produce(s != nullptr, out, [&] {
+        message_request_check(message_cids, n, filter, true, exec_indices);   // before the upload: no device work for a refused request
+        return with_uploaded_tipset(store_of(s), t, [&](Store* st, TipsetDev& td) {
+            return generate_message_log_proof(st, td, message_cids, n, filter, flags, exec_indices);
+        });
     });
 }
-void* ipcfp_store_stream(ipcfp_store* s) { return s ? (void*)reinterpret_cast<Store*>(s)->stream : nullptr; }
+void* ipcfp_store_stream(ipcfp_store* s) { return s ? (void*)store_of(s)->stream : nullptr; }
 
 ipcfp_status ipcfp_read_storage_slots(ipcfp_store* s, const uint8_t root[IPCFP_CID_LEN], const uint8_t* slots, uint64_t k, ipcfp_slot_result** out) {
-    return guard([&] {
-        if (!s || !out || !root || (k && !slots)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = read_storage_slots(reinterpret_cast<Store*>(s), root, slots, k);
-    });
+    return produce(s && root && (!k || slots), out, [&] { return read_storage_slots(store_of(s), root, slots, k); });
 }
 void ipcfp_slot_result_free(ipcfp_slot_result* r) { if (r) slot_result_free(r); }
 
 ipcfp_status ipcfp_generate_storage_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* specs, uint64_t n,
                                            ipcfp_storage_result** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
+    return produce(s != nullptr, out, [&] {
         if (!t) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
-        *out = generate_storage_proofs(reinterpret_cast<Store*>(s), t->child_cid, t->child_parent_state_root, specs, n);
+        return generate_storage_proofs(store_of(s), t->child_cid, t->child_parent_state_root, specs, n);
     });
 }
 void ipcfp_storage_result_free(ipcfp_storage_result* r) { if (r) storage_result_free(r); }
@@ -372,107 +361,58 @@ void ipcfp_storage_result_free(ipcfp_storage_result* r) { if (r) storage_result_
 // generate_proof_bundle (proofs/generator.rs:25-95): the tipset uploaded, then the resident call's body without flags
 ipcfp_status ipcfp_generate_proof_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                          const ipcfp_event_spec* especs, uint64_t n_especs, ipcfp_bundle** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_proof_bundle(st, td, sspecs, n_sspecs, especs, n_especs, 0);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_proof_bundle(st, td, sspecs, n_sspecs, especs, n_especs, 0); });
 }
 ipcfp_status ipcfp_generate_proof_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                                   const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_bundle** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_proof_bundle(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, especs, n_especs, flags);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_proof_bundle(st, td, sspecs, n_sspecs, especs, n_especs, flags); });
 }
 ipcfp_status ipcfp_generate_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                                 const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = generate_log_bundle(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, filters, n_filters, flags);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_log_bundle(st, td, sspecs, n_sspecs, filters, n_filters, flags); });
 }
 ipcfp_status ipcfp_generate_log_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                        const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_bundle** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        *out = generate_log_bundle(st, td, sspecs, n_sspecs, filters, n_filters, flags);
-    });
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_log_bundle(st, td, sspecs, n_sspecs, filters, n_filters, flags); });
 }
 void ipcfp_bundle_free(ipcfp_bundle* b) { delete reinterpret_cast<BundleBox*>(b); }
 
-static void plan_fetch_log_bundle(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs, const ipcfp_log_filter* filters,
-                                  uint64_t n_filters, ipcfp_fetch_plan** out) {
-    std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
-    plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, nullptr, 0, box->plan, filters, n_filters);
-    box->fill();
-    *out = &box.release()->r;
-}
 ipcfp_status ipcfp_plan_fetch_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                        const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
-        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
-        plan_fetch(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), sspecs, n_sspecs, especs, n_especs, box->plan);
-        box->fill();
-        *out = &box.release()->r;
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        plan_flags_check(flags);
+        return make_plan([&](FetchPlan& p) { plan_fetch(st, td, sspecs, n_sspecs, especs, n_especs, p); });
     });
 }
 ipcfp_status ipcfp_plan_fetch(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                               const ipcfp_event_spec* especs, uint64_t n_especs, uint32_t flags, ipcfp_fetch_plan** out) {
-    return guard([&] {
-        if (!s || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
-        Store* st = reinterpret_cast<Store*>(s);
-        TipsetDev td;
-        tipset_upload(st, t, td);
-        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
-        plan_fetch(st, td, sspecs, n_sspecs, especs, n_especs, box->plan);
-        box->fill();
-        *out = &box.release()->r;
+    return produce(s != nullptr, out, [&] {
+        plan_flags_check(flags);
+        return with_uploaded_tipset(store_of(s), t, [&](Store* st, TipsetDev& td) {
+            return make_plan([&](FetchPlan& p) { plan_fetch(st, td, sspecs, n_sspecs, especs, n_especs, p); });
+        });
     });
 }
 ipcfp_status ipcfp_plan_fetch_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                                   const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_fetch_plan** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
-        plan_fetch_log_bundle(s, t, sspecs, n_sspecs, filters, n_filters, out);
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        plan_flags_check(flags);
+        return make_plan([&](FetchPlan& p) { plan_fetch(st, td, sspecs, n_sspecs, nullptr, 0, p, filters, n_filters); });
     });
 }
 // the bundle plan of one filter and no storage spec; a refused filter has no index
 ipcfp_status ipcfp_plan_fetch_log_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_log_filter* filter, uint32_t flags, ipcfp_fetch_plan** out) {
-    return guard([&] {
-        if (!s || !t || !out || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
+    return produce(s && t && filter, out, [&] {
+        plan_flags_check(flags);
         log_filter_check(filter);
-        plan_fetch_log_bundle(s, t, nullptr, 0, filter, 1, out);
+        return make_plan([&](FetchPlan& p) { plan_fetch(store_of(s), tipset_of(t), nullptr, 0, nullptr, 0, p, filter, 1); });
     });
 }
 ipcfp_status ipcfp_plan_fetch_message_log_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n,
                                                    const ipcfp_log_filter* filter, uint32_t flags, ipcfp_fetch_plan** out) {
-    return guard([&] {
-        if (!s || !t || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        if (flags) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for a fetch plan");
-        std::unique_ptr<FetchPlanBox> box(new FetchPlanBox());
-        plan_fetch_messages(reinterpret_cast<Store*>(s), *reinterpret_cast<TipsetDev*>(t), message_cids, n, filter, box->plan);
-        box->fill();
-        *out = &box.release()->r;
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        plan_flags_check(flags);
+        return make_plan([&](FetchPlan& p) { plan_fetch_messages(st, td, message_cids, n, filter, p); });
     });
 }
 void ipcfp_fetch_plan_free(ipcfp_fetch_plan* p) { delete reinterpret_cast<FetchPlanBox*>(p); }
@@ -483,11 +423,9 @@ struct ResolveBox {
 };
 ipcfp_status ipcfp_resolve_addresses(ipcfp_store* s, const uint8_t state_root[IPCFP_CID_LEN], const ipcfp_address* addrs, uint64_t n,
                                      ipcfp_resolve_result** out) {
-    return guard([&] {
-        if (!s || !state_root || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
+    return produce(s && state_root, out, [&] {
         std::unique_ptr<ResolveBox> box(new ResolveBox());
-        resolve_addresses(reinterpret_cast<Store*>(s), state_root, addrs, n, box->out);
+        resolve_addresses(store_of(s), state_root, addrs, n, box->out);
         ipcfp_resolve_result& r = box->r;
         memset(&r, 0, sizeof r);
         r.n = n;
@@ -499,7 +437,7 @@ ipcfp_status ipcfp_resolve_addresses(ipcfp_store* s, const uint8_t state_root[IP
         box->out.wit.fill(r.witness);
         r.ms_total = box->out.ms_total;
         r.ms_lookup = box->out.ms_lookup;
-        *out = &box.release()->r;
+        return &box.release()->r;
     });
 }
 void ipcfp_resolve_result_free(ipcfp_resolve_result* r) { delete reinterpret_cast<ResolveBox*>(r); }
@@ -520,7 +458,7 @@ ipcfp_status ipcfp_verify_event_proofs(ipcfp_store* s, const ipcfp_tipset_desc* 
                                        uint64_t blob_size, const ipcfp_event_spec* filter, uint8_t* results) {
     return guard([&] {
         if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, filter, results);
+        verify_event_proofs(store_of(s), t, proofs, n, blob, blob_size, filter, results);
     });
 }
 // check_event = the set of one filter; a refused filter has no index
@@ -528,7 +466,7 @@ ipcfp_status ipcfp_verify_event_proofs_log(ipcfp_store* s, const ipcfp_tipset_de
                                            uint64_t blob_size, const ipcfp_log_filter* filter, uint8_t* results) {
     return guard([&] {
         if (!s || !filter) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        try { verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filter, 1); }
+        try { verify_event_proofs(store_of(s), t, proofs, n, blob, blob_size, nullptr, results, filter, 1); }
         catch (Error& e) {
             if (e.status == IPCFP_ERR_INVALID_ARG && e.index == 0) e.index = UINT64_MAX;
             throw;
@@ -539,33 +477,27 @@ ipcfp_status ipcfp_verify_event_proofs_any(ipcfp_store* s, const ipcfp_tipset_de
                                            uint64_t blob_size, const ipcfp_log_filter* filters, uint64_t n_filters, uint8_t* results) {
     return guard([&] {
         if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        verify_event_proofs(reinterpret_cast<Store*>(s), t, proofs, n, blob, blob_size, nullptr, results, filters, n_filters);
+        verify_event_proofs(store_of(s), t, proofs, n, blob, blob_size, nullptr, results, filters, n_filters);
     });
 }
 ipcfp_status ipcfp_verify_storage_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n, uint8_t* results) {
     return guard([&] {
         if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        verify_storage_proofs(reinterpret_cast<Store*>(s), t, proofs, n, results);
+        verify_storage_proofs(store_of(s), t, proofs, n, results);
     });
 }
 
 ipcfp_status ipcfp_verify_bundle_json(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
                                       ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_event_spec* filter,
                                       ipcfp_bundle_verdict** out) {
-    return guard([&] {
-        if (!json || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, filter);
-    });
+    return produce(json != nullptr, out, [&] { return verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, filter); });
 }
 ipcfp_status ipcfp_verify_bundle_json_any(const char* json, uint64_t len, int device, ipcfp_trusted_parent_ts_fn trusted_parent,
                                           ipcfp_trusted_child_header_fn trusted_child, void* trust_ctx, const ipcfp_log_filter* filters,
                                           uint64_t n_filters, ipcfp_bundle_verdict** out) {
-    return guard([&] {
-        if (!json || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
+    return produce(json != nullptr, out, [&] {
         LogFilterSet::check(filters, n_filters);
-        *out = verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, nullptr, filters, n_filters);
+        return verify_bundle_json(json, len, device, trusted_parent, trusted_child, trust_ctx, nullptr, filters, n_filters);
     });
 }
 void ipcfp_bundle_verdict_free(ipcfp_bundle_verdict* v) { if (v) bundle_verdict_free(v); }
@@ -577,24 +509,18 @@ ipcfp_status ipcfp_comm_unique_id(uint8_t id[IPCFP_COMM_ID_BYTES]) {
     });
 }
 ipcfp_status ipcfp_comm_init(const uint8_t id[IPCFP_COMM_ID_BYTES], uint32_t world_size, uint32_t rank, int device, ipcfp_comm** out) {
-    return guard([&] {
-        if (!id || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
-        *out = reinterpret_cast<ipcfp_comm*>(comm_init(id, world_size, rank, device));
-    });
+    return produce(id != nullptr, out, [&] { return reinterpret_cast<ipcfp_comm*>(comm_init(id, world_size, rank, device)); });
 }
 void ipcfp_comm_destroy(ipcfp_comm* c) { if (c) comm_destroy(reinterpret_cast<Comm*>(c)); }
 ipcfp_status ipcfp_generate_event_proof_sharded(ipcfp_comm* c, ipcfp_store* s, ipcfp_tipset* t, const ipcfp_event_spec* spec, const uint64_t* bounds,
                                                 uint32_t flags, ipcfp_event_result** out) {
-    return guard([&] {
-        if (!c || !s || !t || !bounds || !out) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
-        *out = nullptr;
+    return produce(c && s && t && bounds, out, [&] {
         Comm* cm = reinterpret_cast<Comm*>(c);
         const uint32_t W = comm_world(cm), r = comm_rank(cm);
-        TipsetDev& td = *reinterpret_cast<TipsetDev*>(t);
+        TipsetDev& td = tipset_of(t);
         for (uint32_t k = 0; k < W; k++) if (bounds[k] > bounds[k + 1]) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must ascend");
         if (bounds[0] != 0 || bounds[W] != td.n_receipts) throw Error(IPCFP_ERR_INVALID_ARG, "shard bounds must cover [0, n_receipts)");
-        *out = generate_event_proof(reinterpret_cast<Store*>(s), td, spec, flags, true, bounds[r], bounds[r + 1], cm);
+        return generate_event_proof(store_of(s), td, spec, flags, true, bounds[r], bounds[r + 1], cm);
     });
 }
 

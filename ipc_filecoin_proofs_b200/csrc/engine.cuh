@@ -213,6 +213,13 @@ ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_
 // filter null: every log extract_evm_log accepts. exec_indices[j] (host): request j's execution position, UINT64_MAX when not executed.
 ipcfp_event_result* generate_message_log_proof(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter,
                                                uint32_t flags, uint64_t* exec_indices);
+// The refusals of a message call, made before any device work: null CIDs with a nonzero count (with_exec: or null exec_indices, which
+// the generators write and the fetch plan does not take), more than IPCFP_MESSAGE_MAX CIDs, a refused filter (null: every log)
+void message_request_check(const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, bool with_exec, const uint64_t* exec_indices);
+// The host half of EventMatcher::new (events/generator.rs:30-35): m = the spec's t1 = ascii_to_bytes32(topic_1) and actor filter, t0 zero
+// (keccak256 of the signature is the caller's, on the device). A spec or field that is null is refused with the message `refusal`.
+struct Matcher;
+void event_matcher(const ipcfp_event_spec* spec, const char* refusal, Matcher& m);
 // plan.cu's selection: has_sel[i] (device, n_receipts) = the receipt has an events root and is selected by message_cids (n*38, host)
 // against the execution order exo (the tipset's, built on this store); left as it is when nothing is selected
 void message_selection_mask(Store* s, TipsetDev& td, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint8_t* has_sel);

@@ -1000,7 +1000,7 @@ struct EventCall {
         t_enter = std::chrono::steady_clock::now();
         LogFilterHost lfh;
         if constexpr (std::is_same_v<P, Matcher>) {
-            if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+            event_matcher(spec, "event spec has null fields", mh);
             siglen = strlen(spec->event_signature);
         } else {
             log_filter_build(filter, lfh);
@@ -1023,16 +1023,8 @@ struct EventCall {
         const size_t sig_cap = (siglen + 64) & ~(size_t)63;
         static_assert(sizeof(P) <= 1024, "the predicate must fit its staging slot");
         uint8_t* d_head = ob->stage(1024 + sig_cap, [&](uint8_t* hs) {
-            memset(&mh, 0, sizeof mh);
-            if constexpr (std::is_same_v<P, Matcher>) {
-                size_t n1 = strlen(spec->topic_1);
-                uint8_t t1[32];
-                memset(t1, 0, 32);
-                memcpy(t1, spec->topic_1, n1 < 32 ? n1 : 32);  // ascii_to_bytes32 (evm.rs:72-78)
-                memcpy(mh.t1, t1, 32);
-                mh.actor = spec->actor_id_filter;
-                mh.has_actor = spec->has_actor_id_filter ? 1 : 0;
-            } else {
+            if constexpr (!std::is_same_v<P, Matcher>) {   // the Matcher is event_matcher's, above
+                memset(&mh, 0, sizeof mh);
                 if (!lfh.dev.empty()) {   // through pinned memory that lives as long as the call: no host synchronisation
                     sets_h = PinnedArray(s->pool, lfh.dev.size() * 8);
                     memcpy(sets_h.p, lfh.dev.data(), lfh.dev.size() * 8);
@@ -1271,11 +1263,29 @@ ipcfp_event_result* generate_log_proof(Store* s, TipsetDev& td, const ipcfp_log_
     return c.fill();
 }
 
+void event_matcher(const ipcfp_event_spec* spec, const char* refusal, Matcher& m) {
+    if (!spec || !spec->event_signature || !spec->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, refusal);
+    memset(&m, 0, sizeof m);
+    const size_t n1 = strlen(spec->topic_1);
+    memcpy(m.t1, spec->topic_1, n1 < 32 ? n1 : 32);   // ascii_to_bytes32 (evm.rs:72-78)
+    m.actor = spec->actor_id_filter;
+    m.has_actor = spec->has_actor_id_filter ? 1 : 0;
+}
+
+void message_request_check(const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, bool with_exec, const uint64_t* exec_indices) {
+    if (with_exec) {
+        if (n && (!message_cids || !exec_indices)) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs or exec indices with a nonzero count");
+    } else if (n && !message_cids) {
+        throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs with a nonzero count");
+    }
+    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+    if (filter) log_filter_check(filter);
+}
+
 // the same call with its receipt loop restricted to the receipts of the given messages (filter null: every log extract_evm_log accepts)
 ipcfp_event_result* generate_message_log_proof(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter,
                                                uint32_t flags, uint64_t* exec_indices) {
-    if (n && (!message_cids || !exec_indices)) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs or exec indices with a nonzero count");
-    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+    message_request_check(message_cids, n, filter, true, exec_indices);
     ipcfp_log_filter any;
     memset(&any, 0, sizeof any);
     EventCall<LogFilter> c(s, td, nullptr, flags, false, 0, 0, nullptr);

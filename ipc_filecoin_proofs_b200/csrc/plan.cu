@@ -110,8 +110,8 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     fs.build(log_filters, n_log_filters);
     const bool events = n_especs || n_log_filters;   // the event path's rules (1–3) apply
     if (n_sspecs && !td.has_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
-    for (uint64_t k = 0; k < n_especs; k++)
-        if (!especs[k].event_signature || !especs[k].topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "event spec has null fields");
+    std::vector<Matcher> mh(n_especs);
+    for (uint64_t k = 0; k < n_especs; k++) event_matcher(&especs[k], "event spec has null fields", mh[k]);
     s->use();
     cudaStream_t st = s->stream;
     IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
@@ -133,16 +133,10 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
     }
     if (n_sspecs) { root(td.child_cid, PK_BLOCK); root(td.child_state_root, PK_BLOCK); }
     const uint64_t nh = kinds.size();
-    std::vector<Matcher> mh(n_especs);
     std::vector<uint64_t> sig_off(n_especs);
     std::vector<uint32_t> sig_len(n_especs);
     std::vector<uint8_t> sigs;
     for (uint64_t k = 0; k < n_especs; k++) {
-        memset(&mh[k], 0, sizeof(Matcher));
-        const size_t n1 = strlen(especs[k].topic_1);
-        memcpy(mh[k].t1, especs[k].topic_1, n1 < 32 ? n1 : 32);   // ascii_to_bytes32 (evm.rs:72-78)
-        mh[k].actor = especs[k].actor_id_filter;
-        mh[k].has_actor = especs[k].has_actor_id_filter ? 1 : 0;
         sig_off[k] = sigs.size();
         sig_len[k] = (uint32_t)strlen(especs[k].event_signature);
         sigs.insert(sigs.end(), especs[k].event_signature, especs[k].event_signature + sig_len[k]);
@@ -272,11 +266,9 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
 // TxMeta or message-AMT block is missing, or one does not decode, which the generator then reports — no receipt is taken, and the round
 // is the base roots, the TxMeta blocks and the message AMTs. Once it is built, the receipts rules 1 and 3 take are the selected ones.
 void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, FetchPlan& out) {
-    if (n && !message_cids) throw Error(IPCFP_ERR_INVALID_ARG, "null message CIDs with a nonzero count");
-    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message CIDs than IPCFP_MESSAGE_MAX");
+    message_request_check(message_cids, n, filter, false, nullptr);
     ipcfp_log_filter any;
     memset(&any, 0, sizeof any);
-    if (filter) log_filter_check(filter);
     s->use();
     AsyncBuf<uint8_t> has(td.n_receipts + 64, s->stream);
     has.zero();

@@ -126,20 +126,13 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
     }
     AsyncBuf<Matcher> d_filter;
     if (filter) {
-        if (!filter->event_signature || !filter->topic_1) throw Error(IPCFP_ERR_INVALID_ARG, "filter spec has null fields");
         Matcher m;
-        memset(&m, 0, sizeof m);
+        event_matcher(filter, "filter spec has null fields", m);
+        m.has_actor = 0;   // check_event compares the topics only
         // keccak256(signature) on the device through the batched-hash entry (K2)
-        uint8_t t0[32];
         uint64_t off0 = 0;
         uint32_t len0 = (uint32_t)strlen(filter->event_signature);
-        hash_batch(1, (const uint8_t*)filter->event_signature, len0, &off0, &len0, 1, s->device, t0);
-        memcpy(m.t0, t0, 32);
-        uint8_t t1[32];
-        memset(t1, 0, 32);
-        size_t n1 = strlen(filter->topic_1);
-        memcpy(t1, filter->topic_1, n1 < 32 ? n1 : 32);
-        memcpy(m.t1, t1, 32);
+        hash_batch(1, (const uint8_t*)filter->event_signature, len0, &off0, &len0, 1, s->device, (uint8_t*)m.t0);
         d_filter.alloc(1, st);
         IPCFP_CUDA(cudaMemcpyAsync(d_filter.p, &m, sizeof m, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaStreamSynchronize(st));   // m is a stack object
