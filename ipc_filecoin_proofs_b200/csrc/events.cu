@@ -146,10 +146,7 @@ __device__ __forceinline__ void setup_receipts_root(const SetupArgs& a) {
     uint64_t cnt;
     amt_root_begin(r, 0, bw, h, cnt);
     AmtNodeHdr hd;
-    amt_node_begin(r, 3, hd);
-    uint32_t nv = rd_array(r);
-    for (uint32_t v = 0; v < nv && !r.err; v++) parse_receipt(r);
-    amt_node_finish(r, hd, nv, h);
+    (void)amt_node_get(r, 3, h, 0, hd, [](Rd& rv, bool) { (void)parse_receipt(rv); });
     if (r.err) report_error(a.err, ST_RECEIPTS_ROOT, 0, DC_DECODE, r.err);
 }
 

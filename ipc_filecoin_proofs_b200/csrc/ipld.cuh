@@ -132,6 +132,50 @@ __device__ __forceinline__ void amt_root_begin(Rd& r, int version, uint32_t& bw,
     height = r.err ? 0 : (uint32_t)h;
     count = rd_uint(r);
 }
+// One whole node, values included, `lvl` levels above the leaves: every value goes through dec(r, keep), keep set for the value in
+// slot idx (serde decodes them all). Returns that value's rank, 0xffffffff when slot idx is empty; r.err on a decode error.
+template <class Dec>
+__device__ __forceinline__ uint32_t amt_node_get(Rd& r, uint32_t bw, uint32_t lvl, uint32_t idx, AmtNodeHdr& h, Dec&& dec) {
+    amt_node_begin(r, bw, h);
+    const uint32_t want = bm_test(h.bm, idx) ? bm_rank(h.bm, idx) : 0xffffffffu;
+    const uint32_t nv = rd_array(r);
+    for (uint32_t v = 0; v < nv && !r.err; v++) dec(r, v == want);
+    amt_node_finish(r, h, nv, lvl);
+    return want;
+}
+// Amt::load(root).get(i) (fvm_ipld_amt [UPSTREAM]) of the version-0 or version-3 AMT rooted at block root_blk, each node on the path
+// decoded whole by amt_node_get; dec keeps the value found. 1 = Some (its node in *leaf), 0 = None, <0 = -DevCode with *detail.
+// wbits (may be null): each child reached is marked there. missing (may be null): on -DC_MISSING, the CID of the child the store lacks.
+template <class Dec>
+static __device__ int amt_get(const StoreView& s, uint32_t root_blk, int version, uint64_t i, Dec&& dec, const uint8_t** leaf, uint32_t* detail,
+                              uint32_t* wbits = nullptr, const uint8_t** missing = nullptr) {
+    uint32_t len;
+    const uint8_t* p = store_block(s, root_blk, len);
+    Rd r(p, len);
+    uint32_t bw, lvl;
+    uint64_t cnt;
+    amt_root_begin(r, version, bw, lvl, cnt);
+    if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
+    const bool in_range = i < pow_sat(bw, lvl + 1);   // checked after the root node has decoded, as `load` decodes it first
+    for (;;) {
+        AmtNodeHdr h;
+        const uint32_t want = amt_node_get(r, bw, lvl, (uint32_t)((i / pow_sat(bw, lvl)) & ((1u << bw) - 1)), h, dec);
+        if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
+        if (!in_range || want == 0xffffffffu) return 0;
+        if (h.nl == 0) {
+            if (lvl != 0) return 0;
+            *leaf = p;
+            return 1;
+        }
+        const uint8_t* link = p + h.links_off + 43 * want + 5;
+        const int32_t child = store_lookup(s, link);
+        if (child < 0) { *detail = 0; if (missing) *missing = link; return -(int)DC_MISSING; }
+        if (wbits) witness_mark(s, wbits, (uint32_t)child);
+        p = store_block(s, (uint32_t)child, len);
+        r = Rd(p, len);
+        lvl--;
+    }
+}
 
 // ------------------------------------------------------------------ StampedEvent + extract_evm_log
 struct EvLog {
@@ -346,14 +390,15 @@ __device__ __forceinline__ bool event_matches(const uint8_t* p, const EvLog& ev,
 __device__ __forceinline__ uint32_t topic_offset(const EvLog& ev, uint32_t k) { return ev.case_a ? ev.toff[0] + 32 * k : ev.toff[k]; }
 
 // ------------------------------------------------------------------ Receipt = [exit_code, return_data, gas_used, events_root|null]
-__device__ __forceinline__ void parse_receipt(Rd& r) {
+// returns the offset of the events root's CID bytes, 0xffffffff for null
+__device__ __forceinline__ uint32_t parse_receipt(Rd& r) {
     rd_array_exact(r, 4);
     uint64_t ec = rd_uint(r);
     if (!r.err && ec > 0xffffffffull) rd_fail(r, CE_RANGE);
     uint32_t l;
     (void)rd_bytes(r, l);
     (void)rd_uint(r);
-    (void)rd_opt_cid(r);
+    return rd_opt_cid(r);
 }
 
 // ------------------------------------------------------------------ HAMT (fvm_ipld_hamt v3 layout)

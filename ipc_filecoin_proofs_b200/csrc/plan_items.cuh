@@ -79,7 +79,8 @@ __device__ __forceinline__ bool plan_receipt_matches(const StoreView* s_dev, uin
 
 // ---- rules 3 and 4 are paths: each one is followed through the blocks the store holds up to the first it lacks, which is returned
 // (nullptr: the path ends in the store). The present blocks are marked in `needed` (rank bitmap).
-// Amt::get(i) of the receipts AMT with pass 2's bounds (receipts_get).
+// Amt::get(i) of the receipts AMT, pass 2's receipts_get. Only a child link can be missing: the root node's decode and the range check
+// after it never name a block.
 __device__ __forceinline__ const uint8_t* plan_receipt_path(const StoreView& s, const uint8_t* receipts_root, uint64_t i, uint32_t* needed) {
     const int32_t rb = store_lookup(s, receipts_root);
     if (rb < 0) return nullptr;   // the root itself is a PK_BLOCK item

@@ -13,30 +13,10 @@ namespace ipcfp {
 // storage_proof_one fails on the same blocks: DC_MISSING (rec.missing names the block), DC_DECODE, DC_ACTOR_NOT_FOUND (no actor ID 1).
 static __device__ bool resolve_init(const StoreView& s, Recorder& rec, const uint8_t* state_root, const uint8_t*& address_map, Fail& f) {
     address_map = nullptr;
-    const int32_t sb = rec_get(s, rec, state_root);
-    if (sb < 0) SFAIL(DC_MISSING, 2);
-    uint32_t sl;
-    const uint8_t* sp = store_block(s, (uint32_t)sb, sl);
-    Rd sr(sp, sl);
-    rd_array_exact(sr, 3);
-    const uint64_t ver = rd_uint(sr);
-    if (!sr.err && ver > 5) rd_fail(sr, CE_RANGE);
-    const uint32_t actors_off = rd_cid(sr);
-    (void)rd_cid(sr);
-    rd_end(sr);
-    if (sr.err) SFAIL(DC_DECODE, sr.err);
-    const uint8_t key[2] = {0x00, 0x01};   // Address::new_id(1).to_bytes()
-    bool found;
-    ValueRef vr;
-    if (!hamt_get(s, rec, sp + actors_off, 5, HV_ACTOR_STATE, key, 2, found, vr, f)) return false;
-    if (!found) SFAIL(DC_ACTOR_NOT_FOUND, 0);
-    uint32_t abl;
-    const uint8_t* abp = store_block(s, vr.blk, abl);
-    Rd ar(abp, abl);
-    ar.pos = vr.off;
-    uint32_t state_off;
-    parse_actor_state(ar, state_off);
-    const int32_t ib = rec_get(s, rec, abp + state_off);
+    uint8_t key[11];
+    const uint8_t* state_cid;
+    if (!actor_state(s, rec, state_root, key, id_address_key(1, key), state_cid, f)) return false;
+    const int32_t ib = rec_get(s, rec, state_cid);
     if (ib < 0) SFAIL(DC_MISSING, 3);
     uint32_t il;
     const uint8_t* ip = store_block(s, (uint32_t)ib, il);

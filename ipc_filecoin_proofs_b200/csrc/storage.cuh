@@ -206,24 +206,25 @@ do_hamt:
     return true;
 }
 
-// HeaderLite (common/decode.rs:100-124): returns offset of parent_state_root CID bytes
-static __device__ uint32_t header_parent_state_root(Rd& r) {
+// HeaderLite (common/decode.rs:100-124): the fields the generators and verifiers read
+struct HeaderFields { uint32_t parents_off, n_parents, psr_off, receipts_off, messages_off; int64_t height; };
+__device__ __forceinline__ void header_fields(Rd& r, HeaderFields& h) {
     rd_array_exact(r, 16);
     for (int i = 0; i < 5; i++) rd_skip_any(r);
-    uint32_t np = rd_array(r);
-    for (uint32_t i = 0; i < np && !r.err; i++) (void)rd_cid(r);
+    h.n_parents = rd_array(r);
+    h.parents_off = r.pos;
+    for (uint32_t i = 0; i < h.n_parents && !r.err; i++) (void)rd_cid(r);
     rd_skip_any(r);
-    (void)rd_int(r);
-    uint32_t psr = rd_cid(r);
-    (void)rd_cid(r);
-    (void)rd_cid(r);
+    h.height = rd_int(r);
+    h.psr_off = rd_cid(r);
+    h.receipts_off = rd_cid(r);
+    h.messages_off = rd_cid(r);
     rd_skip_any(r);
     (void)rd_uint(r);
     rd_skip_any(r);
     (void)rd_uint(r);
     rd_skip_any(r);
     rd_end(r);
-    return psr;
 }
 // EvmStateV6 / V5 (common/decode.rs:48-97): offset of contract_state CID bytes
 static __device__ bool try_evm_state(const uint8_t* p, uint32_t len, int fields, uint32_t& cs_off) {
@@ -239,6 +240,55 @@ static __device__ bool try_evm_state(const uint8_t* p, uint32_t len, int fields,
     if (rd_peek_null(r)) r.pos++; else rd_skip_any(r);
     rd_end(r);
     return !r.err;
+}
+
+// Address::new_id(id).to_bytes(), the actors-HAMT key: protocol 0, then the ID as a varint; returns its length
+__device__ __forceinline__ uint32_t id_address_key(uint64_t id, uint8_t key[11]) {
+    uint32_t kl = 0;
+    key[kl++] = 0;
+    while (id >= 0x80) { key[kl++] = (uint8_t)(id | 0x80); id >>= 7; }
+    key[kl++] = (uint8_t)id;
+    return kl;
+}
+// get_actor_state (common/decode.rs:17-42): StateRoot [version ≤ 5, actors, info] → actors HAMT (width 5) → the ActorState under key;
+// state_cid points at its state CID. DC_ACTOR_NOT_FOUND when the actor is absent.
+__device__ __forceinline__ bool actor_state(const StoreView& s, Recorder& rec, const uint8_t* state_root, const uint8_t* key, uint32_t keylen,
+                                            const uint8_t*& state_cid, Fail& f) {
+    const int32_t sb = rec_get(s, rec, state_root);
+    if (sb < 0) SFAIL(DC_MISSING, 2);
+    uint32_t sl;
+    const uint8_t* sp = store_block(s, (uint32_t)sb, sl);
+    Rd sr(sp, sl);
+    rd_array_exact(sr, 3);
+    const uint64_t ver = rd_uint(sr);
+    if (!sr.err && ver > 5) rd_fail(sr, CE_RANGE);
+    const uint32_t actors_off = rd_cid(sr);
+    (void)rd_cid(sr);
+    rd_end(sr);
+    if (sr.err) SFAIL(DC_DECODE, sr.err);
+    bool found;
+    ValueRef vr;
+    if (!hamt_get(s, rec, sp + actors_off, 5, HV_ACTOR_STATE, key, keylen, found, vr, f)) return false;
+    if (!found) SFAIL(DC_ACTOR_NOT_FOUND, 0);
+    uint32_t abl;
+    const uint8_t* abp = store_block(s, vr.blk, abl);
+    Rd ar(abp, abl);
+    ar.pos = vr.off;
+    uint32_t state_off;
+    parse_actor_state(ar, state_off);
+    state_cid = abp + state_off;
+    return true;
+}
+// parse_evm_state (common/decode.rs:48-97): the EVM state at state_cid, EvmStateV6 else V5; root points at its contract-state CID
+__device__ __forceinline__ bool contract_storage_root(const StoreView& s, Recorder& rec, const uint8_t* state_cid, const uint8_t*& root, Fail& f) {
+    const int32_t eb = rec_get(s, rec, state_cid);
+    if (eb < 0) SFAIL(DC_MISSING, 3);
+    uint32_t el;
+    const uint8_t* ep = store_block(s, (uint32_t)eb, el);
+    uint32_t cs_off;
+    if (!try_evm_state(ep, el, 6, cs_off) && !try_evm_state(ep, el, 5, cs_off)) SFAIL(DC_DECODE, CE_FIELD);
+    root = ep + cs_off;
+    return true;
 }
 
 struct StorageArgs {
@@ -262,48 +312,17 @@ static __device__ bool storage_proof_one(const StorageArgs& a, uint64_t t, Recor
     uint32_t hl;
     const uint8_t* hp = store_block(s, (uint32_t)hb, hl);
     Rd hr(hp, hl);
-    uint32_t psr_off = header_parent_state_root(hr);
+    HeaderFields hf;
+    header_fields(hr, hf);
     if (hr.err) SFAIL(DC_DECODE, hr.err);
-    const uint8_t* psr = hp + psr_off;
+    const uint8_t* psr = hp + hf.psr_off;
     if (!cid38_equal(psr, a.state_root_json)) SFAIL(DC_STATE_MISMATCH, 0);
     rec.note((uint32_t)hb);  // collector.add_cid(child_cid) (:41)
-    // load_actor_and_storage_root (:106-134) — get_actor_state (common/decode.rs:17-42)
-    int32_t sb = rec_get(s, rec, psr);  // add_cid(parent_state_root) + state_recorder.get
-    if (sb < 0) SFAIL(DC_MISSING, 2);
-    uint32_t sl;
-    const uint8_t* sp = store_block(s, (uint32_t)sb, sl);
-    Rd sr(sp, sl);
-    rd_array_exact(sr, 3);
-    uint64_t ver = rd_uint(sr);
-    if (!sr.err && ver > 5) rd_fail(sr, CE_RANGE);
-    uint32_t actors_off = rd_cid(sr);
-    (void)rd_cid(sr);
-    rd_end(sr);
-    if (sr.err) SFAIL(DC_DECODE, sr.err);
+    // load_actor_and_storage_root (:106-134): add_cid(parent_state_root) + state_recorder.get, get_actor_state, parse_evm_state
     uint8_t key[11];
-    uint32_t kl = 0;
-    key[kl++] = 0;
-    uint64_t id = a.specs[t].actor_id;
-    while (id >= 0x80) { key[kl++] = (uint8_t)(id | 0x80); id >>= 7; }
-    key[kl++] = (uint8_t)id;
-    bool found;
-    ValueRef vr;
-    if (!hamt_get(s, rec, sp + actors_off, 5, HV_ACTOR_STATE, key, kl, found, vr, f)) return false;
-    if (!found) SFAIL(DC_ACTOR_NOT_FOUND, 0);
-    uint32_t abl;
-    const uint8_t* abp = store_block(s, vr.blk, abl);
-    Rd ar(abp, abl);
-    ar.pos = vr.off;
-    uint32_t state_off;
-    parse_actor_state(ar, state_off);
-    const uint8_t* state_cid = abp + state_off;
-    int32_t eb = rec_get(s, rec, state_cid);
-    if (eb < 0) SFAIL(DC_MISSING, 3);
-    uint32_t el;
-    const uint8_t* ep = store_block(s, (uint32_t)eb, el);
-    uint32_t cs_off;
-    if (!try_evm_state(ep, el, 6, cs_off) && !try_evm_state(ep, el, 5, cs_off)) SFAIL(DC_DECODE, CE_FIELD);
-    const uint8_t* storage_root = ep + cs_off;
+    const uint32_t kl = id_address_key(a.specs[t].actor_id, key);
+    const uint8_t *state_cid, *storage_root;
+    if (!actor_state(s, rec, psr, key, kl, state_cid, f) || !contract_storage_root(s, rec, state_cid, storage_root, f)) return false;
     // read_storage_value (:137-155)
     SlotValue sv;
     if (!read_storage_slot(s, rec, storage_root, a.specs[t].slot, sv, f)) return false;

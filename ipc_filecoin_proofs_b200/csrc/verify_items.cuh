@@ -12,27 +12,6 @@ namespace ipcfp {
 
 #define ST_VERIFY 9u
 
-// HeaderLite (common/decode.rs:100-118) fields the verifier needs
-struct HeaderFields { uint32_t parents_off, n_parents, psr_off, receipts_off, messages_off; int64_t height; };
-__device__ __forceinline__ void header_fields(Rd& r, HeaderFields& h) {
-    rd_array_exact(r, 16);
-    for (int i = 0; i < 5; i++) rd_skip_any(r);
-    h.n_parents = rd_array(r);
-    h.parents_off = r.pos;
-    for (uint32_t i = 0; i < h.n_parents && !r.err; i++) (void)rd_cid(r);
-    rd_skip_any(r);
-    h.height = rd_int(r);
-    h.psr_off = rd_cid(r);
-    h.receipts_off = rd_cid(r);
-    h.messages_off = rd_cid(r);
-    rd_skip_any(r);
-    (void)rd_uint(r);
-    rd_skip_any(r);
-    (void)rd_uint(r);
-    rd_skip_any(r);
-    rd_end(r);
-}
-
 struct VerifyTipsetArgs {
     StoreView store;
     const uint8_t* parent_cids;   // device, n_parents*38 (from the proof / the caller's tipset)
@@ -112,92 +91,6 @@ __device__ __forceinline__ void verify_txmeta_item(const StoreView& s, const uin
     if (!ok || !digest_eq(d, c)) report_error(err, ST_VERIFY, 0, DC_CID_MISMATCH, (uint32_t)k);
 }
 
-// Amtv0<Receipt>.get(i) WITHOUT recording; returns 1 Some (events root offset in *ev_off, 0xffffffff = None), 0 None, <0 -DevCode
-static __device__ int receipts_get_value(const StoreView& s, uint32_t root_blk, uint64_t i, const uint8_t** blk_out, uint32_t* ev_off, uint32_t* detail) {
-    uint32_t len;
-    const uint8_t* p = store_block(s, root_blk, len);
-    Rd r(p, len);
-    uint32_t bw, height;
-    uint64_t cnt;
-    amt_root_begin(r, 0, bw, height, cnt);
-    if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
-    bool in_range = i < pow_sat(3, height + 1);
-    uint32_t lvl = height;
-    // (the root node is decoded by `load` whatever the index)
-    for (;;) {
-        AmtNodeHdr h;
-        amt_node_begin(r, 3, h);
-        uint32_t nv = rd_array(r);
-        uint32_t idx = (uint32_t)((i / pow_sat(3, lvl)) & 7);
-        uint32_t want = bm_test(h.bm, idx) ? bm_rank(h.bm, idx) : 0xffffffffu;
-        uint32_t found_off = 0xfffffffeu;
-        for (uint32_t v = 0; v < nv && !r.err; v++) {
-            rd_array_exact(r, 4);
-            uint64_t ec = rd_uint(r);
-            if (!r.err && ec > 0xffffffffull) rd_fail(r, CE_RANGE);
-            uint32_t l;
-            (void)rd_bytes(r, l);
-            (void)rd_uint(r);
-            uint32_t eo = rd_opt_cid(r);
-            if (v == want) found_off = eo;
-        }
-        amt_node_finish(r, h, nv, lvl);
-        if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
-        if (!in_range) return 0;
-        if (h.nl == 0) {
-            if (lvl != 0 || want == 0xffffffffu) return 0;
-            *blk_out = p; *ev_off = found_off;
-            return 1;
-        }
-        if (want == 0xffffffffu) return 0;
-        int32_t child = store_lookup(s, p + h.links_off + 43 * want + 5);
-        if (child < 0) { *detail = 0; return -(int)DC_MISSING; }
-        p = store_block(s, (uint32_t)child, len);
-        r = Rd(p, len);
-        lvl--;
-    }
-}
-// Amt<StampedEvent>(v3).get(j): 1 Some (event in ev, its block in *blk_out), 0 None, <0 -DevCode
-static __device__ int events_get_value(const StoreView& s, uint32_t root_blk, uint64_t j, const uint8_t** blk_out, EvLog& ev, uint32_t* detail) {
-    uint32_t len;
-    const uint8_t* p = store_block(s, root_blk, len);
-    Rd r(p, len);
-    uint32_t bw, height;
-    uint64_t cnt;
-    amt_root_begin(r, 3, bw, height, cnt);
-    if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
-    const bool in_range = j < pow_sat(bw, height + 1);
-    uint32_t lvl = height;
-    for (;;) {
-        AmtNodeHdr h;
-        amt_node_begin(r, bw, h);
-        uint32_t nv = rd_array(r);
-        const uint32_t width_mask = (1u << bw) - 1u;
-        uint32_t idx = (uint32_t)((j / pow_sat(bw, lvl)) & width_mask);
-        uint32_t want = bm_test(h.bm, idx) ? bm_rank(h.bm, idx) : 0xffffffffu;
-        bool got = false;
-        for (uint32_t v = 0; v < nv && !r.err; v++) {
-            EvLog e;
-            decode_stamped_event(r, e);
-            if (v == want && !r.err) { ev = e; got = true; }
-        }
-        amt_node_finish(r, h, nv, lvl);
-        if (r.err) { *detail = r.err; return -(int)DC_DECODE; }
-        if (!in_range) return 0;
-        if (h.nl == 0) {
-            if (lvl != 0 || !got) return 0;
-            *blk_out = p;
-            return 1;
-        }
-        if (want == 0xffffffffu) return 0;
-        int32_t child = store_lookup(s, p + h.links_off + 43 * want + 5);
-        if (child < 0) { *detail = 0; return -(int)DC_MISSING; }
-        p = store_block(s, (uint32_t)child, len);
-        r = Rd(p, len);
-        lvl--;
-    }
-}
-
 // check_event: matches_log of a spec (events/generator.rs:38-40), without its actor filter; nullptr: no predicate
 __device__ __forceinline__ bool verify_check(const Matcher* f, const uint8_t* eblk, const EvLog& ev) {
     if (f) {
@@ -245,14 +138,16 @@ __device__ __forceinline__ void verify_event_item(const VerifyEventArgsT<F>& a, 
     if (*a.receipts_root_blk == 0xffffffffu) { report_error(a.err, ST_VERIFY, t, DC_MISSING, 4); return; }
     uint32_t detail = 0, ev_off = 0;
     const uint8_t* rblk = nullptr;
-    int got = receipts_get_value(s, *a.receipts_root_blk, p.exec_index, &rblk, &ev_off, &detail);
+    int got = amt_get(s, *a.receipts_root_blk, 0, p.exec_index, [&](Rd& r, bool keep) { const uint32_t o = parse_receipt(r); if (keep) ev_off = o; },
+                      &rblk, &detail);
     if (got < 0) { report_error(a.err, ST_VERIFY, t, (uint32_t)(-got), detail); return; }
     if (got == 0 || ev_off == 0xffffffffu) return;
     int32_t eb = store_lookup(s, rblk + ev_off);
     if (eb < 0) { report_error(a.err, ST_VERIFY, t, DC_MISSING, 5); return; }
     EvLog ev;
     const uint8_t* eblk = nullptr;
-    got = events_get_value(s, (uint32_t)eb, p.event_index, &eblk, ev, &detail);
+    got = amt_get(s, (uint32_t)eb, 3, p.event_index, [&](Rd& r, bool keep) { EvLog e; decode_stamped_event(r, e); if (keep && !r.err) ev = e; },
+                  &eblk, &detail);
     if (got < 0) { report_error(a.err, ST_VERIFY, t, (uint32_t)(-got), detail); return; }
     if (got == 0) return;
     // verify_event_data_matches (:257-290)
@@ -289,50 +184,20 @@ __device__ __forceinline__ void verify_storage_item(const VerifyStorageArgs& a, 
     uint32_t hl;
     const uint8_t* hp = store_block(s, (uint32_t)hb, hl);
     Rd hr(hp, hl);
-    uint32_t psr_off = header_parent_state_root(hr);
+    HeaderFields hf;
+    header_fields(hr, hf);
     if (hr.err) { report_error(a.err, ST_VERIFY, t, DC_DECODE, hr.err); return; }
-    const uint8_t* psr = hp + psr_off;
+    const uint8_t* psr = hp + hf.psr_off;
     if (!cid38_equal(psr, a.state_root_json)) return;
     // verify_actor_state (:117-132): get_actor_state (common/decode.rs:17-42)
-    int32_t sb = store_lookup(s, psr);
-    if (sb < 0) { report_error(a.err, ST_VERIFY, t, DC_MISSING, 2); return; }
-    uint32_t sl;
-    const uint8_t* sp = store_block(s, (uint32_t)sb, sl);
-    Rd sr(sp, sl);
-    rd_array_exact(sr, 3);
-    uint64_t ver = rd_uint(sr);
-    if (!sr.err && ver > 5) rd_fail(sr, CE_RANGE);
-    uint32_t actors_off = rd_cid(sr);
-    (void)rd_cid(sr);
-    rd_end(sr);
-    if (sr.err) { report_error(a.err, ST_VERIFY, t, DC_DECODE, sr.err); return; }
-    uint8_t key[11];
-    uint32_t kl = 0;
-    key[kl++] = 0;
-    uint64_t id = p.actor_id;
-    while (id >= 0x80) { key[kl++] = (uint8_t)(id | 0x80); id >>= 7; }
-    key[kl++] = (uint8_t)id;
-    bool found;
-    ValueRef vr;
     Fail f{0, 0};
-    if (!hamt_get(s, rec, sp + actors_off, 5, HV_ACTOR_STATE, key, kl, found, vr, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
-    if (!found) { report_error(a.err, ST_VERIFY, t, DC_ACTOR_NOT_FOUND, 0); return; }
-    uint32_t abl;
-    const uint8_t* abp = store_block(s, vr.blk, abl);
-    Rd ar(abp, abl);
-    ar.pos = vr.off;
-    uint32_t state_off;
-    parse_actor_state(ar, state_off);
-    const uint8_t* state_cid = abp + state_off;
+    uint8_t key[11];
+    const uint8_t* state_cid;
+    if (!actor_state(s, rec, psr, key, id_address_key(p.actor_id, key), state_cid, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
     if (!cid38_equal(state_cid, p.actor_state_cid)) return;
     // verify_storage_root (:135-150)
-    int32_t eb = store_lookup(s, state_cid);
-    if (eb < 0) { report_error(a.err, ST_VERIFY, t, DC_MISSING, 3); return; }
-    uint32_t el;
-    const uint8_t* ep = store_block(s, (uint32_t)eb, el);
-    uint32_t cs_off;
-    if (!try_evm_state(ep, el, 6, cs_off) && !try_evm_state(ep, el, 5, cs_off)) { report_error(a.err, ST_VERIFY, t, DC_DECODE, CE_FIELD); return; }
-    const uint8_t* storage_root = ep + cs_off;
+    const uint8_t* storage_root;
+    if (!contract_storage_root(s, rec, state_cid, storage_root, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
     if (!cid38_equal(storage_root, p.storage_root)) return;
     // verify_storage_value (:153-170)
     SlotValue sv;
