@@ -440,7 +440,9 @@ void ipcfp_parsed_blocks_free(ipcfp_parsed_blocks* p);
  * and all texts together under 4 GiB. Any other input (whitespace, other member orders, escapes, error responses, repeated or missing ids,
  * and every invalid text) goes through ipcfp_blocks_from_rpc_json instead, with the same result.
  * Such a store has no caller blob for by-reference offsets to point into: every generate call on it with IPCFP_WITNESS_BY_REFERENCE
- * returns IPCFP_ERR_UNSUPPORTED (IPCFP_RESULT_JSON reads the store itself and works). info (may be NULL): which path ran and its times. */
+ * returns IPCFP_ERR_UNSUPPORTED (IPCFP_RESULT_JSON reads the store itself and works). info (may be NULL): which path ran and its times.
+ * ipcfp_store_create_car fills the same struct, its three fields meaning the same for the CAR's bytes: parsed on the device or by the
+ * host parser (ipcfp_blocks_from_car), wall time until the blocks were in the arena, the device parse's kernel time. */
 typedef struct ipcfp_store_json_info {
     uint32_t parsed_on_device;   /* 1: the device parsed the texts; 0: ipcfp_blocks_from_rpc_json did                                 */
     float ms_parse;              /* wall time until the blocks were in the store's arena (copy of the texts included), before the index  */
@@ -449,6 +451,37 @@ typedef struct ipcfp_store_json_info {
 } ipcfp_store_json_info;
 ipcfp_status ipcfp_store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts,
                                          int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info);
+
+/* ------------------------------------------------------------------------------------------
+ * The block store straight from a CARv1 archive (https://ipld.io/specs/transport/car/carv1/): what Filecoin.ChainExport, `lotus chain
+ * export` and the published snapshots (once decompressed) hold. Varints are unsigned LEB128 below 2^63 in minimal encoding. The rules,
+ * checked in file order (the first failure wins):
+ *   1. the header: a varint H >= 1, then H bytes inside the buffer that are exactly one DAG-CBOR map (minimal heads, definite lengths)
+ *      with the keys "roots" (an array of CIDs: tag 42 over a byte string whose first byte is 0x00; checked for form only, not returned)
+ *      and "version" (an unsigned integer), in either order, each once. Its entries are read in order: a version other than 1 →
+ *      IPCFP_ERR_UNSUPPORTED (a CARv2 starts with the header {"version": 2}); anything else malformed, a key missing and bytes left over
+ *      inside H included → IPCFP_ERR_DECODE; both with index UINT64_MAX;
+ *   2. sections from the header's end to len, k = 0, 1, …: a varint L; L = 0, or L bytes not all inside the buffer (a truncated varint
+ *      included) → IPCFP_ERR_DECODE at k; the section starts with a CID that must decode under the CID spec (else IPCFP_ERR_DECODE at k)
+ *      and be the store's form, CIDv1 with a one-byte codec, a three-byte multihash code and a 32-byte digest: 38 bytes (else
+ *      IPCFP_ERR_UNSUPPORTED at k: CIDv0, sha2-256, identity, a two-byte codec); the block is the rest of the section, possibly empty;
+ *      a block of 2^32 bytes or more → IPCFP_ERR_UNSUPPORTED at k.
+ * ipcfp_blocks_from_car (host C++, no device): the sections in file order, block k = section k. blocks.cids (n*38), and blocks.offsets /
+ * blocks.lengths index `car` itself; blocks.blob is NULL and blocks.blob_size = len (the convention of IPCFP_WITNESS_BY_REFERENCE).
+ * car NULL or out NULL → IPCFP_ERR_INVALID_ARG. Released with ipcfp_parsed_blocks_free.
+ * ------------------------------------------------------------------------------------------ */
+ipcfp_status ipcfp_blocks_from_car(const uint8_t* car, uint64_t len, ipcfp_parsed_blocks** out);
+/* The same bytes straight to a new store. In every case the store, status and index are those of ipcfp_blocks_from_car followed by
+ * ipcfp_store_create(blocks.cids, blocks.offsets, blocks.lengths, car, len, n, device, flags): the arena is the CAR, index k is section
+ * k (ipcfp_store_first_bad_block included: IPCFP_ERR_CID_MISMATCH at the section index under IPCFP_STORE_VERIFY_CIDS, *out then set),
+ * the rules of ipcfp_store_create apply (duplicate CIDs stay as duplicate entries, the lowest index wins; fewer than 2^31 blocks), and
+ * IPCFP_WITNESS_BY_REFERENCE offsets index `car`. The CAR is copied to the device once (pinned memory from ipcfp_host_alloc copies at
+ * PCIe rate; pageable memory works too) and its sections are found there, whatever its blocks hold. A CAR the device path does not
+ * accept (every invalid CAR) goes through ipcfp_blocks_from_car, over the same device copy, for its status and index; so does any CAR
+ * when the device has no room for the parse's scratch (about 0.4 bytes per CAR byte, plus 48 bytes per candidate section). info (may be NULL) is the ipcfp_store_json_info of ipcfp_store_create_rpc_json, with its
+ * fields' meanings: parsed_on_device (1: the device found the sections; 0: ipcfp_blocks_from_car did), ms_parse (wall time until the
+ * blocks and their arrays were on the device, the copy included, before the index), ms_kernels (device parse only: its kernels' time). */
+ipcfp_status ipcfp_store_create_car(const uint8_t* car, uint64_t len, int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info);
 
 /* read_storage_slot (src/proofs/storage/decode.rs:36-97), batched over k slot keys against one
  * contract_state root, with a RecordingBlockStore-equivalent witness. */

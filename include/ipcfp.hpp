@@ -342,6 +342,13 @@ class GpuBlockstore {
         check(ipcfp_store_create(cids, offsets, lengths, blob, blob_size, n_blocks, device, verify ? IPCFP_STORE_VERIFY_CIDS : 0u, &h), "ipcfp_store_create");
         return GpuBlockstore(h, device);
     }
+    // a CARv1 archive held in memory (ipcfp_store_create_car): block k is section k; by-reference offsets index `car`, which the caller
+    // keeps for as long as it reads such witnesses. Pass verify for bytes from an untrusted source.
+    static GpuBlockstore from_car(const uint8_t* car, uint64_t len, int device = 0, bool verify = true, ipcfp_store_json_info* info = nullptr) {
+        ipcfp_store* h = nullptr;
+        check(ipcfp_store_create_car(car, len, device, verify ? IPCFP_STORE_VERIFY_CIDS : 0u, &h, info), "ipcfp_store_create_car");
+        return GpuBlockstore(h, device);
+    }
     // load_witness_store (events/verifier.rs:78-89, storage/verifier.rs:66-77) — with the CID check `put_keyed` leaves out
     static GpuBlockstore from_witness(const std::vector<ProofBlock>& blocks, int device = 0) {
         std::vector<std::pair<Cid, std::vector<uint8_t>>> kv;

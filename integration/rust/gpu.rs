@@ -126,6 +126,28 @@ impl GpuBlockstore {
         }
         Ok(Self { h, kept_blob: if keep { Some(blob) } else { None } })
     }
+    /// A CARv1 archive (`lotus chain export`, `Filecoin.ChainExport`, a decompressed snapshot) as the store, its sections found on the
+    /// GPU (`ipcfp_store_create_car`): block k is section k, and the store keeps `car`, which by-reference witnesses index.
+    pub fn from_car(car: Vec<u8>, device: i32, verify: bool) -> Result<Self> {
+        let mut h = std::ptr::null_mut();
+        let st = unsafe {
+            sys::ipcfp_store_create_car(
+                car.as_ptr(),
+                car.len() as u64,
+                device,
+                if verify { sys::IPCFP_STORE_VERIFY_CIDS } else { 0 },
+                &mut h,
+                std::ptr::null_mut(),
+            )
+        };
+        if st != sys::IPCFP_OK {
+            if !h.is_null() {
+                unsafe { sys::ipcfp_store_destroy(h) };
+            }
+            check(st)?;
+        }
+        Ok(Self { h, kept_blob: Some(car) })
+    }
     /// The witness of a bundle as a store of its own (every block CID-checked): what the verifiers replay against.
     pub fn from_witness(blocks: &[ProofBlock], device: i32) -> Result<Self> {
         Self::ingest(blocks.iter().map(|b| (&b.cid, b.data.as_slice())), device, true)

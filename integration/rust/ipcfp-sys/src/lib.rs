@@ -157,6 +157,9 @@ extern "C" {
     pub fn ipcfp_parsed_blocks_free(p: *mut ipcfp_parsed_blocks);
     pub fn ipcfp_store_create_rpc_json(cids: *const u8, n_blocks: u64, texts: *const *const c_char, text_lens: *const u64, n_texts: u64,
                                        device: c_int, flags: u32, out: *mut *mut ipcfp_store, info: *mut ipcfp_store_json_info) -> ipcfp_status;
+    pub fn ipcfp_blocks_from_car(car: *const u8, len: u64, out: *mut *mut ipcfp_parsed_blocks) -> ipcfp_status;
+    pub fn ipcfp_store_create_car(car: *const u8, len: u64, device: c_int, flags: u32, out: *mut *mut ipcfp_store,
+                                  info: *mut ipcfp_store_json_info) -> ipcfp_status;
     pub fn ipcfp_generate_event_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, spec: *const ipcfp_event_spec, flags: u32,
                                                out: *mut *mut ipcfp_event_result) -> ipcfp_status;
     pub fn ipcfp_generate_log_proof_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, filter: *const ipcfp_log_filter, flags: u32,

@@ -80,6 +80,8 @@ SIGNATURES = {
     "ipcfp_blocks_from_rpc_json": (_st, [_vp, _u64, _P(C.c_char_p), _P(_u64), _u64, _PP(A.ParsedBlocksC)]),
     "ipcfp_parsed_blocks_free": (None, [_P(A.ParsedBlocksC)]),
     "ipcfp_store_create_rpc_json": (_st, [_vp, _u64, _P(C.c_char_p), _P(_u64), _u64, _int, _u32, _P(_vp), _P(A.StoreJsonInfoC)]),
+    "ipcfp_blocks_from_car": (_st, [_vp, _u64, _PP(A.ParsedBlocksC)]),
+    "ipcfp_store_create_car": (_st, [_vp, _u64, _int, _u32, _P(_vp), _P(A.StoreJsonInfoC)]),
     "ipcfp_read_storage_slots": (_st, [_vp, _vp, _vp, _u64, _PP(A.SlotResultC)]),
     "ipcfp_slot_result_free": (None, [_P(A.SlotResultC)]),
     "ipcfp_generate_storage_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _PP(A.StorageResultC)]),
@@ -333,6 +335,22 @@ class BlockStore:
         self._adopt(st, h)
         return self
 
+    @classmethod
+    def from_car(cls, car, device=0, verify_cids=False):
+        """ipcfp_store_create_car: the store straight from a CARv1 archive (bytes, bytearray, mmap or a uint8 numpy array); block k is
+        section k and by-reference offsets index `car`. The sections are found on the device; `.car_info` tells which path ran and its
+        times. Failures raise IpcfpError (status, section index) with `.first_bad_block` as BlockStore() sets it."""
+        buf = _car_view(car)
+        self = cls.__new__(cls)
+        self.device, self._h = device, None
+        h, info = C.c_void_p(), A.StoreJsonInfoC()
+        st = lib().ipcfp_store_create_car(buf.ctypes.data, buf.size, device, A.STORE_VERIFY_CIDS if verify_cids else 0, C.byref(h),
+                                          C.byref(info))
+        self.car_info = A.StoreJsonInfoPy(bool(info.parsed_on_device), float(info.ms_parse), float(info.ms_kernels))
+        self._adopt(st, h)
+        self.n_blocks = lib().ipcfp_store_n_blocks(h)
+        return self
+
     def get(self, cid):
         cid = _u8(cid)
         ln = C.c_uint32()
@@ -551,6 +569,27 @@ def blocks_from_rpc_json(cids, texts):
     arr, lens, keep = _text_array(texts)
     return _result("ipcfp_blocks_from_rpc_json", A.ParsedBlocksC, lambda c: A.witness_from_c(c.blocks), "ipcfp_parsed_blocks_free",
                    cids.ctypes.data if cids.size else None, len(cids), arr, lens, len(keep))
+
+
+def _car_view(car):
+    """The bytes of a CAR (bytes, bytearray, mmap, or a numpy array of uint8) as a flat uint8 array over the same memory where possible."""
+    if isinstance(car, np.ndarray):
+        if car.dtype != np.uint8:
+            raise TypeError("a CAR array must be uint8")
+        buf = np.ascontiguousarray(car).reshape(-1)
+    else:
+        buf = np.frombuffer(car, dtype=np.uint8)
+    return buf if buf.size else np.zeros(1, np.uint8)[:0]
+
+
+def blocks_from_car(car):
+    """ipcfp_blocks_from_car (host parser, no device): the sections of a CARv1 in file order, as an A.WitnessPy whose offsets index the
+    CAR itself (its blob is a view of `car`). Failures raise IpcfpError with the status and the section index include/ipcfp.h gives."""
+    buf = _car_view(car)
+    w = _result("ipcfp_blocks_from_car", A.ParsedBlocksC, lambda c: A.witness_from_c(c.blocks), "ipcfp_parsed_blocks_free",
+                buf.ctypes.data, buf.size)
+    w.blob = buf
+    return w
 
 
 def fetch_plan_to_rpc_json(cids, first_id=0):

@@ -221,7 +221,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* k_rb_* | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* k_rb_* k_car_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }
@@ -248,6 +248,14 @@ ipcfp_status ipcfp_store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks,
     return make_store(out, [&] {
         ipcfp_store_json_info si;
         Store* s = store_create_rpc_json(cids, n_blocks, texts, text_lens, n_texts, device, flags, si);
+        if (info) *info = si;
+        return s;
+    });
+}
+ipcfp_status ipcfp_store_create_car(const uint8_t* car, uint64_t len, int device, uint32_t flags, ipcfp_store** out, ipcfp_store_json_info* info) {
+    return make_store(out, [&] {
+        ipcfp_store_json_info si;
+        Store* s = store_create_car(car, len, device, flags, si);
         if (info) *info = si;
         return s;
     });

@@ -84,6 +84,7 @@ constexpr uint32_t HW_UNION_PARTS_WORDS = 2 * MAX_WORLD;                      //
 constexpr uint32_t HW_JP_META_WORDS = 17;                                     // json_parse.cu: JpMeta
 constexpr uint32_t HW_RJ_META_WORDS = 2;                                      // rpc_json.cu: RjMeta
 constexpr uint32_t HW_RB_META_WORDS = 4;                                      // rpc_blocks.cu: RbMeta
+constexpr uint32_t HW_CAR_META_WORDS = 2;                                     // car.cu: CarMeta
 enum HostWord : uint32_t {
     HW_PROLOGUE = DW_COUNT,
     HW_JSON_TOTALS = HW_PROLOGUE + HW_PROLOGUE_WORDS,
@@ -94,7 +95,8 @@ enum HostWord : uint32_t {
     HW_JP_META = HW_UNION_PARTS + HW_UNION_PARTS_WORDS,
     HW_RJ_META = HW_JP_META + HW_JP_META_WORDS,
     HW_RB_META = HW_RJ_META + HW_RJ_META_WORDS,
-    HW_END = HW_RB_META + HW_RB_META_WORDS
+    HW_CAR_META = HW_RB_META + HW_RB_META_WORDS,
+    HW_END = HW_CAR_META + HW_CAR_META_WORDS
 };
 constexpr uint32_t HW_COUNT = 1024;
 static_assert(DW_JSON_TOTAL2 < DW_COUNT, "a mirrored slot never reaches a host-only region (they start at DW_COUNT)");
@@ -135,6 +137,7 @@ struct Store {
     std::vector<uint32_t> class_rank;                  // rank of each class in `Cid` Ord
     uint64_t first_bad = UINT64_MAX;
     bool caller_blob = true;   // false: made from JSON-RPC texts (rpc_blocks.cu), no caller blob for IPCFP_WITNESS_BY_REFERENCE offsets
+                               // (a store made from a CAR keeps true: its blob is the caller's CAR)
     std::shared_ptr<PinnedPool> pool;
     // small persistent scratch
     DevBuf<unsigned long long> dev_words;  // DW_COUNT slots (DevWord)
@@ -180,11 +183,16 @@ void check_device(int device);
 //   store_shell → store_alloc_blocks → (fill cids_dev, offsets, lengths, arena + 16) → store_index → store_verify_all
 Store* store_shell(int device);   // stream, events, counters; no block yet
 void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev);
+// … its two halves, for a caller that fills the arena before it knows n (car.cu): the arena, then the per-block arrays and the index
+void store_alloc_arena(Store* s, uint64_t blob_size);
+void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev);
 void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws);
 void store_verify_all(Store* s);
 // rpc_blocks.cu — ipcfp_store_create_rpc_json (info: which path ran, its times)
 Store* store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts, int device,
                              uint32_t flags, ipcfp_store_json_info& info);
+// car.cu — ipcfp_store_create_car (info: which path ran, its times)
+Store* store_create_car(const uint8_t* car, uint64_t len, int device, uint32_t flags, ipcfp_store_json_info& info);
 // n_words device words at src_dev (null: the mirrored dev_words[dst_first ..]) → host_words[dst_first ..) through mapped host memory,
 // on `stream` (null: the store's stream): a tiny kernel instead of a D2H copy, so the read-back never queues behind a large copy on
 // the copy engine

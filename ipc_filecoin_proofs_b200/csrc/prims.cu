@@ -153,6 +153,27 @@ void bitmap_to_indices(const uint32_t* bits, uint64_t nbits, uint32_t* out, uint
     k_bitmap_scatter<<<div_up(nwords, 256), 256, 0, st>>>(bits, nwords, word_prefix, out); IPCFP_LAUNCH_CHECK();
 }
 
+// 64-bit positions
+__global__ void k_bitmap_scatter64(const uint32_t* bits, uint64_t nwords, const uint64_t* word_prefix, uint64_t* out) {
+    uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= nwords) return;
+    uint32_t x = bits[w];
+    uint64_t o = word_prefix[w];
+    while (x) {
+        int b = __ffs((int)x) - 1;
+        out[o++] = w * 32 + (uint64_t)b;
+        x &= x - 1;
+    }
+}
+void bitmap_count64(const uint32_t* bits, uint64_t nbits, uint64_t* total_dev, uint64_t* word_prefix, uint64_t* scratch, cudaStream_t st) {
+    scan_impl(bits, word_prefix, (nbits + 31) / 32, total_dev, scratch, st, LoadPopc());
+}
+void bitmap_scatter64(const uint32_t* bits, uint64_t nbits, const uint64_t* word_prefix, uint64_t* out, cudaStream_t st) {
+    const uint64_t nwords = (nbits + 31) / 32;
+    if (nwords == 0) return;
+    k_bitmap_scatter64<<<div_up(nwords, 256), 256, 0, st>>>(bits, nwords, word_prefix, out); IPCFP_LAUNCH_CHECK();
+}
+
 // ------------------------------------------------------------------------------------------ radix sort
 static constexpr int RS_THREADS = 256;
 static constexpr int RS_WARPS = RS_THREADS / 32;

@@ -17,6 +17,10 @@ void exclusive_scan_u32(const uint32_t* in, uint64_t* out, uint64_t n, uint64_t*
 // word_prefix: u64[nwords] scratch. out: u32[≥ popcount]. *total_dev receives the count.
 void bitmap_to_indices(const uint32_t* bits, uint64_t nbits, uint32_t* out, uint64_t* total_dev, uint64_t* word_prefix,
                        uint64_t* scratch, cudaStream_t st);
+// The same in two steps, with 64-bit positions (bitmaps of 2^32 bits or more), so that the caller can size `out` by the count:
+// bitmap_count64 sets word_prefix and *total_dev; bitmap_scatter64 then writes the positions (out: u64[total]).
+void bitmap_count64(const uint32_t* bits, uint64_t nbits, uint64_t* total_dev, uint64_t* word_prefix, uint64_t* scratch, cudaStream_t st);
+void bitmap_scatter64(const uint32_t* bits, uint64_t nbits, const uint64_t* word_prefix, uint64_t* out, cudaStream_t st);
 
 // Stable radix sort of n (key,val) pairs by the `nbits` low bits of key (8-bit digits, LSD).
 // keys/vals are sorted in place using the alt buffers as ping-pong space.

@@ -14,6 +14,7 @@
 
 #include "../../include/ipcfp.h"
 #include "json_value.h"
+#include "parsed_blocks.h"
 
 namespace ipcfp { void set_last_error(const std::string& msg, uint64_t index); }   // capi.cu
 
@@ -82,12 +83,7 @@ void read_text(const char* text, uint64_t len, uint64_t n, uint64_t& pos, std::v
     if (ps.p != ps.e) bad();   // trailing bytes
 }
 
-struct ParsedBlocks {
-    ipcfp_parsed_blocks pub;   // FIRST member: the handle is a pointer to it
-    std::vector<uint8_t> cids, blob;
-    std::vector<uint64_t> offsets;
-    std::vector<uint32_t> lengths;
-};
+using ParsedBlocks = ParsedBlocksBox;
 
 void build(ParsedBlocks& P, const uint8_t* cids, uint64_t n, const char* const* texts, const uint64_t* lens, uint64_t n_texts) {
     if ((n && !cids) || (n_texts && (!texts || !lens))) bad();

@@ -324,11 +324,19 @@ Store* store_shell(int device) {
 
 void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev) {
     if (n >= 0x7fffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^31 blocks in one store");
-    s->n = n;
+    store_alloc_arena(s, blob_size);
+    store_alloc_index(s, n, cids_dev);
+}
+
+// device allocations
+// (from the process-wide device pool: a store created right after one of similar size was destroyed allocates nothing)
+void store_alloc_arena(Store* s, uint64_t blob_size) {
     s->blob_size = blob_size;
-    // device allocations
-    // (from the process-wide device pool: a store created right after one of similar size was destroyed allocates nothing)
     s->arena.alloc_pooled(blob_size + 48 + 512);   // + room for whole aligned chunks around the last block (pass-1 staging copies CH-aligned chunks)
+}
+
+void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev) {
+    s->n = n;
     s->offsets.alloc_pooled(n + 1);
     s->lengths.alloc_pooled(n + 1);
     s->digests.alloc_pooled(n + 1);
