@@ -494,6 +494,109 @@ ipcfp_status ipcfp_generate_storage_proofs(ipcfp_store* s, const ipcfp_tipset_de
                                            uint64_t n_specs, ipcfp_storage_result** out);
 void ipcfp_storage_result_free(ipcfp_storage_result* r);
 
+/* ------------------------------------------------------------------------------------------
+ * Storage paths: a Solidity value named by its access path, with the slots derived and read on the device (DESIGN.md §3, "Storage
+ * paths"). A path is the declared slot p of a state variable (base_slot, u256 big-endian) and a list of steps; all slot arithmetic is
+ * mod 2^256, as in the EVM:
+ *   IPCFP_PATH_MAPPING  slot = keccak256(key ‖ slot). A value-type key is its 32-byte padded form (the caller's); a bytes / string key is
+ *                       its raw bytes, 0 to IPCFP_PATH_MAX_KEY of them.
+ *   IPCFP_PATH_ARRAY    a dynamic array at slot: slot = keccak256(slot) + (index / per_slot) * elem_slots; the array's length word (the
+ *                       slot before the step) is proven too.
+ *   IPCFP_PATH_STATIC   a static array at slot: slot = slot + (index / per_slot) * elem_slots.
+ *   IPCFP_PATH_FIELD    a struct member: slot = slot + index (the member's slot offset).
+ * per_slot = 32 / elem_bytes when the elements are packed (elem_slots = 1 and elem_bytes 1..32), else 1; a packed element sits
+ * byte_offset = (index % per_slot) * elem_bytes bytes above the low-order end of its word.
+ * kind IPCFP_PATH_WORDS reads n_words (1..IPCFP_PATH_MAX_WORDS) consecutive slots from the final slot: a value type, a whole struct or a
+ * static array. kind IPCFP_PATH_BYTES reads a Solidity bytes / string at the final slot: its header word h, then
+ *   h & 1 == 0  short: length = (h & 0xff) / 2, which must be <= 31; the bytes are the word's high-order bytes;
+ *   h & 1 == 1  long: length = (h - 1) / 2, which must be >= 32; the bytes are in ceil(length / 32) slots from keccak256(slot).
+ * A path's EXPANDED SPECS are (actor_id, slot) pairs in this order: the length word of every ARRAY step, in step order; then the value
+ * words (the n_words slots, or the header word followed by the data slots in ascending order). The expanded specs of the paths of one
+ * call are concatenated in path order.
+ * ------------------------------------------------------------------------------------------ */
+#define IPCFP_PATH_MAX_PATHS 65536u  /* paths of one call: a failure's index keeps the path in 16 bits beside its spec's position       */
+#define IPCFP_PATH_MAX_STEPS 32u     /* steps of one path: one thread derives a path, and every ARRAY step adds a spec to it           */
+#define IPCFP_PATH_MAX_KEY 1024u     /* bytes of one MAPPING key: one thread absorbs it into Keccak-256 (at most 8 blocks of 136 bytes) */
+#define IPCFP_PATH_MAX_WORDS 256u    /* n_words of a WORDS path: a proof per word, 8 KiB of value                                      */
+#define IPCFP_PATH_MAX_BYTES 4096u   /* length of a BYTES value: at most 128 data slots, so one path asks for at most 160 KiB of proof
+                                        recorder lists in wave 2 (128 x 320 words)                                                     */
+enum { IPCFP_PATH_MAPPING = 0, IPCFP_PATH_ARRAY = 1, IPCFP_PATH_STATIC = 2, IPCFP_PATH_FIELD = 3 };
+enum { IPCFP_PATH_WORDS = 0, IPCFP_PATH_BYTES = 1 };
+/* Per-path status (not a call failure: the path's proofs are still emitted) */
+enum {
+    IPCFP_PATH_OK = 0,
+    IPCFP_PATH_INDEX_OUT_OF_RANGE = 1,  /* an ARRAY index at or beyond its proven length word (the first such step decides)          */
+    IPCFP_PATH_BAD_BYTES = 2,           /* a header word Solidity refuses with Panic 0x22: short with length > 31, long with < 32      */
+    IPCFP_PATH_TOO_LONG = 3             /* a long bytes / string over IPCFP_PATH_MAX_BYTES: only its header word is proven              */
+};
+typedef struct ipcfp_path_step {
+    uint32_t op;              /* IPCFP_PATH_MAPPING / _ARRAY / _STATIC / _FIELD                                   */
+    uint32_t key_len;         /* MAPPING: bytes at key                                                             */
+    const uint8_t* key;       /* MAPPING                                                                           */
+    uint64_t index;           /* ARRAY / STATIC: the element index; FIELD: the member's slot offset                */
+    uint32_t elem_slots;      /* ARRAY / STATIC: slots per element, >= 1                                           */
+    uint32_t elem_bytes;      /* ARRAY / STATIC: 0 (not packed) or the packed element's size, 1..32                */
+} ipcfp_path_step;
+typedef struct ipcfp_storage_path {
+    uint64_t actor_id;
+    uint8_t base_slot[32];    /* the state variable's declared slot p, u256 big-endian                               */
+    uint32_t n_steps;
+    uint32_t kind;            /* IPCFP_PATH_WORDS / IPCFP_PATH_BYTES                                                 */
+    const ipcfp_path_step* steps;
+    uint32_t n_words;         /* WORDS: 1..IPCFP_PATH_MAX_WORDS; BYTES: ignored                                      */
+    uint32_t _pad;
+} ipcfp_storage_path;
+typedef struct ipcfp_path_value {
+    uint32_t status;          /* IPCFP_PATH_*                                                                        */
+    uint32_t valid;           /* ipcfp_verify_storage_paths: 1 when every expanded spec has a proof that verifies; generate: 1 */
+    uint8_t slot[32];         /* the final slot                                                                      */
+    uint32_t byte_offset;     /* a packed last ARRAY / STATIC step: the element's byte offset above the word's low end; else 0 */
+    uint32_t _pad;
+    uint64_t first_spec;      /* the path's expanded specs: specs[first_spec .. first_spec + n_specs)                 */
+    uint64_t n_specs;
+    uint64_t value_off;       /* the value: value_blob[value_off .. value_off + value_len) — WORDS: the 32-byte words; BYTES:
+                                 the decoded bytes (status OK or INDEX_OUT_OF_RANGE with a valid header; else 0 bytes) */
+    uint64_t value_len;
+} ipcfp_path_value;
+typedef struct ipcfp_path_result {
+    uint64_t n_paths;
+    const ipcfp_path_value* paths;
+    uint64_t n_specs;
+    const ipcfp_storage_spec* specs;    /* the expanded specs of every path, concatenated in path order                     */
+    const uint8_t* value_blob;
+    uint64_t value_blob_size;
+    ipcfp_storage_result* storage;      /* generate: the proofs of specs (owned by this result); verify: NULL               */
+    /* device time (CUDA events on the store's stream), milliseconds: the whole call, slot derivation, wave 1 (the fixed specs), wave
+     * 2 (the data slots, derived and proven), the witness and per-spec lists; host_syncs: host synchronisations the call made */
+    float ms_total, ms_slots, ms_wave1, ms_wave2, ms_witness;
+    uint32_t host_syncs;
+} ipcfp_path_result;
+/* Proofs of storage paths. `storage` is, byte for byte, what ipcfp_generate_storage_proofs gives for `specs` (the proofs, the witness
+ * union, the per-spec witness lists); every proof is an ordinary StorageProof, and the expanded specs go into every bundle and planner
+ * call as ordinary ipcfp_storage_spec. flags: IPCFP_WITNESS_BY_REFERENCE only (any other bit: IPCFP_ERR_INVALID_ARG).
+ * Flow: slot derivation (one thread per path, chained Keccak-256 and u256 adds), wave 1 (the fixed specs: length words and value or
+ * header words), the expansion (each BYTES path's data-slot count and every path's status from wave 1's words, then a scan), wave 2
+ * (the data slots keccak256(slot) + j, derived and proven on the device into the same witness bitmap), one witness materialisation.
+ * Host synchronisations: four — the size of wave 2 after the expansion, then the three every storage result takes: the witness
+ * count, the end of the witness copy, the end of the call.
+ * Failures have the statuses of ipcfp_generate_storage_proofs; the index is the first failing path, and within it the first failing
+ * spec in expanded order decides the status. IPCFP_ERR_INVALID_ARG before any device work: a NULL array with a nonzero count, more than
+ * IPCFP_PATH_MAX_PATHS paths or IPCFP_PATH_MAX_STEPS steps, a key over IPCFP_PATH_MAX_KEY, an unknown op or kind, elem_bytes over 32,
+ * elem_slots = 0, n_words of 0 or over IPCFP_PATH_MAX_WORDS, a tipset without child_parent_state_root. *out is released with
+ * ipcfp_path_result_free. */
+ipcfp_status ipcfp_generate_storage_path_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_path* paths, uint64_t n,
+                                                         uint32_t flags, ipcfp_path_result** out);
+/* (the fetch round of this call, ipcfp_plan_fetch_storage_paths_resident, is declared with the other planners below) */
+/* Checks storage-path claims against a bundle's storage proofs: every proof is replayed by ipcfp_verify_storage_proofs over the witness
+ * store (its failures fail the call, index = the proof). Then, per path, the expanded specs are derived on the device with the length
+ * and header words taken from the proofs themselves; each (actor_id, slot) must have a proof in the list that verifies (the first in
+ * (actor_id, slot) order when several do). The result's paths[i].valid, status and value are the path's verdict, `specs` the expanded
+ * specs derived, `storage` NULL. A proof whose value was changed, a data slot left out or a length word that lies makes the path invalid.
+ * Refusals are the generate call's. *out is released with ipcfp_path_result_free. */
+ipcfp_status ipcfp_verify_storage_paths(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n_proofs,
+                                        const ipcfp_storage_path* paths, uint64_t n_paths, ipcfp_path_result** out);
+void ipcfp_path_result_free(ipcfp_path_result* r);
+
 /* generate_proof_bundle (src/proofs/generator.rs:25-95): the storage specs, then the event specs in order, then the union of every
  * proof's blocks (BTreeSet<(Cid, data)>, built on the device). Equivalent to ipcfp_tipset_upload followed by
  * ipcfp_generate_proof_bundle_resident with flags = 0. */
@@ -563,6 +666,13 @@ ipcfp_status ipcfp_plan_fetch_message_log_resident(ipcfp_store* s, ipcfp_tipset*
  * storage specs fail as in ipcfp_generate_log_bundle_resident / ipcfp_plan_fetch_resident. */
 ipcfp_status ipcfp_plan_fetch_log_bundle_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,
                                                   const ipcfp_log_filter* filters, uint64_t n_filters, uint32_t flags, ipcfp_fetch_plan** out);
+/* One fetch round for ipcfp_generate_storage_path_proofs_resident: rule 4 (the storage path) for every expanded spec known without
+ * reading storage (the length words and the value or header words), and for a BYTES path's data slots once the store can read its
+ * header word (a long header adds one round). From an empty store the rounds end with a store on which the generate call gives what
+ * it gives on the complete store: the same result, or the same status and index. Refusals are the generate call's; any flag bit is
+ * IPCFP_ERR_INVALID_ARG. */
+ipcfp_status ipcfp_plan_fetch_storage_paths_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_path* paths, uint64_t n,
+                                                     uint32_t flags, ipcfp_fetch_plan** out);
 /* The round as one Filecoin.ChainReadObj batch: request k asks for plan->cids[k] with "id": first_id + k, compact JSON
  *   [{"jsonrpc":"2.0","method":"Filecoin.ChainReadObj","params":[{"/":"b…"}],"id":<first_id + k>},…]
  * With first_id = the number of blocks already held, the responses go straight to ipcfp_store_create_rpc_json with

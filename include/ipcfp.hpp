@@ -16,6 +16,8 @@
 //   generate_event_proof(client, &store, parent, child, sig, t1, filter)   generate_event_proof(store, parent, child, receipts, sig, t1, filter)
 //                                                                  — `receipts` is what the reference fetches with client.chain_get_parent_receipts (events/generator.rs:199-204)
 //   generate_storage_proof(&store, parent, child, actor_id, slot)  same                                           (storage/generator.rs:29-67)
+//   (README "Storage Slot Calculation": values in Solidity structures)  StoragePath, generate_storage_path_proofs, plan_fetch_storage_paths,
+//                                                                  verify_storage_paths                           (storage/utils.rs:5-19)
 //   read_storage_slot(&store, &root, &slot)                        same                                           (storage/decode.rs:36-97)
 //   generate_proof_bundle(client, parent, child, sspecs, especs)   generate_proof_bundle(store, parent, child, receipts, sspecs, especs)   (proofs/generator.rs:25-95)
 //   verify_event_proof(&bundle, &trusted_ts, &trusted_child, check_event)  same; check_event is an EventProofSpec (create_event_filter, events/verifier.rs:28-41)
@@ -884,6 +886,163 @@ inline bool verify_storage_proof(const StorageProof& proof, const std::vector<Pr
     uint8_t res = 0;
     check(ipcfp_verify_storage_proofs(store.raw(), &d, &q, 1, &res), "verify_storage_proof");
     return res != 0;
+}
+
+// ------------------------------------------------------------------------------------------ storage paths (ipcfp.h, "Storage paths")
+// A Solidity value by its access path: the declared slot, then steps, then what to read. Each builder step returns a new path:
+//   StoragePath::at(actor, 0).mapping(subnet_id).field(2).bytes()            subnets[id].<string member at slot offset 2>
+struct StoragePath {
+    struct Step { uint32_t op; std::vector<uint8_t> key; uint64_t index; uint32_t elem_slots, elem_bytes; };
+    uint64_t actor_id = 0;
+    H256 base_slot{};
+    std::vector<Step> steps;
+    uint32_t kind = IPCFP_PATH_WORDS;
+    uint32_t n_words = 1;
+
+    static StoragePath at(uint64_t actor_id, const H256& slot) { StoragePath p; p.actor_id = actor_id; p.base_slot = slot; return p; }
+    static StoragePath at(uint64_t actor_id, uint64_t slot) {
+        H256 s{};
+        for (int i = 0; i < 8; i++) s[31 - i] = (uint8_t)(slot >> (8 * i));
+        return at(actor_id, s);
+    }
+    // a value-type key in its 32-byte padded form, or the raw bytes of a bytes / string key
+    StoragePath mapping(const std::vector<uint8_t>& key) const { return with(Step{IPCFP_PATH_MAPPING, key, 0, 0, 0}); }
+    StoragePath mapping(const H256& key) const { return mapping(std::vector<uint8_t>(key.begin(), key.end())); }
+    StoragePath array(uint64_t index, uint32_t elem_slots = 1, uint32_t elem_bytes = 0) const { return with(Step{IPCFP_PATH_ARRAY, {}, index, elem_slots, elem_bytes}); }
+    StoragePath static_array(uint64_t index, uint32_t elem_slots = 1, uint32_t elem_bytes = 0) const {
+        return with(Step{IPCFP_PATH_STATIC, {}, index, elem_slots, elem_bytes});
+    }
+    StoragePath field(uint64_t offset) const { return with(Step{IPCFP_PATH_FIELD, {}, offset, 0, 0}); }
+    StoragePath words(uint32_t n) const { StoragePath p = *this; p.kind = IPCFP_PATH_WORDS; p.n_words = n; return p; }
+    StoragePath bytes() const { StoragePath p = *this; p.kind = IPCFP_PATH_BYTES; p.n_words = 0; return p; }
+
+  private:
+    StoragePath with(Step s) const { StoragePath p = *this; p.steps.push_back(std::move(s)); return p; }
+};
+// One path's outcome: its status (IPCFP_PATH_*), final slot, packed byte offset, value (the words, or the decoded bytes) and its proofs
+// (the StorageProofs of its expanded specs, in expanded order). valid: the verifier's verdict (always true from the generator).
+struct StoragePathValue {
+    uint32_t status = IPCFP_PATH_OK;
+    bool valid = true;
+    H256 slot{};
+    uint32_t byte_offset = 0;
+    std::vector<uint8_t> value;
+    std::vector<StorageProof> proofs;
+};
+struct StoragePathProofs {
+    std::vector<StoragePathValue> paths;
+    std::vector<ProofBlock> blocks;   // the witness union of every proof
+};
+
+namespace detail {
+struct PathsC {
+    std::vector<std::vector<ipcfp_path_step>> steps;
+    std::vector<ipcfp_storage_path> c;
+    explicit PathsC(const std::vector<StoragePath>& paths) {
+        steps.resize(paths.size());
+        for (size_t i = 0; i < paths.size(); i++) {
+            const StoragePath& p = paths[i];
+            for (const auto& s : p.steps)
+                steps[i].push_back(ipcfp_path_step{s.op, (uint32_t)s.key.size(), s.key.empty() ? nullptr : s.key.data(), s.index, s.elem_slots, s.elem_bytes});
+            ipcfp_storage_path q;
+            memset(&q, 0, sizeof q);
+            q.actor_id = p.actor_id;
+            memcpy(q.base_slot, p.base_slot.data(), 32);
+            q.n_steps = (uint32_t)p.steps.size();
+            q.kind = p.kind;
+            q.steps = steps[i].empty() ? nullptr : steps[i].data();
+            q.n_words = p.n_words;
+            c.push_back(q);
+        }
+    }
+};
+// the per-path values of a result; proofs from `proofs` (the result's own, or the caller's for the verifier) when given
+inline std::vector<StoragePathValue> path_values(const ipcfp_path_result& r, const std::vector<StorageProof>* proofs) {
+    std::vector<StoragePathValue> out(r.n_paths);
+    for (uint64_t i = 0; i < r.n_paths; i++) {
+        const ipcfp_path_value& v = r.paths[i];
+        StoragePathValue& o = out[i];
+        o.status = v.status;
+        o.valid = v.valid != 0;
+        memcpy(o.slot.data(), v.slot, 32);
+        o.byte_offset = v.byte_offset;
+        o.value.assign(r.value_blob + v.value_off, r.value_blob + v.value_off + v.value_len);
+        if (proofs) o.proofs.assign(proofs->begin() + v.first_spec, proofs->begin() + v.first_spec + v.n_specs);
+    }
+    return out;
+}
+}  // namespace detail
+
+// ipcfp_generate_storage_path_proofs_resident against (parent, child)'s tipset: every path's value and the StorageProofs of its
+// expanded specs, as generate_storage_proof returns them, with the witness union
+inline StoragePathProofs generate_storage_path_proofs(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<StoragePath>& paths) {
+    TipsetDesc t(parent, child, {});
+    detail::PathsC pc(paths);
+    ipcfp_tipset* tip = nullptr;
+    check(ipcfp_tipset_upload(store.raw(), t.c(), &tip), "ipcfp_tipset_upload");
+    ipcfp_path_result* r = nullptr;
+    const ipcfp_status st = ipcfp_generate_storage_path_proofs_resident(store.raw(), tip, pc.c.data(), pc.c.size(), 0, &r);
+    ipcfp_tipset_free(tip);
+    check(st, "generate_storage_path_proofs");
+    StoragePathProofs out;
+    try {
+        std::vector<StorageProof> proofs;
+        for (uint64_t k = 0; k < r->storage->n_proofs; k++) proofs.push_back(storage_proof(r->storage->proofs[k], t));
+        out.paths = detail::path_values(*r, &proofs);
+        out.blocks = proof_blocks(r->storage->witness);
+    } catch (...) { ipcfp_path_result_free(r); throw; }
+    ipcfp_path_result_free(r);
+    return out;
+}
+// ipcfp_plan_fetch_storage_paths_resident: one fetch round (the CIDs the store lacks, `Cid` order) for generate_storage_path_proofs
+inline std::vector<Cid> plan_fetch_storage_paths(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<StoragePath>& paths) {
+    TipsetDesc t(parent, child, {});
+    detail::PathsC pc(paths);
+    ipcfp_tipset* tip = nullptr;
+    check(ipcfp_tipset_upload(store.raw(), t.c(), &tip), "ipcfp_tipset_upload");
+    ipcfp_fetch_plan* p = nullptr;
+    const ipcfp_status st = ipcfp_plan_fetch_storage_paths_resident(store.raw(), tip, pc.c.data(), pc.c.size(), 0, &p);
+    ipcfp_tipset_free(tip);
+    check(st, "plan_fetch_storage_paths");
+    std::vector<Cid> out;
+    for (uint64_t k = 0; k < p->n_missing; k++) out.push_back(Cid::from_bytes(p->cids + IPCFP_CID_LEN * k));
+    ipcfp_fetch_plan_free(p);
+    return out;
+}
+// ipcfp_verify_storage_paths: the paths' claims against StorageProofs (one child block and state root, as in a bundle) and their blocks,
+// after the trust anchor; per path valid, status and value (proofs left empty). An untrusted child gives every path valid = false.
+inline std::vector<StoragePathValue> verify_storage_paths(const std::vector<StorageProof>& proofs, const std::vector<ProofBlock>& blocks,
+                                                          const std::vector<StoragePath>& paths, const TrustedChildHeader& is_trusted_child_header, int device = 0) {
+    if (proofs.empty()) throw Error(IPCFP_ERR_INVALID_ARG, "verify_storage_paths: no proofs");
+    const Cid child = Cid::try_from(proofs[0].child_block_cid);
+    const Cid psr = Cid::try_from(proofs[0].parent_state_root);
+    std::vector<ipcfp_storage_proof> qs(proofs.size());
+    for (size_t i = 0; i < proofs.size(); i++) {
+        const StorageProof& p = proofs[i];
+        if (p.child_block_cid != proofs[0].child_block_cid || p.parent_state_root != proofs[0].parent_state_root)
+            throw Error(IPCFP_ERR_UNSUPPORTED, "verify_storage_paths: proofs of several child blocks");
+        ipcfp_storage_proof& q = qs[i];
+        memset(&q, 0, sizeof q);
+        q.actor_id = p.actor_id;
+        memcpy(q.actor_state_cid, Cid::try_from(p.actor_state_cid).bytes.data(), IPCFP_CID_LEN);
+        memcpy(q.storage_root, Cid::try_from(p.storage_root).bytes.data(), IPCFP_CID_LEN);
+        memcpy(q.slot, from_hex32(p.slot).data(), 32);
+        memcpy(q.value, from_hex32(p.value).data(), 32);
+    }
+    GpuBlockstore store = GpuBlockstore::from_witness(blocks, device);
+    ipcfp_tipset_desc d;
+    memset(&d, 0, sizeof d);
+    d.child_epoch = proofs[0].child_epoch;
+    d.child_cid = child.bytes.data();
+    d.child_parent_state_root = psr.bytes.data();
+    detail::PathsC pc(paths);
+    ipcfp_path_result* r = nullptr;
+    check(ipcfp_verify_storage_paths(store.raw(), &d, qs.data(), qs.size(), pc.c.data(), pc.c.size(), &r), "verify_storage_paths");
+    std::vector<StoragePathValue> out = detail::path_values(*r, nullptr);
+    ipcfp_path_result_free(r);
+    if (!is_trusted_child_header(proofs[0].child_epoch, child))
+        for (auto& v : out) v.valid = false;
+    return out;
 }
 
 // verify_proof_bundle (proofs/verifier.rs:12-60): every storage proof and every event proof of a UnifiedProofBundle against its

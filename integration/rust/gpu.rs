@@ -495,6 +495,50 @@ pub fn generate_storage_proof_gpu(
     res
 }
 
+/// One Solidity value by its storage path (`ipcfp.h`, "Storage paths"): the caller's `ipcfp_storage_path` (steps and keys borrowed for
+/// the call) → its status, its value (the words, or the decoded bytes) and the proofs of its expanded specs with their blocks, as
+/// `generate_storage_proof_gpu` returns them.
+pub struct StoragePathValue {
+    pub status: u32,
+    pub value: Vec<u8>,
+    pub proofs: Vec<(StorageProof, Vec<ProofBlock>)>,
+}
+pub fn generate_storage_path_proofs_gpu(
+    store: &GpuBlockstore,
+    parent: &ApiTipset,
+    child: &ApiTipset,
+    paths: &[sys::ipcfp_storage_path],
+) -> Result<Vec<StoragePathValue>> {
+    let desc = TipsetDesc::new(parent, child, &[])?;
+    let mut tip = std::ptr::null_mut();
+    check(unsafe { sys::ipcfp_tipset_upload(store.h, &desc.raw(), &mut tip) })?;
+    let mut out = std::ptr::null_mut();
+    let st = unsafe { sys::ipcfp_generate_storage_path_proofs_resident(store.h, tip, paths.as_ptr(), paths.len() as u64, 0, &mut out) };
+    unsafe { sys::ipcfp_tipset_free(tip) };
+    check(st)?;
+    let r = unsafe { &*out };
+    let res = (|| -> Result<Vec<StoragePathValue>> {
+        let s = unsafe { &*r.storage };
+        let all = witness_blocks(&s.witness)?;
+        let mut v = Vec::with_capacity(paths.len());
+        for i in 0..r.n_paths as usize {
+            let pv = unsafe { &*r.paths.add(i) };
+            let value = unsafe { std::slice::from_raw_parts(r.value_blob.add(pv.value_off as usize), pv.value_len as usize) }.to_vec();
+            let mut proofs = Vec::with_capacity(pv.n_specs as usize);
+            for k in pv.first_spec as usize..(pv.first_spec + pv.n_specs) as usize {
+                let p = unsafe { &*s.proofs.add(k) };
+                let (a, b) = unsafe { (*s.spec_witness_offsets.add(k) as usize, *s.spec_witness_offsets.add(k + 1) as usize) };
+                let blocks = (a..b).map(|j| all[unsafe { *s.spec_witness_index.add(j) } as usize].clone()).collect();
+                proofs.push((storage_proof_of(p, child, &desc)?, blocks));
+            }
+            v.push(StoragePathValue { status: pv.status, value, proofs });
+        }
+        Ok(v)
+    })();
+    unsafe { sys::ipcfp_path_result_free(out) };
+    res
+}
+
 /// `resolve_eth_address_to_actor_id` (`src/proofs/common/address.rs:8-62`) from the state tree at `state_root` (the child header's
 /// ParentStateRoot) instead of `Filecoin.EthAddressToFilecoinAddress` + `Filecoin.StateLookupID`: the same validation and messages,
 /// then the Init actor's address map walked on the GPU.

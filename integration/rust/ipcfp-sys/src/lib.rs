@@ -106,6 +106,34 @@ pub struct ipcfp_tipset_info { pub desc: ipcfp_tipset_desc, pub parsed_on_device
 pub struct ipcfp_parsed_blocks { pub blocks: ipcfp_witness }
 #[repr(C)]
 pub struct ipcfp_store_json_info { pub parsed_on_device: u32, pub ms_parse: f32, pub ms_kernels: f32, pub _pad: u32 }
+// Storage paths (ipcfp.h, "Storage paths")
+pub const IPCFP_PATH_MAX_PATHS: u32 = 65536;
+pub const IPCFP_PATH_MAX_STEPS: u32 = 32;
+pub const IPCFP_PATH_MAX_KEY: u32 = 1024;
+pub const IPCFP_PATH_MAX_WORDS: u32 = 256;
+pub const IPCFP_PATH_MAX_BYTES: u32 = 4096;
+pub const IPCFP_PATH_MAPPING: u32 = 0;
+pub const IPCFP_PATH_ARRAY: u32 = 1;
+pub const IPCFP_PATH_STATIC: u32 = 2;
+pub const IPCFP_PATH_FIELD: u32 = 3;
+pub const IPCFP_PATH_WORDS: u32 = 0;
+pub const IPCFP_PATH_BYTES: u32 = 1;
+pub const IPCFP_PATH_OK: u32 = 0;
+pub const IPCFP_PATH_INDEX_OUT_OF_RANGE: u32 = 1;
+pub const IPCFP_PATH_BAD_BYTES: u32 = 2;
+pub const IPCFP_PATH_TOO_LONG: u32 = 3;
+#[repr(C)]
+pub struct ipcfp_path_step { pub op: u32, pub key_len: u32, pub key: *const u8, pub index: u64, pub elem_slots: u32, pub elem_bytes: u32 }
+#[repr(C)]
+pub struct ipcfp_storage_path { pub actor_id: u64, pub base_slot: [u8; 32], pub n_steps: u32, pub kind: u32, pub steps: *const ipcfp_path_step,
+                                pub n_words: u32, pub _pad: u32 }
+#[repr(C)]
+pub struct ipcfp_path_value { pub status: u32, pub valid: u32, pub slot: [u8; 32], pub byte_offset: u32, pub _pad: u32, pub first_spec: u64,
+                              pub n_specs: u64, pub value_off: u64, pub value_len: u64 }
+#[repr(C)]
+pub struct ipcfp_path_result { pub n_paths: u64, pub paths: *const ipcfp_path_value, pub n_specs: u64, pub specs: *const ipcfp_storage_spec,
+                               pub value_blob: *const u8, pub value_blob_size: u64, pub storage: *mut ipcfp_storage_result, pub ms_total: f32,
+                               pub ms_slots: f32, pub ms_wave1: f32, pub ms_wave2: f32, pub ms_witness: f32, pub host_syncs: u32 }
 #[repr(C)]
 pub struct ipcfp_fetch_plan { pub n_missing: u64, pub cids: *const u8, pub n_needed: u64, pub n_levels: u32, pub ms_total: f32 }
 pub const IPCFP_ADDRESS_MAX: usize = 65;
@@ -176,6 +204,13 @@ extern "C" {
     pub fn ipcfp_generate_storage_proofs(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, specs: *const ipcfp_storage_spec, n_specs: u64,
                                          out: *mut *mut ipcfp_storage_result) -> ipcfp_status;
     pub fn ipcfp_storage_result_free(r: *mut ipcfp_storage_result);
+    pub fn ipcfp_generate_storage_path_proofs_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, paths: *const ipcfp_storage_path, n: u64,
+                                                       flags: u32, out: *mut *mut ipcfp_path_result) -> ipcfp_status;
+    pub fn ipcfp_plan_fetch_storage_paths_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, paths: *const ipcfp_storage_path, n: u64,
+                                                   flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_verify_storage_paths(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_storage_proof, n_proofs: u64,
+                                      paths: *const ipcfp_storage_path, n_paths: u64, out: *mut *mut ipcfp_path_result) -> ipcfp_status;
+    pub fn ipcfp_path_result_free(r: *mut ipcfp_path_result);
     pub fn ipcfp_generate_proof_bundle(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,
                                        especs: *const ipcfp_event_spec, n_especs: u64, out: *mut *mut ipcfp_bundle) -> ipcfp_status;
     pub fn ipcfp_generate_proof_bundle_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, sspecs: *const ipcfp_storage_spec, n_sspecs: u64,

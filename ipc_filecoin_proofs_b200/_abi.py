@@ -335,6 +335,35 @@ class StorageResultC(C.Structure):
     ]
 
 
+# Storage paths (include/ipcfp.h, "Storage paths")
+PATH_MAX_PATHS = 65536
+PATH_MAX_STEPS = 32
+PATH_MAX_KEY = 1024
+PATH_MAX_WORDS = 256
+PATH_MAX_BYTES = 4096
+PATH_MAPPING, PATH_ARRAY, PATH_STATIC, PATH_FIELD = 0, 1, 2, 3
+PATH_WORDS, PATH_BYTES = 0, 1
+PATH_OK, PATH_INDEX_OUT_OF_RANGE, PATH_BAD_BYTES, PATH_TOO_LONG = 0, 1, 2, 3
+
+
+class PathStepC(C.Structure):
+    """ipcfp_path_step"""
+    _fields_ = [("op", C.c_uint32), ("key_len", C.c_uint32), ("key", C.c_void_p), ("index", C.c_uint64), ("elem_slots", C.c_uint32),
+                ("elem_bytes", C.c_uint32)]
+
+
+class StoragePathC(C.Structure):
+    """ipcfp_storage_path"""
+    _fields_ = [("actor_id", C.c_uint64), ("base_slot", C.c_uint8 * 32), ("n_steps", C.c_uint32), ("kind", C.c_uint32), ("steps", C.c_void_p),
+                ("n_words", C.c_uint32), ("_pad", C.c_uint32)]
+
+
+class PathValueC(C.Structure):
+    """ipcfp_path_value"""
+    _fields_ = [("status", C.c_uint32), ("valid", C.c_uint32), ("slot", C.c_uint8 * 32), ("byte_offset", C.c_uint32), ("_pad", C.c_uint32),
+                ("first_spec", C.c_uint64), ("n_specs", C.c_uint64), ("value_off", C.c_uint64), ("value_len", C.c_uint64)]
+
+
 class SlotResultC(C.Structure):
     _fields_ = [
         ("n", C.c_uint64),
@@ -360,6 +389,13 @@ class BundleC(C.Structure):
         ("ms_total", C.c_float),
         ("ms_json", C.c_float),
     ]
+
+
+class PathResultC(C.Structure):
+    """ipcfp_path_result"""
+    _fields_ = [("n_paths", C.c_uint64), ("paths", C.c_void_p), ("n_specs", C.c_uint64), ("specs", C.c_void_p), ("value_blob", C.c_void_p),
+                ("value_blob_size", C.c_uint64), ("storage", C.POINTER(StorageResultC)), ("ms_total", C.c_float), ("ms_slots", C.c_float),
+                ("ms_wave1", C.c_float), ("ms_wave2", C.c_float), ("ms_witness", C.c_float), ("host_syncs", C.c_uint32)]
 
 
 def _arr(ptr, n, dtype):
@@ -543,6 +579,42 @@ def slot_result_from_c(r):
     n = int(r.n)
     return SlotResultPy(_arr(r.found, n, np.uint8), _arr(r.raw_len, n, np.uint32), _arr(r.values, n * 32, np.uint8).reshape(n, 32),
                         witness_from_c(r.witness), float(r.ms_total), float(r.ms_lookup), int(r.lookup_nodes), int(r.lookup_bytes))
+
+
+@dataclass
+class PathValuePy:
+    """One path's outcome: status (PATH_*), valid (the verifier's verdict; 1 from the generator), the final slot, the packed byte offset,
+    its expanded specs specs[first_spec : first_spec + n_specs] and its value (the words, or the decoded bytes)."""
+    status: int
+    valid: bool
+    slot: bytes
+    byte_offset: int
+    first_spec: int
+    n_specs: int
+    value: bytes
+
+
+@dataclass
+class PathResultPy:
+    paths: list             # PathValuePy per path
+    specs: list             # the expanded specs, (actor_id, slot) pairs in path order
+    storage: StorageResultPy = None   # generate: the proofs of specs; verify: None
+    timings: dict = field(default_factory=dict)
+    host_syncs: int = 0
+
+
+def path_result_from_c(r):
+    n, m = int(r.n_paths), int(r.n_specs)
+    vals = (PathValueC * max(n, 1)).from_address(r.paths) if n else []
+    blob = C.string_at(r.value_blob, int(r.value_blob_size)) if r.value_blob_size else b""
+    paths = [PathValuePy(int(v.status), bool(v.valid), bytes(v.slot), int(v.byte_offset), int(v.first_spec), int(v.n_specs),
+                         blob[int(v.value_off):int(v.value_off) + int(v.value_len)]) for v in (vals[i] for i in range(n))]
+    raw = _arr(r.specs, m * C.sizeof(StorageSpec), np.uint8)
+    sz = C.sizeof(StorageSpec)
+    specs = [(int.from_bytes(raw[sz * i:sz * i + 8].tobytes(), "little"), raw[sz * i + 8:sz * i + 40].tobytes()) for i in range(m)]
+    st = storage_result_from_c(r.storage.contents) if r.storage else None
+    timings = dict(total=r.ms_total, slots=r.ms_slots, wave1=r.ms_wave1, wave2=r.ms_wave2, witness=r.ms_witness)
+    return PathResultPy(paths, specs, st, timings, int(r.host_syncs))
 
 
 @dataclass

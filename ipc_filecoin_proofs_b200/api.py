@@ -86,6 +86,9 @@ SIGNATURES = {
     "ipcfp_slot_result_free": (None, [_P(A.SlotResultC)]),
     "ipcfp_generate_storage_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _PP(A.StorageResultC)]),
     "ipcfp_storage_result_free": (None, [_P(A.StorageResultC)]),
+    "ipcfp_generate_storage_path_proofs_resident": (_st, [_vp, _vp, _P(A.StoragePathC), _u64, _u32, _PP(A.PathResultC)]),
+    "ipcfp_verify_storage_paths": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _P(A.StoragePathC), _u64, _PP(A.PathResultC)]),
+    "ipcfp_path_result_free": (None, [_P(A.PathResultC)]),
     "ipcfp_generate_proof_bundle": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _PP(A.BundleC)]),
     "ipcfp_generate_proof_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _vp, _u64, _u32, _PP(A.BundleC)]),
     "ipcfp_generate_log_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u64, _u32, _PP(A.BundleC)]),
@@ -97,6 +100,7 @@ SIGNATURES = {
     "ipcfp_plan_fetch_log_resident": (_st, [_vp, _vp, _P(A.LogFilterC), _u32, _PP(A.FetchPlanC)]),
     "ipcfp_plan_fetch_message_log_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u32, _PP(A.FetchPlanC)]),
     "ipcfp_plan_fetch_log_bundle_resident": (_st, [_vp, _vp, _vp, _u64, _P(A.LogFilterC), _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_plan_fetch_storage_paths_resident": (_st, [_vp, _vp, _P(A.StoragePathC), _u64, _u32, _PP(A.FetchPlanC)]),
     "ipcfp_fetch_plan_to_rpc_json": (_st, [_P(A.FetchPlanC), _u64, _P(_vp), _P(_u64)]),
     "ipcfp_resolve_addresses": (_st, [_vp, _vp, _P(A.AddressC), _u64, _PP(A.ResolveResultC)]),
     "ipcfp_resolve_result_free": (None, [_P(A.ResolveResultC)]),
@@ -168,6 +172,7 @@ def _result(fn, out_type, convert, free, *args):
 _EVENT_RESULT = (A.EventResultC, A.event_result_from_c, "ipcfp_event_result_free")
 _BUNDLE = (A.BundleC, A.bundle_from_c, "ipcfp_bundle_free")
 _FETCH_PLAN = (A.FetchPlanC, A.fetch_plan_from_c, "ipcfp_fetch_plan_free")
+_PATH_RESULT = (A.PathResultC, A.path_result_from_c, "ipcfp_path_result_free")
 
 
 def kernel_launch_count():
@@ -262,6 +267,136 @@ def _log_filters_c(log_filters):
 class StorageProofSpec:  # reference src/proofs/generator.rs:12-15
     actor_id: int
     slot: bytes
+
+
+def _u256(x):
+    """an int (mod 2^256, two's complement for negatives) or 32 bytes → 32 big-endian bytes"""
+    if isinstance(x, int):
+        return (x % (1 << 256)).to_bytes(32, "big")
+    x = bytes(x)
+    if len(x) != 32:
+        raise ValueError(f"a slot is 32 bytes, got {len(x)}")
+    return x
+
+
+def encode_key(key, key_type=None):
+    """A mapping key as Solidity hashes it (keccak256(h(k) ‖ p)): value types as their 32-byte padded form — "address" (20 bytes or hex,
+    left-padded), "uint…" / "int…" (two's complement), "bool", "bytes1".."bytes32" (right-padded) — and "bytes" / "string" as their raw
+    bytes. key_type None takes 32 bytes as they are."""
+    if key_type is None:
+        k = bytes(key)
+        if len(k) != 32:
+            raise ValueError("a key without a type must be 32 bytes")
+        return k
+    if key_type == "address":
+        b = bytes.fromhex(key[2:] if key[:2] in ("0x", "0X") else key) if isinstance(key, str) else bytes(key)
+        if len(b) != 20:
+            raise ValueError("an address is 20 bytes")
+        return bytes(12) + b
+    if key_type.startswith("uint") or key_type.startswith("int"):
+        return _u256(int(key))
+    if key_type == "bool":
+        return _u256(1 if key else 0)
+    if key_type in ("bytes", "string"):
+        return key.encode() if isinstance(key, str) else bytes(key)
+    if key_type.startswith("bytes"):
+        n = int(key_type[5:])
+        b = key.encode() if isinstance(key, str) else bytes(key)
+        if not 1 <= n <= 32 or len(b) > n:
+            raise ValueError(f"{key_type} key of {len(b)} bytes")
+        return b + bytes(32 - len(b))
+    raise ValueError(f"unknown key type {key_type!r}")
+
+
+class StoragePath:
+    """A Solidity value by its access path (include/ipcfp.h, "Storage paths"): the state variable's declared slot, then steps —
+    .mapping(key, key_type), .array(index) (dynamic: its length word is proven too), .static(index), .field(offset) — and what to read:
+    .words(n) (a value type, a struct, a static array; the default is one word) or .bytes() (a bytes / string). Each step returns a new
+    path, so a common prefix can be shared:
+        StoragePath(actor, 0).mapping(subnet_id, "bytes32").field(3)     # subnets[id].<member at slot offset 3>
+    Arrays: elem_slots = slots per element; elem_bytes = the size of a packed value-type element (uint8: 1, address: 20), 0 otherwise."""
+
+    def __init__(self, actor_id, base_slot, steps=(), kind=A.PATH_WORDS, n_words=1):
+        self.actor_id = int(actor_id)
+        self.base_slot = _u256(base_slot)
+        self.steps = tuple(steps)
+        self.kind = kind
+        self.n_words = n_words
+
+    def _with(self, step=None, **kw):
+        d = dict(steps=self.steps + ((step,) if step else ()), kind=self.kind, n_words=self.n_words)
+        d.update(kw)
+        return StoragePath(self.actor_id, self.base_slot, **d)
+
+    def mapping(self, key, key_type=None):
+        return self._with((A.PATH_MAPPING, encode_key(key, key_type), 0, 0, 0))
+
+    def array(self, index, elem_slots=1, elem_bytes=0):
+        return self._with((A.PATH_ARRAY, b"", int(index), elem_slots, elem_bytes))
+
+    def static(self, index, elem_slots=1, elem_bytes=0):
+        return self._with((A.PATH_STATIC, b"", int(index), elem_slots, elem_bytes))
+
+    def field(self, offset):
+        return self._with((A.PATH_FIELD, b"", int(offset), 0, 0))
+
+    def words(self, n=1):
+        return self._with(kind=A.PATH_WORDS, n_words=n)
+
+    def bytes(self):
+        return self._with(kind=A.PATH_BYTES, n_words=0)
+
+    @staticmethod
+    def decode(word, value_type="uint256", byte_offset=0):
+        """A packed member of a 32-byte word: its bytes sit byte_offset bytes above the word's low-order end (Solidity packs the first
+        member lowest). value_type: "uintN" / "intN" (int), "bool", "address" (20 bytes), "bytesN" (bytes)."""
+        word = bytes(word)
+        if value_type == "address":
+            size = 20
+        elif value_type == "bool":
+            size = 1
+        elif value_type.startswith("uint") or value_type.startswith("int"):
+            size = int(value_type.lstrip("uint") or 256) // 8
+        elif value_type.startswith("bytes"):
+            size = int(value_type[5:])
+        else:
+            raise ValueError(f"unknown value type {value_type!r}")
+        raw = word[32 - byte_offset - size:32 - byte_offset]
+        if value_type == "bool":
+            return raw != b"\0"
+        if value_type.startswith("uint"):
+            return int.from_bytes(raw, "big")
+        if value_type.startswith("int"):
+            return int.from_bytes(raw, "big", signed=True)
+        return raw
+
+    def as_c(self):
+        """(ipcfp_storage_path, keepalive)"""
+        steps = (A.PathStepC * max(len(self.steps), 1))()
+        keep = [steps]
+        for i, (op, key, index, elem_slots, elem_bytes) in enumerate(self.steps):
+            st = steps[i]
+            st.op, st.index, st.elem_slots, st.elem_bytes = op, index, elem_slots, elem_bytes
+            if key:
+                kb = C.create_string_buffer(key, len(key))
+                keep.append(kb)
+                st.key, st.key_len = C.addressof(kb), len(key)
+        c = A.StoragePathC()
+        c.actor_id = self.actor_id
+        c.base_slot[:] = list(self.base_slot)
+        c.n_steps, c.kind, c.n_words = len(self.steps), self.kind, self.n_words
+        c.steps = C.addressof(steps) if self.steps else None
+        return c, keep
+
+
+def _paths_c(paths):
+    """(ipcfp_storage_path array, count, keepalive) of a sequence of StoragePaths"""
+    cs, keep = [], []
+    for p in paths:
+        c, k = p.as_c()
+        cs.append(c)
+        keep.append(k)
+    return (A.StoragePathC * max(len(cs), 1))(*cs), len(cs), keep
 
 
 class PinnedArray:
@@ -493,6 +628,17 @@ class BlockStore:
         farr, nf, fkeep = _log_filters_c(log_filters)
         return _result(fn, *result, self._h, tipset, sarr, ns, farr, nf, flags)
 
+    def generate_storage_path_proofs_resident(self, tip, paths, flags=0):
+        """ipcfp_generate_storage_path_proofs_resident → A.PathResultPy: the StoragePaths' expanded specs, values and statuses, and
+        .storage, the proofs of the specs (what generate_storage_proofs gives for them). flags: WITNESS_BY_REFERENCE."""
+        arr, n, keep = _paths_c(paths)
+        return _result("ipcfp_generate_storage_path_proofs_resident", *_PATH_RESULT, self._h, tip._h, arr, n, flags)
+
+    def plan_fetch_storage_paths(self, tip, paths, flags=0):
+        """ipcfp_plan_fetch_storage_paths_resident → A.FetchPlanPy: one fetch round for generate_storage_path_proofs_resident."""
+        arr, n, keep = _paths_c(paths)
+        return _result("ipcfp_plan_fetch_storage_paths_resident", *_FETCH_PLAN, self._h, tip._h, arr, n, flags)
+
     def plan_fetch_logs(self, tip, log_filter, flags=0):
         """ipcfp_plan_fetch_log_resident → A.FetchPlanPy: one fetch round for generate_log_proof_resident(tip, log_filter)."""
         f, fkeep = log_filter.as_c()
@@ -636,6 +782,12 @@ def fetch_messages_until_complete(fetch, upload_tipset, message_cids, log_filter
     plan_fetch_messages."""
     return _fetch_loop(lambda store, tip: store.plan_fetch_messages(tip, message_cids, log_filter), fetch, upload_tipset, device, verify_cids,
                        max_rounds)
+
+
+def fetch_storage_paths_until_complete(fetch, upload_tipset, paths, device=0, verify_cids=True, max_rounds=10000):
+    """fetch_until_complete for generate_storage_path_proofs_resident(tip, paths): the same loop, planned with plan_fetch_storage_paths
+    (a long bytes / string value takes one round more: its data slots are known once its header word is)."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch_storage_paths(tip, paths), fetch, upload_tipset, device, verify_cids, max_rounds)
 
 
 def _fetch_loop(plan_round, fetch, upload_tipset, device, verify_cids, max_rounds):
@@ -907,6 +1059,27 @@ def verify_event_proofs_any(witness, ts, result, log_filters, device=0):
 def verify_storage_proofs(witness, ts, result, device=0):
     """verify_storage_proof (storage/verifier.rs:24-63) batched on the GPU over a CID-checked witness store."""
     return _verify(witness, ts, result, device, "ipcfp_verify_storage_proofs", blob=False)
+
+
+def verify_storage_paths(witness, ts, proofs, paths, device=0):
+    """ipcfp_verify_storage_paths over the witness (WitnessPy) as a CID-checked store: proofs — an A.StorageResultPy, a list of
+    A.StorageProofPy or packed ipcfp_storage_proof records — against the StoragePaths → A.PathResultPy (per path: valid, status, value;
+    storage None)."""
+    if hasattr(proofs, "raw_proofs"):
+        raw = proofs.raw_proofs
+    elif isinstance(proofs, np.ndarray):
+        raw = proofs
+    else:
+        raw = A.pack_storage_proofs(proofs)
+    raw = np.ascontiguousarray(raw, dtype=np.uint8)
+    n = raw.size // C.sizeof(A.StorageProofC)
+    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
+    try:
+        d, keep = A.make_tipset_desc(ts)
+        arr, np_, pkeep = _paths_c(paths)
+        return _result("ipcfp_verify_storage_paths", *_PATH_RESULT, store._h, C.byref(d), raw.ctypes.data if n else None, n, arr, np_)
+    finally:
+        store.close()
 
 
 def _hash_batch(fn, messages, device=0):

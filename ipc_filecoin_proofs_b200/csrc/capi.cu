@@ -221,7 +221,7 @@ const char* ipcfp_last_error(void) { return g_last_error.c_str(); }
 uint64_t ipcfp_last_error_index(void) { return g_last_index; }
 const char* ipcfp_version(void) {
     return "ipcfp-b200 0.2 (sm_90a): k_verify_cids k_hash_batch k_build_index sort_by_cid k_pass1_stage k_pass2 k_amt_dense k_amt_expand k_dedup "
-           "k_storage_proofs k_read_slots k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* k_rb_* k_car_* | sharded: k_xb_* k_exec_claim_seg "
+           "k_storage_proofs k_read_slots k_path_* k_verify_events k_verify_storage k_scan k_witness_copy k_witness_emit k_union_mark k_json_* k_jp_* k_rj_* k_rb_* k_car_* | sharded: k_xb_* k_exec_claim_seg "
            "k_exec_mark_dups k_select_positions k_fetch_positions k_part_pack k_merge_* (NCCL via dlopen)";
 }
 uint64_t ipcfp_kernel_launch_count(void) { return g_launches.load(); }
@@ -365,6 +365,23 @@ ipcfp_status ipcfp_generate_storage_proofs(ipcfp_store* s, const ipcfp_tipset_de
     });
 }
 void ipcfp_storage_result_free(ipcfp_storage_result* r) { if (r) storage_result_free(r); }
+
+ipcfp_status ipcfp_generate_storage_path_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_path* paths, uint64_t n, uint32_t flags,
+                                                         ipcfp_path_result** out) {
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_storage_path_proofs(st, td, paths, n, flags); });
+}
+ipcfp_status ipcfp_plan_fetch_storage_paths_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_storage_path* paths, uint64_t n, uint32_t flags,
+                                                     ipcfp_fetch_plan** out) {
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        plan_flags_check(flags);
+        return make_plan([&](FetchPlan& p) { plan_fetch_storage_paths(st, td, paths, n, p); });
+    });
+}
+ipcfp_status ipcfp_verify_storage_paths(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n_proofs,
+                                        const ipcfp_storage_path* paths, uint64_t n_paths, ipcfp_path_result** out) {
+    return produce(s != nullptr, out, [&] { return verify_storage_paths(store_of(s), t, proofs, n_proofs, paths, n_paths); });
+}
+void ipcfp_path_result_free(ipcfp_path_result* r) { if (r) path_result_free(r); }
 
 // generate_proof_bundle (proofs/generator.rs:25-95): the tipset uploaded, then the resident call's body without flags
 ipcfp_status ipcfp_generate_proof_bundle(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_spec* sspecs, uint64_t n_sspecs,

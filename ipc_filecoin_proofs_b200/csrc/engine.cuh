@@ -263,6 +263,14 @@ void plan_fetch(Store* s, TipsetDev& td, const ipcfp_storage_spec* sspecs, uint6
 // ipcfp_plan_fetch_message_log_resident: one round for generate_message_log_proof (filter null: the all-wildcard filter)
 void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, const ipcfp_log_filter* filter, FetchPlan& out);
 
+// storage_path.cu — ipcfp_generate_storage_path_proofs_resident, ipcfp_plan_fetch_storage_paths_resident, ipcfp_verify_storage_paths
+// (DESIGN.md §3, "Storage paths")
+ipcfp_path_result* generate_storage_path_proofs(Store* s, TipsetDev& td, const ipcfp_storage_path* paths, uint64_t n, uint32_t flags);
+void plan_fetch_storage_paths(Store* s, TipsetDev& td, const ipcfp_storage_path* paths, uint64_t n, FetchPlan& out);
+ipcfp_path_result* verify_storage_paths(Store* s, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n_proofs,
+                                        const ipcfp_storage_path* paths, uint64_t n_paths);
+void path_result_free(ipcfp_path_result* r);
+
 // parallel.cu — in-library cross-shard protocol over NCCL (one process per GPU)
 void comm_unique_id(uint8_t* id128);
 Comm* comm_init(const uint8_t* id128, uint32_t world, uint32_t rank, int device);
@@ -331,6 +339,13 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
                                               bool by_ref = false);
 void storage_result_free(ipcfp_storage_result* r);
 const WitnessOut& storage_result_witness(const ipcfp_storage_result* r);
+// generate_storage_proofs' second half: the result of n proofs already on the device in spec order (d_out, their recorder lists d_rec /
+// d_recn, the witness bitmap they marked): copies, one materialize_witness, the per-spec lists. Its two host synchronisations are
+// materialize_witness's, then one at the end; times from s->ev[EV_BEGIN] to s->ev[EV_STORAGE_END].
+ipcfp_storage_result* storage_result_finish(Store* s, const ipcfp_storage_proof* d_out, const uint32_t* d_rec, const uint32_t* d_recn, const uint32_t* wbits,
+                                            uint64_t n, bool by_ref);
+// a storage failure's error key → the Error it throws (status by code, index from the key)
+[[noreturn]] void throw_storage_error(uint64_t key);
 
 // witness.cu — materialise a witness bitmap into a sorted ipcfp_witness (host, pinned)
 struct WitnessOut {

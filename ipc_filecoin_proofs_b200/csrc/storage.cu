@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(128) k_read_slots(SlotArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------ host
-static void throw_storage_error(uint64_t key) {
+void throw_storage_error(uint64_t key) {
     uint32_t code = (uint32_t)(key >> 8) & 0xff, detail = (uint32_t)key & 0xff;
     uint64_t index = (key >> 16) & 0xFFFFFFFFFFull;
     switch (code) {
@@ -172,16 +172,23 @@ ipcfp_storage_result* generate_storage_proofs(Store* s, const uint8_t* child_cid
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
     if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_storage_error(hw[DW_ERR]);
+    return storage_result_finish(s, d_out.p, d_rec.p, d_recn.p, wbits.p, n, by_ref);
+}
+// The result of n proofs on the device in spec order, with their recorder lists and the witness bitmap they marked: the proofs copied
+// back, the witness materialised, the per-spec lists. Timed from s->ev[EV_BEGIN].
+ipcfp_storage_result* storage_result_finish(Store* s, const ipcfp_storage_proof* d_out, const uint32_t* d_rec, const uint32_t* d_recn, const uint32_t* wbits,
+                                            uint64_t n, bool by_ref) {
+    cudaStream_t st = s->stream;
     std::unique_ptr<StorageResultBox> box(new StorageResultBox());
     memset(&box->r, 0, sizeof box->r);
     box->proofs = PinnedArray(s->pool, (n + 1) * sizeof(ipcfp_storage_proof));
     PinnedArray rec(s->pool, (n * REC_CAP + 8) * 4), recn(s->pool, (n + 8) * 4);
     if (n) {
-        IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_out.p, n * sizeof(ipcfp_storage_proof), cudaMemcpyDeviceToHost, st));
-        IPCFP_CUDA(cudaMemcpyAsync(rec.p, d_rec.p, n * REC_CAP * 4, cudaMemcpyDeviceToHost, st));
-        IPCFP_CUDA(cudaMemcpyAsync(recn.p, d_recn.p, n * 4, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaMemcpyAsync(box->proofs.p, d_out, n * sizeof(ipcfp_storage_proof), cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaMemcpyAsync(rec.p, d_rec, n * REC_CAP * 4, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaMemcpyAsync(recn.p, d_recn, n * 4, cudaMemcpyDeviceToHost, st));
     }
-    materialize_witness(s, wbits.p, box->wit, by_ref);
+    materialize_witness(s, wbits, box->wit, by_ref);
     // per-spec Vec<ProofBlock>: map recorded block indices to positions in the sorted union
     PinnedArray& sorted_idx = box->wit.sorted_idx;
     IPCFP_CUDA(cudaEventRecord(s->ev[EV_STORAGE_END], st));
