@@ -592,6 +592,9 @@ ipcfp_status ipcfp_generate_storage_path_proofs_resident(ipcfp_store* s, ipcfp_t
  * and header words taken from the proofs themselves; each (actor_id, slot) must have a proof in the list that verifies (the first in
  * (actor_id, slot) order when several do). The result's paths[i].valid, status and value are the path's verdict, `specs` the expanded
  * specs derived, `storage` NULL. A proof whose value was changed, a data slot left out or a length word that lies makes the path invalid.
+ * A path that is not valid still gets a status and value, read as follows where a spec has no proof that verifies: a length word does
+ * not make the index out of range, a bytes / string header reads as zero (no data slots, an empty value), and any other word is that
+ * of the first proof in the list with the spec's (actor_id, slot), or zero when there is none. Such a value is not proven.
  * Refusals are the generate call's. *out is released with ipcfp_path_result_free. */
 ipcfp_status ipcfp_verify_storage_paths(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_storage_proof* proofs, uint64_t n_proofs,
                                         const ipcfp_storage_path* paths, uint64_t n_paths, ipcfp_path_result** out);

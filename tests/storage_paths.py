@@ -86,6 +86,109 @@ def expand(path, read):
     return [(path.actor_id, s) for s in specs], status, value, slot, off
 
 
+# ------------------------------------------------------------------ random paths and hand-picked edges (the host campaign and the GPU worlds)
+KEY_EDGES = (0, 1, 31, 32, 33, 103, 104, 105, 135, 136, 137, 239, 240, 241, 375, 376, 377, A.PATH_MAX_KEY - 1, A.PATH_MAX_KEY)
+U64_EDGES = (0, 1, 2, 31, 32, 33, 2 ** 32 - 1, 2 ** 32, 2 ** 63, 2 ** 64 - 1)
+
+
+def random_u256(rng):
+    return rng.choice([rng.randrange(16), M - 1 - rng.randrange(16), rng.randrange(M), (1 << rng.randrange(256)) - rng.randrange(3)]) % M
+
+
+def step(rng):
+    op = rng.choice((A.PATH_MAPPING, A.PATH_MAPPING, A.PATH_ARRAY, A.PATH_STATIC, A.PATH_FIELD))
+    if op == A.PATH_MAPPING:
+        n = rng.choice(KEY_EDGES + (32, 32, 20, rng.randrange(A.PATH_MAX_KEY + 1)))
+        return (op, rng.randbytes(n), 0, 0, 0)
+    index = rng.choice(U64_EDGES + (rng.randrange(100), rng.randrange(2 ** 64)))
+    if op == A.PATH_FIELD:
+        return (op, b"", index, 0, 0)
+    es = rng.choice((1, 1, 1, 2, 3, 7, 2 ** 32 - 1))
+    eb = rng.choice((0, 0, 1, 2, 3, 8, 16, 20, 31, 32))
+    return (op, b"", index, es, eb)
+
+
+def header(rng):
+    """a bytes / string header word of every form"""
+    kind = rng.randrange(7)
+    if kind == 0:
+        return bytes(31) + bytes([2 * rng.randrange(32)])                        # short
+    if kind == 1:
+        return rng.randbytes(31) + bytes([2 * rng.randrange(32, 128)])           # short, BAD_BYTES
+    if kind == 2:
+        return b32(2 * rng.choice((32, 33, 63, 64, 65, rng.randrange(32, A.PATH_MAX_BYTES + 1), A.PATH_MAX_BYTES)) + 1)   # long
+    if kind == 3:
+        return b32(2 * rng.randrange(32) + 1)                                    # long, BAD_BYTES
+    if kind == 4:
+        return b32(2 * rng.choice((A.PATH_MAX_BYTES + 1, rng.randrange(A.PATH_MAX_BYTES + 1, 2 ** 64), rng.randrange(M // 2))) + 1)   # TOO_LONG
+    if kind == 5:
+        return rng.randbytes(32)
+    return bytes(32)
+
+
+def case(rng, storage, actors=None):
+    """One random path; its words go into storage. Without actors the path's actor ID is random and storage is one {slot: word};
+    with actors (a sequence of IDs) the actor is drawn from them and storage is {actor: {slot: word}}. The random-number calls
+    without actors are those of the host campaign's seeds, so a seed always gives the same paths."""
+    steps = tuple(step(rng) for _ in range(rng.choice((0, 1, 2, 3, 4, 6, A.PATH_MAX_STEPS))))
+    is_bytes = rng.random() < 0.5
+    actor = rng.randrange(2 ** 64) if actors is None else rng.choice(actors)
+    if is_bytes:
+        p = StoragePath(actor, random_u256(rng), steps, A.PATH_BYTES, 0)
+    else:
+        p = StoragePath(actor, random_u256(rng), steps, A.PATH_WORDS, rng.choice((1, 1, 2, 3, A.PATH_MAX_WORDS)))
+    st = storage if actors is None else storage[actor]
+    lengths, values, slot, _ = derive(p)
+    arrays = [s for s in steps if s[0] == A.PATH_ARRAY]
+    for ls, s in zip(lengths, arrays):
+        if rng.random() < 0.8:
+            st[ls] = rng.choice((b32(s[2] + 1 + rng.randrange(5)), b32(s[2]), b32(max(s[2] - 1, 0)), rng.randbytes(32)))
+    if p.kind == A.PATH_WORDS:
+        for v in values:
+            if rng.random() < 0.7:
+                st[v] = rng.randbytes(32)
+    else:
+        st[slot] = header(rng)
+        base = u256(keccak256(slot))
+        for j in range(A.PATH_MAX_BYTES // 32 + 1):
+            if rng.random() < 0.9:
+                st[b32(base + j)] = rng.randbytes(32)
+    return p
+
+
+EDGE_ACTOR = 7
+
+
+def edges():
+    """hand-picked paths: carries out of the top byte, the caps, every header form on one slot each (actor EDGE_ACTOR)"""
+    top = M - 1
+    P = lambda base, *steps, kind=A.PATH_WORDS, n=1: StoragePath(EDGE_ACTOR, base, steps, kind, n)
+    paths = [P(top, (A.PATH_FIELD, b"", 1, 0, 0)), P(top, (A.PATH_FIELD, b"", 2 ** 64 - 1, 0, 0), n=A.PATH_MAX_WORDS),
+             P(top - 5, (A.PATH_STATIC, b"", 2 ** 64 - 1, 2 ** 32 - 1, 0)), P(0, (A.PATH_STATIC, b"", 2 ** 64 - 1, 1, 1)),
+             P(3, (A.PATH_ARRAY, b"", 2 ** 64 - 1, 2 ** 32 - 1, 0), (A.PATH_FIELD, b"", 2 ** 64 - 1, 0, 0))]
+    paths += [P(5, (A.PATH_MAPPING, (bytes(range(256)) * 4)[:n], 0, 0, 0)) for n in KEY_EDGES]
+    paths += [P(k, (A.PATH_ARRAY, b"", i, 1, eb)) for k, (i, eb) in enumerate((i, eb) for eb in range(1, 33) for i in (0, 31, 32, 63))]
+    paths += [P(9000 + k, kind=A.PATH_BYTES) for k in range(12)]
+    return paths
+
+
+def edge_storage(paths):
+    """{slot: word} for edges(): the twelve header forms with every data slot written, every array length 2^64 - 1"""
+    storage = {}
+    hdr = [bytes(32), bytes(31) + b"\x3e", bytes(31) + b"\x40", b32(2 * 32 + 1), b32(2 * 31 + 1), b32(1),
+           b32(2 * A.PATH_MAX_BYTES + 1), b32(2 * (A.PATH_MAX_BYTES + 1) + 1), b"\xff" * 32, b32(2 * 33 + 1),
+           b32(2 * 65 + 1), b"\xff" * 31 + b"\xfe"]
+    for k, p in enumerate(paths[-12:]):
+        storage[p.base_slot] = hdr[k]
+        base = u256(keccak256(p.base_slot))
+        for j in range(A.PATH_MAX_BYTES // 32 + 1):
+            storage[b32(base + j)] = bytes([j % 256]) * 32
+    for p in paths[:-12]:
+        for ls in derive(p)[0]:
+            storage[ls] = b32(2 ** 64 - 1)
+    return storage
+
+
 def encode_string(slot, s):
     """{slot: word} of a bytes / string value stored at slot"""
     s = bytes(s)
