@@ -84,11 +84,6 @@ struct BundleBox {
         for (auto* e : ev) event_result_free(e);
     }
 };
-struct TimingEvent {
-    cudaEvent_t e = nullptr;
-    TimingEvent() { IPCFP_CUDA(cudaEventCreate(&e)); }
-    ~TimingEvent() { if (e) cudaEventDestroy(e); }
-};
 
 struct FetchPlanBox {
     ipcfp_fetch_plan r;   // must stay first
@@ -128,8 +123,8 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
     st->use();
     const bool by_ref = (flags & IPCFP_WITNESS_BY_REFERENCE) != 0;
     cudaStream_t stream = st->stream;
-    TimingEvent t0, t1, j0, j1;
-    IPCFP_CUDA(cudaEventRecord(t0.e, stream));
+    Event t0, t1, j0, j1;
+    IPCFP_CUDA(cudaEventRecord(t0, stream));
     std::unique_ptr<BundleBox> box(new BundleBox());
     memset(&box->r, 0, sizeof box->r);
     std::vector<const WitnessOut*> lists;
@@ -145,7 +140,7 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
     witness_union(st, lists, box->wit, by_ref);
 
     if (flags & IPCFP_RESULT_JSON) {
-        IPCFP_CUDA(cudaEventRecord(j0.e, stream));
+        IPCFP_CUDA(cudaEventRecord(j0, stream));
         // the records' inputs in ONE upload: storage proofs, every spec's EventProofs with their topics / data offsets rebased into one
         // concatenated data blob, the tipset CIDs the records repeat
         const uint64_t ns = box->r.storage ? box->r.storage->n_proofs : 0;
@@ -177,18 +172,17 @@ static ipcfp_bundle* generate_proof_bundle(Store* st, TipsetDev& td, const ipcfp
                              box->wit.cids_dev.p, box->wit.idx_dev.p, box->wit.n, td.parent_epoch, td.child_epoch, td.n_parents,
                              d.p + o_cids + 76, d.p + o_cids, d.p + o_cids + 38};
         box->r.json_len = render_unified_json(st, ji, box->json);
-        IPCFP_CUDA(cudaEventRecord(j1.e, stream));
+        IPCFP_CUDA(cudaEventRecord(j1, stream));
     }
-    IPCFP_CUDA(cudaEventRecord(t1.e, stream));
+    IPCFP_CUDA(cudaEventRecord(t1, stream));
     IPCFP_CUDA(cudaStreamSynchronize(stream));
     box->r.n_event_results = box->ev.size();
     box->r.events = box->ev.data();
     box->wit.fill(box->r.witness);
-    float ms;
-    IPCFP_CUDA(cudaEventElapsedTime(&ms, t0.e, t1.e)); box->r.ms_total = ms;
+    box->r.ms_total = elapsed_ms(t0, t1);
     if (flags & IPCFP_RESULT_JSON) {
         box->r.json = box->json.as<char>();
-        IPCFP_CUDA(cudaEventElapsedTime(&ms, j0.e, j1.e)); box->r.ms_json = ms;
+        box->r.ms_json = elapsed_ms(j0, j1);
     }
     return &box.release()->r;
 }

@@ -5,7 +5,7 @@
 //
 // Device path, all on the store's stream unless noted:
 //   header                 decoded on the host (car_header, the host parser's own rule)
-//   H2D of the CAR         into arena + 16 in CAR_CHUNK pieces on a copy stream; chunk k is marked once chunk k + 1 has landed
+//   H2D of the CAR         into the store's block bytes in CAR_CHUNK pieces on a copy stream; chunk k is marked once chunk k + 1 has landed
 //                          (a candidate reads 5 bytes before it and 6 from it)
 //   k_car_mark             one thread per 32 bytes: bit s of the bitmap = a candidate CID starts at s (car_items.cuh)
 //   bitmap_count64         the candidate count
@@ -14,11 +14,10 @@
 //   k_car_links            one thread per (candidate, option): where its section ends, as a link to the next candidate; the head
 //   ── host synchronisation 2: the links. The host follows them from the head (a few words per section, no CAR byte) to the payload's end
 //   k_car_gather           one thread per section of the chain: offset, length, CID
-//   store_index + store_verify_all (store.cu)
+//   store_finish (store.cu)
 // The scratch is sized by the candidate count and released before the index is built; when it cannot be allocated, the CAR goes through
 // the host parser like any CAR the device path does not accept.
 #include <algorithm>
-#include <chrono>
 #include <cstring>
 #include <vector>
 
@@ -34,7 +33,7 @@ struct CarMeta {
     unsigned long long n;      // candidates
     unsigned long long head;   // the link to the section at the header's end
 };
-static_assert(sizeof(CarMeta) <= HW_CAR_META_WORDS * 8, "the meta words fit their host words (HW_CAR_META)");
+static_assert(sizeof(CarMeta) <= HW_PARSE_META_WORDS * 8, "the meta words fit their host words (HW_PARSE_META)");
 
 // words [w0, w1) of the bitmap over the payload t[0, len); sections start at or after `first`
 __global__ void __launch_bounds__(256) k_car_mark(const uint8_t* __restrict__ t, uint64_t len, uint64_t first, uint64_t w0, uint64_t w1,
@@ -72,20 +71,7 @@ __global__ void k_car_gather(const uint8_t* __restrict__ t, const uint64_t* __re
     for (uint32_t b = 0; b < IPCFP_CID_LEN; b++) cids[IPCFP_CID_LEN * k + b] = c[b];
 }
 
-using Clock = std::chrono::steady_clock;
-static float ms_since(Clock::time_point t0) { return std::chrono::duration<float, std::milli>(Clock::now() - t0).count(); }
-
 static const uint64_t CAR_CHUNK = 64ull << 20;   // the H2D piece: ipcfp_store_create's chunk (a multiple of 32, so chunks hold whole bitmap words)
-
-struct Events {
-    std::vector<cudaEvent_t> e;
-    cudaEvent_t add(unsigned flags) {
-        e.push_back(nullptr);
-        IPCFP_CUDA(cudaEventCreateWithFlags(&e.back(), flags));
-        return e.back();
-    }
-    ~Events() { for (auto x : e) if (x) cudaEventDestroy(x); }
-};
 
 // b = count elements on `st`; false (nothing allocated) when the device is out of memory
 template <class T> static bool try_alloc(AsyncBuf<T>& b, size_t count, cudaStream_t st) {
@@ -113,22 +99,17 @@ static bool walk(const uint64_t* links, uint64_t n, uint64_t head, std::vector<u
 static void blocks_on_device(Store* s, const uint8_t* car, uint64_t len, uint64_t first, uint32_t flags, ipcfp_store_json_info& info,
                              Clock::time_point t0) {
     cudaStream_t st = s->stream;
-    store_alloc_arena(s, len);
-    uint8_t* t = s->arena.p + 16;
-    IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, 16, st));
-    IPCFP_CUDA(cudaMemsetAsync(t + len, 0, 32 + 512, st));
-    cudaStream_t st2;
-    IPCFP_CUDA(cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking));
-    struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); } } sg{st2};
-    Events ev;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timed;   // around every parse kernel
+    uint8_t* t = store_alloc_arena(s, len, false);
+    ChunkedCopy copy;
+    std::vector<Event> timed;   // a pair around every parse kernel
     auto timed_launch = [&](auto enqueue) {
-        timed.emplace_back(ev.add(cudaEventDefault), ev.add(cudaEventDefault));
-        IPCFP_CUDA(cudaEventRecord(timed.back().first, st));
+        timed.emplace_back();
+        IPCFP_CUDA(cudaEventRecord(timed.back(), st));
         enqueue();
-        IPCFP_CUDA(cudaEventRecord(timed.back().second, st));
+        timed.emplace_back();
+        IPCFP_CUDA(cudaEventRecord(timed.back(), st));
     };
-    DevBuf<uint8_t> cids_dev, sort_ws;
+    DevBuf<uint8_t> cids_dev;
     bool accepted = false;
     {   // the scratch of the device parse: gone before the index is built
         const uint64_t nwords = (len + 31) / 32;
@@ -145,16 +126,13 @@ static void blocks_on_device(Store* s, const uint8_t* car, uint64_t len, uint64_
         const uint64_t n_chunks = div_up(len, CAR_CHUNK);
         cudaEvent_t landed = nullptr;
         for (uint64_t k = 0; k < n_chunks; k++) {
-            const uint64_t c0 = k * CAR_CHUNK, c1 = std::min(len, c0 + CAR_CHUNK);
-            IPCFP_CUDA(cudaMemcpyAsync(t + c0, car + c0, c1 - c0, cudaMemcpyHostToDevice, st2));
-            landed = ev.add(cudaEventDisableTiming);
-            IPCFP_CUDA(cudaEventRecord(landed, st2));
+            landed = copy.copy(t, car, k * CAR_CHUNK, std::min(len, (k + 1) * CAR_CHUNK));
             if (!room) continue;
             if (k) mark(k - 1, landed);
             if (k + 1 == n_chunks) mark(k, landed);
         }
         IPCFP_CUDA(cudaStreamWaitEvent(st, landed, 0));   // the whole CAR is in the arena, whichever path reads it
-        uint64_t* hm = s->host_words.p + HW_CAR_META;
+        uint64_t* hm = s->host_words.p + HW_PARSE_META;
         uint64_t n = 0;
         if (room) {
             timed_launch([&] { bitmap_count64(bits.p, len, (uint64_t*)&meta.p->n, word_prefix.p, scratch.p, st); });
@@ -221,43 +199,20 @@ static void blocks_on_device(Store* s, const uint8_t* car, uint64_t len, uint64_
             first_prefix = w.cids;
         }
     }
-    IPCFP_CUDA(cudaMemsetAsync(s->table.p, 0, s->table.n * 8, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));   // the host arrays go away with `keep`; the parse's times are final
     info.ms_parse = ms_since(t0);
-    if (accepted) {
-        for (auto& e : timed) {
-            float ms;
-            IPCFP_CUDA(cudaEventElapsedTime(&ms, e.first, e.second));
-            info.ms_kernels += ms;
-        }
-    }
-    store_index(s, cids_dev.p, pb ? pb->blocks.cids : nullptr, first_prefix, sort_ws);
-    if (flags & IPCFP_STORE_VERIFY_CIDS) store_verify_all(s);
-    else IPCFP_CUDA(cudaStreamSynchronize(st));
+    if (accepted)
+        for (size_t k = 0; k < timed.size(); k += 2) info.ms_kernels += elapsed_ms(timed[k], timed[k + 1]);
+    store_finish(s, cids_dev.p, pb ? pb->blocks.cids : nullptr, first_prefix, flags);
 }
 
 Store* store_create_car(const uint8_t* car, uint64_t len, int device, uint32_t flags, ipcfp_store_json_info& info) {
-    memset(&info, 0, sizeof info);
-    const Clock::time_point t0 = Clock::now();
-    // the device path needs a device and a header; everything else (and every failure) is the host parser's to report
+    // the device path needs a header; everything else (and every failure) is the host parser's to report
     uint64_t first = 0;
-    if (car && car_header(car, len, first)) {
-        bool have_device = true;
-        try { check_device(device); }
-        catch (const Error&) { have_device = false; }
-        if (have_device) {
-            std::unique_ptr<Store> s(store_shell(device));
-            blocks_on_device(s.get(), car, len, first, flags, info, t0);
-            return s.release();
-        }
-    }
-    ipcfp_parsed_blocks* pb = nullptr;
-    const ipcfp_status st = ipcfp_blocks_from_car(car, len, &pb);
-    if (st != IPCFP_OK) throw Error(st, ipcfp_last_error(), ipcfp_last_error_index());
-    std::unique_ptr<ipcfp_parsed_blocks, void (*)(ipcfp_parsed_blocks*)> keep(pb, ipcfp_parsed_blocks_free);
-    info.ms_parse = ms_since(t0);
-    const ipcfp_witness& w = pb->blocks;
-    return store_create(w.cids, w.offsets, w.lengths, car, len, w.n_blocks, device, flags);
+    return store_create_parsed(
+        device, flags, info, car && car_header(car, len, first),
+        [&](Store* s, Clock::time_point t0) { blocks_on_device(s, car, len, first, flags, info, t0); return true; },
+        [&](ipcfp_parsed_blocks** pb) { return ipcfp_blocks_from_car(car, len, pb); }, car);
 }
 
 }  // namespace ipcfp

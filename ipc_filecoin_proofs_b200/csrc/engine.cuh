@@ -1,6 +1,8 @@
 // engine.cuh — host-side objects of the engine (C++17), shared by the translation units.
 #pragma once
 #include <array>
+#include <chrono>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -49,6 +51,45 @@ struct PinnedArray {
     template <class T> T* as() const { return (T*)p; }
 };
 
+// ---- Timing and copy helpers of the host code
+using Clock = std::chrono::steady_clock;
+inline float ms_since(Clock::time_point t0) { return std::chrono::duration<float, std::milli>(Clock::now() - t0).count(); }
+
+// a CUDA event that lives as long as its owner; converts to cudaEvent_t
+struct Event {
+    cudaEvent_t e = nullptr;
+    explicit Event(unsigned flags = cudaEventDefault) { IPCFP_CUDA(cudaEventCreateWithFlags(&e, flags)); }
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    Event(Event&& o) noexcept : e(o.e) { o.e = nullptr; }
+    ~Event() { if (e) cudaEventDestroy(e); }
+    operator cudaEvent_t() const { return e; }
+};
+inline float elapsed_ms(cudaEvent_t a, cudaEvent_t b) {
+    float ms = 0.f;
+    IPCFP_CUDA(cudaEventElapsedTime(&ms, a, b));
+    return ms;
+}
+
+// H2D copies of byte ranges on a stream of their own, one event per range, so that work on another stream can start on range k while
+// the later ranges are still on the wire. The stream is drained before it is destroyed: the source is read for this object's lifetime.
+struct ChunkedCopy {
+    cudaStream_t st = nullptr;
+    std::vector<Event> landed;
+    ChunkedCopy() { IPCFP_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); }
+    ChunkedCopy(const ChunkedCopy&) = delete;
+    ChunkedCopy& operator=(const ChunkedCopy&) = delete;
+    ~ChunkedCopy() { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
+    // dst[byte0, byte1) = src[byte0, byte1); returns the range's event
+    cudaEvent_t copy(uint8_t* dst, const uint8_t* src, uint64_t byte0, uint64_t byte1) {
+        if (byte1 > byte0) IPCFP_CUDA(cudaMemcpyAsync(dst + byte0, src + byte0, byte1 - byte0, cudaMemcpyHostToDevice, st));
+        landed.emplace_back(cudaEventDisableTiming);
+        IPCFP_CUDA(cudaEventRecord(landed.back(), st));
+        return landed.back();
+    }
+    void wait(cudaStream_t consumer, size_t k) const { IPCFP_CUDA(cudaStreamWaitEvent(consumer, landed[k], 0)); }
+};
+
 // ---- The store's counter words and events
 // dev_words: one slot per counter or fault word a kernel writes. host_words[0, DW_COUNT) mirror them at the same index
 // (publish_words(s, first, n) with first + n <= DW_COUNT); the host-only regions behind the mirror receive other device data.
@@ -81,10 +122,7 @@ constexpr uint32_t HW_ANY_SKIP_WORDS = 2;                                     //
 constexpr uint32_t HW_PARKED_KEY_WORDS = 1;                                   // verify.cu: the TxMeta check's error key
 constexpr uint32_t HW_EXCHANGE_WORDS = 2;                                     // parallel.cu: exchange overflow flag, n_exec
 constexpr uint32_t HW_UNION_PARTS_WORDS = 2 * MAX_WORLD;                      // parallel.cu: [partition size, overflow] per rank
-constexpr uint32_t HW_JP_META_WORDS = 17;                                     // json_parse.cu: JpMeta
-constexpr uint32_t HW_RJ_META_WORDS = 2;                                      // rpc_json.cu: RjMeta
-constexpr uint32_t HW_RB_META_WORDS = 4;                                      // rpc_blocks.cu: RbMeta
-constexpr uint32_t HW_CAR_META_WORDS = 2;                                     // car.cu: CarMeta
+constexpr uint32_t HW_PARSE_META_WORDS = 17;                                  // the meta of a device parse: JpMeta (json_parse.cu), the largest
 enum HostWord : uint32_t {
     HW_PROLOGUE = DW_COUNT,
     HW_JSON_TOTALS = HW_PROLOGUE + HW_PROLOGUE_WORDS,
@@ -92,11 +130,9 @@ enum HostWord : uint32_t {
     HW_PARKED_KEY = HW_ANY_SKIP + HW_ANY_SKIP_WORDS,
     HW_EXCH_OVERFLOW = HW_PARKED_KEY + HW_PARKED_KEY_WORDS, HW_EXCH_N_EXEC = HW_EXCH_OVERFLOW + 1,
     HW_UNION_PARTS = HW_EXCH_OVERFLOW + HW_EXCHANGE_WORDS,
-    HW_JP_META = HW_UNION_PARTS + HW_UNION_PARTS_WORDS,
-    HW_RJ_META = HW_JP_META + HW_JP_META_WORDS,
-    HW_RB_META = HW_RJ_META + HW_RJ_META_WORDS,
-    HW_CAR_META = HW_RB_META + HW_RB_META_WORDS,
-    HW_END = HW_CAR_META + HW_CAR_META_WORDS
+    HW_PARSE_META = HW_UNION_PARTS + HW_UNION_PARTS_WORDS,   // one parse at a time per store: each parses on a fresh store_shell, or
+                                                             // (rpc_json.cu) inside a call on the caller's store, and those are serialised
+    HW_END = HW_PARSE_META + HW_PARSE_META_WORDS
 };
 constexpr uint32_t HW_COUNT = 1024;
 static_assert(DW_JSON_TOTAL2 < DW_COUNT, "a mirrored slot never reaches a host-only region (they start at DW_COUNT)");
@@ -179,15 +215,26 @@ void hash_batch(int which, const uint8_t* blob, uint64_t blob_size, const uint64
                 uint8_t* out);
 void mapping_slots(const uint8_t* keys32, const uint64_t* slot_indices, uint64_t n, int device, uint8_t* out);
 void check_device(int device);
-// the pieces of store_create, for a caller that writes the blocks on the device itself (json_parse.cu):
-//   store_shell → store_alloc_blocks → (fill cids_dev, offsets, lengths, arena + 16) → store_index → store_verify_all
+// the pieces of store_create, for a caller that writes the blocks on the device itself:
+//   store_shell → store_alloc_blocks → (fill cids_dev, offsets, lengths and the blocks) → store_finish
 Store* store_shell(int device);   // stream, events, counters; no block yet
-void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev);
+// n blocks of blob_size bytes: the arena with its pads zeroed (zero_blocks: all of it), the per-block arrays, cids_dev (n*38) and the
+// zeroed hash table, on the store's stream. Returns where block bytes go: offsets index from there.
+uint8_t* store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev, bool zero_blocks);
 // … its two halves, for a caller that fills the arena before it knows n (car.cu): the arena, then the per-block arrays and the index
-void store_alloc_arena(Store* s, uint64_t blob_size);
+uint8_t* store_alloc_arena(Store* s, uint64_t blob_size, bool zero_blocks);
 void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev);
-void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws);
-void store_verify_all(Store* s);
+// the index of the blocks in place, then the CID check of IPCFP_STORE_VERIFY_CIDS in `flags` (first_bad) or a plain synchronisation.
+// cids_host: the CIDs on the host, or null; first_prefix: the first CID's 6 prefix bytes (host). blob: the block bytes still landing,
+// blocks [bounds[k], bounds[k + 1]) in its range k (null: all on the device already).
+void store_finish(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, uint32_t flags,
+                  const ChunkedCopy* blob = nullptr, const std::vector<uint64_t>& bounds = {});
+// A store from input that has a host parser: on_device(store, t0) on a fresh store when try_device and the device is there (false: it
+// declined, and the store is dropped); otherwise host_parse's blocks through store_create, over `blob` (null: the parsed blocks' own).
+// info is cleared first, and again when the device path declines; the host path sets its ms_parse.
+Store* store_create_parsed(int device, uint32_t flags, ipcfp_store_json_info& info, bool try_device,
+                           const std::function<bool(Store*, Clock::time_point)>& on_device,
+                           const std::function<ipcfp_status(ipcfp_parsed_blocks**)>& host_parse, const uint8_t* blob);
 // rpc_blocks.cu — ipcfp_store_create_rpc_json (info: which path ran, its times)
 Store* store_create_rpc_json(const uint8_t* cids, uint64_t n_blocks, const char* const* texts, const uint64_t* text_lens, uint64_t n_texts, int device,
                              uint32_t flags, ipcfp_store_json_info& info);

@@ -14,15 +14,13 @@
 //   k_jp_proofs            one thread per proof: the PODs and the topic / data bytes
 //   trust callbacks (host); if a trusted proof is left:
 //   k_jp_blocks            one warp per block: CID bytes, offset, length, base64 decoded straight into the new store's arena
-//   store_index + store_verify_all (store.cu; host synchronisations of the class check and of the CID check)
+//   store_finish (store.cu; host synchronisations of the class check and of the CID check)
 //   verify_storage_proofs_dev / verify_event_proofs_dev (verify.cu)
-#include <algorithm>
-#include <chrono>
 #include <cstring>
 
 #include "engine.cuh"
 #include "json_parse_items.cuh"
-#include "prims.cuh"
+#include "text_scan.cuh"
 
 namespace ipcfp {
 
@@ -34,7 +32,7 @@ struct JpMeta {
     unsigned long long witness_bytes;
     unsigned long long e_total, b_total;
 };
-static_assert(sizeof(JpMeta) <= HW_JP_META_WORDS * 8, "the meta words fit their host words (HW_JP_META)");
+static_assert(sizeof(JpMeta) <= HW_PARSE_META_WORDS * 8, "the meta words fit their host words (HW_PARSE_META)");
 
 __global__ void __launch_bounds__(256) k_jp_mark(const char* __restrict__ t, uint64_t len, uint32_t* bits, uint64_t nwords) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -135,9 +133,6 @@ struct VerdictBox {
     ~VerdictBox() { if (pb) ipcfp_parsed_bundle_free(pb); }
 };
 
-using Clock = std::chrono::steady_clock;
-static float ms_since(Clock::time_point t0) { return std::chrono::duration<float, std::milli>(Clock::now() - t0).count(); }
-
 // verify_trust_anchors / verify_trust_anchor of the bundle: each callback at most once
 struct Trust { bool child = false, parent = false; };
 static Trust ask_trust(const ipcfp_tipset_desc& t, uint64_t nS, uint64_t nE, ipcfp_trusted_parent_ts_fn trusted_parent,
@@ -199,26 +194,17 @@ static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, in
     catch (const Error&) { return false; }   // the host path meets the same failure where the composition does
     std::unique_ptr<Store> s(store_shell(device));
     cudaStream_t st = s->stream;
-    const uint64_t nwords = (len + 31) / 32, cap = len / JP_MIN_RECORD + 1;
-    AsyncBuf<char> d_text(len + JP_PAD, st);
-    AsyncBuf<uint32_t> bits(nwords + 8, st), pos(len / 8 + 8, st), elen(cap + 1, st), blen(cap + 1, st);
-    AsyncBuf<uint64_t> word_prefix(nwords + 8, st), eoff(cap + 1, st), boff(cap + 1, st),
-        scratch(scan_scratch_elems(std::max(nwords, cap)) + 8, st);
-    AsyncBuf<JpMeta> meta(1, st);
-    IPCFP_CUDA(cudaMemcpyAsync(d_text.p, json, len, cudaMemcpyHostToDevice, st));
-    IPCFP_CUDA(cudaMemsetAsync(d_text.p + len, 0, JP_PAD, st));
-    IPCFP_CUDA(cudaMemsetAsync(meta.p, 0xff, sizeof(JpMeta), st));
-    IPCFP_CUDA(cudaMemsetAsync(&meta.p->witness_bytes, 0, 8, st));
-    k_jp_mark<<<div_up(nwords, 256), 256, 0, st>>>(d_text.p, len, bits.p, nwords); IPCFP_LAUNCH_CHECK();
-    bitmap_to_indices(bits.p, len, pos.p, (uint64_t*)&meta.p->n, word_prefix.p, scratch.p, st);
-    k_jp_records<<<div_up(cap * 32, 128), 128, 0, st>>>(d_text.p, len, pos.p, cap, meta.p, elen.p, blen.p); IPCFP_LAUNCH_CHECK();
-    exclusive_scan_u32(elen.p, eoff.p, cap, (uint64_t*)&meta.p->e_total, scratch.p, st);
-    exclusive_scan_u32(blen.p, boff.p, cap, (uint64_t*)&meta.p->b_total, scratch.p, st);
-    uint64_t* hm = s->host_words.p + HW_JP_META;
-    IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, sizeof(JpMeta), cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 1
-    JpMeta m;
-    memcpy(&m, hm, sizeof m);
+    const uint64_t cap = len / JP_MIN_RECORD + 1;
+    TextScan<JpMeta> sc(s.get(), len, len / 8 + 8, cap, 0xff);
+    AsyncBuf<uint32_t> elen(cap + 1, st), blen(cap + 1, st);
+    AsyncBuf<uint64_t> eoff(cap + 1, st), boff(cap + 1, st);
+    IPCFP_CUDA(cudaMemcpyAsync(sc.text.p, json, len, cudaMemcpyHostToDevice, st));
+    IPCFP_CUDA(cudaMemsetAsync(&sc.meta.p->witness_bytes, 0, 8, st));
+    sc.starts(k_jp_mark);
+    k_jp_records<<<div_up(cap * 32, 128), 128, 0, st>>>(sc.text.p, len, sc.pos.p, cap, sc.meta.p, elen.p, blen.p); IPCFP_LAUNCH_CHECK();
+    exclusive_scan_u32(elen.p, eoff.p, cap, (uint64_t*)&sc.meta.p->e_total, sc.scratch.p, st);
+    exclusive_scan_u32(blen.p, boff.p, cap, (uint64_t*)&sc.meta.p->b_total, sc.scratch.p, st);
+    const JpMeta m = sc.read();   // host synchronisation 1
     if (m.defer != UINT64_MAX || m.n > cap) return false;
     uint64_t cnt[3], first_start[3], last_end[3];
     for (int k = 0; k < 3; k++) { cnt[k] = m.first[k] == UINT64_MAX ? 0 : m.last[k] - m.first[k] + 1; first_start[k] = m.first_start[k]; last_end[k] = m.last_end[k]; }
@@ -246,7 +232,7 @@ static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, in
     AsyncBuf<ipcfp_storage_proof> d_sp(nS + 1, st);
     AsyncBuf<ipcfp_event_proof> d_ep(nE + 1, st);
     AsyncBuf<uint8_t> d_blob(m.e_total + 16, st);
-    if (nS + nE) { k_jp_proofs<<<div_up(nS + nE, 128), 128, 0, st>>>(d_text.p, len, pos.p, nS, nE, eoff.p, d_sp.p, d_ep.p, d_blob.p); IPCFP_LAUNCH_CHECK(); }
+    if (nS + nE) { k_jp_proofs<<<div_up(nS + nE, 128), 128, 0, st>>>(sc.text.p, len, sc.pos.p, nS, nE, eoff.p, d_sp.p, d_ep.p, d_blob.p); IPCFP_LAUNCH_CHECK(); }
     B.sp.resize(nS + 1); B.ep.resize(nE + 1); B.blob.assign(m.e_total + 16, 0);
     B.sres.assign(nS + 1, 0); B.eres.assign(nE + 1, 0);
     if (nS) IPCFP_CUDA(cudaMemcpyAsync(B.sp.data(), d_sp.p, nS * sizeof(ipcfp_storage_proof), cudaMemcpyDeviceToHost, st));
@@ -261,21 +247,18 @@ static bool verify_device_path(VerdictBox& B, const char* json, uint64_t len, in
     if (!tr.child || (!nS && !(tr.parent && nE))) return true;
     // the witness store, decoded straight into its arena
     const Clock::time_point t1 = Clock::now();
-    DevBuf<uint8_t> cids_dev, sort_ws;
-    store_alloc_blocks(s.get(), nB, m.b_total, cids_dev);
-    IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, m.b_total + 48 + 512, st));
-    IPCFP_CUDA(cudaMemsetAsync(s->table.p, 0, s->table.n * 8, st));
+    DevBuf<uint8_t> cids_dev;
+    uint8_t* blocks = store_alloc_blocks(s.get(), nB, m.b_total, cids_dev, true);
     uint8_t prefix[6] = {};
     if (nB) {
-        k_jp_blocks<<<div_up(nB * 32, 128), 128, 0, st>>>(d_text.p, len, pos.p, m.n, m.first[JP_BLOCK], nB, boff.p, cids_dev.p, s->offsets.p, s->lengths.p,
-                                                          s->arena.p + 16);
+        k_jp_blocks<<<div_up(nB * 32, 128), 128, 0, st>>>(sc.text.p, len, sc.pos.p, m.n, m.first[JP_BLOCK], nB, boff.p, cids_dev.p, s->offsets.p,
+                                                          s->lengths.p, blocks);
         IPCFP_LAUNCH_CHECK();
         JpCur c{json, first_start[JP_BLOCK], len};
         c.lit("{\"cid\":[");
         for (int k = 0; k < 6; k++) { uint64_t x = 0; if (k) c.lit(","); c.u64(x); prefix[k] = (uint8_t)x; }
     }
-    store_index(s.get(), cids_dev.p, nullptr, prefix, sort_ws);
-    store_verify_all(s.get());
+    store_finish(s.get(), cids_dev.p, nullptr, prefix, IPCFP_STORE_VERIFY_CIDS);
     if (s->first_bad != UINT64_MAX) throw Error(IPCFP_ERR_CID_MISMATCH, "blake2b-256(block) != CID digest", s->first_bad);
     v.ms_store = ms_since(t1);
     const Clock::time_point t2 = Clock::now();

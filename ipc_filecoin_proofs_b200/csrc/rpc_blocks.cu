@@ -11,15 +11,14 @@
 //                          (all lanes); claims owner[id], writes the id's 16-aligned arena bytes and character count, adds the owned bytes
 //   exclusive_scan_u32     arena offsets by id
 //   ── host synchronisation 1: the meta words. Accepted: no defer, one record per id, every byte of the texts owned.
-//   k_rb_blocks            one warp per id: offset, length, base64 decoded straight into arena + 16 + offset
-//   store_index + store_verify_all (store.cu)
-#include <algorithm>
-#include <chrono>
+//   k_rb_blocks            one warp per id: offset, length, base64 decoded straight into the store's block bytes at offset
+//   store_finish (store.cu)
 #include <cstring>
 
 #include "engine.cuh"
 #include "prims.cuh"
 #include "rpc_blocks_items.cuh"
+#include "text_scan.cuh"
 
 namespace ipcfp {
 
@@ -29,7 +28,7 @@ struct RbMeta {
     unsigned long long owned;   // bytes the records own
     unsigned long long b_total; // arena bytes (16-aligned blocks)
 };
-static_assert(sizeof(RbMeta) <= HW_RB_META_WORDS * 8, "the meta words fit their host words (HW_RB_META)");
+static_assert(sizeof(RbMeta) <= HW_PARSE_META_WORDS * 8, "the meta words fit their host words (HW_PARSE_META)");
 
 __global__ void __launch_bounds__(256) k_rb_mark(const char* __restrict__ t, uint64_t len, uint32_t* bits, uint64_t nwords) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -97,9 +96,6 @@ __global__ void __launch_bounds__(128) k_rb_blocks(const char* __restrict__ t, c
     for (uint64_t g = lane; g < b.n_chars / 4; g += 32) jp_block_group(t, b, g, out);
 }
 
-using Clock = std::chrono::steady_clock;
-static float ms_since(Clock::time_point t0) { return std::chrono::duration<float, std::milli>(Clock::now() - t0).count(); }
-
 #define RB_DIRECT_BYTES (1ull << 20)   // texts this long are copied from the caller's memory; shorter ones are packed first
 #define RB_STAGE_BYTES (16ull << 20)   // one pinned staging chunk (two of them alternate)
 
@@ -107,14 +103,12 @@ static float ms_since(Clock::time_point t0) { return std::chrono::duration<float
 static void upload_texts(Store* s, const char* const* texts, const uint64_t* lens, uint64_t n_texts, char* d) {
     cudaStream_t st = s->stream;
     PinnedArray stage[2];
-    cudaEvent_t done[2] = {};
-    struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int k = 0; k < 2; k++) if (e[k]) cudaEventDestroy(e[k]); } } g{done};
+    Event done[2] = {Event(cudaEventDisableTiming), Event(cudaEventDisableTiming)};   // a buffer's last copy (none yet: complete)
     int cur = 0;
     uint64_t fill = 0, at = 0, chunk_at = 0;
     auto flush = [&] {
         if (!fill) return;
         IPCFP_CUDA(cudaMemcpyAsync(d + chunk_at, stage[cur].p, fill, cudaMemcpyHostToDevice, st));
-        if (!done[cur]) IPCFP_CUDA(cudaEventCreateWithFlags(&done[cur], cudaEventDisableTiming));
         IPCFP_CUDA(cudaEventRecord(done[cur], st));
         cur ^= 1;
         fill = 0;
@@ -131,7 +125,7 @@ static void upload_texts(Store* s, const char* const* texts, const uint64_t* len
         if (fill + L + 1 > RB_STAGE_BYTES) flush();
         if (!fill) {   // a fresh chunk: its buffer's last copy must be done before it is written again
             if (!stage[cur].p) stage[cur] = PinnedArray(s->pool, RB_STAGE_BYTES);
-            if (done[cur]) IPCFP_CUDA(cudaEventSynchronize(done[cur]));
+            IPCFP_CUDA(cudaEventSynchronize(done[cur]));
             chunk_at = at;
         }
         char* h = stage[cur].as<char>() + fill;
@@ -156,80 +150,46 @@ static bool blocks_on_device(Store* s, const uint8_t* cids, uint64_t nb, const c
     }
     if (nb && !cids) return false;
     cudaStream_t st = s->stream;
-    const uint64_t nwords = (len + 31) / 32, cap = len / RB_MIN_RECORD + 1;
-    AsyncBuf<char> d_text(len + JP_PAD, st);
-    AsyncBuf<uint32_t> bits(nwords + 8, st), pos(len / RB_HEAD_LEN + 8, st), owner(nb + 1, st), blen(nb + 1, st), nch(nb + 1, st);
-    AsyncBuf<uint64_t> word_prefix(nwords + 8, st), boff(nb + 1, st), scratch(scan_scratch_elems(std::max(nwords, nb + 1)) + 8, st);
-    AsyncBuf<RbMeta> meta(1, st);
-    upload_texts(s, texts, lens, n_texts, d_text.p);
-    IPCFP_CUDA(cudaMemsetAsync(d_text.p + len, 0, JP_PAD, st));
-    IPCFP_CUDA(cudaMemsetAsync(meta.p, 0, sizeof(RbMeta), st));
+    const uint64_t cap = len / RB_MIN_RECORD + 1;
+    TextScan<RbMeta> sc(s, len, len / RB_HEAD_LEN + 8, nb + 1, 0);
+    AsyncBuf<uint32_t> owner(nb + 1, st), blen(nb + 1, st), nch(nb + 1, st);
+    AsyncBuf<uint64_t> boff(nb + 1, st);
+    upload_texts(s, texts, lens, n_texts, sc.text.p);
     IPCFP_CUDA(cudaMemsetAsync(owner.p, 0xff, (nb + 1) * 4, st));
     IPCFP_CUDA(cudaMemsetAsync(blen.p, 0, (nb + 1) * 4, st));
-    cudaEvent_t tm[4] = {};
-    struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int k = 0; k < 4; k++) if (e[k]) cudaEventDestroy(e[k]); } } g{tm};
-    for (auto& e : tm) IPCFP_CUDA(cudaEventCreate(&e));
+    Event tm[4];
     IPCFP_CUDA(cudaEventRecord(tm[0], st));
-    k_rb_mark<<<div_up(nwords, 256), 256, 0, st>>>(d_text.p, len, bits.p, nwords); IPCFP_LAUNCH_CHECK();
-    bitmap_to_indices(bits.p, len, pos.p, (uint64_t*)&meta.p->n, word_prefix.p, scratch.p, st);
-    k_rb_records<<<div_up(cap * 32, 128), 128, 0, st>>>(d_text.p, len, pos.p, cap, nb, meta.p, owner.p, blen.p, nch.p); IPCFP_LAUNCH_CHECK();
-    if (nb) exclusive_scan_u32(blen.p, boff.p, nb, (uint64_t*)&meta.p->b_total, scratch.p, st);
+    sc.starts(k_rb_mark);
+    k_rb_records<<<div_up(cap * 32, 128), 128, 0, st>>>(sc.text.p, len, sc.pos.p, cap, nb, sc.meta.p, owner.p, blen.p, nch.p); IPCFP_LAUNCH_CHECK();
+    if (nb) exclusive_scan_u32(blen.p, boff.p, nb, (uint64_t*)&sc.meta.p->b_total, sc.scratch.p, st);
     IPCFP_CUDA(cudaEventRecord(tm[1], st));
-    uint64_t* hm = s->host_words.p + HW_RB_META;
-    IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, sizeof(RbMeta), cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 1
-    RbMeta m;
-    memcpy(&m, hm, sizeof m);
+    const RbMeta m = sc.read();   // host synchronisation 1
     if (m.defer || m.n != nb || m.owned != want_owned) return false;
     // the store, its blocks decoded straight into the arena
-    DevBuf<uint8_t> cids_dev, sort_ws;
-    store_alloc_blocks(s, nb, m.b_total, cids_dev);
-    IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, m.b_total + 48 + 512, st));
-    IPCFP_CUDA(cudaMemsetAsync(s->table.p, 0, s->table.n * 8, st));
+    DevBuf<uint8_t> cids_dev;
+    uint8_t* blocks = store_alloc_blocks(s, nb, m.b_total, cids_dev, true);
     if (nb) IPCFP_CUDA(cudaMemcpyAsync(cids_dev.p, cids, nb * IPCFP_CID_LEN, cudaMemcpyHostToDevice, st));
     IPCFP_CUDA(cudaEventRecord(tm[2], st));
     if (nb) {
-        k_rb_blocks<<<div_up(nb * 32, 128), 128, 0, st>>>(d_text.p, pos.p, owner.p, nch.p, nb, boff.p, s->offsets.p, s->lengths.p, s->arena.p + 16);
+        k_rb_blocks<<<div_up(nb * 32, 128), 128, 0, st>>>(sc.text.p, sc.pos.p, owner.p, nch.p, nb, boff.p, s->offsets.p, s->lengths.p, blocks);
         IPCFP_LAUNCH_CHECK();
     }
     IPCFP_CUDA(cudaEventRecord(tm[3], st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    float a, b;
-    IPCFP_CUDA(cudaEventElapsedTime(&a, tm[0], tm[1]));
-    IPCFP_CUDA(cudaEventElapsedTime(&b, tm[2], tm[3]));
     info.parsed_on_device = 1;
     info.ms_parse = ms_since(t0);
-    info.ms_kernels = a + b;
-    store_index(s, cids_dev.p, cids, cids, sort_ws);
-    if (flags & IPCFP_STORE_VERIFY_CIDS) store_verify_all(s);
-    else IPCFP_CUDA(cudaStreamSynchronize(st));
+    info.ms_kernels = elapsed_ms(tm[0], tm[1]) + elapsed_ms(tm[2], tm[3]);
+    store_finish(s, cids_dev.p, cids, cids, flags);
     return true;
 }
 
 Store* store_create_rpc_json(const uint8_t* cids, uint64_t nb, const char* const* texts, const uint64_t* lens, uint64_t n_texts, int device,
                              uint32_t flags, ipcfp_store_json_info& info) {
-    memset(&info, 0, sizeof info);
-    const Clock::time_point t0 = Clock::now();
-    // the device path needs a device and texts to read; everything else (and every failure) is the host path's to report
-    if (n_texts && texts && lens && nb < 0x7fffffffull) {
-        bool have_device = true;
-        try { check_device(device); }
-        catch (const Error&) { have_device = false; }
-        if (have_device) {
-            std::unique_ptr<Store> s(store_shell(device));
-            s->caller_blob = false;
-            if (blocks_on_device(s.get(), cids, nb, texts, lens, n_texts, flags, info, t0)) return s.release();
-            memset(&info, 0, sizeof info);
-        }
-    }
-    const Clock::time_point t1 = Clock::now();
-    ipcfp_parsed_blocks* pb = nullptr;
-    const ipcfp_status st = ipcfp_blocks_from_rpc_json(cids, nb, texts, lens, n_texts, &pb);
-    if (st != IPCFP_OK) throw Error(st, ipcfp_last_error(), ipcfp_last_error_index());
-    std::unique_ptr<ipcfp_parsed_blocks, void (*)(ipcfp_parsed_blocks*)> keep(pb, ipcfp_parsed_blocks_free);
-    info.ms_parse = ms_since(t1);
-    const ipcfp_witness& w = pb->blocks;
-    Store* s = store_create(w.cids, w.offsets, w.lengths, w.blob, w.blob_size, w.n_blocks, device, flags);
+    // the device path needs texts to read; everything else (and every failure) is the host path's to report
+    Store* s = store_create_parsed(
+        device, flags, info, n_texts && texts && lens && nb < 0x7fffffffull,
+        [&](Store* fresh, Clock::time_point t0) { return blocks_on_device(fresh, cids, nb, texts, lens, n_texts, flags, info, t0); },
+        [&](ipcfp_parsed_blocks** pb) { return ipcfp_blocks_from_rpc_json(cids, nb, texts, lens, n_texts, pb); }, nullptr);
     s->caller_blob = false;
     return s;
 }

@@ -10,12 +10,11 @@
 //   ── host synchronisation 1: the record count and the defer word; they size the tipset's events_roots / has_root
 //   k_rj_records           one thread per record: its template and its joints, its 38 CID bytes and flag straight into the tipset's arrays
 //   ── host synchronisation 2: the defer word
-#include <chrono>
 #include <cstring>
 
 #include "engine.cuh"
-#include "prims.cuh"
 #include "rpc_json_items.cuh"
+#include "text_scan.cuh"
 
 namespace ipcfp {
 
@@ -23,7 +22,7 @@ struct RjMeta {
     unsigned long long defer;   // non-zero: not canonical
     unsigned long long n;       // record starts
 };
-static_assert(sizeof(RjMeta) <= HW_RJ_META_WORDS * 8, "the meta words fit their host words (HW_RJ_META)");
+static_assert(sizeof(RjMeta) <= HW_PARSE_META_WORDS * 8, "the meta words fit their host words (HW_PARSE_META)");
 
 __global__ void __launch_bounds__(256) k_rj_mark(const char* __restrict__ t, uint64_t len, uint32_t* bits, uint64_t nwords, RjMeta* meta) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -50,48 +49,32 @@ __global__ void __launch_bounds__(128) k_rj_records(const char* __restrict__ t, 
     has[i] = h;
 }
 
-using Clock = std::chrono::steady_clock;
-
 // the device path for the receipt list; false: not canonical (td's receipt arrays are then to be replaced)
 static bool receipts_on_device(Store* s, const char* text, uint64_t len, TipsetDev& td) {
     if (len < 2 || len >= (1ull << 32) || text[0] != '[' || text[len - 1] != ']') return false;   // record starts are u32
     if (len == 2) { td.n_receipts = 0; return true; }
     cudaStream_t st = s->stream;
-    const uint64_t nwords = (len + 31) / 32, cap = len / RJ_MIN_RECORD + 1;
-    AsyncBuf<char> d_text(len + JP_PAD, st);
-    AsyncBuf<uint32_t> bits(nwords + 8, st), pos(len / RJ_HEAD_LEN + 8, st);
-    AsyncBuf<uint64_t> word_prefix(nwords + 8, st), scratch(scan_scratch_elems(nwords) + 8, st);
-    AsyncBuf<RjMeta> meta(1, st);
-    IPCFP_CUDA(cudaMemsetAsync(d_text.p + len, 0, JP_PAD, st));
-    IPCFP_CUDA(cudaMemsetAsync(meta.p, 0, sizeof(RjMeta), st));
+    const uint64_t cap = len / RJ_MIN_RECORD + 1;
+    TextScan<RjMeta> sc(s, len, len / RJ_HEAD_LEN + 8, 0, 0);
     // straight from the caller's pageable memory: the driver's own pipelined staging beat a copy through two pinned chunks of the pool
     // (8 MB each, filled by one host thread): the whole parse of the 142 MB list of 1 M receipts took 22 ms against 28 ms on an H100 host
-    IPCFP_CUDA(cudaMemcpyAsync(d_text.p, text, len, cudaMemcpyHostToDevice, st));
-    cudaEvent_t tm[4] = {};
-    struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int k = 0; k < 4; k++) if (e[k]) cudaEventDestroy(e[k]); } } g{tm};
-    for (auto& e : tm) IPCFP_CUDA(cudaEventCreate(&e));
+    IPCFP_CUDA(cudaMemcpyAsync(sc.text.p, text, len, cudaMemcpyHostToDevice, st));
+    Event tm[4];
     IPCFP_CUDA(cudaEventRecord(tm[0], st));
-    k_rj_mark<<<div_up(nwords, 256), 256, 0, st>>>(d_text.p, len, bits.p, nwords, meta.p); IPCFP_LAUNCH_CHECK();
-    bitmap_to_indices(bits.p, len, pos.p, (uint64_t*)&meta.p->n, word_prefix.p, scratch.p, st);
+    sc.starts(k_rj_mark, sc.meta.p);
     IPCFP_CUDA(cudaEventRecord(tm[1], st));
-    uint64_t* hm = s->host_words.p + HW_RJ_META;
-    IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, sizeof(RjMeta), cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 1
-    const uint64_t n = hm[1];
-    if (hm[0] || n == 0 || n > cap) return false;
+    const RjMeta m = sc.read();   // host synchronisation 1
+    const uint64_t n = m.n;
+    if (m.defer || n == 0 || n > cap) return false;
     td.n_receipts = n;
     td.events_roots.alloc(n * 38 + 64);
     td.has_root.alloc(n + 64);
     IPCFP_CUDA(cudaEventRecord(tm[2], st));
-    k_rj_records<<<div_up(n, 128), 128, 0, st>>>(d_text.p, len, pos.p, n, td.events_roots.p, td.has_root.p, meta.p); IPCFP_LAUNCH_CHECK();
+    k_rj_records<<<div_up(n, 128), 128, 0, st>>>(sc.text.p, len, sc.pos.p, n, td.events_roots.p, td.has_root.p, sc.meta.p); IPCFP_LAUNCH_CHECK();
     IPCFP_CUDA(cudaEventRecord(tm[3], st));
-    IPCFP_CUDA(cudaMemcpyAsync(hm, meta.p, 8, cudaMemcpyDeviceToHost, st));
-    IPCFP_CUDA(cudaStreamSynchronize(st));   // host synchronisation 2
-    float a, b;
-    IPCFP_CUDA(cudaEventElapsedTime(&a, tm[0], tm[1]));
-    IPCFP_CUDA(cudaEventElapsedTime(&b, tm[2], tm[3]));
-    td.ms_kernels = a + b;
-    return hm[0] == 0;
+    const bool canonical = sc.read().defer == 0;   // host synchronisation 2
+    td.ms_kernels = elapsed_ms(tm[0], tm[1]) + elapsed_ms(tm[2], tm[3]);
+    return canonical;
 }
 
 static void rethrow_parse(ipcfp_status st) {
@@ -116,7 +99,7 @@ void tipset_upload_json(Store* s, const char* parent, uint64_t parent_len, const
         if (dev.n_receipts) { td.events_roots = std::move(dev.events_roots); td.has_root = std::move(dev.has_root); }
         td.parsed_on_device = true;
         td.ms_kernels = dev.ms_kernels;
-        td.ms_parse = std::chrono::duration<float, std::milli>(Clock::now() - t0).count();
+        td.ms_parse = ms_since(t0);
         return;
     }
     keep.reset();
@@ -125,7 +108,7 @@ void tipset_upload_json(Store* s, const char* parent, uint64_t parent_len, const
     keep.reset(pt);
     tipset_upload(s, &pt->desc, td);
     IPCFP_CUDA(cudaStreamSynchronize(s->stream));
-    td.ms_parse = std::chrono::duration<float, std::milli>(Clock::now() - t0).count();
+    td.ms_parse = ms_since(t0);
 }
 
 void tipset_describe(TipsetDev& td, bool with_roots, ipcfp_tipset_info* out) {

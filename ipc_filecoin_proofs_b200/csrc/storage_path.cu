@@ -299,13 +299,6 @@ static std::unique_ptr<PathResultBox> result_box(PathRun& run) {
     return box;
 }
 
-struct PathEvents {
-    cudaEvent_t e[5] = {};
-    PathEvents() { for (auto& x : e) IPCFP_CUDA(cudaEventCreate(&x)); }
-    ~PathEvents() { for (auto& x : e) if (x) cudaEventDestroy(x); }
-    float ms(int a, int b) const { float v = 0.f; IPCFP_CUDA(cudaEventElapsedTime(&v, e[a], e[b])); return v; }
-};
-
 ipcfp_path_result* generate_storage_path_proofs(Store* s, TipsetDev& td, const ipcfp_storage_path* paths, uint64_t n, uint32_t flags) {
     if (flags & ~(uint32_t)IPCFP_WITNESS_BY_REFERENCE) throw Error(IPCFP_ERR_INVALID_ARG, "unknown flag bit for storage paths");
     PathPack pk;
@@ -317,31 +310,31 @@ ipcfp_path_result* generate_storage_path_proofs(Store* s, TipsetDev& td, const i
     s->use();
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
-    PathEvents ev;
+    Event ev[4];
     PathRun run(s, pk, td.child_cid, td.child_state_root);
     IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
     AsyncBuf<uint32_t> wbits((s->n + 31) / 32 + 8, st), w1_rec(run.n_fixed * REC_CAP + 8, st), w1_recn(run.n_fixed + 8, st);
     wbits.zero();
     run.slots();
-    IPCFP_CUDA(cudaEventRecord(ev.e[0], st));
+    IPCFP_CUDA(cudaEventRecord(ev[0], st));
     // wave 1: the fixed specs
     StorageArgs a1 = run.args(run.fixed.p, run.n_fixed, run.w1.p);
     a1.rec_list = w1_rec.p; a1.rec_n = w1_recn.p; a1.wbits = wbits.p; a1.err = dw;
     run.proofs(a1, run.owner1, run.pos1, false, run.w1_ok.p);
-    IPCFP_CUDA(cudaEventRecord(ev.e[1], st));
+    IPCFP_CUDA(cudaEventRecord(ev[1], st));
     PinnedArray words(s->pool, 16);
     run.size(words);   // host synchronisation 1
     // wave 2: the data slots, into the final list; wave 1's results join them there
     AsyncBuf<uint32_t> rec(run.n_specs * REC_CAP + 8, st), recn(run.n_specs + 8, st);
-    IPCFP_CUDA(cudaEventRecord(ev.e[2], st));
+    IPCFP_CUDA(cudaEventRecord(ev[2], st));
     run.place(w1_rec.p, w1_recn.p, rec.p, recn.p);
     w1_rec.release();   // wave 1's lists are in the final ones now: freed in stream order, so a call holds one copy of them
     StorageArgs a2 = run.args(run.specs.p, run.n_specs, run.out.p);
     a2.rec_list = rec.p; a2.rec_n = recn.p; a2.wbits = wbits.p; a2.err = dw;
     run.proofs(a2, run.owner.p, run.pos.p, true, run.ok.p);
     run.values_kernel();
-    IPCFP_CUDA(cudaEventRecord(ev.e[3], st));
+    IPCFP_CUDA(cudaEventRecord(ev[3], st));
     std::unique_ptr<PathResultBox> box = result_box(run);
     uint64_t* hw = s->host_words.p;
     IPCFP_CUDA(cudaMemcpyAsync(hw + DW_ERR, dw, 8, cudaMemcpyDeviceToHost, st));   // read with the witness count's synchronisation
@@ -352,12 +345,10 @@ ipcfp_path_result* generate_storage_path_proofs(Store* s, TipsetDev& td, const i
     }
     ipcfp_path_result& r = box->r;
     r.ms_total = r.storage->ms_total;
-    float t_slots = 0.f;
-    IPCFP_CUDA(cudaEventElapsedTime(&t_slots, s->ev[EV_BEGIN], ev.e[0]));
-    r.ms_slots = t_slots;
-    r.ms_wave1 = ev.ms(0, 1);
-    r.ms_wave2 = ev.ms(2, 3);
-    IPCFP_CUDA(cudaEventElapsedTime(&r.ms_witness, ev.e[3], s->ev[EV_STORAGE_END]));
+    r.ms_slots = elapsed_ms(s->ev[EV_BEGIN], ev[0]);
+    r.ms_wave1 = elapsed_ms(ev[0], ev[1]);
+    r.ms_wave2 = elapsed_ms(ev[2], ev[3]);
+    r.ms_witness = elapsed_ms(ev[3], s->ev[EV_STORAGE_END]);
     r.host_syncs = 4;   // the size, then storage_result_finish's three (witness count, witness copy, end)
     return &box.release()->r;
 }
@@ -393,8 +384,8 @@ ipcfp_path_result* verify_storage_paths(Store* s, const ipcfp_tipset_desc* t, co
     path_pack(paths, n_paths, pk);
     s->use();
     cudaStream_t st = s->stream;
-    PathEvents ev;
-    IPCFP_CUDA(cudaEventRecord(ev.e[4], st));
+    Event ev[5];
+    IPCFP_CUDA(cudaEventRecord(ev[4], st));
     // every proof replayed over the witness store (its Err fails the call)
     std::vector<uint8_t> results(n_proofs + 1, 0);
     verify_storage_proofs(s, t, proofs, n_proofs, results.data());
@@ -417,16 +408,16 @@ ipcfp_path_result* verify_storage_paths(Store* s, const ipcfp_tipset_desc* t, co
     }
     PathRun run(s, pk, nullptr, nullptr);
     run.slots();
-    IPCFP_CUDA(cudaEventRecord(ev.e[0], st));
+    IPCFP_CUDA(cudaEventRecord(ev[0], st));
     if (run.n_fixed) {
         k_path_lookup<<<div_up(run.n_fixed, 128), 128, 0, st>>>(run.fixed.p, run.n_fixed, run.owner1, run.pos1, nullptr, d_proofs.p, d_order.p, d_res.p, n_proofs,
                                                                  run.w1.p, run.w1_ok.p);
         IPCFP_LAUNCH_CHECK();
     }
-    IPCFP_CUDA(cudaEventRecord(ev.e[1], st));
+    IPCFP_CUDA(cudaEventRecord(ev[1], st));
     PinnedArray words(s->pool, 16);
     run.size(words);
-    IPCFP_CUDA(cudaEventRecord(ev.e[2], st));
+    IPCFP_CUDA(cudaEventRecord(ev[2], st));
     run.place(nullptr, nullptr, nullptr, nullptr);
     if (run.n_specs) {
         k_path_lookup<<<div_up(run.n_specs, 128), 128, 0, st>>>(run.specs.p, run.n_specs, run.owner.p, run.pos.p, run.P.paths, d_proofs.p, d_order.p, d_res.p,
@@ -434,14 +425,14 @@ ipcfp_path_result* verify_storage_paths(Store* s, const ipcfp_tipset_desc* t, co
         IPCFP_LAUNCH_CHECK();
     }
     run.values_kernel();
-    IPCFP_CUDA(cudaEventRecord(ev.e[3], st));
+    IPCFP_CUDA(cudaEventRecord(ev[3], st));
     std::unique_ptr<PathResultBox> box = result_box(run);
     IPCFP_CUDA(cudaStreamSynchronize(st));
     ipcfp_path_result& r = box->r;
-    r.ms_slots = ev.ms(4, 0);
-    r.ms_wave1 = ev.ms(0, 1);
-    r.ms_wave2 = ev.ms(2, 3);
-    r.ms_total = ev.ms(4, 3);
+    r.ms_slots = elapsed_ms(ev[4], ev[0]);
+    r.ms_wave1 = elapsed_ms(ev[0], ev[1]);
+    r.ms_wave2 = elapsed_ms(ev[2], ev[3]);
+    r.ms_total = elapsed_ms(ev[4], ev[3]);
     return &box.release()->r;
 }
 

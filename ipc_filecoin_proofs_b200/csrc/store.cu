@@ -251,6 +251,10 @@ void publish_words(Store* s, uint32_t dst_first, uint32_t n_words, const void* s
 __global__ void k_lookup_one(StoreView v, const uint8_t* cid, int32_t* out) { out[0] = store_lookup(v, cid); }
 
 // ------------------------------------------------------------------------------------------ host side
+// The arena: ARENA_HEAD zero bytes in front of block 0 (StoreView::blob), the blob_size block bytes, then ARENA_TAIL zero bytes: pass-1
+// staging copies whole CH-aligned chunks around the last block.
+static const uint64_t ARENA_HEAD = 16, ARENA_TAIL = 32 + 512;
+
 static bool parse_prefix(const uint8_t* p, uint64_t key[4]) {
     size_t pos = 0;
     for (int f = 0; f < 4; f++) {
@@ -274,7 +278,7 @@ static void upload_view(Store* s) {
 }
 static void fill_view(Store* s) {
     StoreView& v = s->view;
-    v.blob = s->arena.p + 16;
+    v.blob = s->arena.p + ARENA_HEAD;
     v.offsets = s->offsets.p; v.lengths = s->lengths.p; v.digests = s->digests.p; v.cls = s->cls.p; v.table = s->table.p;
     v.recs = s->recs.p;
     v.rank_of = s->rank_of.p; v.block_at_rank = s->block_at_rank.p;
@@ -322,17 +326,27 @@ Store* store_shell(int device) {
     return s.release();
 }
 
-void store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev) {
+uint8_t* store_alloc_blocks(Store* s, uint64_t n, uint64_t blob_size, DevBuf<uint8_t>& cids_dev, bool zero_blocks) {
     if (n >= 0x7fffffffull) throw Error(IPCFP_ERR_UNSUPPORTED, "more than 2^31 blocks in one store");
-    store_alloc_arena(s, blob_size);
+    uint8_t* blocks = store_alloc_arena(s, blob_size, zero_blocks);
     store_alloc_index(s, n, cids_dev);
+    return blocks;
 }
 
 // device allocations
 // (from the process-wide device pool: a store created right after one of similar size was destroyed allocates nothing)
-void store_alloc_arena(Store* s, uint64_t blob_size) {
+uint8_t* store_alloc_arena(Store* s, uint64_t blob_size, bool zero_blocks) {
+    cudaStream_t st = s->stream;
     s->blob_size = blob_size;
-    s->arena.alloc_pooled(blob_size + 48 + 512);   // + room for whole aligned chunks around the last block (pass-1 staging copies CH-aligned chunks)
+    s->arena.alloc_pooled(ARENA_HEAD + blob_size + ARENA_TAIL);
+    uint8_t* blocks = s->arena.p + ARENA_HEAD;
+    if (zero_blocks) {
+        IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, s->arena.n, st));
+    } else {
+        IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, ARENA_HEAD, st));
+        IPCFP_CUDA(cudaMemsetAsync(blocks + blob_size, 0, ARENA_TAIL, st));
+    }
+    return blocks;
 }
 
 void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev) {
@@ -347,6 +361,7 @@ void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev) {
     uint64_t slots = 64;
     while (slots < 2 * n) slots <<= 1;
     s->table.alloc_pooled(slots);
+    IPCFP_CUDA(cudaMemsetAsync(s->table.p, 0, slots * 8, s->stream));
     cids_dev.alloc_pooled(n * 38 + 16);
 }
 
@@ -354,7 +369,7 @@ void store_alloc_index(Store* s, uint64_t n, DevBuf<uint8_t>& cids_dev) {
 // offsets / lengths are in the store: everything of the ingest that does not touch block bytes. cids_host: the same CIDs on the host, or
 // null (the rare several-prefix path then reads them back). first_prefix: the first CID's 6 prefix bytes (host). Leaves the view
 // uploaded; the last synchronisation is the class check's.
-void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws) {
+static void store_index(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, DevBuf<uint8_t>& sort_ws) {
     const uint64_t n = s->n;
     cudaStream_t st = s->stream;
     // CID classes: the first CID's prefix is class 0; anything else is discovered by the kernel
@@ -415,15 +430,28 @@ static uint32_t blake2b_class_mask(const Store* s) {
     return mask;
 }
 
-// IPCFP_STORE_VERIFY_CIDS over every block of a store whose blocks are all on the device already; synchronises, sets first_bad
-void store_verify_all(Store* s) {
+void store_finish(Store* s, const uint8_t* cids_dev, const uint8_t* cids_host, const uint8_t* first_prefix, uint32_t flags, const ChunkedCopy* blob,
+                  const std::vector<uint64_t>& bounds) {
     cudaStream_t st = s->stream;
+    DevBuf<uint8_t> sort_ws;   // released (to the device pool) after the final synchronisation
+    store_index(s, cids_dev, cids_host, first_prefix, sort_ws);
+    if (!(flags & IPCFP_STORE_VERIFY_CIDS)) {
+        if (blob) blob->wait(st, blob->landed.size() - 1);   // the blob must have landed before anything reads blocks
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        return;
+    }
+    const uint32_t mask = blake2b_class_mask(s);
     unsigned long long* bad = s->dev_words.p + DW_FIRST_BAD;
     IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
-    if (s->n) { k_verify_cids<<<div_up(s->n, 128), 128, 0, st>>>(s->view, 0, (uint32_t)s->n, blake2b_class_mask(s), bad); IPCFP_LAUNCH_CHECK(); }
+    const std::vector<uint64_t> all{0, s->n};
+    const std::vector<uint64_t>& b = blob ? bounds : all;
+    for (size_t k = 0; k + 1 < b.size(); k++) {   // range k is checked while range k + 1 is on the wire
+        if (blob) blob->wait(st, k);
+        if (b[k + 1] > b[k]) { k_verify_cids<<<div_up(b[k + 1] - b[k], 128), 128, 0, st>>>(s->view, (uint32_t)b[k], (uint32_t)b[k + 1], mask, bad); IPCFP_LAUNCH_CHECK(); }
+    }
     publish_words(s, DW_FIRST_BAD, 1);
     IPCFP_CUDA(cudaStreamSynchronize(st));
-    s->first_bad = s->host_words.p[DW_FIRST_BAD];
+    s->first_bad = s->host_words.p[DW_FIRST_BAD];   // reported by the C ABI as IPCFP_ERR_CID_MISMATCH (handle stays valid)
 }
 
 Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t* lengths, const uint8_t* blob, uint64_t blob_size, uint64_t n,
@@ -433,22 +461,15 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
     if (n && (!cids || !offsets || !lengths || (!blob && blob_size))) throw Error(IPCFP_ERR_INVALID_ARG, "null input array");
     std::unique_ptr<Store> s(store_shell(device));
     cudaStream_t st = s->stream;
-    DevBuf<uint8_t> cids_dev, sort_ws;   // released (to the device pool) when this function returns: after its final sync
-    store_alloc_blocks(s.get(), n, blob_size, cids_dev);
-    const uint64_t slots = s->table.n;
+    DevBuf<uint8_t> cids_dev;   // released (to the device pool) when this function returns: after its final sync
+    uint8_t* blocks = store_alloc_blocks(s.get(), n, blob_size, cids_dev, false);
 
     // H2D. The CID array goes first so the index build overlaps the (much larger) blob copy.
-    cudaStream_t st2;
-    IPCFP_CUDA(cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking));
-    struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } sg{st2};
     if (n) {
         IPCFP_CUDA(cudaMemcpyAsync(cids_dev.p, cids, n * 38, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaMemcpyAsync(s->offsets.p, offsets, n * 8, cudaMemcpyHostToDevice, st));
         IPCFP_CUDA(cudaMemcpyAsync(s->lengths.p, lengths, n * 4, cudaMemcpyHostToDevice, st));
     }
-    IPCFP_CUDA(cudaMemsetAsync(s->arena.p, 0, 16, st2));
-    IPCFP_CUDA(cudaMemsetAsync(s->arena.p + 16 + blob_size, 0, 32 + 512, st2));
-    IPCFP_CUDA(cudaMemsetAsync(s->table.p, 0, slots * 8, st));
 
     // validate offsets / lengths on the host (metadata only); blocks laid out in index order (the usual case) let the blob travel in
     // CHUNKS whose blocks are Blake2b-checked while the next chunk is still on the wire
@@ -458,45 +479,43 @@ Store* store_create(const uint8_t* cids, const uint64_t* offsets, const uint32_t
         if (i && offsets[i] < offsets[i - 1] + lengths[i - 1]) monotonic = false;
     }
     const bool verify = (flags & IPCFP_STORE_VERIFY_CIDS) && n;
-    struct Chunk { uint64_t b0, b1, byte0, byte1; };
-    std::vector<Chunk> chunks;
+    std::vector<uint64_t> bounds{0}, byte_bounds{0};   // chunk k: blocks [bounds[k], bounds[k + 1]), bytes [byte_bounds[k], byte_bounds[k + 1])
     const uint64_t CHUNK_BYTES = 64ull << 20;
     if (monotonic && verify && blob_size > 2 * CHUNK_BYTES) {
-        uint64_t b0 = 0, byte0 = 0;
-        for (uint64_t i = 0; i < n; i++) {
-            const uint64_t end = offsets[i] + lengths[i];
-            if (end - byte0 >= CHUNK_BYTES && i + 1 < n) { chunks.push_back(Chunk{b0, i + 1, byte0, offsets[i + 1]}); b0 = i + 1; byte0 = offsets[i + 1]; }
-        }
-        chunks.push_back(Chunk{b0, n, byte0, blob_size});
-    } else chunks.push_back(Chunk{0, n, 0, blob_size});
-    std::vector<cudaEvent_t> chunk_ev(chunks.size(), nullptr);
-    struct EvGuard { std::vector<cudaEvent_t>& v; ~EvGuard() { for (auto e : v) if (e) cudaEventDestroy(e); } } evg{chunk_ev};
-    for (size_t k = 0; k < chunks.size(); k++) {
-        const Chunk& c = chunks[k];
-        if (c.byte1 > c.byte0) IPCFP_CUDA(cudaMemcpyAsync(s->arena.p + 16 + c.byte0, blob + c.byte0, c.byte1 - c.byte0, cudaMemcpyHostToDevice, st2));
-        IPCFP_CUDA(cudaEventCreateWithFlags(&chunk_ev[k], cudaEventDisableTiming));
-        IPCFP_CUDA(cudaEventRecord(chunk_ev[k], st2));
+        for (uint64_t i = 0; i + 1 < n; i++)
+            if (offsets[i] + lengths[i] - byte_bounds.back() >= CHUNK_BYTES) { bounds.push_back(i + 1); byte_bounds.push_back(offsets[i + 1]); }
     }
-
-    store_index(s.get(), cids_dev.p, cids, cids, sort_ws);
-    if (verify) {
-        const uint32_t mask = blake2b_class_mask(s.get());
-        unsigned long long* bad = s->dev_words.p + DW_FIRST_BAD;
-        IPCFP_CUDA(cudaMemsetAsync(bad, 0xff, 8, st));
-        for (size_t k = 0; k < chunks.size(); k++) {   // chunk k is checked while chunk k+1 is on the wire
-            const Chunk& c = chunks[k];
-            IPCFP_CUDA(cudaStreamWaitEvent(st, chunk_ev[k], 0));
-            if (c.b1 > c.b0) { k_verify_cids<<<div_up(c.b1 - c.b0, 128), 128, 0, st>>>(s->view, (uint32_t)c.b0, (uint32_t)c.b1, mask, bad); IPCFP_LAUNCH_CHECK(); }
-        }
-        publish_words(s.get(), DW_FIRST_BAD, 1);
-        IPCFP_CUDA(cudaStreamSynchronize(st));
-        s->first_bad = s->host_words.p[DW_FIRST_BAD];  // reported by the C ABI as IPCFP_ERR_CID_MISMATCH (handle stays valid)
-    } else {
-        // the blob must have landed before anything reads blocks
-        IPCFP_CUDA(cudaStreamWaitEvent(st, chunk_ev.back(), 0));
-        IPCFP_CUDA(cudaStreamSynchronize(st));
-    }
+    bounds.push_back(n);
+    byte_bounds.push_back(blob_size);
+    ChunkedCopy copy;
+    for (size_t k = 0; k + 1 < bounds.size(); k++) copy.copy(blocks, blob, byte_bounds[k], byte_bounds[k + 1]);
+    store_finish(s.get(), cids_dev.p, cids, cids, verify ? flags : 0, &copy, bounds);
     return s.release();
+}
+
+Store* store_create_parsed(int device, uint32_t flags, ipcfp_store_json_info& info, bool try_device,
+                           const std::function<bool(Store*, Clock::time_point)>& on_device,
+                           const std::function<ipcfp_status(ipcfp_parsed_blocks**)>& host_parse, const uint8_t* blob) {
+    memset(&info, 0, sizeof info);
+    const Clock::time_point t0 = Clock::now();
+    if (try_device) {
+        bool have_device = true;
+        try { check_device(device); }
+        catch (const Error&) { have_device = false; }   // the host path's store_create reports it
+        if (have_device) {
+            std::unique_ptr<Store> s(store_shell(device));
+            if (on_device(s.get(), t0)) return s.release();
+            memset(&info, 0, sizeof info);
+        }
+    }
+    const Clock::time_point t1 = Clock::now();
+    ipcfp_parsed_blocks* pb = nullptr;
+    const ipcfp_status st = host_parse(&pb);
+    if (st != IPCFP_OK) throw Error(st, ipcfp_last_error(), ipcfp_last_error_index());
+    std::unique_ptr<ipcfp_parsed_blocks, void (*)(ipcfp_parsed_blocks*)> keep(pb, ipcfp_parsed_blocks_free);
+    info.ms_parse = ms_since(t1);
+    const ipcfp_witness& w = pb->blocks;
+    return store_create(w.cids, w.offsets, w.lengths, blob ? blob : w.blob, w.blob_size, w.n_blocks, device, flags);
 }
 
 void store_get(Store* s, const uint8_t* cid, uint8_t* buf, uint32_t cap, uint32_t* len, int* found) {
@@ -515,7 +534,7 @@ void store_get(Store* s, const uint8_t* cid, uint8_t* buf, uint32_t cap, uint32_
     IPCFP_CUDA(cudaMemcpy(&off, s->offsets.p + idx, 8, cudaMemcpyDeviceToHost));
     IPCFP_CUDA(cudaMemcpy(&l, s->lengths.p + idx, 4, cudaMemcpyDeviceToHost));
     if (len) *len = l;
-    if (buf && cap) IPCFP_CUDA(cudaMemcpy(buf, s->arena.p + 16 + off, l < cap ? l : cap, cudaMemcpyDeviceToHost));
+    if (buf && cap) IPCFP_CUDA(cudaMemcpy(buf, s->arena.p + ARENA_HEAD + off, l < cap ? l : cap, cudaMemcpyDeviceToHost));
 }
 
 // ------------------------------------------------------------------------------------------ batched hashes

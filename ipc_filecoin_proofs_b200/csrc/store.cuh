@@ -6,7 +6,7 @@
 // (common/blockstore.rs:8-39) becomes one bit per block in a witness bitmap.
 //
 // HBM layout (n blocks, B blob bytes):
-//   arena    : [16 B pad][blob as given, any offsets][16 B pad]      B + 32
+//   arena    : [16 B pad][blob as given, any offsets][tail pad]      (store.cu: ARENA_HEAD, ARENA_TAIL)
 //   offsets  : u64[n]    lengths: u32[n]
 //   digests  : Digest[n] (32 B, raw digest bytes)       cls: u8[n] (CID prefix class)
 //   table    : u64[2^k], k = ceil(log2(2n)); slot = fingerprint32 << 32 | (block index + 1)
