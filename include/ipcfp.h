@@ -722,6 +722,102 @@ ipcfp_status ipcfp_address_parse(const char* text, uint64_t len, ipcfp_address* 
 ipcfp_status ipcfp_address_from_eth(const uint8_t eth[20], ipcfp_address* out);
 
 /* ------------------------------------------------------------------------------------------
+ * Actor proofs: what the state tree holds for an address — its actor ID, code, head, nonce (sequence), balance and delegated (f410)
+ * address, and for an EVM actor its bytecode CID and hash, EVM nonce and storage root — or a proof that the address or actor is absent
+ * (DESIGN.md §2 "Actor proofs", §3). The account half of eth_getProof. A request is an ipcfp_address:
+ *   protocol 0 (ID)   the actors HAMT under the child header's ParentStateRoot, key Address::new_id(id).to_bytes();
+ *   any other         first the Init actor's address_map (the path of ipcfp_resolve_addresses) under the same ParentStateRoot, then
+ *                     the actors HAMT under the ID found there.
+ * Every block of both walks goes into the proof's witness: the child header, the StateRoot, the Init path (actors HAMT to ID 1, the
+ * InitState) and the address_map path for a non-ID address, the actors HAMT path, the EVM state of an EVM actor and, with
+ * IPCFP_ACTOR_WITH_CODE, its bytecode block.
+ * Decode contract of the new fields (the rest is DESIGN.md §3's):
+ *   ActorState   [code, head, sequence, balance, delegated | null], exactly; delegated must be bytes Address::from_bytes accepts;
+ *   balance      fvm bigint_ser: empty bytes = 0; else a sign byte (0 plus, 1 minus; anything else: IPCFP_ERR_DECODE) followed by the
+ *                big-endian magnitude, at most 32 bytes (more: IPCFP_ERR_DECODE; total supply is below 2^91). A zero magnitude is
+ *                never negative;
+ *   EVM actors   those whose code is one of evm_code_cids (the EVM actor code CIDs of the network's manifests; the caller's input, n_evm
+ *                may be 0). Their head is read as EvmStateV6, else V5 (the rule of storage proofs); neither: IPCFP_ERR_DECODE. The head
+ *                of any other actor is not read.
+ * ------------------------------------------------------------------------------------------ */
+#define IPCFP_ACTOR_MAX 65536u          /* requests of one call                                                                */
+#define IPCFP_ACTOR_WITH_CODE 0x20u     /* flag: the bytecode block of every EVM actor joins its witness and its bytes the code blob */
+enum {
+    IPCFP_ACTOR_FOUND = 0,              /* the actor and every field below                                                     */
+    IPCFP_ACTOR_NO_ADDRESS = 1,         /* a non-ID address proven absent from the address_map; actor_id and the fields are 0   */
+    IPCFP_ACTOR_NO_ACTOR = 2            /* actor_id proven absent from the actors HAMT; the fields are 0                        */
+};
+/* 400 bytes, 8-byte aligned; every byte not named by a field is zero. Offsets: actor_id 0, sequence 8, evm_nonce 16, code_off 24,
+ * code_len 32, status 40, balance_negative 44, has_delegated 45, is_evm 46, balance 48, code 80, head 118, bytecode_cid 156,
+ * contract_state 194, bytecode_hash 232, address 264, delegated 330. */
+typedef struct ipcfp_actor_proof {
+    uint64_t actor_id;                  /* the ID (an ID address's own, or the address_map's value)                               */
+    uint64_t sequence;                  /* ActorState.sequence (the nonce)                                                        */
+    uint64_t evm_nonce;                 /* EVM actors: the EVM state's nonce                                                      */
+    uint64_t code_off, code_len;        /* IPCFP_ACTOR_WITH_CODE, EVM actors: the bytecode, code_blob[code_off .. +code_len)       */
+    uint32_t status;                    /* IPCFP_ACTOR_*                                                                          */
+    uint8_t balance_negative;
+    uint8_t has_delegated;
+    uint8_t is_evm;                     /* code is one of evm_code_cids                                                           */
+    uint8_t _pad0;
+    uint8_t balance[32];                /* big-endian magnitude                                                                   */
+    uint8_t code[IPCFP_CID_LEN];        /* ActorState.code                                                                        */
+    uint8_t head[IPCFP_CID_LEN];        /* ActorState.state                                                                       */
+    uint8_t bytecode_cid[IPCFP_CID_LEN];   /* EVM actors                                                                         */
+    uint8_t contract_state[IPCFP_CID_LEN]; /* EVM actors: the storage root storage proofs read (their storage_root)             */
+    uint8_t bytecode_hash[32];          /* EVM actors: keccak256 of the bytecode                                                  */
+    ipcfp_address address;              /* the request                                                                            */
+    ipcfp_address delegated;            /* has_delegated: ActorState.delegated_address                                            */
+    uint8_t _pad1[4];
+} ipcfp_actor_proof;
+typedef struct ipcfp_actor_result {
+    uint64_t n_proofs;
+    const ipcfp_actor_proof* proofs;        /* in request order                                                                   */
+    ipcfp_witness witness;                  /* union over all proofs, `Cid` order                                                 */
+    const uint64_t* proof_witness_offsets;  /* n_proofs+1                                                                         */
+    const uint32_t* proof_witness_index;    /* per proof: indices into witness (its blocks), ascending                            */
+    const uint8_t* code_blob;               /* IPCFP_ACTOR_WITH_CODE: the bytecodes, in proof order                               */
+    uint64_t code_blob_size;
+    /* device time (CUDA events on the store's stream), milliseconds: the whole call, the Init walk, the proofs' walks, the code gather,
+     * the witness and per-proof lists; host_syncs: host synchronisations the call made */
+    float ms_total, ms_init, ms_walk, ms_code, ms_witness;
+    uint32_t host_syncs;
+} ipcfp_actor_result;
+/* Proofs of n addresses against a resident tipset. Anchored as storage proofs are: the child header's ParentStateRoot must equal the
+ * tipset's child_parent_state_root (else IPCFP_ERR_STATE_ROOT_MISMATCH), and the header is in every proof's witness. flags:
+ *   IPCFP_WITNESS_BY_REFERENCE  the witness comes by reference (blob NULL, offsets into the blob the store was created from);
+ *   IPCFP_ACTOR_WITH_CODE       the bytecode block of every EVM actor (raw codec 0x55, Blake2b-256: a second CID prefix in the store)
+ *                               joins the proof's witness and its bytes the code blob; keccak256 of the bytes must equal bytecode_hash,
+ *                               else IPCFP_ERR_DECODE.
+ * The Init path runs once per call, and only when some address is not an ID address. Absent addresses and actors are answers (status),
+ * not failures. Missing blocks, decode errors, a state-tree without an Init actor (IPCFP_ERR_ACTOR_NOT_FOUND) and a state-root mismatch
+ * fail the call with the first failing proof's index, as ipcfp_generate_storage_proofs does. IPCFP_ERR_INVALID_ARG before any device
+ * work: bytes that are not an Address (ipcfp_resolve_addresses' rule; the index names the request), NULL arrays with nonzero counts, more
+ * than IPCFP_ACTOR_MAX requests, another flag bit, a tipset without child_parent_state_root. Host synchronisations: four — the error
+ * word (with the bytecode lengths), the witness count, the end of the witness copy, the end of the call. *out is released with
+ * ipcfp_actor_result_free. */
+ipcfp_status ipcfp_generate_actor_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_address* addrs, uint64_t n,
+                                                  const uint8_t* evm_code_cids /* n_evm*38 */, uint64_t n_evm, uint32_t flags,
+                                                  ipcfp_actor_result** out);
+/* ipcfp_tipset_upload, then the resident call */
+ipcfp_status ipcfp_generate_actor_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_address* addrs, uint64_t n,
+                                         const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags, ipcfp_actor_result** out);
+void ipcfp_actor_result_free(ipcfp_actor_result* r);
+/* One ChainReadObj round for the call above: the blocks its walks would read that the store lacks, as far as the blocks it holds tell
+ * (the bytecode blocks with IPCFP_ACTOR_WITH_CODE). From an empty store the rounds end with a store on which the generate call gives what
+ * it gives on the complete store. flags: those of the generate call; refusals are its refusals. */
+ipcfp_status ipcfp_plan_fetch_actor_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_address* addrs, uint64_t n,
+                                                    const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags, ipcfp_fetch_plan** out);
+/* Replays every proof on the witness store (create it with IPCFP_STORE_VERIFY_CIDS): the header and its ParentStateRoot against t, the
+ * Init path and the address_map for a non-ID address, the actors HAMT, every field, the EVM state of an actor whose code is in
+ * evm_code_cids, and with IPCFP_ACTOR_WITH_CODE the bytecode block (its length must be code_len and its keccak256 bytecode_hash).
+ * Absence claims are checked by walking to the absence again. results[i] = 1 when proof i states exactly what the witness holds. A
+ * missing witness block or a decode error fails the call at that proof, as ipcfp_verify_storage_proofs does; refusals are the generate
+ * call's (an address of a proof that is not an Address, an unknown status is a 0 verdict). */
+ipcfp_status ipcfp_verify_actor_proofs(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_actor_proof* proofs, uint64_t n,
+                                       const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags, uint8_t* results);
+
+/* ------------------------------------------------------------------------------------------
  * Wire format (src/proofs/common/bundle.rs:10-45, src/proofs/events/bundle.rs:5-30, src/proofs/storage/bundle.rs:5-14): the JSON
  * `serde_json::to_string` gives for UnifiedProofBundle / EventProofBundle — struct field order, compact, CIDs as "bafy2bzace…"
  * strings, "0x" lower-case hex, base64 block data (ProofBlock.cid as the byte array cid 0.11's Serialize emits). t supplies the

@@ -643,6 +643,85 @@ inline uint64_t resolve_eth_address_to_actor_id(GpuBlockstore& store, const Cid&
     return r.actor_ids[0];
 }
 
+// ipcfp_generate_actor_proofs: what the state tree under the child header's ParentStateRoot holds for each address. A proof keeps the C
+// record (its fields are the account's: actor_id, sequence, balance, code, head, delegated, the EVM fields) and, with code, the bytecode.
+struct ActorProof {
+    ipcfp_actor_proof c;
+    std::vector<uint8_t> bytecode;       // with_code, EVM actors
+    std::vector<size_t> witness;         // indices into ActorProofs::blocks
+};
+struct ActorProofs {
+    std::vector<ActorProof> proofs;
+    std::vector<ProofBlock> blocks;      // the union, `Cid` order
+};
+namespace detail {
+inline std::vector<uint8_t> cid_bytes(const std::vector<Cid>& cids) {
+    std::vector<uint8_t> out;
+    for (const Cid& c : cids) out.insert(out.end(), c.bytes.begin(), c.bytes.end());
+    return out;
+}
+// the descriptor of a child block and its ParentStateRoot: the fields an actor proof reads (no receipts: the root is a placeholder)
+struct ActorDesc {
+    std::array<uint8_t, IPCFP_CID_LEN> receipts{};
+    ipcfp_tipset_desc d;
+    ActorDesc(const Cid& child, const Cid& parent_state_root) {
+        memset(&d, 0, sizeof d);
+        d.child_cid = child.bytes.data();
+        d.child_parent_state_root = parent_state_root.bytes.data();
+        d.receipts_root = receipts.data();
+    }
+};
+}  // namespace detail
+inline ActorProofs generate_actor_proofs(GpuBlockstore& store, const Cid& child, const Cid& parent_state_root, const std::vector<ipcfp_address>& addrs,
+                                         const std::vector<Cid>& evm_code_cids, bool with_code) {
+    detail::ActorDesc t(child, parent_state_root);
+    const std::vector<uint8_t> evm = detail::cid_bytes(evm_code_cids);
+    ipcfp_actor_result* r = nullptr;
+    check(ipcfp_generate_actor_proofs(store.raw(), &t.d, addrs.data(), addrs.size(), evm.data(), evm_code_cids.size(),
+                                      with_code ? IPCFP_ACTOR_WITH_CODE : 0u, &r), "generate_actor_proofs");
+    ActorProofs out;
+    for (uint64_t i = 0; i < r->n_proofs; i++) {
+        ActorProof p;
+        p.c = r->proofs[i];
+        p.bytecode.assign(r->code_blob + p.c.code_off, r->code_blob + p.c.code_off + p.c.code_len);
+        p.witness.assign(r->proof_witness_index + r->proof_witness_offsets[i], r->proof_witness_index + r->proof_witness_offsets[i + 1]);
+        out.proofs.push_back(std::move(p));
+    }
+    out.blocks = proof_blocks(r->witness);
+    ipcfp_actor_result_free(r);
+    return out;
+}
+// ipcfp_plan_fetch_actor_proofs_resident: one fetch round (the CIDs the store lacks, `Cid` order) for generate_actor_proofs
+inline std::vector<Cid> plan_fetch_actor_proofs(GpuBlockstore& store, const Cid& child, const Cid& parent_state_root, const std::vector<ipcfp_address>& addrs,
+                                                const std::vector<Cid>& evm_code_cids, bool with_code) {
+    detail::ActorDesc t(child, parent_state_root);
+    const std::vector<uint8_t> evm = detail::cid_bytes(evm_code_cids);
+    ipcfp_tipset* tip = nullptr;
+    check(ipcfp_tipset_upload(store.raw(), &t.d, &tip), "ipcfp_tipset_upload");
+    ipcfp_fetch_plan* p = nullptr;
+    const ipcfp_status st = ipcfp_plan_fetch_actor_proofs_resident(store.raw(), tip, addrs.data(), addrs.size(), evm.data(), evm_code_cids.size(),
+                                                                   with_code ? IPCFP_ACTOR_WITH_CODE : 0u, &p);
+    ipcfp_tipset_free(tip);
+    check(st, "plan_fetch_actor_proofs");
+    std::vector<Cid> out;
+    for (uint64_t k = 0; k < p->n_missing; k++) out.push_back(Cid::from_bytes(p->cids + IPCFP_CID_LEN * k));
+    ipcfp_fetch_plan_free(p);
+    return out;
+}
+// ipcfp_verify_actor_proofs over the proofs' blocks (a store of them with every block checked against its CID): one verdict per proof
+inline std::vector<bool> verify_actor_proofs(const ActorProofs& ap, const Cid& child, const Cid& parent_state_root, const std::vector<Cid>& evm_code_cids,
+                                             bool with_code, int device = 0) {
+    GpuBlockstore store = GpuBlockstore::from_witness(ap.blocks, device);
+    detail::ActorDesc t(child, parent_state_root);
+    const std::vector<uint8_t> evm = detail::cid_bytes(evm_code_cids);
+    std::vector<ipcfp_actor_proof> qs;
+    for (const ActorProof& p : ap.proofs) qs.push_back(p.c);
+    std::vector<uint8_t> res(qs.size() + 1, 0);
+    check(ipcfp_verify_actor_proofs(store.raw(), &t.d, qs.data(), qs.size(), evm.data(), evm_code_cids.size(), with_code ? IPCFP_ACTOR_WITH_CODE : 0u,
+                                    res.data()), "verify_actor_proofs");
+    return std::vector<bool>(res.begin(), res.begin() + qs.size());
+}
+
 // the UnifiedProofBundle of an ipcfp_bundle, which it frees
 inline UnifiedProofBundle unified_bundle(ipcfp_bundle* b, const TipsetDesc& t) {
     UnifiedProofBundle u;

@@ -561,6 +561,73 @@ pub fn resolve_eth_address_to_actor_id_gpu(store: &GpuBlockstore, state_root: &C
     Ok(id)
 }
 
+/// An actor proof: the C record (actor_id, sequence, balance, code, head, delegated address, the EVM fields, `status`) with the bytecode
+/// when asked for, and the blocks that prove it.
+pub struct ActorProofGpu {
+    pub proof: sys::ipcfp_actor_proof,
+    pub bytecode: Vec<u8>,
+    pub blocks: Vec<ProofBlock>,
+}
+
+/// `ipcfp_generate_actor_proofs`: what the state tree under `child`'s ParentStateRoot holds for each address (`Address::to_bytes()`),
+/// or a proven absence. `evm_code_cids`: the EVM actor code CIDs of the network's manifests; `with_code`: the bytecode joins the proof.
+pub fn generate_actor_proofs_gpu(
+    store: &GpuBlockstore,
+    child: &Cid,
+    parent_state_root: &Cid,
+    addresses: &[Vec<u8>],
+    evm_code_cids: &[Cid],
+    with_code: bool,
+) -> Result<Vec<ActorProofGpu>> {
+    let mut addrs = Vec::with_capacity(addresses.len());
+    for a in addresses {
+        if a.is_empty() || a.len() > sys::IPCFP_ADDRESS_MAX {
+            bail!("address of {} bytes", a.len());
+        }
+        let mut c = sys::ipcfp_address { len: a.len() as u8, bytes: [0u8; sys::IPCFP_ADDRESS_MAX] };
+        c.bytes[..a.len()].copy_from_slice(a);
+        addrs.push(c);
+    }
+    let mut evm = Vec::with_capacity(CID_LEN * evm_code_cids.len());
+    for c in evm_code_cids {
+        evm.extend_from_slice(&cid38(c)?);
+    }
+    let (child_b, root_b, receipts) = (cid38(child)?, cid38(parent_state_root)?, [0u8; CID_LEN]);
+    let mut d: sys::ipcfp_tipset_desc = unsafe { std::mem::zeroed() };
+    d.child_cid = child_b.as_ptr();
+    d.child_parent_state_root = root_b.as_ptr();
+    d.receipts_root = receipts.as_ptr();   // not read by actor proofs
+    let flags = if with_code { sys::IPCFP_ACTOR_WITH_CODE } else { 0 };
+    let mut out = std::ptr::null_mut();
+    check(unsafe {
+        sys::ipcfp_generate_actor_proofs(store.h, &d, addrs.as_ptr(), addrs.len() as u64, evm.as_ptr(), evm_code_cids.len() as u64, flags, &mut out)
+    })?;
+    let r = unsafe { &*out };
+    let result = (|| {
+        let all = witness_blocks(&r.witness)?;
+        let mut proofs = Vec::with_capacity(r.n_proofs as usize);
+        for i in 0..r.n_proofs as usize {
+            let p = unsafe { *r.proofs.add(i) };
+            let bytecode = if p.code_len > 0 {
+                unsafe { std::slice::from_raw_parts(r.code_blob.add(p.code_off as usize), p.code_len as usize) }.to_vec()
+            } else {
+                Vec::new()
+            };
+            let (lo, hi) = unsafe { (*r.proof_witness_offsets.add(i), *r.proof_witness_offsets.add(i + 1)) };
+            let blocks = (lo..hi)
+                .map(|k| {
+                    let b = &all[unsafe { *r.proof_witness_index.add(k as usize) } as usize];
+                    ProofBlock { cid: b.cid, data: b.data.clone() }
+                })
+                .collect();
+            proofs.push(ActorProofGpu { proof: p, bytecode, blocks });
+        }
+        Ok(proofs)
+    })();
+    unsafe { sys::ipcfp_actor_result_free(out) };
+    result
+}
+
 /// `generate_proof_bundle` (`src/proofs/generator.rs:25-95`): ONE store built from everything the RPC layer fetched for this tipset
 /// pair, storage specs first, then event specs, then the `BTreeSet<(Cid, Vec<u8>)>` union of the witnesses.
 pub fn generate_proof_bundle_gpu(

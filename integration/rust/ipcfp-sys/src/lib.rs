@@ -24,6 +24,7 @@ pub const IPCFP_SHARDED_UNION_TO_HOST: u32 = 0x2;
 pub const IPCFP_SHARDED_UNION_FULL: u32 = 0x4;
 pub const IPCFP_WITNESS_BY_REFERENCE: u32 = 0x8;
 pub const IPCFP_RESULT_JSON: u32 = 0x10;
+pub const IPCFP_ACTOR_WITH_CODE: u32 = 0x20;
 pub const IPCFP_COMM_ID_BYTES: usize = 128;
 
 #[repr(C)] pub struct ipcfp_store { _p: [u8; 0] }
@@ -143,6 +144,21 @@ pub struct ipcfp_address { pub len: u8, pub bytes: [u8; IPCFP_ADDRESS_MAX] }
 #[repr(C)]
 pub struct ipcfp_resolve_result { pub n: u64, pub actor_ids: *const u64, pub status: *const ipcfp_status, pub init_status: ipcfp_status, pub _pad: u32,
                                   pub n_missing: u64, pub missing_cids: *const u8, pub witness: ipcfp_witness, pub ms_total: f32, pub ms_lookup: f32 }
+pub const IPCFP_ACTOR_MAX: u64 = 65536;
+pub const IPCFP_ACTOR_FOUND: u32 = 0;
+pub const IPCFP_ACTOR_NO_ADDRESS: u32 = 1;
+pub const IPCFP_ACTOR_NO_ACTOR: u32 = 2;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct ipcfp_actor_proof { pub actor_id: u64, pub sequence: u64, pub evm_nonce: u64, pub code_off: u64, pub code_len: u64, pub status: u32,
+                               pub balance_negative: u8, pub has_delegated: u8, pub is_evm: u8, pub _pad0: u8, pub balance: [u8; 32],
+                               pub code: [u8; 38], pub head: [u8; 38], pub bytecode_cid: [u8; 38], pub contract_state: [u8; 38],
+                               pub bytecode_hash: [u8; 32], pub address: ipcfp_address, pub delegated: ipcfp_address, pub _pad1: [u8; 4] }
+#[repr(C)]
+pub struct ipcfp_actor_result { pub n_proofs: u64, pub proofs: *const ipcfp_actor_proof, pub witness: ipcfp_witness,
+                                pub proof_witness_offsets: *const u64, pub proof_witness_index: *const u32, pub code_blob: *const u8,
+                                pub code_blob_size: u64, pub ms_total: f32, pub ms_init: f32, pub ms_walk: f32, pub ms_code: f32, pub ms_witness: f32,
+                                pub host_syncs: u32 }
 #[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
                           pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
@@ -243,6 +259,15 @@ extern "C" {
     pub fn ipcfp_resolve_result_free(r: *mut ipcfp_resolve_result);
     pub fn ipcfp_address_parse(text: *const c_char, len: u64, out: *mut ipcfp_address) -> ipcfp_status;
     pub fn ipcfp_address_from_eth(eth: *const u8, out: *mut ipcfp_address) -> ipcfp_status;
+    pub fn ipcfp_generate_actor_proofs_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, addrs: *const ipcfp_address, n: u64,
+                                                evm_code_cids: *const u8, n_evm: u64, flags: u32, out: *mut *mut ipcfp_actor_result) -> ipcfp_status;
+    pub fn ipcfp_generate_actor_proofs(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, addrs: *const ipcfp_address, n: u64,
+                                       evm_code_cids: *const u8, n_evm: u64, flags: u32, out: *mut *mut ipcfp_actor_result) -> ipcfp_status;
+    pub fn ipcfp_actor_result_free(r: *mut ipcfp_actor_result);
+    pub fn ipcfp_plan_fetch_actor_proofs_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, addrs: *const ipcfp_address, n: u64,
+                                                  evm_code_cids: *const u8, n_evm: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_verify_actor_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_actor_proof, n: u64,
+                                     evm_code_cids: *const u8, n_evm: u64, flags: u32, results: *mut u8) -> ipcfp_status;
 
     pub fn ipcfp_bundle_to_json(b: *const ipcfp_bundle, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_event_result_to_json(r: *const ipcfp_event_result, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;

@@ -29,6 +29,7 @@ SHARDED_UNION_TO_HOST = 0x2
 SHARDED_UNION_FULL = 0x4
 WITNESS_BY_REFERENCE = 0x8
 RESULT_JSON = 0x10
+ACTOR_WITH_CODE = 0x20
 COMM_ID_BYTES = 128
 
 
@@ -295,6 +296,78 @@ def resolve_result_from_c(r):
     return ResolveResultPy(_arr(r.actor_ids, n, np.uint64), _arr(r.status, n, np.int32), int(r.init_status),
                            _arr(r.missing_cids, m * CID_LEN, np.uint8).reshape(m, CID_LEN), witness_from_c(r.witness), float(r.ms_total),
                            float(r.ms_lookup))
+
+
+# Actor proofs (include/ipcfp.h, "Actor proofs")
+ACTOR_MAX = 65536
+ACTOR_FOUND, ACTOR_NO_ADDRESS, ACTOR_NO_ACTOR = 0, 1, 2
+
+
+class ActorProofC(C.Structure):
+    """ipcfp_actor_proof (400 bytes)."""
+    _fields_ = [("actor_id", C.c_uint64), ("sequence", C.c_uint64), ("evm_nonce", C.c_uint64), ("code_off", C.c_uint64), ("code_len", C.c_uint64),
+                ("status", C.c_uint32), ("balance_negative", C.c_uint8), ("has_delegated", C.c_uint8), ("is_evm", C.c_uint8), ("_pad0", C.c_uint8),
+                ("balance", C.c_uint8 * 32), ("code", C.c_uint8 * CID_LEN), ("head", C.c_uint8 * CID_LEN), ("bytecode_cid", C.c_uint8 * CID_LEN),
+                ("contract_state", C.c_uint8 * CID_LEN), ("bytecode_hash", C.c_uint8 * 32), ("address", AddressC), ("delegated", AddressC),
+                ("_pad1", C.c_uint8 * 4)]
+
+
+class ActorResultC(C.Structure):
+    """ipcfp_actor_result (ipcfp_generate_actor_proofs_resident)."""
+    _fields_ = [("n_proofs", C.c_uint64), ("proofs", C.c_void_p), ("witness", Witness), ("proof_witness_offsets", C.c_void_p),
+                ("proof_witness_index", C.c_void_p), ("code_blob", C.c_void_p), ("code_blob_size", C.c_uint64), ("ms_total", C.c_float),
+                ("ms_init", C.c_float), ("ms_walk", C.c_float), ("ms_code", C.c_float), ("ms_witness", C.c_float), ("host_syncs", C.c_uint32)]
+
+
+@dataclass
+class ActorProof:
+    """What the state tree holds for `address` (Address::to_bytes()): status ACTOR_*, the actor ID, ActorState's code, head, sequence,
+    balance (a signed int) and delegated address (bytes or None), and for an EVM actor its bytecode CID and hash, EVM nonce, storage root
+    (contract_state) and, with ACTOR_WITH_CODE, its bytecode."""
+    address: bytes
+    status: int
+    actor_id: int
+    code: bytes
+    head: bytes
+    sequence: int
+    balance: int
+    delegated: bytes
+    is_evm: bool
+    bytecode_cid: bytes
+    bytecode_hash: bytes
+    evm_nonce: int
+    contract_state: bytes
+    bytecode: bytes = None
+
+
+def actor_proof_from_c(p, blob=b""):
+    mag = int.from_bytes(bytes(p.balance), "big")
+    return ActorProof(p.address.to_bytes(), int(p.status), int(p.actor_id), bytes(p.code), bytes(p.head), int(p.sequence),
+                      -mag if p.balance_negative else mag, p.delegated.to_bytes() if p.has_delegated else None, bool(p.is_evm),
+                      bytes(p.bytecode_cid), bytes(p.bytecode_hash), int(p.evm_nonce), bytes(p.contract_state),
+                      blob[int(p.code_off):int(p.code_off) + int(p.code_len)] if p.code_len and blob else None)
+
+
+@dataclass
+class ActorResultPy:
+    proofs: list            # ActorProof per request
+    witness: "WitnessPy"
+    proof_witness: list     # per proof: indices into witness
+    raw_proofs: np.ndarray  # packed ipcfp_actor_proof records (for the verifier)
+    timings: dict = field(default_factory=dict)
+    host_syncs: int = 0
+
+
+def actor_result_from_c(r):
+    n = int(r.n_proofs)
+    raw = _arr(r.proofs, n * C.sizeof(ActorProofC), np.uint8)
+    blob = C.string_at(r.code_blob, int(r.code_blob_size)) if r.code_blob_size else b""
+    recs = (ActorProofC * max(n, 1)).from_buffer_copy(raw.tobytes() or bytes(C.sizeof(ActorProofC)))
+    offs = _arr(r.proof_witness_offsets, n + 1, np.uint64)
+    idx = _arr(r.proof_witness_index, int(offs[-1]) if n else 0, np.uint32)
+    timings = dict(total=r.ms_total, init=r.ms_init, walk=r.ms_walk, code=r.ms_code, witness=r.ms_witness)
+    return ActorResultPy([actor_proof_from_c(recs[i], blob) for i in range(n)], witness_from_c(r.witness),
+                         [idx[int(offs[i]):int(offs[i + 1])].tolist() for i in range(n)], raw, timings, int(r.host_syncs))
 
 
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)

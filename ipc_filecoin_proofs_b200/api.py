@@ -106,6 +106,11 @@ SIGNATURES = {
     "ipcfp_resolve_result_free": (None, [_P(A.ResolveResultC)]),
     "ipcfp_address_parse": (_st, [C.c_char_p, _u64, _P(A.AddressC)]),
     "ipcfp_address_from_eth": (_st, [_vp, _P(A.AddressC)]),
+    "ipcfp_generate_actor_proofs_resident": (_st, [_vp, _vp, _P(A.AddressC), _u64, _vp, _u64, _u32, _PP(A.ActorResultC)]),
+    "ipcfp_generate_actor_proofs": (_st, [_vp, _P(A.TipsetDesc), _P(A.AddressC), _u64, _vp, _u64, _u32, _PP(A.ActorResultC)]),
+    "ipcfp_actor_result_free": (None, [_P(A.ActorResultC)]),
+    "ipcfp_plan_fetch_actor_proofs_resident": (_st, [_vp, _vp, _P(A.AddressC), _u64, _vp, _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_verify_actor_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _u32, _vp]),
     "ipcfp_bundle_to_json": (_st, _TO_JSON),
     "ipcfp_event_result_to_json": (_st, _TO_JSON),
     "ipcfp_json_free": (None, [_vp]),
@@ -654,6 +659,20 @@ class BlockStore:
         return _result("ipcfp_resolve_addresses", A.ResolveResultC, A.resolve_result_from_c, "ipcfp_resolve_result_free", self._h,
                        root.ctypes.data, addrs, len(addresses))
 
+    def generate_actor_proofs_resident(self, tip, addresses, evm_code_cids=(), with_code=False, flags=0):
+        """ipcfp_generate_actor_proofs_resident → A.ActorResultPy: per address (an int actor ID, "f…" / "t…" text, "0x…" Ethereum
+        address or Address::to_bytes()) its actor's fields, or a proven absence. evm_code_cids: the EVM actor code CIDs (38 bytes each).
+        with_code: ACTOR_WITH_CODE (the bytecode joins the proof). flags: WITNESS_BY_REFERENCE."""
+        addrs, n, ev, n_ev, fl = _actor_args(addresses, evm_code_cids, with_code, flags)
+        return _result("ipcfp_generate_actor_proofs_resident", A.ActorResultC, A.actor_result_from_c, "ipcfp_actor_result_free", self._h,
+                       tip._h, addrs, n, ev.ctypes.data if n_ev else None, n_ev, fl)
+
+    def plan_fetch_actor_proofs(self, tip, addresses, evm_code_cids=(), with_code=False, flags=0):
+        """ipcfp_plan_fetch_actor_proofs_resident → A.FetchPlanPy: one fetch round for generate_actor_proofs_resident."""
+        addrs, n, ev, n_ev, fl = _actor_args(addresses, evm_code_cids, with_code, flags)
+        return _result("ipcfp_plan_fetch_actor_proofs_resident", *_FETCH_PLAN, self._h, tip._h, addrs, n, ev.ctypes.data if n_ev else None,
+                       n_ev, fl)
+
     def close(self):
         if self._h:
             lib().ipcfp_store_destroy(self._h)
@@ -893,6 +912,56 @@ def resolve_until_complete(fetch, state_root, addresses, device=0, verify_cids=T
         store.close()
         store = make_store()
     raise RuntimeError("resolve_until_complete: no fixed point after %d rounds" % max_rounds)
+
+
+def actor_address(a):
+    """An actor proof's request → Address::to_bytes(): an int is an actor ID, text is "0x…" (address_from_eth) or "f…" / "t…"
+    (address_parse), bytes are taken as they are."""
+    if isinstance(a, int):
+        if not 0 <= a < 2 ** 64:
+            raise ValueError(f"actor ID {a} out of range")
+        out = bytearray([0])
+        while a >= 0x80:
+            out.append((a & 0x7F) | 0x80)
+            a >>= 7
+        out.append(a)
+        return bytes(out)
+    if isinstance(a, str):
+        return address_from_eth(a) if a.startswith("0x") else address_parse(a)
+    return bytes(a)
+
+
+def _actor_args(addresses, evm_code_cids, with_code, flags):
+    raw = [actor_address(a) for a in addresses]
+    ev = np.ascontiguousarray(np.frombuffer(b"".join(bytes(c) for c in evm_code_cids), dtype=np.uint8)) if len(evm_code_cids) else np.zeros(0, np.uint8)
+    if ev.size % A.CID_LEN:
+        raise ValueError("evm_code_cids must be 38-byte CIDs")
+    return A.make_addresses(raw), len(raw), ev, ev.size // A.CID_LEN, flags | (A.ACTOR_WITH_CODE if with_code else 0)
+
+
+def fetch_actor_proofs_until_complete(fetch, upload_tipset, addresses, evm_code_cids=(), with_code=False, device=0, verify_cids=True,
+                                      max_rounds=10000):
+    """fetch_until_complete for generate_actor_proofs_resident(tip, addresses, evm_code_cids, with_code): the same loop, planned with
+    plan_fetch_actor_proofs."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch_actor_proofs(tip, addresses, evm_code_cids, with_code), fetch, upload_tipset, device,
+                       verify_cids, max_rounds)
+
+
+def verify_actor_proofs(witness, ts, result, evm_code_cids=(), with_code=False, device=0):
+    """ipcfp_verify_actor_proofs over the witness (WitnessPy) as a CID-checked store: every proof of `result` (A.ActorResultPy, or packed
+    ipcfp_actor_proof records) replayed against the tipset `ts` → list of bools."""
+    raw = np.ascontiguousarray(result.raw_proofs if hasattr(result, "raw_proofs") else result, dtype=np.uint8)
+    n = raw.size // C.sizeof(A.ActorProofC)
+    _, _, ev, n_ev, fl = _actor_args([], evm_code_cids, with_code, 0)
+    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
+    try:
+        d, keep = A.make_tipset_desc(ts)
+        res = np.zeros(max(n, 1), dtype=np.uint8)
+        _check(lib().ipcfp_verify_actor_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, ev.ctypes.data if n_ev else None, n_ev,
+                                               fl, res.ctypes.data))
+        return [bool(x) for x in res[:n]]
+    finally:
+        store.close()
 
 
 def tipset_desc_from_json(parent_text, child_text, receipts_text):

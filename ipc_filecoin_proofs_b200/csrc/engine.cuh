@@ -446,6 +446,28 @@ void resolve_addresses(Store* s, const uint8_t* state_root, const ipcfp_address*
 void address_parse(const char* text, uint64_t len, ipcfp_address& out);
 void address_from_eth(const uint8_t eth[20], ipcfp_address& out);
 
+// actor.cu — ipcfp_generate_actor_proofs_resident (DESIGN.md §2, "Actor proofs"); the planner (plan.cu) and the verifier (verify.cu) share
+// its refusals and its upload
+struct ActorArgs;
+// the refusals made before any device work (include/ipcfp.h); returns the number of addresses that are not ID addresses
+uint64_t actor_request_check(const ipcfp_address* addrs, uint64_t n, const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags);
+// one upload of a call's inputs (the child CID, the state root, the EVM code CIDs, the addresses) on the store's stream
+struct ActorUpload {
+    AsyncBuf<uint8_t> d;
+    uint64_t o_evm = 0, o_addrs = 0;
+    ActorUpload(Store* s, const uint8_t* child_cid, const uint8_t* state_root, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm,
+                uint64_t n_evm);
+    void fill(ActorArgs& a, const StoreView& v, uint64_t n, uint64_t n_evm, uint32_t flags) const;   // inputs, sizes, flags
+};
+ipcfp_actor_result* generate_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm_code_cids, uint64_t n_evm,
+                                          uint32_t flags);
+void actor_result_free(ipcfp_actor_result* r);
+// plan.cu — ipcfp_plan_fetch_actor_proofs_resident; verify.cu — ipcfp_verify_actor_proofs
+void plan_fetch_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm_code_cids, uint64_t n_evm,
+                             uint32_t flags, FetchPlan& out);
+void verify_actor_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_actor_proof* proofs, uint64_t n, const uint8_t* evm_code_cids,
+                         uint64_t n_evm, uint32_t flags, uint8_t* results);
+
 // json.cu — IPCFP_RESULT_JSON: the EventProofBundle text of one call from what is on the device after k_witness_emit (all pointers device)
 struct JsonInputs {
     const ipcfp_event_proof* proofs;   // n_proofs slots as pass 2 wrote them (skipped slots included)

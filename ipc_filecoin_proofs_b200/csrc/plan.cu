@@ -96,6 +96,13 @@ __global__ void __launch_bounds__(128) k_plan_storage(StorageArgs a, uint32_t* n
     if (c) plan_miss(miss, ctr, c);
 }
 
+__global__ void __launch_bounds__(128) k_plan_actors(ActorArgs a, uint32_t* needed, uint8_t* miss, unsigned long long* ctr) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.n) return;
+    const uint8_t* c = plan_actor_path(a, t, needed);
+    if (c) plan_miss(miss, ctr, c);
+}
+
 __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, unsigned long long* out) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t c = w < nwords ? (uint32_t)__popc(bits[w]) : 0u;
@@ -284,6 +291,44 @@ void plan_fetch_messages(Store* s, TipsetDev& td, const uint8_t* message_cids, u
     }
     if (have_order) message_selection_mask(s, td, exo, message_cids, n, has.p);
     plan_fetch(s, td, nullptr, 0, nullptr, 0, out, filter ? filter : &any, 1, has.p);
+}
+
+// ipcfp_plan_fetch_actor_proofs_resident: each request's walks up to the first block the store lacks (plan_actor_path), one thread each
+void plan_fetch_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm, uint64_t n_evm, uint32_t flags,
+                             FetchPlan& out) {
+    actor_request_check(addrs, n, evm, n_evm, flags);
+    if (!td.has_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+    s->use();
+    cudaStream_t st = s->stream;
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_BEGIN], st));
+    const uint64_t nwords = (s->n + 31) / 32 + 1;
+    ActorUpload up(s, td.child_cid, td.child_state_root, addrs, n, evm, n_evm);
+    ActorArgs a{};
+    up.fill(a, s->view, n, n_evm, flags);
+    AsyncBuf<uint32_t> needed(nwords, st);
+    needed.zero();
+    AsyncBuf<unsigned long long> ctr(PC_COUNT, st);
+    ctr.zero();
+    AsyncBuf<uint8_t> miss(38 * n + 16, st);
+    if (n) { k_plan_actors<<<div_up(n, 128), 128, 0, st>>>(a, needed.p, miss.p, ctr.p); IPCFP_LAUNCH_CHECK(); }
+    k_plan_popc<<<div_up(nwords, 256), 256, 0, st>>>(needed.p, nwords, ctr.p + PC_NEEDED); IPCFP_LAUNCH_CHECK();
+    PinnedArray hc(s->pool, PC_COUNT * 8);
+    IPCFP_CUDA(cudaMemcpyAsync(hc.p, ctr.p, PC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    const uint64_t n_miss = hc.as<unsigned long long>()[PC_MISSING];
+    out.n_needed = hc.as<unsigned long long>()[PC_NEEDED];
+    out.n_levels = 0;
+    uint64_t m = 0, mixed = UINT64_MAX;
+    if (n_miss) {
+        AsyncBuf<uint8_t> sorted(38 * n_miss + 16, st);
+        m = sort_unique_cids(st, miss.p, n_miss, sorted.p, &mixed);
+        out.cids.resize(38 * m);
+        IPCFP_CUDA(cudaMemcpyAsync(out.cids.data(), sorted.p, 38 * m, cudaMemcpyDeviceToHost, st));
+    }
+    IPCFP_CUDA(cudaEventRecord(s->ev[EV_END], st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    IPCFP_CUDA(cudaEventElapsedTime(&out.ms_total, s->ev[EV_BEGIN], s->ev[EV_END]));
+    if (mixed != UINT64_MAX) sort_cids_host(out.cids);
 }
 
 }  // namespace ipcfp

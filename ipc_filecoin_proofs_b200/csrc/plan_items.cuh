@@ -4,6 +4,7 @@
 // amt_node_begin (ipld.cuh), walk_events and receipts_get (events_items.cuh), storage_proof_one (storage.cuh).
 #pragma once
 #include "events_items.cuh"
+#include "actor_items.cuh"
 #include "storage.cuh"
 
 namespace ipcfp {
@@ -97,6 +98,22 @@ __device__ __forceinline__ const uint8_t* plan_storage_path(const StorageArgs& a
     ipcfp_storage_proof q;
     Fail f{0, 0};
     if (storage_proof_one(a, t, rec, q, f) || f.code != DC_MISSING) return nullptr;
+    return rec.missing;
+}
+// ipcfp_generate_actor_proofs_resident for request t: the header, the Init path (a non-ID address; the generator walks it once per
+// call, the planner once per request), then actor_proof_one. A path the generator fails on for another reason ends here.
+__device__ __forceinline__ const uint8_t* plan_actor_path(const ActorArgs& a, uint64_t t, uint32_t* needed) {
+    Recorder rec{nullptr, 0, needed, false};
+    rec.rank_of = a.store.rank_of;
+    Fail f{0, 0}, init_fail{0, 0};
+    const uint8_t* psr;
+    if (!actor_header(a, rec, psr, f)) return f.code == DC_MISSING ? rec.missing : nullptr;
+    const uint8_t* map = nullptr;
+    if (a.addrs[t].bytes[0] != 0 && !resolve_init(a.store, rec, psr, map, init_fail)) return init_fail.code == DC_MISSING ? rec.missing : nullptr;
+    ipcfp_actor_proof q;
+    memset(&q, 0, sizeof q);
+    uint64_t cb;
+    if (actor_proof_one(a, a.addrs[t], map, init_fail, rec, q, cb, f) || f.code != DC_MISSING) return nullptr;
     return rec.missing;
 }
 

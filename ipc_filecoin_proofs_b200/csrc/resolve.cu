@@ -68,42 +68,11 @@ __global__ void __launch_bounds__(128) k_resolve(ResolveArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------ host: address codecs
-// unsigned_varint::decode::u64 followed by "no bytes left" (fvm_shared from_leb_bytes): at most 10 bytes, minimal, no overflow
-static bool leb_u64(const uint8_t* p, uint32_t n, uint32_t& used, uint64_t& v) {
-    v = 0;
-    for (uint32_t i = 0; i < n && i < 10; i++) {
-        const uint64_t b = p[i] & 0x7f;
-        if (i == 9 && b > 1) return false;
-        v |= b << (7 * i);
-        if (!(p[i] & 0x80)) {
-            if (i > 0 && p[i] == 0) return false;   // a trailing zero group is not minimal
-            used = i + 1;
-            return true;
-        }
-    }
-    return false;
-}
 static uint32_t leb_put(uint64_t v, uint8_t* out) {
     uint32_t k = 0;
     while (v >= 0x80) { out[k++] = (uint8_t)(v | 0x80); v >>= 7; }
     out[k++] = (uint8_t)v;
     return k;
-}
-
-// fvm_shared Address::from_bytes accepts a; *id = the ID of a protocol-0 address
-static bool address_valid(const ipcfp_address& a, uint64_t* id) {
-    if (a.len < 1 || a.len > IPCFP_ADDRESS_MAX) return false;
-    const uint8_t* p = a.bytes + 1;
-    const uint32_t n = a.len - 1u;
-    uint32_t used;
-    uint64_t v;
-    switch (a.bytes[0]) {
-        case 0: if (!leb_u64(p, n, used, v) || used != n) return false; if (id) *id = v; return true;
-        case 1: case 2: return n == 20;
-        case 3: return n == 48;
-        case 4: return leb_u64(p, n, used, v) && n - used <= 54;
-        default: return false;
-    }
 }
 
 // BLAKE2b with a 4-byte digest (the address checksum): RFC 7693, unkeyed

@@ -9,6 +9,38 @@
 
 namespace ipcfp {
 
+// unsigned_varint::decode::u64 followed by "no bytes left" (fvm_shared from_leb_bytes): at most 10 bytes, minimal, no overflow
+__host__ __device__ inline bool leb_u64(const uint8_t* p, uint32_t n, uint32_t& used, uint64_t& v) {
+    v = 0;
+    for (uint32_t i = 0; i < n && i < 10; i++) {
+        const uint64_t b = p[i] & 0x7f;
+        if (i == 9 && b > 1) return false;
+        v |= b << (7 * i);
+        if (!(p[i] & 0x80)) {
+            if (i > 0 && p[i] == 0) return false;   // a trailing zero group is not minimal
+            used = i + 1;
+            return true;
+        }
+    }
+    return false;
+}
+// fvm_shared Address::from_bytes accepts bytes[0, len); *id = the ID of a protocol-0 address
+__host__ __device__ inline bool address_bytes_valid(const uint8_t* bytes, uint32_t len, uint64_t* id) {
+    if (len < 1 || len > IPCFP_ADDRESS_MAX) return false;
+    const uint8_t* p = bytes + 1;
+    const uint32_t n = len - 1u;
+    uint32_t used = 0;
+    uint64_t v = 0;
+    switch (bytes[0]) {
+        case 0: if (!leb_u64(p, n, used, v) || used != n) return false; if (id) *id = v; return true;
+        case 1: case 2: return n == 20;
+        case 3: return n == 48;
+        case 4: return leb_u64(p, n, used, v) && n - used <= 54;
+        default: return false;
+    }
+}
+__host__ __device__ inline bool address_valid(const ipcfp_address& a, uint64_t* id) { return address_bytes_valid(a.bytes, a.len, id); }
+
 // The Init path: the address_map root of the state tree at state_root (a pointer into the store's block arena). Fails as
 // storage_proof_one fails on the same blocks: DC_MISSING (rec.missing names the block), DC_DECODE, DC_ACTOR_NOT_FOUND (no actor ID 1).
 static __device__ bool resolve_init(const StoreView& s, Recorder& rec, const uint8_t* state_root, const uint8_t*& address_map, Fail& f) {

@@ -207,4 +207,39 @@ void verify_storage_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp
     if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
 }
 
+// ------------------------------------------------------------------------------------------ actor proofs
+__global__ void __launch_bounds__(128) k_verify_actors(VerifyActorArgs a) {
+    const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= a.n || (threadIdx.x & 31)) return;
+    verify_actor_item(a, t);
+}
+
+void verify_actor_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_actor_proof* proofs, uint64_t n, const uint8_t* evm, uint64_t n_evm,
+                         uint32_t flags, uint8_t* results) {
+    s->use();
+    if (!t || !t->child_cid || !t->child_parent_state_root) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor lacks child_cid / parent_state_root");
+    if (n && (!proofs || !results)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+    actor_request_check(nullptr, 0, evm, n_evm, flags);
+    if (n > IPCFP_ACTOR_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more than IPCFP_ACTOR_MAX proofs");
+    for (uint64_t i = 0; i < n; i++)
+        if (!address_valid(proofs[i].address, nullptr)) throw Error(IPCFP_ERR_INVALID_ARG, "bytes that are not an Address", i);
+    if (n == 0) return;
+    cudaStream_t st = s->stream;
+    unsigned long long* dw = s->dev_words.p;
+    uint64_t* hw = s->host_words.p;
+    IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
+    ActorUpload up(s, t->child_cid, t->child_parent_state_root, nullptr, 0, evm, n_evm);
+    AsyncBuf<ipcfp_actor_proof> d_proofs(n, st);
+    AsyncBuf<uint8_t> d_res(n + 16, st);
+    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_actor_proof), cudaMemcpyHostToDevice, st));
+    VerifyActorArgs a{};
+    up.fill(a.g, s->view, 0, n_evm, flags);
+    a.proofs = d_proofs.p; a.n = n; a.results = d_res.p; a.err = dw;
+    k_verify_actors<<<div_up(n * 32, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK();
+    IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
+}
+
 }  // namespace ipcfp

@@ -6,6 +6,7 @@
 #include "engine.cuh"
 #include "events_items.cuh"
 #include "hashes.cuh"
+#include "actor_items.cuh"
 #include "storage.cuh"
 
 namespace ipcfp {
@@ -204,6 +205,41 @@ __device__ __forceinline__ void verify_storage_item(const VerifyStorageArgs& a, 
     if (!read_storage_slot(s, rec, storage_root, p.slot, sv, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
     for (int q = 0; q < 32; q++) if (sv.v32[q] != p.value[q]) return;
     a.results[t] = 1;
+}
+
+struct VerifyActorArgs {
+    ActorArgs g;                        // the generator's inputs: the tipset's CIDs, the EVM code CIDs, with_code
+    const ipcfp_actor_proof* proofs;
+    uint64_t n;
+    uint8_t* results;
+    unsigned long long* err;
+};
+__device__ __forceinline__ bool actor_claims_equal(const ipcfp_actor_proof& q, const ipcfp_actor_proof& p, bool with_code) {
+    bool eq = q.status == p.status && q.actor_id == p.actor_id && q.sequence == p.sequence && q.evm_nonce == p.evm_nonce &&
+              q.balance_negative == p.balance_negative && q.has_delegated == p.has_delegated && q.is_evm == p.is_evm &&
+              q.delegated.len == p.delegated.len && (!with_code || q.code_len == p.code_len);
+    for (int i = 0; i < 32; i++) eq &= q.balance[i] == p.balance[i] && q.bytecode_hash[i] == p.bytecode_hash[i];
+    for (int i = 0; i < 38; i++)
+        eq &= q.code[i] == p.code[i] && q.head[i] == p.head[i] && q.bytecode_cid[i] == p.bytecode_cid[i] && q.contract_state[i] == p.contract_state[i];
+    for (uint32_t i = 0; eq && i < q.delegated.len; i++) eq &= q.delegated.bytes[i] == p.delegated.bytes[i];
+    return eq;
+}
+// Proof t is replayed on the witness (the generator's walk for its address, the Init path included) and must state what the replay
+// finds, absences included. A header naming another ParentStateRoot is a false verdict, as in verify_storage_item.
+__device__ __forceinline__ void verify_actor_item(const VerifyActorArgs& a, uint64_t t) {
+    const ipcfp_actor_proof& p = a.proofs[t];
+    a.results[t] = 0;
+    Recorder rec{nullptr, 0, nullptr, false};   // the verifier records nothing
+    Fail f{0, 0}, init_fail{0, 0};
+    const uint8_t* psr;
+    if (!actor_header(a.g, rec, psr, f)) { if (f.code != DC_STATE_MISMATCH) report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
+    const uint8_t* map = nullptr;
+    if (p.address.bytes[0] != 0 && !resolve_init(a.g.store, rec, psr, map, init_fail)) { report_error(a.err, ST_VERIFY, t, init_fail.code, init_fail.detail); return; }
+    ipcfp_actor_proof q;
+    memset(&q, 0, sizeof q);
+    uint64_t cb;
+    if (!actor_proof_one(a.g, p.address, map, init_fail, rec, q, cb, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
+    a.results[t] = actor_claims_equal(q, p, a.g.with_code != 0);
 }
 
 }  // namespace ipcfp
