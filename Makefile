@@ -4,7 +4,7 @@ NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CSRC      := ipc_filecoin_proofs_b200/csrc
 NVFLAGS   := -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr
-CU_SRCS   := $(CSRC)/store.cu $(CSRC)/events.cu $(CSRC)/storage.cu $(CSRC)/storage_path.cu $(CSRC)/witness.cu $(CSRC)/prims.cu $(CSRC)/parallel.cu $(CSRC)/verify.cu $(CSRC)/json.cu $(CSRC)/json_parse.cu $(CSRC)/rpc_json.cu $(CSRC)/rpc_blocks.cu $(CSRC)/car.cu $(CSRC)/plan.cu $(CSRC)/resolve.cu $(CSRC)/actor.cu $(CSRC)/capi.cu
+CU_SRCS   := $(CSRC)/store.cu $(CSRC)/events.cu $(CSRC)/storage.cu $(CSRC)/storage_path.cu $(CSRC)/witness.cu $(CSRC)/prims.cu $(CSRC)/parallel.cu $(CSRC)/verify.cu $(CSRC)/json.cu $(CSRC)/json_parse.cu $(CSRC)/rpc_json.cu $(CSRC)/rpc_blocks.cu $(CSRC)/car.cu $(CSRC)/plan.cu $(CSRC)/resolve.cu $(CSRC)/actor.cu $(CSRC)/message_proof.cu $(CSRC)/capi.cu
 CU_OBJS   := $(CU_SRCS:.cu=.o)
 CU_HDRS   := $(wildcard $(CSRC)/*.cuh) include/ipcfp.h
 LIB       := ipc_filecoin_proofs_b200/libipcfp.so
@@ -54,6 +54,6 @@ clean:
 
 # The host-compiled device headers (tests/host_fuzz) and the JSON parser under AddressSanitizer + UBSan (DESIGN.md §7.12)
 sanitize:
-	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_tail_bytes_host.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py tests/test_rpc_json_host.py tests/test_rpc_blocks_host.py tests/test_car_host.py tests/test_plan_fetch_host.py tests/test_resolve_host.py tests/test_log_filter_host.py tests/test_log_bundle_host.py tests/test_message_proof_host.py tests/test_storage_paths_host.py tests/test_actor_host.py -q
+	IPCFP_HOST_FUZZ_SANITIZE=1 python -m pytest tests/test_host_fuzz.py tests/test_tail_bytes_host.py tests/test_bundle_json.py tests/test_json_items_host.py tests/test_json_unified_host.py tests/test_json_parse_host.py tests/test_rpc_json_host.py tests/test_rpc_blocks_host.py tests/test_car_host.py tests/test_plan_fetch_host.py tests/test_resolve_host.py tests/test_log_filter_host.py tests/test_log_bundle_host.py tests/test_message_proof_host.py tests/test_storage_paths_host.py tests/test_actor_host.py tests/test_message_proofs_host.py -q
 
 .PHONY: all clean sanitize

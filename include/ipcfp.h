@@ -818,6 +818,102 @@ ipcfp_status ipcfp_verify_actor_proofs(ipcfp_store* witness_store, const ipcfp_t
                                        const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags, uint8_t* results);
 
 /* ------------------------------------------------------------------------------------------
+ * Message proofs: whether a message executed in the tipset pair and how it ended — its receipt's exit code, return data, gas used and
+ * events root — and, with IPCFP_MESSAGE_WITH_BODY, the message itself (DESIGN.md §2 "Message proofs", §3). The status / gasUsed half of
+ * eth_getTransactionReceipt, with the fields eth_getTransactionByHash returns. A request is a message CID as the parent blocks' message
+ * AMTs hold it (the request of ipcfp_generate_message_log_proof_resident); duplicates are allowed. Request j's execution position is
+ * found in the execution order the event calls rebuild, and its receipt is Amtv0<Receipt>::get(exec_index) under the tipset's
+ * receipts_root. The tipset's RPC receipt list (events_roots, n_receipts) and every events AMT are not read.
+ * Decode contract of the new fields (the rest is DESIGN.md §3's):
+ *   Receipt        [exit_code, return_data, gas_used, events_root | null], exactly; exit_code at most 2^32-1, gas_used a u64;
+ *   message block  decided by its shape: array(10) is a Message [version, to, from, sequence, value, gas_limit, gas_fee_cap, gas_premium,
+ *                  method_num, params]; array(2) is a SignedMessage [Message, Signature]; anything else is IPCFP_ERR_DECODE.
+ *                  version, sequence, gas_limit and method_num are unsigned integers (a negative one: IPCFP_ERR_DECODE); to and from
+ *                  bytes Address::from_bytes accepts; value, gas_fee_cap and gas_premium TokenAmounts (the balance rule of actor
+ *                  proofs); params bytes; the Signature bytes whose first byte is its type, 1 secp256k1, 2 BLS or 3 delegated (any
+ *                  other byte, or no byte: IPCFP_ERR_DECODE). Nothing may follow the block's one item.
+ * ------------------------------------------------------------------------------------------ */
+#define IPCFP_MESSAGE_WITH_BODY 0x40u   /* flag: the message block of every executed request joins the witness; its fields are decoded */
+enum {
+    IPCFP_MESSAGE_EXECUTED = 0,         /* executed, with its receipt in every receipt field                                       */
+    IPCFP_MESSAGE_NOT_EXECUTED = 1,     /* not in the execution order; exec_index is UINT64_MAX and every other field is 0          */
+    IPCFP_MESSAGE_NO_RECEIPT = 2        /* executed, but the receipts AMT has no entry at exec_index; the receipt fields are 0      */
+};
+/* 400 bytes, 8-byte aligned; every byte not named by a field is zero. Offsets: exec_index 0, gas_used 8, return_off 16, return_len 24,
+ * version 32, sequence 40, gas_limit 48, method_num 56, params_off 64, params_len 72, status 80, exit_code 84, has_events_root 88,
+ * has_body 89, sig_type 90, value_negative 91, gas_fee_cap_negative 92, gas_premium_negative 93, value 96, gas_fee_cap 128,
+ * gas_premium 160, message_cid 192, events_root 230, to 268, from 334. */
+typedef struct ipcfp_message_proof {
+    uint64_t exec_index;                /* position in the execution order; UINT64_MAX when not executed                          */
+    uint64_t gas_used;                  /* Receipt.gas_used                                                                       */
+    uint64_t return_off, return_len;    /* Receipt.return_data: data_blob[return_off .. +return_len) (return_off 0 when empty)     */
+    uint64_t version;                   /* with the body: Message.version                                                         */
+    uint64_t sequence;                  /* with the body: Message.sequence (the nonce)                                            */
+    uint64_t gas_limit;                 /* with the body: Message.gas_limit                                                       */
+    uint64_t method_num;                /* with the body: Message.method_num                                                      */
+    uint64_t params_off, params_len;    /* with the body: Message.params, data_blob[params_off .. +params_len) (0 when empty)      */
+    uint32_t status;                    /* IPCFP_MESSAGE_*                                                                        */
+    uint32_t exit_code;                 /* Receipt.exit_code                                                                      */
+    uint8_t has_events_root;
+    uint8_t has_body;                   /* IPCFP_MESSAGE_WITH_BODY and the message executed: the body fields are set              */
+    uint8_t sig_type;                   /* with the body: 0 for a Message block, else the Signature's type byte (1, 2 or 3)        */
+    uint8_t value_negative, gas_fee_cap_negative, gas_premium_negative;
+    uint8_t _pad0[2];
+    uint8_t value[32];                  /* with the body: big-endian magnitudes                                                   */
+    uint8_t gas_fee_cap[32];
+    uint8_t gas_premium[32];
+    uint8_t message_cid[IPCFP_CID_LEN]; /* the request                                                                            */
+    uint8_t events_root[IPCFP_CID_LEN]; /* has_events_root: Receipt.events_root                                                   */
+    ipcfp_address to;                   /* with the body: Message.to                                                              */
+    ipcfp_address from;                 /* with the body: Message.from                                                            */
+} ipcfp_message_proof;
+typedef struct ipcfp_message_result {
+    uint64_t n_proofs;
+    const ipcfp_message_proof* proofs;  /* in request order                                                                       */
+    const uint8_t* data_blob;           /* per proof: its return data, then its params                                            */
+    uint64_t data_blob_size;
+    ipcfp_witness witness;              /* one union, `Cid` order: the base witness, every parent's message AMTs, the receipts root,
+                                         * each executed request's receipts-AMT path and, with the body, the message blocks        */
+    uint64_t n_exec;                    /* length of the execution order                                                          */
+    /* device time (CUDA events on the store's stream), milliseconds: the whole call, the execution order (the requests' sort, the
+     * message-AMT walk and the dedup), the selection and per-request walks, the data-blob gather, the witness; host_syncs: the call's host synchronisations when the message
+     * AMTs take the dense walk (the general walk adds its own) */
+    float ms_total, ms_exec_order, ms_walk, ms_gather, ms_witness;
+    uint32_t host_syncs;
+} ipcfp_message_result;
+/* Proofs of n messages against a resident tipset. flags: IPCFP_WITNESS_BY_REFERENCE (the witness comes by reference, as for the event
+ * calls) and IPCFP_MESSAGE_WITH_BODY. Not executed and no receipt are answers (status), not failures: the first is proven by the message
+ * AMTs, which are in the base witness, the second by the receipts-AMT path up to the node that shows the entry absent.
+ * Failures: a fault in a header, a TxMeta, a message AMT or the receipts root carries the status and index the message-log call reports
+ * for it; then the first fault in request order — a missing or undecodable receipts-AMT node, receipt or message block — with the
+ * request's index; then a base-witness block the store lacks (IPCFP_ERR_MISSING_BLOCK). IPCFP_ERR_INVALID_ARG before any device work:
+ * message_cids NULL with n > 0, n > IPCFP_MESSAGE_MAX, another flag bit. Host synchronisations: five when the message AMTs take the dense
+ * walk — the walk's, the error word with the data lengths, the witness count, the end of the witness copy, the end of the call.
+ * *out is released with ipcfp_message_result_free. */
+ipcfp_status ipcfp_generate_message_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids /* n*38 */, uint64_t n,
+                                                    uint32_t flags, ipcfp_message_result** out);
+/* ipcfp_tipset_upload, then the resident call */
+ipcfp_status ipcfp_generate_message_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const uint8_t* message_cids, uint64_t n, uint32_t flags,
+                                           ipcfp_message_result** out);
+void ipcfp_message_result_free(ipcfp_message_result* r);
+/* One ChainReadObj round for the call above: while the execution order cannot be built, the headers, the receipts root, the TxMetas and
+ * the message AMTs the store lacks; once it can, also each executed request's receipts-AMT path up to the first block the store lacks
+ * and, with IPCFP_MESSAGE_WITH_BODY, its message block. No events AMT is planned. From an empty store the rounds end with a store on
+ * which the generate call gives what it gives on the complete store. flags and refusals are the generate call's. */
+ipcfp_status ipcfp_plan_fetch_message_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n, uint32_t flags,
+                                                      ipcfp_fetch_plan** out);
+/* Replays every proof on the witness store (create it with IPCFP_STORE_VERIFY_CIDS). The tipset is anchored as ipcfp_verify_event_proofs
+ * anchors it: the child header and the parent headers against t, the TxMeta recompute and the execution order rebuilt from the witness.
+ * Then per proof: its position in that order (UINT64_MAX when absent) must be exec_index, the receipt at that position (or its absence)
+ * every receipt field with the return data compared against data_blob, and with IPCFP_MESSAGE_WITH_BODY the message block every body
+ * field with the params compared against data_blob. results[i] = 1 when proof i states exactly what the witness holds, its unnamed
+ * bytes zero; headers that do not match t give 0 for every proof. A missing witness block or a decode error fails the call at that
+ * proof, as ipcfp_verify_actor_proofs does. IPCFP_ERR_INVALID_ARG: NULL arrays with n > 0, n > IPCFP_MESSAGE_MAX, a flag bit other
+ * than IPCFP_MESSAGE_WITH_BODY and IPCFP_WITNESS_BY_REFERENCE. */
+ipcfp_status ipcfp_verify_message_proofs(ipcfp_store* witness_store, const ipcfp_tipset_desc* t, const ipcfp_message_proof* proofs, uint64_t n,
+                                         const uint8_t* data_blob, uint64_t data_blob_size, uint32_t flags, uint8_t* results);
+
+/* ------------------------------------------------------------------------------------------
  * Wire format (src/proofs/common/bundle.rs:10-45, src/proofs/events/bundle.rs:5-30, src/proofs/storage/bundle.rs:5-14): the JSON
  * `serde_json::to_string` gives for UnifiedProofBundle / EventProofBundle — struct field order, compact, CIDs as "bafy2bzace…"
  * strings, "0x" lower-case hex, base64 block data (ProofBlock.cid as the byte array cid 0.11's Serialize emits). t supplies the

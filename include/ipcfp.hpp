@@ -722,6 +722,75 @@ inline std::vector<bool> verify_actor_proofs(const ActorProofs& ap, const Cid& c
     return std::vector<bool>(res.begin(), res.begin() + qs.size());
 }
 
+// ipcfp_generate_message_proofs: whether each message executed in the tipset pair and how it ended (its receipt), and with_body the
+// message itself. A proof keeps the C record (status, exec_index, exit_code, gas_used, events_root, the body fields) with its return
+// data and params; the witness is one union for all proofs.
+struct MessageProof {
+    ipcfp_message_proof c;
+    std::vector<uint8_t> return_data;
+    std::vector<uint8_t> params;         // with_body
+};
+struct MessageProofs {
+    std::vector<MessageProof> proofs;
+    std::vector<ProofBlock> blocks;      // the union, `Cid` order
+};
+inline MessageProofs generate_message_proofs(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                             const std::vector<Cid>& message_cids, bool with_body = false) {
+    TipsetDesc t(parent, child, receipts);
+    const std::vector<uint8_t> cids = detail::cid_bytes(message_cids);
+    ipcfp_message_result* r = nullptr;
+    check(ipcfp_generate_message_proofs(store.raw(), t.c(), cids.empty() ? nullptr : cids.data(), message_cids.size(),
+                                        with_body ? IPCFP_MESSAGE_WITH_BODY : 0u, &r), "generate_message_proofs");
+    MessageProofs out;
+    for (uint64_t i = 0; i < r->n_proofs; i++) {
+        MessageProof p;
+        p.c = r->proofs[i];
+        p.return_data.assign(r->data_blob + p.c.return_off, r->data_blob + p.c.return_off + p.c.return_len);
+        p.params.assign(r->data_blob + p.c.params_off, r->data_blob + p.c.params_off + p.c.params_len);
+        out.proofs.push_back(std::move(p));
+    }
+    out.blocks = proof_blocks(r->witness);
+    ipcfp_message_result_free(r);
+    return out;
+}
+// ipcfp_plan_fetch_message_proofs_resident: one fetch round (the CIDs the store lacks, `Cid` order) for generate_message_proofs
+inline std::vector<Cid> plan_fetch_message_proofs(GpuBlockstore& store, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                                  const std::vector<Cid>& message_cids, bool with_body = false) {
+    TipsetDesc t(parent, child, receipts);
+    const std::vector<uint8_t> cids = detail::cid_bytes(message_cids);
+    ipcfp_tipset* tip = nullptr;
+    check(ipcfp_tipset_upload(store.raw(), t.c(), &tip), "ipcfp_tipset_upload");
+    ipcfp_fetch_plan* p = nullptr;
+    const ipcfp_status st = ipcfp_plan_fetch_message_proofs_resident(store.raw(), tip, cids.empty() ? nullptr : cids.data(), message_cids.size(),
+                                                                     with_body ? IPCFP_MESSAGE_WITH_BODY : 0u, &p);
+    ipcfp_tipset_free(tip);
+    check(st, "plan_fetch_message_proofs");
+    std::vector<Cid> out;
+    for (uint64_t k = 0; k < p->n_missing; k++) out.push_back(Cid::from_bytes(p->cids + IPCFP_CID_LEN * k));
+    ipcfp_fetch_plan_free(p);
+    return out;
+}
+// ipcfp_verify_message_proofs over the proofs' blocks (a store of them with every block checked against its CID): one verdict per proof
+inline std::vector<bool> verify_message_proofs(const MessageProofs& mp, const ApiTipset& parent, const ApiTipset& child, const std::vector<ApiReceipt>& receipts,
+                                               bool with_body = false, int device = 0) {
+    GpuBlockstore store = GpuBlockstore::from_witness(mp.blocks, device);
+    TipsetDesc t(parent, child, receipts);
+    std::vector<ipcfp_message_proof> qs;
+    std::vector<uint8_t> blob;   // each proof's return data, then its params, as the generator lays them out
+    for (const MessageProof& p : mp.proofs) {
+        ipcfp_message_proof q = p.c;
+        q.return_off = p.return_data.empty() ? 0 : blob.size();
+        blob.insert(blob.end(), p.return_data.begin(), p.return_data.end());
+        q.params_off = p.params.empty() ? 0 : blob.size();
+        blob.insert(blob.end(), p.params.begin(), p.params.end());
+        qs.push_back(q);
+    }
+    std::vector<uint8_t> res(qs.size() + 1, 0);
+    check(ipcfp_verify_message_proofs(store.raw(), t.c(), qs.data(), qs.size(), blob.empty() ? nullptr : blob.data(), blob.size(),
+                                      with_body ? IPCFP_MESSAGE_WITH_BODY : 0u, res.data()), "verify_message_proofs");
+    return std::vector<bool>(res.begin(), res.begin() + qs.size());
+}
+
 // the UnifiedProofBundle of an ipcfp_bundle, which it frees
 inline UnifiedProofBundle unified_bundle(ipcfp_bundle* b, const TipsetDesc& t) {
     UnifiedProofBundle u;

@@ -741,6 +741,49 @@ pub fn generate_message_log_proof_gpu(
     Ok((res?, idx.into_iter().map(|i| if i == u64::MAX { None } else { Some(i) }).collect()))
 }
 
+/// A message proof: the C record (`status`, `exec_index`, `exit_code`, `gas_used`, `events_root`, and with the body the message's
+/// fields) with its return data and params. The witness is one union for all proofs.
+pub struct MessageProofGpu {
+    pub proof: sys::ipcfp_message_proof,
+    pub return_data: Vec<u8>,
+    pub params: Vec<u8>,
+}
+
+/// `ipcfp_generate_message_proofs`: whether each message (`message_cids`, as the parent blocks' message AMTs hold them) executed in the
+/// tipset pair and how it ended, from the receipts AMT under the child header; `with_body`: the message block joins the witness and its
+/// fields the proof. → (one proof per message in request order, the witness union in `Cid` order)
+pub fn generate_message_proofs_gpu(
+    store: &GpuBlockstore,
+    parent: &ApiTipset,
+    child: &ApiTipset,
+    receipts: &[ApiReceipt],
+    message_cids: &[Cid],
+    with_body: bool,
+) -> Result<(Vec<MessageProofGpu>, Vec<ProofBlock>)> {
+    let desc = TipsetDesc::new(parent, child, receipts)?;
+    let mut cids = Vec::with_capacity(message_cids.len() * CID_LEN);
+    for c in message_cids {
+        cids.extend_from_slice(&cid38(c)?);
+    }
+    let flags = if with_body { sys::IPCFP_MESSAGE_WITH_BODY } else { 0 };
+    let mut out = std::ptr::null_mut();
+    check(unsafe { sys::ipcfp_generate_message_proofs(store.h, &desc.raw(), cids.as_ptr(), message_cids.len() as u64, flags, &mut out) })?;
+    let r = unsafe { &*out };
+    let result = (|| {
+        let bytes = |off: u64, len: u64| {
+            if len == 0 { Vec::new() } else { unsafe { std::slice::from_raw_parts(r.data_blob.add(off as usize), len as usize) }.to_vec() }
+        };
+        let mut proofs = Vec::with_capacity(r.n_proofs as usize);
+        for i in 0..r.n_proofs as usize {
+            let p = unsafe { *r.proofs.add(i) };
+            proofs.push(MessageProofGpu { proof: p, return_data: bytes(p.return_off, p.return_len), params: bytes(p.params_off, p.params_len) });
+        }
+        Ok((proofs, witness_blocks(&r.witness)?))
+    })();
+    unsafe { sys::ipcfp_message_result_free(out) };
+    result
+}
+
 /// The UnifiedProofBundle of an `ipcfp_bundle`, which it frees.
 fn unified_bundle_of(out: *mut sys::ipcfp_bundle, parent: &ApiTipset, child: &ApiTipset, desc: &TipsetDesc) -> Result<UnifiedProofBundle> {
     let b = unsafe { &*out };

@@ -25,6 +25,7 @@ pub const IPCFP_SHARDED_UNION_FULL: u32 = 0x4;
 pub const IPCFP_WITNESS_BY_REFERENCE: u32 = 0x8;
 pub const IPCFP_RESULT_JSON: u32 = 0x10;
 pub const IPCFP_ACTOR_WITH_CODE: u32 = 0x20;
+pub const IPCFP_MESSAGE_WITH_BODY: u32 = 0x40;
 pub const IPCFP_COMM_ID_BYTES: usize = 128;
 
 #[repr(C)] pub struct ipcfp_store { _p: [u8; 0] }
@@ -159,6 +160,21 @@ pub struct ipcfp_actor_result { pub n_proofs: u64, pub proofs: *const ipcfp_acto
                                 pub proof_witness_offsets: *const u64, pub proof_witness_index: *const u32, pub code_blob: *const u8,
                                 pub code_blob_size: u64, pub ms_total: f32, pub ms_init: f32, pub ms_walk: f32, pub ms_code: f32, pub ms_witness: f32,
                                 pub host_syncs: u32 }
+pub const IPCFP_MESSAGE_EXECUTED: u32 = 0;
+pub const IPCFP_MESSAGE_NOT_EXECUTED: u32 = 1;
+pub const IPCFP_MESSAGE_NO_RECEIPT: u32 = 2;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct ipcfp_message_proof { pub exec_index: u64, pub gas_used: u64, pub return_off: u64, pub return_len: u64, pub version: u64, pub sequence: u64,
+                                 pub gas_limit: u64, pub method_num: u64, pub params_off: u64, pub params_len: u64, pub status: u32, pub exit_code: u32,
+                                 pub has_events_root: u8, pub has_body: u8, pub sig_type: u8, pub value_negative: u8, pub gas_fee_cap_negative: u8,
+                                 pub gas_premium_negative: u8, pub _pad0: [u8; 2], pub value: [u8; 32], pub gas_fee_cap: [u8; 32],
+                                 pub gas_premium: [u8; 32], pub message_cid: [u8; 38], pub events_root: [u8; 38], pub to: ipcfp_address,
+                                 pub from: ipcfp_address }
+#[repr(C)]
+pub struct ipcfp_message_result { pub n_proofs: u64, pub proofs: *const ipcfp_message_proof, pub data_blob: *const u8, pub data_blob_size: u64,
+                                  pub witness: ipcfp_witness, pub n_exec: u64, pub ms_total: f32, pub ms_exec_order: f32, pub ms_walk: f32,
+                                  pub ms_gather: f32, pub ms_witness: f32, pub host_syncs: u32 }
 #[repr(C)]
 pub struct ipcfp_bundle { pub storage: *mut ipcfp_storage_result, pub n_event_results: u64, pub events: *mut *mut ipcfp_event_result, pub witness: ipcfp_witness,
                           pub json: *const c_char, pub json_len: u64, pub ms_total: f32, pub ms_json: f32 }
@@ -268,6 +284,15 @@ extern "C" {
                                                   evm_code_cids: *const u8, n_evm: u64, flags: u32, out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
     pub fn ipcfp_verify_actor_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_actor_proof, n: u64,
                                      evm_code_cids: *const u8, n_evm: u64, flags: u32, results: *mut u8) -> ipcfp_status;
+    pub fn ipcfp_generate_message_proofs_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, message_cids: *const u8, n: u64, flags: u32,
+                                                  out: *mut *mut ipcfp_message_result) -> ipcfp_status;
+    pub fn ipcfp_generate_message_proofs(s: *mut ipcfp_store, t: *const ipcfp_tipset_desc, message_cids: *const u8, n: u64, flags: u32,
+                                         out: *mut *mut ipcfp_message_result) -> ipcfp_status;
+    pub fn ipcfp_message_result_free(r: *mut ipcfp_message_result);
+    pub fn ipcfp_plan_fetch_message_proofs_resident(s: *mut ipcfp_store, t: *mut ipcfp_tipset, message_cids: *const u8, n: u64, flags: u32,
+                                                    out: *mut *mut ipcfp_fetch_plan) -> ipcfp_status;
+    pub fn ipcfp_verify_message_proofs(witness_store: *mut ipcfp_store, t: *const ipcfp_tipset_desc, proofs: *const ipcfp_message_proof, n: u64,
+                                       data_blob: *const u8, data_blob_size: u64, flags: u32, results: *mut u8) -> ipcfp_status;
 
     pub fn ipcfp_bundle_to_json(b: *const ipcfp_bundle, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;
     pub fn ipcfp_event_result_to_json(r: *const ipcfp_event_result, t: *const ipcfp_tipset_desc, out: *mut *mut c_char, out_len: *mut u64) -> ipcfp_status;

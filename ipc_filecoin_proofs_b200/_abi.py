@@ -370,6 +370,90 @@ def actor_result_from_c(r):
                          [idx[int(offs[i]):int(offs[i + 1])].tolist() for i in range(n)], raw, timings, int(r.host_syncs))
 
 
+# Message proofs (include/ipcfp.h, "Message proofs")
+MESSAGE_WITH_BODY = 0x40
+MESSAGE_EXECUTED, MESSAGE_NOT_EXECUTED, MESSAGE_NO_RECEIPT = 0, 1, 2
+
+
+class MessageProofC(C.Structure):
+    """ipcfp_message_proof (400 bytes)."""
+    _fields_ = [("exec_index", C.c_uint64), ("gas_used", C.c_uint64), ("return_off", C.c_uint64), ("return_len", C.c_uint64),
+                ("version", C.c_uint64), ("sequence", C.c_uint64), ("gas_limit", C.c_uint64), ("method_num", C.c_uint64),
+                ("params_off", C.c_uint64), ("params_len", C.c_uint64), ("status", C.c_uint32), ("exit_code", C.c_uint32),
+                ("has_events_root", C.c_uint8), ("has_body", C.c_uint8), ("sig_type", C.c_uint8), ("value_negative", C.c_uint8),
+                ("gas_fee_cap_negative", C.c_uint8), ("gas_premium_negative", C.c_uint8), ("_pad0", C.c_uint8 * 2),
+                ("value", C.c_uint8 * 32), ("gas_fee_cap", C.c_uint8 * 32), ("gas_premium", C.c_uint8 * 32),
+                ("message_cid", C.c_uint8 * CID_LEN), ("events_root", C.c_uint8 * CID_LEN), ("to", AddressC), ("from_", AddressC)]
+
+
+class MessageResultC(C.Structure):
+    """ipcfp_message_result (ipcfp_generate_message_proofs_resident)."""
+    _fields_ = [("n_proofs", C.c_uint64), ("proofs", C.c_void_p), ("data_blob", C.c_void_p), ("data_blob_size", C.c_uint64),
+                ("witness", Witness), ("n_exec", C.c_uint64), ("ms_total", C.c_float), ("ms_exec_order", C.c_float), ("ms_walk", C.c_float),
+                ("ms_gather", C.c_float), ("ms_witness", C.c_float), ("host_syncs", C.c_uint32)]
+
+
+@dataclass
+class MessageProof:
+    """Whether `message_cid` executed (status MESSAGE_*, exec_index or None) and its receipt: exit code, return data, gas used and events
+    root (bytes or None). With the body (has_body): the Message fields, value / gas_fee_cap / gas_premium as signed ints, to / from as
+    Address::to_bytes(), and sig_type (0 for an unsigned Message)."""
+    message_cid: bytes
+    status: int
+    exec_index: int
+    exit_code: int
+    return_data: bytes
+    gas_used: int
+    events_root: bytes
+    has_body: bool = False
+    version: int = 0
+    to: bytes = b""
+    from_: bytes = b""
+    sequence: int = 0
+    value: int = 0
+    gas_limit: int = 0
+    gas_fee_cap: int = 0
+    gas_premium: int = 0
+    method_num: int = 0
+    params: bytes = b""
+    sig_type: int = 0
+
+
+def _signed(mag, negative):
+    m = int.from_bytes(bytes(mag), "big")
+    return -m if negative else m
+
+
+def message_proof_from_c(p, blob=b""):
+    ro, rl, po, pl = int(p.return_off), int(p.return_len), int(p.params_off), int(p.params_len)
+    return MessageProof(bytes(p.message_cid), int(p.status), None if p.exec_index == 2 ** 64 - 1 else int(p.exec_index), int(p.exit_code),
+                        blob[ro:ro + rl], int(p.gas_used), bytes(p.events_root) if p.has_events_root else None, bool(p.has_body),
+                        int(p.version), p.to.to_bytes() if p.has_body else b"", p.from_.to_bytes() if p.has_body else b"", int(p.sequence),
+                        _signed(p.value, p.value_negative), int(p.gas_limit), _signed(p.gas_fee_cap, p.gas_fee_cap_negative),
+                        _signed(p.gas_premium, p.gas_premium_negative), int(p.method_num), blob[po:po + pl], int(p.sig_type))
+
+
+@dataclass
+class MessageResultPy:
+    proofs: list            # MessageProof per request
+    witness: "WitnessPy"
+    data_blob: bytes
+    raw_proofs: np.ndarray  # packed ipcfp_message_proof records (for the verifier)
+    n_exec: int = 0
+    timings: dict = field(default_factory=dict)
+    host_syncs: int = 0
+
+
+def message_result_from_c(r):
+    n = int(r.n_proofs)
+    raw = _arr(r.proofs, n * C.sizeof(MessageProofC), np.uint8)
+    blob = C.string_at(r.data_blob, int(r.data_blob_size)) if r.data_blob_size else b""
+    recs = (MessageProofC * max(n, 1)).from_buffer_copy(raw.tobytes() or bytes(C.sizeof(MessageProofC)))
+    timings = dict(total=r.ms_total, exec_order=r.ms_exec_order, walk=r.ms_walk, gather=r.ms_gather, witness=r.ms_witness)
+    return MessageResultPy([message_proof_from_c(recs[i], blob) for i in range(n)], witness_from_c(r.witness), blob, raw, int(r.n_exec),
+                           timings, int(r.host_syncs))
+
+
 TrustedParentFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32)
 TrustedChildFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.c_void_p)
 

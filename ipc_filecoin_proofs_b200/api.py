@@ -111,6 +111,11 @@ SIGNATURES = {
     "ipcfp_actor_result_free": (None, [_P(A.ActorResultC)]),
     "ipcfp_plan_fetch_actor_proofs_resident": (_st, [_vp, _vp, _P(A.AddressC), _u64, _vp, _u64, _u32, _PP(A.FetchPlanC)]),
     "ipcfp_verify_actor_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _u32, _vp]),
+    "ipcfp_generate_message_proofs_resident": (_st, [_vp, _vp, _vp, _u64, _u32, _PP(A.MessageResultC)]),
+    "ipcfp_generate_message_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _u32, _PP(A.MessageResultC)]),
+    "ipcfp_message_result_free": (None, [_P(A.MessageResultC)]),
+    "ipcfp_plan_fetch_message_proofs_resident": (_st, [_vp, _vp, _vp, _u64, _u32, _PP(A.FetchPlanC)]),
+    "ipcfp_verify_message_proofs": (_st, [_vp, _P(A.TipsetDesc), _vp, _u64, _vp, _u64, _u32, _vp]),
     "ipcfp_bundle_to_json": (_st, _TO_JSON),
     "ipcfp_event_result_to_json": (_st, _TO_JSON),
     "ipcfp_json_free": (None, [_vp]),
@@ -673,6 +678,20 @@ class BlockStore:
         return _result("ipcfp_plan_fetch_actor_proofs_resident", *_FETCH_PLAN, self._h, tip._h, addrs, n, ev.ctypes.data if n_ev else None,
                        n_ev, fl)
 
+    def generate_message_proofs_resident(self, tip, message_cids, with_body=False, flags=0):
+        """ipcfp_generate_message_proofs_resident → A.MessageResultPy: per message CID ((n, 38) bytes, as the message AMTs hold them)
+        whether it executed and its receipt; with_body: MESSAGE_WITH_BODY (the message block joins the witness and its fields the
+        proof). flags: WITNESS_BY_REFERENCE."""
+        cids = np.ascontiguousarray(message_cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+        return _result("ipcfp_generate_message_proofs_resident", A.MessageResultC, A.message_result_from_c, "ipcfp_message_result_free",
+                       self._h, tip._h, cids.ctypes.data if cids.size else None, len(cids), flags | (A.MESSAGE_WITH_BODY if with_body else 0))
+
+    def plan_fetch_message_proofs(self, tip, message_cids, with_body=False, flags=0):
+        """ipcfp_plan_fetch_message_proofs_resident → A.FetchPlanPy: one fetch round for generate_message_proofs_resident."""
+        cids = np.ascontiguousarray(message_cids, dtype=np.uint8).reshape(-1, A.CID_LEN)
+        return _result("ipcfp_plan_fetch_message_proofs_resident", *_FETCH_PLAN, self._h, tip._h, cids.ctypes.data if cids.size else None,
+                       len(cids), flags | (A.MESSAGE_WITH_BODY if with_body else 0))
+
     def close(self):
         if self._h:
             lib().ipcfp_store_destroy(self._h)
@@ -959,6 +978,30 @@ def verify_actor_proofs(witness, ts, result, evm_code_cids=(), with_code=False, 
         res = np.zeros(max(n, 1), dtype=np.uint8)
         _check(lib().ipcfp_verify_actor_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, ev.ctypes.data if n_ev else None, n_ev,
                                                fl, res.ctypes.data))
+        return [bool(x) for x in res[:n]]
+    finally:
+        store.close()
+
+
+def fetch_message_proofs_until_complete(fetch, upload_tipset, message_cids, with_body=False, device=0, verify_cids=True, max_rounds=10000):
+    """fetch_until_complete for generate_message_proofs_resident(tip, message_cids, with_body): the same loop, planned with
+    plan_fetch_message_proofs."""
+    return _fetch_loop(lambda store, tip: store.plan_fetch_message_proofs(tip, message_cids, with_body), fetch, upload_tipset, device,
+                       verify_cids, max_rounds)
+
+
+def verify_message_proofs(witness, ts, result, with_body=False, data_blob=None, device=0):
+    """ipcfp_verify_message_proofs over the witness (WitnessPy) as a CID-checked store: every proof of `result` (A.MessageResultPy, or
+    packed ipcfp_message_proof records with their data_blob) replayed against the tipset `ts` → list of bools."""
+    raw = np.ascontiguousarray(result.raw_proofs if hasattr(result, "raw_proofs") else result, dtype=np.uint8)
+    blob = np.frombuffer(result.data_blob if data_blob is None else data_blob, dtype=np.uint8)
+    n = raw.size // C.sizeof(A.MessageProofC)
+    store = BlockStore(witness.cids, witness.offsets, witness.lengths, witness.blob, device, verify_cids=True)
+    try:
+        d, keep = A.make_tipset_desc(ts)
+        res = np.zeros(max(n, 1), dtype=np.uint8)
+        _check(lib().ipcfp_verify_message_proofs(store._h, C.byref(d), raw.ctypes.data if n else None, n, blob.ctypes.data if blob.size else None,
+                                                 blob.size, A.MESSAGE_WITH_BODY if with_body else 0, res.ctypes.data))
         return [bool(x) for x in res[:n]]
     finally:
         store.close()

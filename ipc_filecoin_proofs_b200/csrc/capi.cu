@@ -473,6 +473,32 @@ ipcfp_status ipcfp_address_from_eth(const uint8_t eth[20], ipcfp_address* out) {
     });
 }
 
+ipcfp_status ipcfp_generate_message_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n, uint32_t flags,
+                                                    ipcfp_message_result** out) {
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_message_proofs(st, td, message_cids, n, flags); });
+}
+ipcfp_status ipcfp_generate_message_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const uint8_t* message_cids, uint64_t n, uint32_t flags,
+                                           ipcfp_message_result** out) {
+    return produce(s != nullptr, out, [&] {
+        message_proof_check(message_cids, n, flags);   // before the upload: no device work for a refused request
+        return with_uploaded_tipset(store_of(s), t, [&](Store* st, TipsetDev& td) { return generate_message_proofs(st, td, message_cids, n, flags); });
+    });
+}
+void ipcfp_message_result_free(ipcfp_message_result* r) { if (r) message_result_free(r); }
+ipcfp_status ipcfp_plan_fetch_message_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const uint8_t* message_cids, uint64_t n, uint32_t flags,
+                                                      ipcfp_fetch_plan** out) {
+    return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) {
+        return make_plan([&](FetchPlan& p) { plan_fetch_message_proofs(st, td, message_cids, n, flags, p); });
+    });
+}
+ipcfp_status ipcfp_verify_message_proofs(ipcfp_store* s, const ipcfp_tipset_desc* t, const ipcfp_message_proof* proofs, uint64_t n,
+                                         const uint8_t* data_blob, uint64_t data_blob_size, uint32_t flags, uint8_t* results) {
+    return guard([&] {
+        if (!s) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+        verify_message_proofs(store_of(s), t, proofs, n, data_blob, data_blob_size, flags, results);
+    });
+}
+
 ipcfp_status ipcfp_generate_actor_proofs_resident(ipcfp_store* s, ipcfp_tipset* t, const ipcfp_address* addrs, uint64_t n,
                                                   const uint8_t* evm_code_cids, uint64_t n_evm, uint32_t flags, ipcfp_actor_result** out) {
     return on_tipset(s, t, out, [&](Store* st, TipsetDev& td) { return generate_actor_proofs(st, td, addrs, n, evm_code_cids, n_evm, flags); });

@@ -278,6 +278,19 @@ void event_matcher(const ipcfp_event_spec* spec, const char* refusal, Matcher& m
 // plan.cu's selection: has_sel[i] (device, n_receipts) = the receipt has an events root and is selected by message_cids (n*38, host)
 // against the execution order exo (the tipset's, built on this store); left as it is when nothing is selected
 void message_selection_mask(Store* s, TipsetDev& td, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint8_t* has_sel);
+// message proofs (message_proof.cu): the execution order of td built with its witness (k_setup's base witness, every message AMT, the
+// receipts root; n_receipts only sizes the walk), and request j's position in it. Faults of the message AMTs and the receipts root are
+// thrown as generate_message_log_proof throws them; a base-witness block the store lacks is left in missing_base. The call's device
+// words are the walk's; DW_N_EXEC is published (read it after the next synchronisation).
+struct MessagePositions {
+    AsyncBuf<uint32_t> wbits;          // the witness bitmap, by Cid rank
+    AsyncBuf<uint64_t> exec_indices;   // n+1: UINT64_MAX where the message is not executed
+    uint32_t receipts_root_blk = 0;
+    bool missing_base = false;
+};
+void message_positions(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, uint32_t flags, MessagePositions& out);
+// … and the same positions in an execution order already built (exo): exec_indices (device, n) as message_positions gives them
+void message_exec_indices(Store* s, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint64_t* exec_indices);
 // verify.cu — batched verifiers over a witness store; n_log_filters > 0: check_event is "matches at least one of log_filters[]", in place
 // of `filter`
 void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* proofs, uint64_t n, const uint8_t* data_blob, uint64_t blob_size,
@@ -462,6 +475,14 @@ struct ActorUpload {
 ipcfp_actor_result* generate_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm_code_cids, uint64_t n_evm,
                                           uint32_t flags);
 void actor_result_free(ipcfp_actor_result* r);
+// message_proof.cu — ipcfp_generate_message_proofs_resident (DESIGN.md §2, "Message proofs"); its refusals come before any device work
+void message_proof_check(const uint8_t* message_cids, uint64_t n, uint32_t flags);
+ipcfp_message_result* generate_message_proofs(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, uint32_t flags);
+void message_result_free(ipcfp_message_result* r);
+// plan.cu — ipcfp_plan_fetch_message_proofs_resident; verify.cu — ipcfp_verify_message_proofs
+void plan_fetch_message_proofs(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, uint32_t flags, FetchPlan& out);
+void verify_message_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_message_proof* proofs, uint64_t n, const uint8_t* data_blob,
+                           uint64_t blob_size, uint32_t flags, uint8_t* results);
 // plan.cu — ipcfp_plan_fetch_actor_proofs_resident; verify.cu — ipcfp_verify_actor_proofs
 void plan_fetch_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs, uint64_t n, const uint8_t* evm_code_cids, uint64_t n_evm,
                              uint32_t flags, FetchPlan& out);

@@ -562,6 +562,7 @@ struct ExecOrderBuild {
     AsyncBuf<uint64_t> g_base[2];
     bool dense_used = false, xch_early = false;
     std::optional<WitnessBuilder> wbuild;
+    bool early_copy = true;   // with witness: snapshot the witness and start its copy behind the walk (false: the caller materialises wbits)
     uint64_t nraw = 0;
     bool xch_stale = false;
     // dedup
@@ -810,7 +811,7 @@ struct ExecOrderBuild {
     // Witness snapshot: base witness + every message-AMT block are final at this point — start moving them to the host while pass 1 /
     // pass 2 run (witness.cu). Publishes the error word, frontier counters, witness counts, dense-walk flag and gather split.
     void snapshot_and_sync(bool with_prologue) {
-        if (with_witness) wbuild->snapshot(wbits.p);
+        if (wbuild) wbuild->snapshot(wbits.p);
         publish_words(s, 0, DW_SPLIT_BYTES + 1);
         if (with_prologue) publish_prologue();
         IPCFP_CUDA(cudaStreamSynchronize(st));
@@ -829,7 +830,7 @@ struct ExecOrderBuild {
             xch_early = xch->all_early;
             if (xch_early) xch->start_exchange(exec_raw.p);
         }
-        if (with_witness) {
+        if (with_witness && early_copy) {
             wbuild.emplace(s);
             wbuild->by_ref = by_ref;
         }
@@ -868,7 +869,7 @@ struct ExecOrderBuild {
             xch->agree_slices(pend_tx, pend_err, 0);
             throw_first(xch->g_tx, xch->g_err);
         }
-        if (with_witness) wbuild->start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_SPLIT_IDX], hw[DW_SPLIT_BYTES]);
+        if (wbuild) wbuild->start_copy(hw[DW_WIT_A], hw[DW_WIT_A_BYTES], hw[DW_SPLIT_IDX], hw[DW_SPLIT_BYTES]);
         if (xch && !xch_early) {
             // LATE H0 (some shard could not promise its slice before its walk was over): agree on the slices now and start the exchange
             xch->agree_slices(IPCFP_NO_ERROR, IPCFP_NO_ERROR, nraw);
@@ -1308,6 +1309,39 @@ void build_execution_order(Store* s, uint32_t n_parents, const uint8_t* txmeta_c
     out.n_exec = b.hw[DW_N_EXEC];
     out.exec_raw = std::move(b.exec_raw);
     out.exec_idx = std::move(b.exec_idx);
+}
+
+void message_positions(Store* s, TipsetDev& td, const uint8_t* message_cids, uint64_t n, uint32_t flags, MessagePositions& out) {
+    ExecOrderBuild ob(s, &td, td.n_parents, td.txmeta_cids.data(), flags & IPCFP_WITNESS_BY_REFERENCE);
+    ob.early_copy = false;
+    ob.stage(0, [](uint8_t*) {});
+    MsgRequests msg;
+    msg.stage(s, message_cids, n);   // read by the walk's synchronisation
+    ob.build(nullptr, 0, nullptr);
+    cudaStream_t st = s->stream;
+    out.exec_indices.alloc(n + 1, st);
+    IPCFP_CUDA(cudaMemsetAsync(out.exec_indices.p, 0xff, (n + 1) * 8, st));
+    // every executed position is selectable (no receipt count bounds it); the bitmap k_msg_select fills is not read
+    AsyncBuf<uint32_t> sel_bits((ob.nraw + 31) / 32 + 8, st);
+    msg.select(st, ob.exec_raw.p, ob.exec_idx.p, ob.n_exec_dev, ob.nraw, UINT64_MAX, out.exec_indices.p, sel_bits.p);
+    publish_words(s, DW_N_EXEC, 1);
+    out.wbits = std::move(ob.wbits);
+    out.receipts_root_blk = ob.receipts_root_blk;
+    out.missing_base = ob.missing_base;
+}
+
+void message_exec_indices(Store* s, const ExecOrderOut& exo, const uint8_t* message_cids, uint64_t n, uint64_t* exec_indices) {
+    cudaStream_t st = s->stream;
+    IPCFP_CUDA(cudaMemsetAsync(exec_indices, 0xff, n * 8, st));
+    if (!n || !exo.n_exec) return;
+    MsgRequests req;
+    req.stage(s, message_cids, n);
+    AsyncBuf<unsigned long long> n_exec(1, st);
+    AsyncBuf<uint32_t> sel_bits((exo.n_exec + 31) / 32 + 8, st);   // k_msg_select's bitmap, not read
+    const unsigned long long ne = exo.n_exec;
+    IPCFP_CUDA(cudaMemcpyAsync(n_exec.p, &ne, 8, cudaMemcpyHostToDevice, st));
+    req.select(st, exo.exec_raw.p, exo.exec_idx.p, n_exec.p, exo.n_exec, UINT64_MAX, exec_indices, sel_bits.p);
+    IPCFP_CUDA(cudaStreamSynchronize(st));   // the host copies above are read until here
 }
 
 __global__ void k_msg_mask(const uint8_t* __restrict__ has_root, const uint32_t* __restrict__ sel_bits, uint64_t n, uint8_t* has_sel) {

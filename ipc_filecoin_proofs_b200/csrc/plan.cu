@@ -103,6 +103,15 @@ __global__ void __launch_bounds__(128) k_plan_actors(ActorArgs a, uint32_t* need
     if (c) plan_miss(miss, ctr, c);
 }
 
+__global__ void __launch_bounds__(128) k_plan_messages(MsgProofArgs a, const uint8_t* receipts_root, uint32_t* needed, uint8_t* miss,
+                                                       unsigned long long* ctr) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.n) return;
+    const uint8_t* m[2];
+    const uint32_t k = plan_message_path(a, receipts_root, t, needed, m);
+    for (uint32_t i = 0; i < k; i++) plan_miss(miss, ctr, m[i]);
+}
+
 __global__ void k_plan_popc(const uint32_t* __restrict__ bits, uint64_t nwords, unsigned long long* out) {
     const uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t c = w < nwords ? (uint32_t)__popc(bits[w]) : 0u;
@@ -329,6 +338,70 @@ void plan_fetch_actor_proofs(Store* s, TipsetDev& td, const ipcfp_address* addrs
     IPCFP_CUDA(cudaStreamSynchronize(st));
     IPCFP_CUDA(cudaEventElapsedTime(&out.ms_total, s->ev[EV_BEGIN], s->ev[EV_END]));
     if (mixed != UINT64_MAX) sort_cids_host(out.cids);
+}
+
+// ipcfp_plan_fetch_message_proofs_resident: the base (headers, receipts root, TxMetas, message AMTs: the message-log planner's rules with no
+// receipt taken); once the execution order can be built, each executed request's receipts-AMT path up to the first block the store lacks
+// and, with the body, its message block. No events AMT is planned.
+void plan_fetch_message_proofs(Store* s, TipsetDev& td, const uint8_t* cids, uint64_t n, uint32_t flags, FetchPlan& out) {
+    message_proof_check(cids, n, flags);
+    s->use();
+    cudaStream_t st = s->stream;
+    Event ev[2];
+    IPCFP_CUDA(cudaEventRecord(ev[0], st));
+    {
+        ipcfp_log_filter any;
+        memset(&any, 0, sizeof any);
+        AsyncBuf<uint8_t> none(td.n_receipts + 64, st);
+        none.zero();
+        plan_fetch(s, td, nullptr, 0, nullptr, 0, out, &any, 1, none.p);
+    }
+    auto finish = [&] {
+        IPCFP_CUDA(cudaEventRecord(ev[1], st));
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        out.ms_total = elapsed_ms(ev[0], ev[1]);
+    };
+    ExecOrderOut exo;
+    try {
+        build_execution_order(s, td.n_parents, td.txmeta_cids.data(), exo);
+    } catch (Error& e) {
+        // a block the walk lacks, or one that does not decode (the generator reports it): the base plan is the round
+        if (e.status != IPCFP_ERR_MISSING_BLOCK && e.status != IPCFP_ERR_DECODE) throw;
+        finish();
+        return;
+    }
+    if (!n) { finish(); return; }
+    AsyncBuf<uint64_t> pos(n + 1, st);
+    message_exec_indices(s, exo, cids, n, pos.p);
+    AsyncBuf<uint8_t> d_in(64 + 38 * n + 16, st), miss(2 * 38 * n + 16, st);
+    IPCFP_CUDA(cudaMemcpyAsync(d_in.p, td.receipts_root, 38, cudaMemcpyHostToDevice, st));
+    IPCFP_CUDA(cudaMemcpyAsync(d_in.p + 64, cids, 38 * n, cudaMemcpyHostToDevice, st));
+    const uint64_t nwords = (s->n + 31) / 32 + 1;
+    AsyncBuf<uint32_t> needed(nwords, st);
+    needed.zero();
+    AsyncBuf<unsigned long long> ctr(PC_COUNT, st);
+    ctr.zero();
+    MsgProofArgs a{};
+    a.store = s->view; a.cids = d_in.p + 64; a.exec_indices = pos.p; a.n = n; a.with_body = (flags & IPCFP_MESSAGE_WITH_BODY) ? 1 : 0;
+    k_plan_messages<<<div_up(n, 128), 128, 0, st>>>(a, d_in.p, needed.p, miss.p, ctr.p); IPCFP_LAUNCH_CHECK();
+    k_plan_popc<<<div_up(nwords, 256), 256, 0, st>>>(needed.p, nwords, ctr.p + PC_NEEDED); IPCFP_LAUNCH_CHECK();
+    PinnedArray hc(s->pool, PC_COUNT * 8);
+    IPCFP_CUDA(cudaMemcpyAsync(hc.p, ctr.p, PC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    const uint64_t n_miss = hc.as<unsigned long long>()[PC_MISSING];
+    out.n_needed += hc.as<unsigned long long>()[PC_NEEDED];   // the paths' blocks are none of the base's
+    if (n_miss) {
+        std::vector<uint8_t> more(38 * n_miss);
+        IPCFP_CUDA(cudaMemcpyAsync(more.data(), miss.p, 38 * n_miss, cudaMemcpyDeviceToHost, st));
+        IPCFP_CUDA(cudaStreamSynchronize(st));
+        out.cids.insert(out.cids.end(), more.begin(), more.end());
+        sort_cids_host(out.cids);
+        std::vector<uint8_t> u;   // unique, in `Cid` order
+        for (uint64_t k = 0; k < out.cids.size() / 38; k++)
+            if (u.empty() || memcmp(u.data() + u.size() - 38, out.cids.data() + 38 * k, 38)) u.insert(u.end(), out.cids.begin() + 38 * k, out.cids.begin() + 38 * k + 38);
+        out.cids.swap(u);
+    }
+    finish();
 }
 
 }  // namespace ipcfp

@@ -5,6 +5,7 @@
 #pragma once
 #include "events_items.cuh"
 #include "actor_items.cuh"
+#include "message_proof_items.cuh"
 #include "storage.cuh"
 
 namespace ipcfp {
@@ -115,6 +116,23 @@ __device__ __forceinline__ const uint8_t* plan_actor_path(const ActorArgs& a, ui
     uint64_t cb;
     if (actor_proof_one(a, a.addrs[t], map, init_fail, rec, q, cb, f) || f.code != DC_MISSING) return nullptr;
     return rec.missing;
+}
+
+// message proofs: request t's receipts-AMT path (plan_receipt_path) at its execution position and, with the body, its message block.
+// Writes the CIDs the store lacks to miss (at most two) and returns how many; a request that was not executed reads nothing.
+__device__ __forceinline__ uint32_t plan_message_path(const MsgProofArgs& a, const uint8_t* receipts_root, uint64_t t, uint32_t* needed,
+                                                      const uint8_t* miss[2]) {
+    const uint64_t e = a.exec_indices[t];
+    if (e == UINT64_MAX) return 0;
+    uint32_t k = 0;
+    if (const uint8_t* m = plan_receipt_path(a.store, receipts_root, e, needed)) miss[k++] = m;
+    if (a.with_body) {
+        const uint8_t* c = a.cids + 38 * t;
+        const int32_t b = store_lookup(a.store, c);
+        if (b < 0) miss[k++] = c;
+        else witness_mark(a.store, needed, (uint32_t)b);
+    }
+    return k;
 }
 
 }  // namespace ipcfp

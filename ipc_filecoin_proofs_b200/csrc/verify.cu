@@ -67,21 +67,17 @@ void verify_event_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event
     verify_event_proofs_dev(s, t, d_proofs.p, n, d_blob.p, blob_size, filter, results, log_filters, n_log_filters);
 }
 
-// the proofs and their data blob (blob_size bytes + 16 of padding) already on the device, on the store's device
-void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
-                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
-    if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
-    if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
-    LogFilterSet fs;
-    fs.build(log_filters, n_log_filters);
-    if (n == 0) return;
+// Once per call, what every proof of a tipset rests on: k_verify_tipset on the witness (d_flags[0]: the headers are consistent, [1]: the
+// receipts root's block), then — consistent headers only — the TxMeta recompute and the execution order exo. Failures throw at the first
+// proof. The error word is reset for the proofs' kernel.
+static void verify_anchor(Store* s, const ipcfp_tipset_desc* t, AsyncBuf<uint32_t>& d_flags, ExecOrderOut& exo) {
     cudaStream_t st = s->stream;
     unsigned long long* dw = s->dev_words.p;
     uint64_t* hw = s->host_words.p;
     const uint32_t P = t->n_parents;
     IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
-    AsyncBuf<uint8_t> d_cids(38ull * (2 * P + 2) + 64, st), d_res(n + 16, st);
-    AsyncBuf<uint32_t> d_flags(8, st);
+    AsyncBuf<uint8_t> d_cids(38ull * (2 * P + 2) + 64, st);
+    d_flags.alloc(8, st);
     IPCFP_CUDA(cudaMemcpyAsync(d_cids.p, t->child_cid, 38, cudaMemcpyHostToDevice, st));
     if (P) IPCFP_CUDA(cudaMemcpyAsync(d_cids.p + 38, t->parent_cids, 38ull * P, cudaMemcpyHostToDevice, st));
     uint8_t* d_tx = d_cids.p + 38ull * (P + 1);
@@ -97,7 +93,6 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));
     if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
-    ExecOrderOut exo;
     if (h_flags[0]) {
         // collect_exec_list(verify_txmeta = true) once for the whole batch: TxMeta recompute, then the engine's own message-AMT walk
         // + first-seen dedup (the same kernels generate_event_proof uses), on the TxMeta links taken from the parent HEADERS
@@ -124,6 +119,23 @@ void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_e
         if (tx_key != IPCFP_NO_ERROR) throw_verify_error(tx_key);
         IPCFP_CUDA(cudaMemsetAsync(dw, 0xff, 8, st));
     }
+}
+
+// the proofs and their data blob (blob_size bytes + 16 of padding) already on the device, on the store's device
+void verify_event_proofs_dev(Store* s, const ipcfp_tipset_desc* t, const ipcfp_event_proof* d_proofs, uint64_t n, const uint8_t* d_blob, uint64_t blob_size,
+                             const ipcfp_event_spec* filter, uint8_t* results, const ipcfp_log_filter* log_filters, uint64_t n_log_filters) {
+    if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
+    if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
+    LogFilterSet fs;
+    fs.build(log_filters, n_log_filters);
+    if (n == 0) return;
+    cudaStream_t st = s->stream;
+    unsigned long long* dw = s->dev_words.p;
+    uint64_t* hw = s->host_words.p;
+    AsyncBuf<uint8_t> d_res(n + 16, st);
+    AsyncBuf<uint32_t> d_flags;
+    ExecOrderOut exo;
+    verify_anchor(s, t, d_flags, exo);
     AsyncBuf<Matcher> d_filter;
     if (filter) {
         Matcher m;
@@ -236,6 +248,52 @@ void verify_actor_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_actor
     up.fill(a.g, s->view, 0, n_evm, flags);
     a.proofs = d_proofs.p; a.n = n; a.results = d_res.p; a.err = dw;
     k_verify_actors<<<div_up(n * 32, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK();
+    IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    if (hw[DW_ERR] != IPCFP_NO_ERROR) throw_verify_error(hw[DW_ERR]);
+}
+
+// ------------------------------------------------------------------------------------------ message proofs
+__global__ void __launch_bounds__(128) k_verify_messages(VerifyMessageArgs a) {
+    const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= a.g.n || (threadIdx.x & 31)) return;
+    verify_message_item(a, t);
+}
+
+void verify_message_proofs(Store* s, const ipcfp_tipset_desc* t, const ipcfp_message_proof* proofs, uint64_t n, const uint8_t* data_blob,
+                           uint64_t blob_size, uint32_t flags, uint8_t* results) {
+    s->use();
+    if (!t || !t->child_cid || (t->n_parents && !t->parent_cids)) throw Error(IPCFP_ERR_INVALID_ARG, "tipset descriptor has null fields");
+    if (t->n_parents > 64) throw Error(IPCFP_ERR_UNSUPPORTED, "too many parent blocks");
+    if ((n && (!proofs || !results)) || (blob_size && !data_blob)) throw Error(IPCFP_ERR_INVALID_ARG, "null argument");
+    message_proof_check(nullptr, 0, flags & ~(uint32_t)IPCFP_WITNESS_BY_REFERENCE);
+    if (n > IPCFP_MESSAGE_MAX) throw Error(IPCFP_ERR_INVALID_ARG, "more message proofs than IPCFP_MESSAGE_MAX");
+    if (n == 0) return;
+    cudaStream_t st = s->stream;
+    unsigned long long* dw = s->dev_words.p;
+    uint64_t* hw = s->host_words.p;
+    AsyncBuf<ipcfp_message_proof> d_proofs(n, st);
+    AsyncBuf<uint8_t> d_blob(blob_size + 16, st), d_res(n + 16, st), d_cids(38 * n + 16, st);
+    IPCFP_CUDA(cudaMemcpyAsync(d_proofs.p, proofs, n * sizeof(ipcfp_message_proof), cudaMemcpyHostToDevice, st));
+    if (blob_size) IPCFP_CUDA(cudaMemcpyAsync(d_blob.p, data_blob, blob_size, cudaMemcpyHostToDevice, st));
+    std::vector<uint8_t> cids(38 * n);
+    for (uint64_t i = 0; i < n; i++) memcpy(cids.data() + 38 * i, proofs[i].message_cid, 38);
+    IPCFP_CUDA(cudaMemcpyAsync(d_cids.p, cids.data(), 38 * n, cudaMemcpyHostToDevice, st));
+    AsyncBuf<uint32_t> d_flags;
+    ExecOrderOut exo;
+    verify_anchor(s, t, d_flags, exo);
+    // every proof's position in the rebuilt order, found as the generator finds it (UINT64_MAX: not executed)
+    AsyncBuf<uint64_t> d_pos(n + 1, st);
+    message_exec_indices(s, exo, cids.data(), n, d_pos.p);
+    uint32_t h_root = 0xffffffffu;
+    IPCFP_CUDA(cudaMemcpyAsync(&h_root, d_flags.p + 1, 4, cudaMemcpyDeviceToHost, st));
+    IPCFP_CUDA(cudaStreamSynchronize(st));
+    VerifyMessageArgs a{};
+    a.g.store = s->view; a.g.cids = d_cids.p; a.g.exec_indices = d_pos.p; a.g.n = n; a.g.receipts_root_blk = h_root;
+    a.g.with_body = (flags & IPCFP_MESSAGE_WITH_BODY) ? 1 : 0; a.g.err = dw;
+    a.proofs = d_proofs.p; a.blob = d_blob.p; a.blob_size = blob_size; a.consistent = d_flags.p; a.results = d_res.p;
+    k_verify_messages<<<div_up(n * 32, 128), 128, 0, st>>>(a); IPCFP_LAUNCH_CHECK();
     IPCFP_CUDA(cudaMemcpyAsync(results, d_res.p, n, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaMemcpyAsync(hw, dw, 8, cudaMemcpyDeviceToHost, st));
     IPCFP_CUDA(cudaStreamSynchronize(st));

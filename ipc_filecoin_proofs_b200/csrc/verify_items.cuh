@@ -7,6 +7,7 @@
 #include "events_items.cuh"
 #include "hashes.cuh"
 #include "actor_items.cuh"
+#include "message_proof_items.cuh"
 #include "storage.cuh"
 
 namespace ipcfp {
@@ -240,6 +241,41 @@ __device__ __forceinline__ void verify_actor_item(const VerifyActorArgs& a, uint
     uint64_t cb;
     if (!actor_proof_one(a.g, p.address, map, init_fail, rec, q, cb, f)) { report_error(a.err, ST_VERIFY, t, f.code, f.detail); return; }
     a.results[t] = actor_claims_equal(q, p, a.g.with_code != 0);
+}
+
+struct VerifyMessageArgs {
+    MsgProofArgs g;                     // the generator's inputs: the proofs' message CIDs, their positions in the rebuilt order, with_body
+    const ipcfp_message_proof* proofs;
+    const uint8_t* blob;                // the caller's data blob, blob_size bytes (+ 16 of padding)
+    uint64_t blob_size;
+    const uint32_t* consistent;
+    uint8_t* results;
+};
+__device__ __forceinline__ bool blob_equal(const uint8_t* blob, uint64_t blob_size, uint64_t off, uint64_t len, const uint8_t* x) {
+    if (off > blob_size || len > blob_size - off) return false;
+    for (uint64_t i = 0; i < len; i++) if (blob[off + i] != x[i]) return false;
+    return true;
+}
+// Proof t is replayed on the witness — its position in the rebuilt execution order, the receipt at that position, with the body the
+// message block — and must state exactly what the replay finds: every field, the return data and params against the caller's blob.
+__device__ __forceinline__ void verify_message_item(const VerifyMessageArgs& a, uint64_t t) {
+    const ipcfp_message_proof& p = a.proofs[t];
+    a.results[t] = 0;
+    if (!*a.consistent) return;
+    ipcfp_message_proof q;
+    memset(&q, 0, sizeof q);
+    const uint8_t *ret, *par;
+    Fail f{0, 0};
+    if (a.g.exec_indices[t] != UINT64_MAX && a.g.receipts_root_blk == 0xffffffffu) { report_error(a.g.err, ST_VERIFY, t, DC_MISSING, 4); return; }
+    if (!message_proof_one(a.g, t, q, ret, par, f)) { report_error(a.g.err, ST_VERIFY, t, f.code, f.detail); return; }
+    q.return_off = p.return_off;
+    q.params_off = p.params_off;
+    const uint8_t* x = reinterpret_cast<const uint8_t*>(&q);
+    const uint8_t* y = reinterpret_cast<const uint8_t*>(&p);
+    for (size_t i = 0; i < sizeof q; i++) if (x[i] != y[i]) return;   // the generator's records are zero where no field is
+    if (ret && !blob_equal(a.blob, a.blob_size, p.return_off, p.return_len, ret)) return;
+    if (par && !blob_equal(a.blob, a.blob_size, p.params_off, p.params_len, par)) return;
+    a.results[t] = 1;
 }
 
 }  // namespace ipcfp
